@@ -1,7 +1,7 @@
 // grk_ref_bench -- the reference arm of bench.py: times the UNMODIFIED reference's own public API,
 // grk_compress() into a memory stream and grk_decompress() from it (grok.h; the flow follows the
 // reference's examples/core/core_compress.cpp and core_decompress.cpp), on caller-provided planes.
-// Built by baseline/build_ref.sh against baseline/_ref/bin/libgrokj2k.so; called from bench.py and the
+// Built by oracle/build_ref.sh against oracle/_ref/grok/bin/libgrokj2k.so; called from bench.py and the
 // interop tests through ctypes.  Test / measurement infrastructure -- the product never links it.
 #include <chrono>
 #include <cstdint>

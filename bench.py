@@ -13,8 +13,8 @@ decoded once per step.
   roofline  the dominant memory-bound kernel: the fused DC-shift + RCT + level-1 5/3 DWT
           (k_dwt53_fwd<3>): algorithmic bytes = samples x 8 B (one 4-byte read + one 4-byte
           write per sample per level, SURVEY.md 8d) / CUDA-event duration of that launch
-  cpu_baseline  the UNMODIFIED reference library (baseline/_ref/bin/libgrokj2k.so.1, built from
-          /root/reference by baseline/build_ref.sh): grk_compress() into a memory stream +
+  cpu_baseline  the UNMODIFIED reference library (oracle/_ref/grok/bin/libgrokj2k.so.1, built from
+          the reference tree by oracle/build_ref.sh): grk_compress() into a memory stream +
           grk_decompress() from it (grok.cpp L1025 ff.; harness baseline/grk_ref_bench.cpp), same
           image, all host threads and one thread; the round-1 kernel composite (oracle/_ref) is
           kept as a second, labelled figure
@@ -22,6 +22,9 @@ decoded once per step.
 `--impl reference` times that CPU path (grk_compress + grk_decompress) as the step.  N>1 (torchrun): one process per GPU, each
 rank runs the whole workload on its own image ("weak": tiles shard with no data-path
 collective; NCCL only carries the barrier / max-reduction and the coded-size gather).
+
+`--dump-outputs DIR` writes, after the timed steps, what the last device-resident step computed (see dump_outputs()).
+The image is generated from a fixed seed, so two builds given the same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -57,11 +60,11 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s), not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -123,6 +126,17 @@ class ClockSampler:
                     reasons.add(n)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def gpu_info(index):
+    """The card a number was measured on: its name and the power limit it runs under (both part of the number)."""
+    try:
+        name, limit = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                                     stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip().split(", ")
+        return {"name": name, "power_limit_w": float(limit)}
+    except Exception:
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -227,7 +241,7 @@ def cpu_quota():
 
 
 # ------------------------------------------------------------------------------------------------
-# The reference itself: libgrokj2k's public API on memory streams (tests/grok_ref.py -> baseline/_ref)
+# The reference itself: libgrokj2k's public API on memory streams (tests/grok_ref.py -> oracle/_ref/grok)
 # ------------------------------------------------------------------------------------------------
 def grok_setup(img, w=W, h=H):
     import grok_ref as R
@@ -308,7 +322,7 @@ def run_reference(args, rank, world):
     img = make_image()
     st = grok_setup(img)
     if st is None:
-        print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref (libgrokj2k built from /root/reference) is not in the tree"}))
+        print(json.dumps({"impl": "reference", "unavailable": "oracle/_ref/grok (libgrokj2k built from the reference tree) is not in the tree"}))
         return
     grok_tune_threads(st)
     for _ in range(args.warmup):
@@ -334,7 +348,7 @@ def run_reference(args, rank, world):
             "decode_only": {"value": W * H / float(np.mean(decs)) / 1e6, "unit": "Mpixels/s", "ms": float(np.mean(decs)) * 1e3},
             "cpu_baseline": {"value": val, "unit": "Mpixels/s", "cores": st["threads"], "cpu_quota": cpu_quota(), "kind": "reference",
                              "sample": "whole image (64 of 64 tiles) per step: grk_compress() + grk_decompress() of the unmodified "
-                                       "libgrokj2k (baseline/_ref) on memory streams, TLM + PLT, %d threads" % st["threads"]},
+                                       "libgrokj2k (oracle/_ref/grok) on memory streams, TLM + PLT, %d threads" % st["threads"]},
             "e2e": {"value": val, "unit": "Mpixels/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line))
 
@@ -488,7 +502,7 @@ def run_config4(args, rank, world, local):
                            "timing": "host wall clock around the K steps incl. barriers, max over ranks (the step ends on the host: the code stream is in host memory)",
                            "codestream_bytes": int(cs_len), **info},
                 "e2e": {"value": pix / dt / 1e6, "unit": "Mpixels/s", "h2d_bytes_per_step": int(W4 * H4 * NC4 * 2), "d2h_bytes_per_step": int(cs_len)},
-                "clocks": clocks}
+                "gpu": gpu_info(local), "clocks": clocks}
         print(json.dumps(line))
     if dist is not None:
         dist.barrier()
@@ -504,7 +518,11 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--workload", default="config2", choices=["config2", "config4"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last device-resident step computed as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.workload != "config2":
+        raise SystemExit("bench.py: --dump-outputs covers the config2 workload")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -572,6 +590,11 @@ def main():
     launches = lib.b2k_launch_count() - l0
     job.download(out)
     assert all(np.array_equal(a, b) for a, b in zip(out, planes)), "device-resident round trip is not lossless"
+    dumped = None
+    if args.dump_outputs and rank == 0:
+        res = job.fetch_result()
+        dumped = dump_outputs(args.dump_outputs, out, res)
+        res.free()
     pipe = None
     if world == 1 or bool(os.environ.get("B2K_BENCH_ALL_LEGS")):
         # extra: the same K round trips with the block-coder stage pipelined over 2 block ranges on 2 streams
@@ -630,10 +653,10 @@ def main():
             e2e_step()
         barrier()
         t0 = time.perf_counter()
-        for _ in range(max(3, args.steps // 2)):
+        for _ in range(args.steps):
             e2e_step()
         barrier()
-        dt_e2e32 = (time.perf_counter() - t0) / max(3, args.steps // 2)
+        dt_e2e32 = (time.perf_counter() - t0) / args.steps
         assert all(np.array_equal(a, b) for a, b in zip(out, planes)), "e2e (no host packing) round trip is not lossless"
         G.set_host_threads(-1)
 
@@ -649,10 +672,10 @@ def main():
             file_step()
         barrier()
         t0 = time.perf_counter()
-        for _ in range(max(3, args.steps // 2)):
+        for _ in range(args.steps):
             cs_len = file_step()
         barrier()
-        dt_file = (time.perf_counter() - t0) / max(3, args.steps // 2)
+        dt_file = (time.perf_counter() - t0) / args.steps
         assert all(np.array_equal(a, b) for a, b in zip(out, planes)), "codestream round trip is not lossless"
 
         # ---------------- same, 16-bit sample containers (b2k_encode16 / b2k_decode16) ----------------
@@ -721,7 +744,7 @@ def main():
 
         streamed(3 * depth + 3)           # warm-up: every worker's engine has built its job, the pinned result arenas exist
         barrier()
-        n_stream = max(16, args.steps)
+        n_stream = args.steps
         dt_stream = streamed(n_stream) / n_stream
         barrier()
         enc_stream.end()
@@ -755,7 +778,7 @@ def main():
             "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "i32", "data": "synthetic",
             "config": {"workload": WORKLOAD, "timing": "CUDA events around the K queued steps, max over ranks; host wall clock of the same region incl. barriers: %.3f ms/step" % (wall_dev / args.steps * 1e3), "per_gpu": "one 8192x8192x3 image (64 tiles) per rank", "numa_node": numa, "cpus_per_rank": ncpus,
-                       "l2": "inputs (805 MB of planes per step) are larger than the 126 MB L2",
+                       "l2": "inputs (805 MB of planes per step) are larger than the 50 MB L2",
                        "coded_bytes": int(nbytes), "blocks": int(nbk),
                        "ht_encode_Mblocks_s": nbk / (stage[1] / args.steps * 1e-3) / 1e6,
                        "ht_decode_Mblocks_s": nbk / (stage[2] / args.steps * 1e-3) / 1e6,
@@ -770,12 +793,12 @@ def main():
                     "api": "b2k_encode + b2k_decode (include/grok_b200.h), host int32 planes (the gpup_image layout); samples "
                            "<= 16 bit cross PCIe in 16-bit containers, narrowed/widened per chunk by host_threads host threads"},
             "gpu_launches": int(launches),
+            "gpu": gpu_info(local),
             "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": "k_dwt53_fwd<3> (DC shift + RCT + level-1 5/3, all 64 tiles x 3 comps)",
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "peak_source": peak_src, "frac_of_nominal_8000_GBs": achieved / 8000.0,
-                         "algorithmic_bytes_per_launch": int(l1_bytes),
-                         "ms_per_launch": l1_ms, "traffic": TRAFFIC_NCU},
+                         "peak_source": peak_src, "algorithmic_bytes_per_launch": int(l1_bytes),
+                         "ms_per_launch": l1_ms},
         }
         if pipe is not None:
             line["device_pipelined"] = pipe
@@ -809,7 +832,7 @@ def main():
                 cb = {"value": W * H / sec / 1e6, "unit": "Mpixels/s", "cores": gs["threads"], "cpu_quota": cpu_quota(),
                       "kind": "reference", "host": cpu_model(),
                       "sample": "whole image (64 of 64 tiles), best of 3 passes: grk_compress() + grk_decompress() of the unmodified "
-                                "libgrokj2k (baseline/_ref) on memory streams, TLM + PLT",
+                                "libgrokj2k (oracle/_ref/grok) on memory streams, TLM + PLT",
                       "encode_only_Mpix_s": W * H / info["enc_s"] / 1e6, "decode_only_Mpix_s": W * H / info["dec_s"] / 1e6, **info}
                 # one thread, on a 2048x2048 corner (4 of 64 tiles) so that it stays bounded
                 g1 = grok_setup(img, 2048, 2048)
@@ -824,7 +847,7 @@ def main():
                                                    "device_resident": value / cb["value"]}
             else:
                 line["cpu_baseline"] = {"value": None, "unit": "Mpixels/s", "cores": 0, "kind": "reference",
-                                        "sample": "baseline/_ref not built"}
+                                        "sample": "oracle/_ref/grok not built"}
             st = cpu_reference_setup(img)
             if st is not None:   # round 1's figure, kept for continuity: kernels only, no T2 / streams / scheduler
                 tune_reference_threads(st)
@@ -832,6 +855,8 @@ def main():
                 line["cpu_kernel_composite"] = {"value": W * H / sec / 1e6, "unit": "Mpixels/s", "cores": st["threads"],
                                                 "sample": "whole image, best of 2: the reference's HT coder + forward DWT kernels and its "
                                                           "grk_bench_dwt_53 hook driven by oracle/ref_shim (no T2, no streams)", **info}
+        if dumped is not None:
+            line["dump_outputs"] = dumped
         print(json.dumps(line))
     if dist is not None:
         dist.barrier()
@@ -839,11 +864,25 @@ def main():
     eng.close()
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum of one k_dwt53_fwd<3> launch, from the committed `ncu --set full` capture
-# of THIS kernel version (profiles/r02v_dwt53_fwd_ncu_full_summary.txt, captured 2026-09-24 on the round-2 bulk-copy
-# kernel: 877.08 MB read + 762.23 MB written = 1.018 x the algorithmic bytes).  A constant, not a per-run counter:
-# re-capture when the kernel changes.
-TRAFFIC_NCU = 1639311616
+DUMP_SAMPLES = 1 << 21   # per decoded plane; the coded-byte sample is twice that
+
+
+def dump_outputs(dirname, out, res):
+    """What a caller of the device-resident round trip receives from its last step: the decoded planes and the coded
+    code blocks.  Both are larger than is worth keeping, so a fixed, seeded sample of positions is written (float32,
+    ~41 MB in all): decoded_c<k>.npy (samples of plane k), coded_bytes.npy (bytes of the concatenated block arena) and
+    block_lengths.npy (every block's coded length, float64).  Returns {name: shape}."""
+    d = os.path.abspath(os.path.expanduser(dirname))
+    os.makedirs(d, exist_ok=True)
+    rng = np.random.default_rng(SEED)
+    pix = np.sort(rng.integers(0, W * H, DUMP_SAMPLES))
+    arrays = {"decoded_c%d" % c: p.reshape(-1)[pix].astype(np.float32) for c, p in enumerate(out)}
+    pos = np.sort(rng.integers(0, max(1, res.num_bytes), 2 * DUMP_SAMPLES))
+    arrays["coded_bytes"] = res.bytes[pos].astype(np.float32)
+    arrays["block_lengths"] = res.blocks["length"].astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), a)
+    return {"dir": d, "arrays": {k: list(a.shape) for k, a in arrays.items()}}
 
 if __name__ == "__main__":
     main()

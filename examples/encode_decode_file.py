@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Encode an image to an HTJ2K file on the GPU and read it back (needs a B200; uses only the public API).
+"""Encode an image to an HTJ2K file on the GPU and read it back (needs an H100; uses only the public API).
 
   python examples/encode_decode_file.py in.ppm out.jph [--lossy] [--tile 1024]      # PGM / PPM (8 or 16 bit) in, .jph or .j2c out
   python examples/encode_decode_file.py --decode in.jph out.ppm

@@ -1,6 +1,6 @@
-"""grok_b200 -- host-side Python mirror of the B200 JPEG 2000 tile engine's C ABI.
+"""grok_b200 -- host-side Python mirror of the JPEG 2000 tile engine's C ABI.
 
-The product is ``libgrokj2k_plugin.so`` (hand-written sm_100a CUDA behind the C ABI of
+The product is ``libgrokj2k_plugin.so`` (hand-written sm_90a CUDA behind the C ABI of
 ``include/grok_b200.h``); this module is only the ctypes doorway tests, ``bench.py`` and Python
 hosts use.  It mirrors the reference's plugin surface (``src/lib/core/plugin/plugin_interface.h``,
 ``gpup/gpu_plugin_shared.h``): same entry-point names, argument meaning and return convention

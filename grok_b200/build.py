@@ -1,4 +1,4 @@
-"""Build libgrokj2k_plugin.so (CUDA kernels + C ABI) in-tree with nvcc for sm_100a."""
+"""Build libgrokj2k_plugin.so (CUDA kernels + C ABI) in-tree with nvcc for sm_90a (H100)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgrokj2k_plugin.so")
 SOURCES = ["engine.cu", "dwt.cu", "ht_enc.cu", "ht_dec.cu", "geometry.cpp", "plugin.cpp", "plugin_decode.cpp", "host_pack.cpp", "codestream.cpp", "stream.cpp", "plugin_batch.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function", "--use_fast_math=false"]
 FLAGS = [f for f in FLAGS if not f.startswith("--use_fast_math")]
 
@@ -41,7 +41,7 @@ def build(force=False, verbose=False):
             raise RuntimeError("nvcc failed on " + src)
         if verbose and out:
             print(out.decode())
-    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-lpthread"]
+    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-lpthread"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -1,6 +1,6 @@
 /*
  * grok_b200/csrc/dwt.cu -- forward / inverse lifting DWT (reversible 5/3, irreversible 9/7) for
- * sm_100a, one decomposition level per launch, with the DC level shift and the RCT / ICT
+ * sm_90a, one decomposition level per launch, with the DC level shift and the RCT / ICT
  * multi-component transform fused into the finest level.
  *
  * What it replaces in the reference (CPU, Highway SIMD + Taskflow):
@@ -10,7 +10,7 @@
  *                                                     wavelet/WaveletReverse97.cpp L837-857, L950-
  *             DecompressRev / DecompressIrrev         point_transform/mct.cpp L201-256, L318-391
  *
- * B200 design (not a port of the column-strip SIMD loops):
+ * Design (not a port of the column-strip SIMD loops):
  *   - one warp = one job = (tile component(s), 8*strip_w-column strip, row segment).  Each lane
  *     owns 8 consecutive canvas columns (two 128-bit loads per row).  The reference's
  *     "all columns, then all rows" double pass is fused: rows stream through a register

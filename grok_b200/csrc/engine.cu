@@ -1,5 +1,5 @@
 /*
- * grok_b200/csrc/engine.cu -- the B200 tile engine behind include/grok_b200.h.
+ * grok_b200/csrc/engine.cu -- the tile engine behind include/grok_b200.h.
  *
  * Replaces, for the tiles it is given, the per-tile pipeline of the reference
  *   encode: TileProcessorCompress::preCompressTile / buildCompressDAG / doCompress
@@ -67,7 +67,7 @@ struct b2k_engine
  * Jobs come and go with the coding (every windowed decode is a new virtual image, SURVEY 8f N3) and cudaMalloc /
  * cudaFree synchronise the device and cost milliseconds per gigabyte.  Freed job buffers are kept per device and
  * handed out again to requests of about the same size (best fit, at most 25 % slack); the cache is trimmed, largest
- * first, above B2K_DEV_CACHE_GB (default 32). */
+ * first, above B2K_DEV_CACHE_GB (default 16: a fifth of an H100's 80 GB, more than config 4's job needs). */
 namespace {
 struct DevCache
 {
@@ -81,7 +81,7 @@ size_t dev_cache_limit()
 {
   static const size_t v = [] {
     const char* e = getenv("B2K_DEV_CACHE_GB");
-    return (size_t)(e ? atof(e) : 32.0) << 30;
+    return (size_t)(e ? atof(e) : 16.0) << 30;
   }();
   return v;
 }

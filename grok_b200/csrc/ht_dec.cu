@@ -1,5 +1,5 @@
 /*
- * grok_b200/csrc/ht_dec.cu -- HTJ2K (ITU-T T.814) cleanup-pass block DECODER for sm_100a, one
+ * grok_b200/csrc/ht_dec.cu -- HTJ2K (ITU-T T.814) cleanup-pass block DECODER for sm_90a, one
  * warp per code block, fused with the T1 post-processing (dequantisation into the Mallat buffer).
  *
  * Replaces (reference, CPU): T1OJPH::decompress            t1/part15/CoderOJPH.cpp L212-262

@@ -1,5 +1,5 @@
 /*
- * grok_b200/csrc/ht_enc.cu -- HTJ2K (ITU-T T.814) cleanup-pass block ENCODER for sm_100a,
+ * grok_b200/csrc/ht_enc.cu -- HTJ2K (ITU-T T.814) cleanup-pass block ENCODER for sm_90a,
  * one warp per code block, fused with the T1 pre-processing (sign-magnitude conversion and,
  * for the irreversible path, scalar quantisation).
  *
@@ -44,10 +44,10 @@ namespace {
 #define ENC_MIN_CTAS 1
 #endif
 /* warps (= code blocks in flight) per CTA, at most: ONE persistent CTA per SM.  For 64-wide blocks a warp needs 9.3 KB of
-   shared memory and the CTA 8.3 KB of tables: 20 warps = 194 KB.  Measured on config 2 (tools/build_variant.py):
-   20 x 1 CTA 1.53 ms, 5 x 4 CTAs 1.66 ms (same warps per SM, but four table copies and 228 KB of shared memory leave the
-   L1 its minimum), 16 x 1 1.68, 23 x 1 1.53, 10 x 2 1.63.  Launches with wider blocks (more shared memory per warp) run
-   with fewer warps per CTA: the kernel takes its warp count from blockDim. */
+   shared memory and the CTA 8.3 KB of tables: 20 warps = 194 KB of the 227 KB a block may opt into on sm_90, so one CTA
+   per SM, its tables loaded once (several smaller CTAs per SM would each carry a copy of the tables and leave the L1
+   its minimum).  ENC_WARPS_N / ENC_MIN_CTAS let tools/build_variant.py build other shapes for A/B runs.  Launches with
+   wider blocks (more shared memory per warp) run with fewer warps per CTA: the kernel takes its warp count from blockDim. */
 constexpr int ENC_WARPS = ENC_WARPS_N;
 constexpr int UNIT_QUADS = 8;       /* quads per unit (even: the VLC stream codes quads in pairs) */
 constexpr int MS_RING_WORDS = 128;  /* 4096 bits: < 1024 left by the last drain + one 2048-bit gather batch */
@@ -983,7 +983,7 @@ void b2k_launch_ht_encode(const HtBlockDesc* d_blocks, HtBlockOut* d_out, uint8_
   const size_t table_bytes = 2 * 2048 * sizeof(uint16_t) + 64 * sizeof(uint16_t), smem_max = 227 * 1024;
   /* as many warps per CTA as the opt-in maximum of shared memory holds */
   uint32_t cta_warps = (uint32_t)std::max<size_t>(1, std::min<size_t>(ENC_WARPS, (smem_max - table_bytes) / (warp_words * sizeof(uint32_t))));
-  int dev = 0, sms = 148, per_sm = 1;
+  int dev = 0, sms = 132, per_sm = 1;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   if(nblocks < (uint32_t)sms * cta_warps) /* a small launch: fewer warps per CTA, every SM still gets one */
@@ -995,7 +995,7 @@ void b2k_launch_ht_encode(const HtBlockDesc* d_blocks, HtBlockOut* d_out, uint8_
   once.run([&] {
     for(Kernel k : variants)
     {
-      cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); /* the opt-in maximum of sm_100 */
+      cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); /* the opt-in maximum of sm_90 */
       /* the kernel lives on shared memory (staged samples, per-lane bit strings): without this hint the driver may
          size the carve-out for fewer CTAs per SM than fit */
       cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);

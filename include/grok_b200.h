@@ -1,5 +1,5 @@
 /*
- * include/grok_b200.h -- C ABI of libgrokj2k_plugin.so, the B200-native JPEG 2000 tile engine.
+ * include/grok_b200.h -- C ABI of libgrokj2k_plugin.so, the CUDA (sm_90a, H100) JPEG 2000 tile engine.
  *
  * Two groups of entry points:
  *

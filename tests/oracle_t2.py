@@ -8,7 +8,7 @@ so that the two can be compared byte for byte.  It follows the reference's write
   tag tree              t2/TagTree.h (encode with threshold, value known once written)
   bit stuffing          t1_t2 BitIO: after a 0xFF byte the next one carries 7 bits; flush appends a byte after 0xFF
 Pinning: whole codestreams written this way are byte-identical to grk_compress's (the real libgrokj2k built by
-baseline/build_ref.sh; tests/test_interop.py, COM marker aside), and OpenJPEG decodes them (tests/test_codestream.py).
+oracle/build_ref.sh; tests/test_interop.py, COM marker aside), and OpenJPEG decodes them (tests/test_codestream.py).
 Pure Python loops: small cases only."""
 import numpy as np
 

@@ -518,8 +518,7 @@ def test_refinement_passes_of_foreign_streams(engine, case):
 def test_corrupt_streams_are_rejected_or_decoded_never_fatal(engine):
     """Damaged block tables / byte arenas (flipped bytes, garbage Scup, wrong lengths, impossible bit-plane
     counts, bogus refinement segments): b2k_decode either decodes or reports rejected blocks (-2) or a bad
-    table (-1); it never faults, and the engine decodes a clean stream right afterwards.  (Run under
-    compute-sanitizer memcheck in profiles/r01g_memcheck.txt.)"""
+    table (-1); it never faults, and the engine decodes a clean stream right afterwards."""
     w, h = 256, 192
     cp = G.make_coding(w, h, 3, 12, numres=4)
     planes = P.synthetic_image(w, h, 3, 12, seed=5)

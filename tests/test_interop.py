@@ -1,6 +1,6 @@
 """Interop parity gate against the REAL reference library (BASELINE.md 3.6).
 
-baseline/_ref/bin/libgrokj2k.so.1 is the unmodified GrokImageCompression/Grok built by baseline/build_ref.sh
+oracle/_ref/grok/bin/libgrokj2k.so.1 is the unmodified GrokImageCompression/Grok built by oracle/build_ref.sh
 (SURVEY.md 8c recipe); tests/grok_ref.py drives its public API (grk_compress / grk_decompress on memory streams).
 What is pinned here, on the reference's own outputs:
 
@@ -13,22 +13,24 @@ What is pinned here, on the reference's own outputs:
   <= 8-bit irreversible images through its 16-bit fixed-point engine: a different algorithm; there the bar is
   the reference's own <= 2 codes, GrkPluginBatchMemoryTest.cpp L35-45).
 
-The CPU tests use the oracle as the block coder (no GPU), the `-m gpu` tests the CUDA engine.  Everything skips
-when baseline/_ref was not built (no reference tree at build time)."""
+The CPU tests use the oracle as the block coder (no GPU), the `-m gpu` tests the CUDA engine.  Where the library is
+not built, Grok's outputs come from the record in tests/golden/ (tests/grok_golden.py): digests of its code streams
+and decodes, seeded samples where a comparison has a tolerance."""
 import numpy as np
 import pytest
 
 import grok_b200 as G
+import grok_golden as GG
 import grok_ref as R
 import oracle_pipeline as P
+from grok_golden import grok
 from test_codestream import oracle_decode, oracle_encode
-
-pytestmark = pytest.mark.skipif(not R.available(), reason="baseline/_ref (the reference library) is not built")
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _grok():
-    R.init(4)
+    if R.available():
+        R.init(4)
     yield
 
 
@@ -52,6 +54,17 @@ def grok_compress(args, planes):
                        irreversible=args.get("irreversible", False), tlm=True, plt=True, cblk=args.get("cblk", (64, 64)),
                        precinct=args.get("grok_precinct"))
     return np.frombuffer(bytes(cs), np.uint8)
+
+
+def grok_stream(args, seed, ours):
+    """grk_compress's code stream of synth(args, seed), live or from the record (then rebuilt from ours)"""
+    return GG.grok_stream(GG.key("stream", args, seed), ours, grok(lambda: grok_compress(args, synth(args, seed))))
+
+
+def grok_decode(cs, args, reduce=0):
+    """a callable giving grk_decompress's planes of cs (None without the library)"""
+    w, h, n = args["width"], args["height"], args["numcomps"]
+    return grok(lambda: R.decompress(cs, -(-w >> reduce), -(-h >> reduce), n, reduce=reduce)[0])
 
 
 def block_bytes(table, data, i):
@@ -96,12 +109,10 @@ def test_reversible_codestream_is_byte_identical_to_grok(args):
     planes = synth(args)
     table, data, _ = oracle_encode(cp, planes)
     ours = G.codestream_write(cp, table, data, G.CS_TLM | G.CS_PLT)
-    theirs = grok_compress(args, planes)
+    theirs = grok_stream(args, 5, ours)
     assert bytes(ours) == strip_com(theirs)
     # Grok decodes ours exactly
-    dec, _, _ = R.decompress(ours, args["width"], args["height"], args["numcomps"])
-    for a, b in zip(dec, planes):
-        assert np.array_equal(a, b)
+    GG.same(GG.key("grok decode of ours", args, 5), planes, grok_decode(ours, args))
     # we decode Grok's exactly, block bytes equal
     cp2, blocks = G.codestream_parse(theirs)
     assert len(blocks) == len(table)
@@ -117,11 +128,11 @@ def test_precinct_spec_shorter_than_resolutions_matches_grok():
     (CodeStreamCompress.cpp L793-825).  The packet order then depends on the derived precinct grid."""
     args = dict(width=600, height=500, numcomps=3, prec=12, numres=5)
     planes = synth(args)
-    theirs, _ = R.compress(planes, 12, numres=5, tlm=True, plt=True, precinct=(128, 128))
-    theirs = np.frombuffer(bytes(theirs), np.uint8)
     cp = G.make_coding(precincts=[(max(128 >> k, 2),) * 2 for k in range(5)][::-1], **args)
     table, data, _ = oracle_encode(cp, planes)
     ours = G.codestream_write(cp, table, data, G.CS_TLM | G.CS_PLT)
+    theirs = GG.grok_stream(GG.key("stream, -c [128,128]", args, 5), ours,
+                            grok(lambda: R.compress(planes, 12, numres=5, tlm=True, plt=True, precinct=(128, 128))[0]))
     assert bytes(ours) == strip_com(theirs)
 
 
@@ -131,16 +142,14 @@ def test_irreversible_blocks_are_byte_identical_to_grok(args):
     planes = synth(args)
     table, data, _ = oracle_encode(cp, planes)
     ours = G.codestream_write(cp, table, data, G.CS_TLM | G.CS_PLT)
-    theirs = grok_compress(args, planes)
+    theirs = grok_stream(args, 5, ours)
     cp2, blocks = G.codestream_parse(theirs)
     same = sum(int(np.array_equal(block_bytes(table, data, i), block_bytes(blocks, theirs, i))) for i in range(len(table)))
     assert same == len(table), "%d of %d irreversible code blocks equal Grok's" % (same, len(table))
     assert bytes(ours) == strip_com(theirs)
     # decode: ours of theirs == Grok's of theirs, sample for sample (precision >= 9)
-    gd, _, _ = R.decompress(theirs, args["width"], args["height"], args["numcomps"])
     od = oracle_decode(cp2, blocks, theirs)
-    for a, b in zip(gd, od):
-        assert np.array_equal(a, b)
+    GG.same(GG.key("grok decode", args, 5), od, grok_decode(theirs, args))
 
 
 def test_irreversible_8bit_decode_within_reference_tolerance():
@@ -150,14 +159,13 @@ def test_irreversible_8bit_decode_within_reference_tolerance():
     cp = mk(args)
     planes = synth(args)
     table, data, _ = oracle_encode(cp, planes)
-    theirs = grok_compress(args, planes)
+    ours = G.codestream_write(cp, table, data, G.CS_TLM | G.CS_PLT)
+    theirs = grok_stream(args, 5, ours)
     cp2, blocks = G.codestream_parse(theirs)
     for i in range(len(table)):
         assert np.array_equal(block_bytes(table, data, i), block_bytes(blocks, theirs, i))
-    gd, _, _ = R.decompress(theirs, 320, 256, 3)
     od = oracle_decode(cp2, blocks, theirs)
-    for a, b in zip(gd, od):
-        assert np.abs(a.astype(np.int64) - b).max() <= 2
+    GG.close(GG.key("grok decode", args, 5), od, grok_decode(theirs, args), tol=2)
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -168,20 +176,22 @@ def test_irreversible_8bit_decode_within_reference_tolerance():
 def test_gpu_codestream_is_byte_identical_to_grok_and_decodes_it(engine, args):
     cp = mk(args)
     planes = synth(args, seed=9)
-    theirs = grok_compress(args, planes)
     ours = engine.encode_codestream(cp, planes, flags=G.CS_TLM | G.CS_PLT)
+    theirs = grok_stream(args, 9, ours)
     assert bytes(ours) == strip_com(theirs), "GPU codestream differs from grk_compress's"
-    # Grok decodes the GPU's stream; the GPU decodes Grok's stream; both equal Grok decoding its own
+    # Grok decodes the GPU's stream; the GPU decodes Grok's stream; both equal Grok decoding its own (from the record,
+    # the two streams are one apart from the COM segment, so Grok's decodes of them are one too)
     w, h, n = args["width"], args["height"], args["numcomps"]
-    g_of_ours, _, _ = R.decompress(ours, w, h, n)
-    g_of_theirs, _, _ = R.decompress(theirs, w, h, n)
+    if R.available():
+        for a, b in zip(R.decompress(ours, w, h, n)[0], R.decompress(theirs, w, h, n)[0]):
+            assert np.array_equal(a, b)
     _, ours_of_theirs = engine.decode_codestream(theirs)
-    for a, b, c, src in zip(g_of_ours, g_of_theirs, ours_of_theirs, planes):
-        assert np.array_equal(a, b)
-        if args.get("irreversible"):
-            assert np.abs(c.astype(np.int64) - b).max() <= 1      # device inverse 9/7 vs Grok's host inverse
-        else:
-            assert np.array_equal(c, src) and np.array_equal(b, src)
+    if args.get("irreversible"):      # device inverse 9/7 vs Grok's host inverse
+        GG.close(GG.key("grok decode", args, 9), ours_of_theirs, grok_decode(theirs, args), tol=1)
+    else:
+        for c, src in zip(ours_of_theirs, planes):
+            assert np.array_equal(c, src)
+        GG.same(GG.key("grok decode", args, 9), planes, grok_decode(theirs, args))
 
 
 @pytest.mark.gpu
@@ -190,8 +200,8 @@ def test_gpu_config2_tiles_match_grok_at_full_tile_size(engine):
     args = dict(width=2048, height=2048, numcomps=3, prec=12, tile=(1024, 1024))
     cp = mk(args)
     planes = P.synthetic_image(2048, 2048, 3, 12, seed=20260924)
-    theirs = grok_compress(args, planes)
     ours = engine.encode_codestream(cp, planes, flags=G.CS_TLM | G.CS_PLT)
+    theirs = GG.grok_stream(GG.key("stream", args, 20260924), ours, grok(lambda: grok_compress(args, planes)))
     assert bytes(ours) == strip_com(theirs)
     _, rec = engine.decode_codestream(theirs)
     for a, b in zip(rec, planes):
@@ -210,15 +220,17 @@ def test_config3_full_size_single_tile_irreversible_matches_grok(engine):
     w = h = 8192
     cp = G.make_coding(w, h, 3, 12, numres=6, irreversible=True)
     planes = P.synthetic_image(w, h, 3, 12, seed=20260925)
-    R.init(0)
-    theirs, _ = R.compress(planes, 12, numres=6, irreversible=True, tlm=True, plt=True)
-    theirs = np.frombuffer(bytes(theirs), np.uint8)
     ours = engine.encode_codestream(cp, planes, flags=G.CS_TLM | G.CS_PLT)
+
+    def compress():
+        R.init(0)
+        return R.compress(planes, 12, numres=6, irreversible=True, tlm=True, plt=True)[0]
+    args = dict(width=w, height=h, numcomps=3, prec=12, numres=6, irreversible=True)
+    theirs = GG.grok_stream(GG.key("stream", args, 20260925), ours, grok(compress))
     assert bytes(ours) == strip_com(theirs)
     _, rec = engine.decode_codestream(theirs)
-    gd, _, _ = R.decompress(theirs, w, h, 3)
-    for a, b, s in zip(rec, gd, planes):
-        assert np.abs(a.astype(np.int64) - b).max() <= 1
+    GG.close(GG.key("grok decode", args, 20260925), rec, grok_decode(theirs, args), tol=1)
+    for a, s in zip(rec, planes):
         err = (a.astype(np.float64) - s)
         assert 10 * np.log10(4095.0 ** 2 / (err ** 2).mean()) > 50.0
 
@@ -236,9 +248,6 @@ def test_config4_full_size_sharded_tiles_match_grok(engine):
         ty, tx = divmod(t, 16)
         for c in range(4):
             planes[c][ty * 1024:(ty + 1) * 1024, tx * 1024:(tx + 1) * 1024] = (base[c] + 257 * t) & 0xFFFF
-    R.init(0)
-    theirs, _ = R.compress(planes, 16, tile=(1024, 1024), numres=6, tlm=True, plt=True, mct=1)
-    theirs = np.frombuffer(bytes(theirs), np.uint8)
     shards = []
     for rem in (0, 1):
         r = engine.encode(cp, planes, tile_mod=2, tile_rem=rem)
@@ -247,6 +256,12 @@ def test_config4_full_size_sharded_tiles_match_grok(engine):
     merged = G.merge_shards(cp, shards)
     ours = G.codestream_write(cp, merged.blocks, merged.bytes, G.CS_TLM | G.CS_PLT, num_tiles=256)
     merged.free()
+
+    def compress():
+        R.init(0)
+        return R.compress(planes, 16, tile=(1024, 1024), numres=6, tlm=True, plt=True, mct=1)[0]
+    args = dict(width=w, height=h, numcomps=4, prec=16, tile=(1024, 1024), numres=6, mct=1)
+    theirs = GG.grok_stream(GG.key("stream", args, 20260926), ours, grok(compress))
     assert bytes(ours) == strip_com(theirs)
     del ours, shards
     _, rec = engine.decode_codestream(theirs)
@@ -289,13 +304,9 @@ def test_window_and_reduce_parse_matches_grok(args, window, reduce):
     grk_decompress at `reduce` gives the reference for the resolution, the window is a crop of it."""
     cp = mk(args)
     planes = synth(args, seed=12)
-    theirs = grok_compress(args, planes)
+    table, data, _ = oracle_encode(cp, planes)
+    theirs = grok_stream(args, 12, G.codestream_write(cp, table, data, G.CS_TLM | G.CS_PLT))
     w, h, n = args["width"], args["height"], args["numcomps"]
-    rw, rh = -(-w >> reduce), -(-h >> reduce)
-    ref, _, _ = R.decompress(theirs, rw, rh, n, reduce=reduce)                # Grok's own reduced decode of the whole image
-    if reduce == 0 and not args.get("irreversible"):
-        for a, b in zip(ref, planes):
-            assert np.array_equal(a, b)
     vcp, blocks = _parse_window(theirs, window, reduce)
     rec = oracle_decode(vcp, blocks, theirs)
     sh = (1 << reduce) - 1
@@ -305,8 +316,16 @@ def test_window_and_reduce_parse_matches_grok(args, window, reduce):
     if window is not None:       # tile-granular: at most the touched tiles are decoded
         tw, th = args.get("tile", (w, h))
         assert (vcp.x1 - vcp.x0) <= ((-(-window[2] // tw) - window[0] // tw) * tw + sh) >> reduce
-    for a, b in zip(rec, ref):
-        assert np.array_equal(a[y0 - vcp.y0:y1 - vcp.y0, x0 - vcp.x0:x1 - vcp.x0], b[y0:y1, x0:x1])
+    whole = grok_decode(theirs, args, reduce)                # Grok's own reduced decode of the whole image
+
+    def ref():
+        planes_r = whole()
+        if reduce == 0 and not args.get("irreversible"):
+            for a, b in zip(planes_r, planes):
+                assert np.array_equal(a, b)
+        return [b[y0:y1, x0:x1] for b in planes_r]
+    GG.same(GG.key("grok decode %s reduce %d" % (window, reduce), args, 12),
+            [a[y0 - vcp.y0:y1 - vcp.y0, x0 - vcp.x0:x1 - vcp.x0] for a in rec], ref if whole else None)
 
 
 @pytest.mark.parametrize("irreversible", [False, True])
@@ -316,7 +335,8 @@ def test_window_parse_keeps_exactly_the_blocks_a_window_can_depend_on(irreversib
     decode, and most of the touched tiles' coded bytes are not needed."""
     args = dict(width=768, height=640, numcomps=1, prec=12, tile=(512, 512), numres=6, irreversible=irreversible)
     planes = synth(args, seed=21)
-    theirs = grok_compress(args, planes)
+    table, data, _ = oracle_encode(mk(args), planes)
+    theirs = grok_stream(args, 21, G.codestream_write(mk(args), table, data, G.CS_TLM | G.CS_PLT))
     fcp, fblocks = G.codestream_parse(theirs)
     full = oracle_decode(fcp, fblocks, theirs)
     rng = np.random.default_rng(7)
@@ -338,14 +358,14 @@ def test_window_parse_keeps_exactly_the_blocks_a_window_can_depend_on(irreversib
 @pytest.mark.parametrize("args,window,reduce", WINDOW_CASES)
 def test_gpu_window_and_reduce_decode_matches_grok(engine, args, window, reduce):
     planes = synth(args, seed=12)
-    theirs = grok_compress(args, planes)
+    theirs = grok_stream(args, 12, engine.encode_codestream(mk(args), planes, flags=G.CS_TLM | G.CS_PLT))
     w, h, n = args["width"], args["height"], args["numcomps"]
-    ref, _, _ = R.decompress(theirs, -(-w >> reduce), -(-h >> reduce), n, reduce=reduce)
+    whole = grok_decode(theirs, args, reduce)
     _, got = engine.decode_window(theirs, window, reduce)
     sh = (1 << reduce) - 1
     x0, y0, x1, y1 = [(v + sh) >> reduce for v in ((0, 0, w, h) if window is None else window)]
-    for a, b in zip(got, ref):
-        assert np.array_equal(a, b[y0:y1, x0:x1])
+    GG.same(GG.key("grok decode %s reduce %d" % (window, reduce), args, 12), got,
+            (lambda: [b[y0:y1, x0:x1] for b in whole()]) if whole else None)
 
 
 @pytest.mark.gpu

@@ -19,5 +19,5 @@ for src, p in procs:
     if p.returncode:
         sys.stderr.write(o.decode()); raise SystemExit("nvcc failed on " + src)
 lib = os.path.join(out, "libgrokj2k_plugin.so")
-subprocess.check_call([B.NVCC, "-shared", "-o", lib] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-lpthread"])
+subprocess.check_call([B.NVCC, "-shared", "-o", lib] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-lpthread"])
 print(lib)

@@ -1,4 +1,4 @@
-"""Summarise an `ncu --set full` report: python tools/ncu_extract.py report.ncu-rep > profiles/xxx.txt"""
+"""Summarise an `ncu --set full` report: python tools/ncu_extract.py report.ncu-rep > summary.txt"""
 import csv, subprocess, sys, io
 WANT = ['gpu__time_duration.sum', 'dram__bytes_read.sum', 'dram__bytes_write.sum',
         'dram__throughput.avg.pct_of_peak_sustained_elapsed', 'sm__throughput.avg.pct_of_peak_sustained_elapsed',
