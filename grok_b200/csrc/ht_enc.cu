@@ -56,11 +56,50 @@ constexpr int VLC_UNIT_WORDS = 5;   /* 4 pairs * <= 30 bits = 120 bits -> 4 word
 constexpr int OFFS_WORDS = 34;      /* exclusive prefix sums of the 32 units' string lengths + the total */
 constexpr int MEL_CAP = 256;        /* reference buffer is 192 bytes (L555); more is an error there */
 
+#ifdef ENC_PHASE_CLOCKS
+/* ENC_PHASE_CLOCKS (tools/enc_phases.py builds it with tools/build_variant.py): every warp adds the clock64() cycles it
+   spends in each phase of k_ht_encode to g_enc_phase.  Lane p keeps phase p's sum in one register, so the instrumented
+   kernel needs two more 64-bit registers, not one per phase (some instances then spill 8 bytes; the product has no spills).  Slots past the phases: blocks coded, warp cycles from start
+   to exit and the same span in %globaltimer nanoseconds (their ratio is the SM clock while the kernel runs). */
+enum
+{
+  PH_SETUP, PH_STAGE, PH_CODE, PH_MEL, PH_SCAN, PH_MS, PH_VLC, PH_TERM, PH_N,
+  PH_BLOCKS = PH_N, PH_WARP_CYCLES, PH_WARP_NS, PH_SLOTS
+};
+__device__ unsigned long long g_enc_phase[PH_SLOTS];
+__device__ __forceinline__ unsigned long long enc_globaltimer()
+{
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#define PHASE_MARK(p)                                                          \
+  do                                                                           \
+  {                                                                            \
+    const long long t_ = clock64();                                            \
+    ph_acc += lane == (p) ? (unsigned long long)(t_ - ph_t) : 0ull;            \
+    ph_t = t_;                                                                 \
+  } while(0)
+#else
+#define PHASE_MARK(p) do {} while(0)
+#endif
+
 __device__ __forceinline__ unsigned lanemask_lt()
 {
   unsigned m;
   asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));
   return m;
+}
+
+/* pulls the 128-byte lines of [p, p + bytes) into L2: no registers held, no shared memory, nothing waits for it.  A plain
+   per-thread prefetch, one line per instruction, because lanes prefetch different rows: the bulk form
+   (cp.async.bulk.prefetch.L2) takes a warp-uniform address, so per-lane rows compile to a loop over the lanes, and it
+   measured slower (1.94 against 1.90 ms per encode of config 2, H100 80GB HBM3 at 400 W). */
+__device__ __forceinline__ void prefetch_l2(const void* p, uint32_t bytes)
+{
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+  for(uintptr_t l = a & ~(uintptr_t)127; l < a + bytes; l += 128)
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(l) : "memory");
 }
 
 /* 15 bits starting at absolute bit position pos; bits at or beyond `tail` read as `fill`
@@ -427,6 +466,12 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
   __syncthreads();
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#ifdef ENC_PHASE_CLOCKS
+  unsigned long long ph_acc = 0;
+  long long ph_t = clock64();
+  const long long ph_c0 = ph_t;
+  const unsigned long long ph_g0 = enc_globaltimer();
+#endif
   uint32_t* stage = warp_base + (size_t)warp * warp_words;
   uint32_t* ms_scr = stage + lay.stage_words;
   uint32_t* vlc_scr = ms_scr + 32u * lay.ms_w;
@@ -478,6 +523,36 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
   for(int y0 = 0; y0 < h; y0 += 2 * R)
   {
     /* ---- stage: sample rows y0-1 .. y0+2R-1, converted to (mu << 1) | sign --------------------------- */
+    PHASE_MARK(PH_SETUP);
+    /* the rows the warp stages next -- the next round's, or in the last round the first round's rows of the warp's next
+       block -- are pulled into L2 (one row per lane) while this round is coded: without it the staging loads go to HBM
+       and staging took 40 % of a warp's cycles (tools/enc_phases.py).  The next block's descriptor is read here, the
+       prefetch issued after staging, so that the staging loads overlap its latency. */
+    const uint8_t* pf_row = nullptr;
+    uint32_t pf_bytes = 0;
+    if(y0 + 2 * R < h)
+    {
+      const int gy = y0 + 2 * R + lane;
+      if(lane < 2 * R && gy < h)
+      {
+        pf_row = static_cast<const uint8_t*>(B.coef) + (size_t)gy * B.pitch * 4u;
+        pf_bytes = 4u * (uint32_t)w;
+      }
+    }
+    else
+    {
+      const uint32_t nxt = bidx + gridDim.x * cta_warps;
+      if(nxt < nblocks)
+      {
+        const HtBlockDesc* N = blocks + nxt;
+        const uint32_t nw = N->w, nh = N->h;
+        if(lane < 2 * (int)enc_rows_per_round(nw) && lane < (int)nh)
+        {
+          pf_row = static_cast<const uint8_t*>(N->coef) + (size_t)lane * N->pitch * 4u;
+          pf_bytes = 4u * nw;
+        }
+      }
+    }
     __syncwarp();
     {
       const uint32_t* cbase = reinterpret_cast<const uint32_t*>(B.coef);
@@ -553,6 +628,9 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
       }
     }
     __syncwarp();
+    if(pf_row)
+      prefetch_l2(pf_row, pf_bytes);
+    PHASE_MARK(PH_STAGE);
 
     /* ---- code: lane = unit; the staged rows hold R * upr units, 32 at a time (more than one trip only for
        blocks wider than 32 units, where R = 1) ------------------------------------------------------------ */
@@ -707,6 +785,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
         *vwp = (uint32_t)vacc;
     }
     __syncwarp();
+    PHASE_MARK(PH_CODE);
 
     /* ---- join: MEL events, unit by unit in coding order: quad 2p, quad 2p+1, pair p ---- */
     if(__any_sync(0xffffffffu, mel_has != 0))
@@ -730,6 +809,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
         }
       }
     }
+    PHASE_MARK(PH_MEL);
     /* ---- join: where each unit's strings start (one scan for both: MagSgn < 2^17 bits per round, VLC < 2^14) ---- */
     {
       uint32_t x = mlen | (vlen << 17);
@@ -750,6 +830,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
       }
     }
     __syncwarp();
+    PHASE_MARK(PH_SCAN);
     /* ---- join: MagSgn.  64 ring words (2048 bits) are gathered from the units' strings at a time, two words per
        lane, and 128 bytes leave whenever 1024 bits are queued. ---- */
     {
@@ -777,6 +858,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
         __syncwarp();
       }
     }
+    PHASE_MARK(PH_MS);
     /* ---- join: VLC, 128 bytes out when 1024 bits are queued, else 32 whenever 256 are ---- */
     {
       const uint32_t total = offs_v[32], t0 = vlc_tail;
@@ -805,6 +887,7 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
         __syncwarp();
       }
     }
+    PHASE_MARK(PH_VLC);
     } /* unit trips */
   }
 
@@ -872,7 +955,17 @@ __global__ void __launch_bounds__(ENC_WARPS * 32, ENC_MIN_CTAS)
       o.total = 0xFFFFFFFFu; /* the reference raises "mel encoder's buffer is full" here */
     outs[bidx] = o;
   }
+  PHASE_MARK(PH_TERM);
+#ifdef ENC_PHASE_CLOCKS
+  ph_acc += lane == PH_BLOCKS ? 1ull : 0ull;
+#endif
   } /* block loop */
+#ifdef ENC_PHASE_CLOCKS
+  const unsigned long long ph_cycles = (unsigned long long)(clock64() - ph_c0), ph_ns = enc_globaltimer() - ph_g0;
+  ph_acc += lane == PH_WARP_CYCLES ? ph_cycles : lane == PH_WARP_NS ? ph_ns : 0ull;
+  if(lane < PH_SLOTS)
+    atomicAdd(&g_enc_phase[lane], ph_acc);
+#endif
 }
 
 /* lengths -> exclusive byte offsets.  One CTA of 1024 threads, SCAN_ITEMS consecutive blocks per thread and round:
@@ -945,7 +1038,36 @@ __global__ void __launch_bounds__(1024) k_scan_lengths(const HtBlockOut* __restr
     offsets[n] = carry_s;
 }
 
-/* compaction: MagSgn|MEL from the slot head, VLC from the slot tail (warp per block) */
+/* byte j of a block's coded bytes: MagSgn|MEL (slot[0, front)) followed by VLC (vsrc[0, ...)) */
+__device__ __forceinline__ uint32_t coded_byte(const uint8_t* slot, const uint8_t* vsrc, uint32_t front, uint32_t j)
+{
+  return j < front ? slot[j] : vsrc[j - front];
+}
+
+/* bytes j .. j+3 of the same, little-endian.  Inside one of the two pieces: the two aligned words that hold them, funnel-
+   shifted (both words hold at least one of the four bytes, so neither read leaves the piece's words); across the seam,
+   byte by byte. */
+__device__ __forceinline__ uint32_t coded_word(const uint8_t* slot, const uint8_t* vsrc, uint32_t front, uint32_t j)
+{
+  if(j + 4u <= front || j >= front)
+  {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(j >= front ? vsrc + (j - front) : slot + j);
+    const uint32_t* p = reinterpret_cast<const uint32_t*>(a & ~(uintptr_t)3);
+    const uint32_t sh = (uint32_t)(a & 3u);
+    const uint32_t lo = p[0];
+    return sh ? __funnelshift_r(lo, p[1], 8u * sh) : lo;
+  }
+  uint32_t v = 0;
+#pragma unroll
+  for(int k = 0; k < 4; ++k)
+    v |= coded_byte(slot, vsrc, front, j + k) << (8 * k);
+  return v;
+}
+
+/* compaction: MagSgn|MEL from the slot head, VLC from the slot tail (warp per block).  The destination's whole 4-byte words
+   are written as words, four per lane in flight (byte-wide copies left the kernel bound by load latency); the up to three
+   bytes at each end share their words with the neighbouring blocks and are written as bytes. */
+constexpr int GATHER_UNROLL = 4;
 __global__ void k_ht_gather(const HtBlockDesc* __restrict__ blocks, const HtBlockOut* __restrict__ outs,
                             const uint64_t* __restrict__ offsets, const uint8_t* __restrict__ scratch,
                             uint8_t* __restrict__ bytes, uint32_t nblocks, uint64_t cap)
@@ -959,12 +1081,35 @@ __global__ void k_ht_gather(const HtBlockDesc* __restrict__ blocks, const HtBloc
     return; /* arena too small: the host notices from the offsets and re-gathers */
   const uint8_t* slot = scratch + blocks[bidx].slot_off;
   uint8_t* dst = bytes + offsets[bidx];
-  const uint32_t front = o.ms_len + o.mel_len;
-  for(uint32_t i = lane; i < front; i += 32)
-    dst[i] = slot[i];
+  const uint32_t front = o.ms_len + o.mel_len, total = front + o.vlc_len;
   const uint8_t* vsrc = slot + blocks[bidx].slot_cap - o.vlc_len;
-  for(uint32_t i = lane; i < o.vlc_len; i += 32)
-    dst[front + i] = vsrc[i];
+  const uint32_t head = (uint32_t)(-reinterpret_cast<uintptr_t>(dst) & 3u); /* bytes before the first whole word */
+  if(total < head + 4u)
+  {
+    for(uint32_t i = lane; i < total; i += 32)
+      dst[i] = (uint8_t)coded_byte(slot, vsrc, front, i);
+    return;
+  }
+  const uint32_t words = (total - head) >> 2, tail0 = head + 4u * words;
+  if((uint32_t)lane < head)
+    dst[lane] = (uint8_t)coded_byte(slot, vsrc, front, lane);
+  if((uint32_t)lane < total - tail0)
+    dst[tail0 + lane] = (uint8_t)coded_byte(slot, vsrc, front, tail0 + lane);
+  uint32_t* dw = reinterpret_cast<uint32_t*>(dst + head);
+  for(uint32_t w0 = lane; w0 < words; w0 += 32 * GATHER_UNROLL)
+  {
+    uint32_t v[GATHER_UNROLL];
+#pragma unroll
+    for(int k = 0; k < GATHER_UNROLL; ++k)
+    {
+      const uint32_t w = w0 + 32u * k;
+      v[k] = w < words ? coded_word(slot, vsrc, front, head + 4u * w) : 0u;
+    }
+#pragma unroll
+    for(int k = 0; k < GATHER_UNROLL; ++k)
+      if(w0 + 32u * k < words)
+        dw[w0 + 32u * k] = v[k];
+  }
 }
 
 } /* namespace */
@@ -1009,6 +1154,22 @@ void b2k_launch_ht_encode(const HtBlockDesc* d_blocks, HtBlockOut* d_out, uint8_
   kern<<<grid, cta_warps * 32, smem, st>>>(d_blocks, d_out, d_scratch, nblocks, lay);
   b2k_count_launch();
 }
+
+#ifdef ENC_PHASE_CLOCKS
+/* copies up to n of the ENC_PHASE_CLOCKS counters (layout: the PH_ enum) to out, zeroes them, returns how many there are */
+extern "C" B2K_API int32_t b2k_enc_phase_clocks(uint64_t* out, int32_t n)
+{
+  unsigned long long h[PH_SLOTS] = {};
+  if(cudaMemcpyFromSymbol(h, g_enc_phase, sizeof(h)) != cudaSuccess)
+    return -1;
+  const unsigned long long zero[PH_SLOTS] = {};
+  if(cudaMemcpyToSymbol(g_enc_phase, zero, sizeof(zero)) != cudaSuccess)
+    return -1;
+  for(int i = 0; i < n && i < PH_SLOTS; ++i)
+    out[i] = h[i];
+  return PH_SLOTS;
+}
+#endif
 
 /* words of shared memory one warp needs to stage the sample rows of one round of a w-wide block */
 uint32_t b2k_ht_encode_stage_words(uint32_t w)
