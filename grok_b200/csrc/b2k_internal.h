@@ -47,9 +47,8 @@ struct DwtLevelDesc
   int32_t lo[3], hi[3];/* inverse: clamp range after the shift is restored */
   uint16_t nstrips, nsegs, strip_w, pairs_per_seg;
   uint8_t first_level; /* 1: samples are integers from the image (apply shift / MCT) */
-  uint8_t in_is_u16;   /* finest level only: 0 = 32-bit samples, 1 = uint16, 2 = int16 containers */
   uint8_t comp0;       /* first component this descriptor covers */
-  uint8_t pad;
+  uint8_t pad[2];
 };
 
 /* ---- one code block for the HT coder kernels ------------------------------------------------
@@ -78,10 +77,8 @@ struct HtBlockOut /* written by the encoder kernel */
 };
 
 /* kernel launchers (dwt.cu, ht_enc.cu, ht_dec.cu) */
-void b2k_launch_dwt_fwd(const DwtLevelDesc* d_descs, int ndesc, int max_jobs, int nc, bool irreversible,
-                        bool in_u16, cudaStream_t st);
-void b2k_launch_dwt_inv(const DwtLevelDesc* d_descs, int ndesc, int max_jobs, int nc, bool irreversible, bool out_u16,
-                        cudaStream_t st);
+void b2k_launch_dwt_fwd(const DwtLevelDesc* d_descs, int ndesc, int max_jobs, int nc, bool irreversible, cudaStream_t st);
+void b2k_launch_dwt_inv(const DwtLevelDesc* d_descs, int ndesc, int max_jobs, int nc, bool irreversible, cudaStream_t st);
 /* numres = 1: DC shift + colour transform only (forward: image -> coefficient planes; else back, rounded and clamped) */
 void b2k_launch_point_transform(const DwtLevelDesc* d_descs, int ndesc, uint32_t max_w, uint32_t max_h, int nc, bool irreversible,
                                 bool forward, cudaStream_t st);

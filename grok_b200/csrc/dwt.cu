@@ -69,28 +69,6 @@ __device__ __forceinline__ void load8_w32(const int32_t* __restrict__ row, int r
       v[i] = __ldg(row + mirror_rel(rel + i, n));
   }
 }
-__device__ __forceinline__ void load8_u16(const uint16_t* __restrict__ row, int rel, int n, int sgnd, int (&v)[8])
-{
-  const uint16_t* p = row + rel;
-  if(rel >= 0 && rel + 8 <= n && ((reinterpret_cast<uintptr_t>(p) & 15) == 0))
-  {
-    const uint4 a = __ldg(reinterpret_cast<const uint4*>(p));
-    v[0] = a.x & 0xFFFF; v[1] = a.x >> 16; v[2] = a.y & 0xFFFF; v[3] = a.y >> 16;
-    v[4] = a.z & 0xFFFF; v[5] = a.z >> 16; v[6] = a.w & 0xFFFF; v[7] = a.w >> 16;
-  }
-  else
-  {
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-      v[i] = __ldg(row + mirror_rel(rel + i, n));
-  }
-  if(sgnd)
-  {
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-      v[i] = (int)(int16_t)v[i];
-  }
-}
 
 /* 4 consecutive band samples (inverse transform): idx0 = first band-relative index wanted,
  * mirrored per element through the interleaved domain when out of range */
@@ -115,36 +93,6 @@ __device__ __forceinline__ void load4_band(const int32_t* __restrict__ row, int 
       /* a length-1 line mirrors onto a sample of the other parity: that band is empty */
       v[i] = ((um & 1) == odd) ? __ldg(row + ((um >> 1) - kb0)) : 0;
     }
-  }
-}
-
-__device__ __forceinline__ void store4(int32_t* __restrict__ row, int col, const int (&v)[4], unsigned validmask)
-{
-  int32_t* p = row + col;
-  if(validmask == 0xF && ((reinterpret_cast<uintptr_t>(p) & 15) == 0))
-    *reinterpret_cast<int4*>(p) = make_int4(v[0], v[1], v[2], v[3]);
-  else
-  {
-#pragma unroll
-    for(int i = 0; i < 4; ++i)
-      if(validmask & (1u << i))
-        p[i] = v[i];
-  }
-}
-__device__ __forceinline__ void store8(int32_t* __restrict__ row, int col, const int (&v)[8], unsigned validmask)
-{
-  int32_t* p = row + col;
-  if(validmask == 0xFF && ((reinterpret_cast<uintptr_t>(p) & 15) == 0))
-  {
-    reinterpret_cast<int4*>(p)[0] = make_int4(v[0], v[1], v[2], v[3]);
-    reinterpret_cast<int4*>(p)[1] = make_int4(v[4], v[5], v[6], v[7]);
-  }
-  else
-  {
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-      if(validmask & (1u << i))
-        p[i] = v[i];
   }
 }
 
@@ -174,9 +122,103 @@ __device__ __forceinline__ bool decode_job(const DwtLevelDesc& D, Job& J)
 }
 
 /* =============================================================================================
- * forward, finest-level sample fetch: integers from the image, + DC shift, + RCT / ICT
+ * DC shift + colour transforms of the finest level, for N sample positions of NC components (one
+ * component: the DC shift alone).  The level-1 DWT kernels, their degenerate jobs and
+ * k_point_transform all call these.  The irreversible ones spell out every rounding with _rn
+ * intrinsics, in the reference build's operand order: that build contracts a_r*r + a_g*g + a_b*b
+ * into two FMAs and the inverse ICT into FMA / FNMA, and the coded bytes are pinned against
+ * libgrokj2k (tests/test_interop.py).
  * =========================================================================================== */
-template <int NC, bool U16>
+/* forward RCT: mct.cpp L497-531 */
+template <int NC, int N>
+__device__ __forceinline__ void rct_fwd(const DwtLevelDesc& D, int (&x)[NC][N])
+{
+#pragma unroll
+  for(int i = 0; i < N; ++i)
+  {
+    if constexpr(NC == 3)
+    {
+      const int r = x[0][i] + D.shift[0], g = x[1][i] + D.shift[1], b = x[2][i] + D.shift[2];
+      x[0][i] = ((g + g) + b + r) >> 2;
+      x[1][i] = b - g;
+      x[2][i] = r - g;
+    }
+    else
+      x[0][i] += D.shift[0];
+  }
+}
+
+/* forward ICT: mct.cpp L584-636 */
+template <int NC, int N>
+__device__ __forceinline__ void ict_fwd(const DwtLevelDesc& D, const int (&x)[NC][N], float (&out)[NC][N])
+{
+  const float a_r = 0.299f, a_g = 0.587f, a_b = 0.114f;
+  const float cb = __fdiv_rn(0.5f, __fsub_rn(1.0f, a_b)), cr = __fdiv_rn(0.5f, __fsub_rn(1.0f, a_r));
+#pragma unroll
+  for(int i = 0; i < N; ++i)
+  {
+    if constexpr(NC == 3)
+    {
+      const float r = (float)(x[0][i] + D.shift[0]), g = (float)(x[1][i] + D.shift[1]), b = (float)(x[2][i] + D.shift[2]);
+      const float y = __fmaf_rn(a_b, b, __fmaf_rn(a_g, g, __fmul_rn(a_r, r)));
+      out[0][i] = y;
+      out[1][i] = __fmul_rn(cb, __fsub_rn(b, y));
+      out[2][i] = __fmul_rn(cr, __fsub_rn(r, y));
+    }
+    else
+      out[0][i] = (float)(x[0][i] + D.shift[0]);
+  }
+}
+
+/* inverse RCT, DC shift and clamp to the sample range: mct.cpp L201-256 */
+template <int NC, int N>
+__device__ __forceinline__ void rct_inv(const DwtLevelDesc& D, int (&x)[NC][N])
+{
+#pragma unroll
+  for(int i = 0; i < N; ++i)
+  {
+    if constexpr(NC == 3)
+    {
+      const int y = x[0][i], u = x[1][i], w = x[2][i];
+      const int gg = y - ((u + w) >> 2);
+      x[0][i] = w + gg;
+      x[1][i] = gg;
+      x[2][i] = u + gg;
+    }
+#pragma unroll
+    for(int c = 0; c < NC; ++c)
+      x[c][i] = min(max(x[c][i] - D.shift[c], D.lo[c]), D.hi[c]);
+  }
+}
+
+/* inverse ICT, rounding, DC shift and clamp to the sample range: mct.cpp L318-391 */
+template <int NC, int N>
+__device__ __forceinline__ void ict_inv(const DwtLevelDesc& D, const float (&x)[NC][N], int (&out)[NC][N])
+{
+#pragma unroll
+  for(int i = 0; i < N; ++i)
+  {
+    float f[NC];
+    if constexpr(NC == 3)
+    {
+      const float y = x[0][i], u = x[1][i], w = x[2][i];
+      f[0] = __fmaf_rn(w, 1.402f, y);
+      f[1] = __fmaf_rn(-w, 0.71414f, __fmaf_rn(-u, 0.34413f, y));
+      f[2] = __fmaf_rn(u, 1.772f, y);
+    }
+    else
+      f[0] = x[0][i];
+#pragma unroll
+    for(int c = 0; c < NC; ++c)
+      out[c][i] = min(max(__float2int_rn(f[c]) - D.shift[c], D.lo[c]), D.hi[c]);
+  }
+}
+
+/* =============================================================================================
+ * forward sample fetch: integers from the image at the finest level (+ DC shift, + RCT / ICT),
+ * the previous level's LL coefficients elsewhere
+ * =========================================================================================== */
+template <int NC>
 __device__ __forceinline__ void fetch_int_rows(const DwtLevelDesc& D, const Job& J, int v, int (&out)[NC][8])
 {
   const int r = mirror_rel(v - D.v0, J.hn);
@@ -190,75 +232,48 @@ __device__ __forceinline__ void fetch_int_rows(const DwtLevelDesc& D, const Job&
         out[c][i] = 0;
       continue;
     }
-    if(U16)
-      load8_u16(reinterpret_cast<const uint16_t*>(D.in[c]) + (size_t)r * D.in_pitch, J.ulane - D.u0, J.wn,
-                D.in_is_u16 == 2, out[c]);
-    else
-      load8_w32(reinterpret_cast<const int32_t*>(D.in[c]) + (size_t)r * D.in_pitch, J.ulane - D.u0, J.wn, out[c]);
+    load8_w32(reinterpret_cast<const int32_t*>(D.in[c]) + (size_t)r * D.in_pitch, J.ulane - D.u0, J.wn, out[c]);
   }
 }
 
-/* reversible: mct.cpp L497-531 */
-template <int NC, bool U16>
-__device__ __forceinline__ void fetch53(const DwtLevelDesc& D, const Job& J, int v, int (&out)[NC][8])
+/* a fetched row -> the values the 5/3 lifting starts from */
+template <int NC>
+__device__ __forceinline__ void to_coeffs53(const DwtLevelDesc& D, int (&x)[NC][8])
 {
   if(D.first_level)
-  {
-    fetch_int_rows<NC, U16>(D, J, v, out);
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-    {
-      if(NC == 3)
-      {
-        const int r = out[0][i] + D.shift[0], g = out[1][i] + D.shift[1], b = out[2][i] + D.shift[2];
-        out[0][i] = ((g + g) + b + r) >> 2;
-        out[1][i] = b - g;
-        out[2][i] = r - g;
-      }
-      else
-        out[0][i] += D.shift[0];
-    }
-  }
-  else
-    fetch_int_rows<NC, false>(D, J, v, out);
+    rct_fwd<NC>(D, x);
 }
 
-/* irreversible: mct.cpp L584-636; float conversion of the finest level WaveletFwd.cpp L658-681 */
-template <int NC, bool U16>
-__device__ __forceinline__ void fetch97(const DwtLevelDesc& D, const Job& J, int v, float (&out)[NC][8])
+/* a fetched row -> the values the 9/7 lifting starts from; the float conversion of the finest level
+   is WaveletFwd.cpp L658-681, other levels hold float bits */
+template <int NC>
+__device__ __forceinline__ void to_coeffs97(const DwtLevelDesc& D, const int (&raw)[NC][8], float (&out)[NC][8])
 {
-  int raw[NC][8];
   if(D.first_level)
-  {
-    fetch_int_rows<NC, U16>(D, J, v, raw);
-    const float a_r = 0.299f, a_g = 0.587f, a_b = 0.114f;
-    const float cb = __fdiv_rn(0.5f, __fsub_rn(1.0f, a_b)), cr = __fdiv_rn(0.5f, __fsub_rn(1.0f, a_r));
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-    {
-      if(NC == 3)
-      {
-        const float r = (float)(raw[0][i] + D.shift[0]), g = (float)(raw[1][i] + D.shift[1]),
-                    b = (float)(raw[2][i] + D.shift[2]);
-        /* the reference build contracts a_r*r + a_g*g + a_b*b into two FMAs (pinned against libgrokj2k, tests/test_interop.py) */
-        const float y = __fmaf_rn(a_b, b, __fmaf_rn(a_g, g, __fmul_rn(a_r, r)));
-        out[0][i] = y;
-        out[1][i] = __fmul_rn(cb, __fsub_rn(b, y));
-        out[2][i] = __fmul_rn(cr, __fsub_rn(r, y));
-      }
-      else
-        out[0][i] = (float)(raw[0][i] + D.shift[0]);
-    }
-  }
+    ict_fwd<NC>(D, raw, out);
   else
   {
-    fetch_int_rows<NC, false>(D, J, v, raw);
 #pragma unroll
     for(int c = 0; c < NC; ++c)
 #pragma unroll
       for(int i = 0; i < 8; ++i)
         out[c][i] = __int_as_float(raw[c][i]);
   }
+}
+
+template <int NC>
+__device__ __forceinline__ void fetch53(const DwtLevelDesc& D, const Job& J, int v, int (&out)[NC][8])
+{
+  fetch_int_rows<NC>(D, J, v, out);
+  to_coeffs53<NC>(D, out);
+}
+
+template <int NC>
+__device__ __forceinline__ void fetch97(const DwtLevelDesc& D, const Job& J, int v, float (&out)[NC][8])
+{
+  int raw[NC][8];
+  fetch_int_rows<NC>(D, J, v, raw);
+  to_coeffs97<NC>(D, raw, out);
 }
 
 /* ---- sub-band row stores (Mallat layout: TileComponentWindow.h L241-264) -------------------- */
@@ -278,37 +293,74 @@ __device__ __forceinline__ BandGeom band_geom(const DwtLevelDesc& D)
   return g;
 }
 
-/* lo[4]/hi[4]: horizontally transformed samples of one vertical row (vertical low if !vhigh) */
-__device__ __forceinline__ void store_band_rows(const DwtLevelDesc& D, const Job& J, const BandGeom& g, int c, int j,
-                                                bool vhigh, const int (&lo)[4], const int (&hi)[4])
+/* per-lane constants of the sub-band stores */
+struct StoreCtx
 {
-  const int v = 2 * j + (vhigh ? 1 : 0);
-  if(!J.owner || v < D.v0 || v >= D.v1)
-    return;
-  unsigned mlo = 0, mhi = 0;
-#pragma unroll
-  for(int i = 0; i < 4; ++i)
+  unsigned mlo, mhi;
+  bool vec_ll, vec_lo, vec_hi; /* all four samples valid and the 16-byte store is aligned */
+  int col_ll, col_lo, col_hi; /* column of the lane's first low sample in the LL plane / in the
+                                 Mallat buffer, and of its first high sample */
+};
+__device__ __forceinline__ StoreCtx store_ctx(const DwtLevelDesc& D, const Job& J, const BandGeom& g)
+{
+  StoreCtx s;
+  s.mlo = s.mhi = 0;
+  if(J.owner)
   {
-    const int ue = J.ulane + 2 * i;
-    if(ue >= D.u0 && ue < D.u1)
-      mlo |= 1u << i;
-    if(ue + 1 >= D.u0 && ue + 1 < D.u1)
-      mhi |= 1u << i;
+#pragma unroll
+    for(int i = 0; i < 4; ++i)
+    {
+      const int ue = J.ulane + 2 * i;
+      if(ue >= D.u0 && ue < D.u1)
+        s.mlo |= 1u << i;
+      if(ue + 1 >= D.u0 && ue + 1 < D.u1)
+        s.mhi |= 1u << i;
+    }
   }
   const int k0 = J.ulane >> 1;
+  s.col_ll = k0 - g.x0l;
+  s.col_lo = k0 - g.x0l;
+  s.col_hi = g.snx + k0 - g.x0h;
+  /* row pitches are multiples of 4 elements (engine allocates 128-byte multiples) */
+  const bool pitch_ok = ((D.ll_pitch | D.c_pitch) & 3u) == 0;
+  s.vec_ll = pitch_ok && s.mlo == 0xF && (((reinterpret_cast<uintptr_t>(D.out_ll[0]) >> 2) + (unsigned)s.col_ll) & 3u) == 0;
+  s.vec_lo = pitch_ok && s.mlo == 0xF && (((reinterpret_cast<uintptr_t>(D.out_c[0]) >> 2) + (unsigned)s.col_lo) & 3u) == 0;
+  s.vec_hi = pitch_ok && s.mhi == 0xF && (((reinterpret_cast<uintptr_t>(D.out_c[0]) >> 2) + (unsigned)s.col_hi) & 3u) == 0;
+  return s;
+}
+__device__ __forceinline__ void store4v(int32_t* __restrict__ p, const int (&v)[4], unsigned mask, bool vec)
+{
+  if(vec)
+    *reinterpret_cast<int4*>(p) = make_int4(v[0], v[1], v[2], v[3]);
+  else
+  {
+#pragma unroll
+    for(int i = 0; i < 4; ++i)
+      if(mask & (1u << i))
+        p[i] = v[i];
+  }
+}
+/* lo[4]/hi[4]: horizontally transformed samples of one vertical row (vertical low if !vhigh) */
+__device__ __forceinline__ void store_rows(const DwtLevelDesc& D, const BandGeom& g, const StoreCtx& S, int c, int j,
+                                           bool vhigh, const int (&lo)[4], const int (&hi)[4])
+{
+  const int v = 2 * j + (vhigh ? 1 : 0);
+  if(v < D.v0 || v >= D.v1 || (S.mlo | S.mhi) == 0)
+    return;
+  /* all components of a descriptor share the alignment of component 0 (planes are equally laid out) */
   if(!vhigh)
   {
     /* LL -> out_ll, HL -> Mallat top-right */
-    int32_t* llrow = reinterpret_cast<int32_t*>(D.out_ll[c]) + (size_t)(j - g.y0l) * D.ll_pitch;
-    store4(llrow, k0 - g.x0l, lo, mlo);
-    int32_t* crow = reinterpret_cast<int32_t*>(D.out_c[c]) + (size_t)(j - g.y0l) * D.c_pitch;
-    store4(crow, g.snx + k0 - g.x0h, hi, mhi);
+    const int r = j - g.y0l;
+    store4v(reinterpret_cast<int32_t*>(D.out_ll[c]) + (r * (int)D.ll_pitch + S.col_ll), lo, S.mlo, S.vec_ll);
+    store4v(reinterpret_cast<int32_t*>(D.out_c[c]) + (r * (int)D.c_pitch + S.col_hi), hi, S.mhi, S.vec_hi);
   }
   else
   {
-    int32_t* crow = reinterpret_cast<int32_t*>(D.out_c[c]) + (size_t)(g.sny + j - g.y0h) * D.c_pitch;
-    store4(crow, k0 - g.x0l, lo, mlo);
-    store4(crow, g.snx + k0 - g.x0h, hi, mhi);
+    const int r = g.sny + j - g.y0h;
+    int32_t* crow = reinterpret_cast<int32_t*>(D.out_c[c]) + r * (int)D.c_pitch;
+    store4v(crow + S.col_lo, lo, S.mlo, S.vec_lo);
+    store4v(crow + S.col_hi, hi, S.mhi, S.vec_hi);
   }
 }
 
@@ -383,13 +435,9 @@ __device__ __forceinline__ void hfwd97(const float (&r)[8], int wn, float invK, 
   }
 }
 
-/* =============================================================================================
- * staged row fetch for the forward kernels: every lane prefetches ITS OWN 8 samples of the next
- * row pairs into a private shared-memory slot with cp.async (LDGSTS, 16 bytes per copy, L1
- * bypass) and reads them back later, so STAGES-1 row pairs (x NC components) are in flight per
- * warp without holding registers.  No cross-lane traffic -> no barrier; edge lanes (mirrored or
- * unaligned columns) fill their slot with ordinary loads.
- * =========================================================================================== */
+/* ---- asynchronous copies into shared memory -------------------------------------------------
+ * cp.async (LDGSTS): 16 or 4 bytes per lane and instruction, L1 bypass for the 16-byte ones;
+ * completion is tracked per thread by commit groups. */
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src)
 {
   const unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
@@ -443,17 +491,113 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity)
                : "memory");
 }
 
-template <int NC, bool U16>
+/* =============================================================================================
+ * the per-warp staging pipeline of all four DWT kernels: each warp owns DWT_STAGES shared-memory
+ * slots of one row pair (Stage::PAIRB bytes), plus one mbarrier per slot, so DWT_STAGES-1 row pairs
+ * are in flight while one is lifted, without holding registers.  Pair t sits in slot
+ * (t - tfirst) % DWT_STAGES.  A warp whose lanes are all interior (`bulk`) has lane 0 fill a slot
+ * with bulk copies that complete on the slot's mbarrier; any other warp fills it with cp.async.
+ * A commit group is closed on every step, filled or not, so that wait_group DWT_STAGES-1 always
+ * leaves exactly the pair about to be read complete.
+ * Stage::COOPERATIVE: the cp.async fill has each lane copy samples other lanes read, so the warp
+ * syncs after the wait, and before every refill on both paths.  Otherwise each lane's cp.async
+ * slot is private and only the bulk path (lane 0 writes every lane's samples) syncs before a refill.
+ * =========================================================================================== */
+constexpr int DWT_STAGES = 3;
+
+template <class Stage>
+struct WarpPipe
+{
+  /* dynamic shared memory of a CTA: every warp's slots, then every warp's mbarriers */
+  static constexpr size_t SLOT_BYTES = (size_t)B2K_WARPS_PER_CTA * DWT_STAGES * Stage::PAIRB;
+  static constexpr size_t SMEM_BYTES = SLOT_BYTES + (size_t)B2K_WARPS_PER_CTA * DWT_STAGES * sizeof(uint64_t);
+
+  uint8_t* slots;
+  uint64_t* bars;
+  int tfirst, tlast, tfill;
+  bool bulk;
+
+  __device__ __forceinline__ WarpPipe(uint8_t* smem, bool bulk_, int tfirst_, int tlast_)
+      : slots(smem + (size_t)(threadIdx.x >> 5) * DWT_STAGES * Stage::PAIRB),
+        bars(reinterpret_cast<uint64_t*>(smem + SLOT_BYTES) + (threadIdx.x >> 5) * DWT_STAGES), tfirst(tfirst_),
+        tlast(tlast_), tfill(tfirst_), bulk(bulk_)
+  {
+  }
+  /* fill_bulk(slot, t, bar) runs on lane 0 only; fill_async(slot, t) on every lane */
+  template <class Bulk, class Async>
+  __device__ __forceinline__ void refill(const Bulk& fill_bulk, const Async& fill_async)
+  {
+    if(tfill <= tlast)
+    {
+      const int slot = (tfill - tfirst) % DWT_STAGES;
+      uint8_t* st = slots + (size_t)slot * Stage::PAIRB;
+      if(bulk)
+      {
+        if((threadIdx.x & 31) == 0)
+        {
+          mbar_expect_tx(bars + slot, Stage::PAIRB);
+          fill_bulk(st, tfill, bars + slot);
+        }
+      }
+      else
+        fill_async(st, tfill);
+    }
+    cp_async_commit();
+    ++tfill;
+  }
+  template <class Bulk, class Async>
+  __device__ __forceinline__ void prime(const Bulk& fill_bulk, const Async& fill_async)
+  {
+    if(bulk)
+    {
+      if((threadIdx.x & 31) == 0)
+      {
+#pragma unroll
+        for(int s = 0; s < DWT_STAGES; ++s)
+          mbar_init(bars + s, 1);
+        mbar_fence_init();
+      }
+      __syncwarp();
+    }
+#pragma unroll
+    for(int s = 0; s < DWT_STAGES - 1; ++s)
+      refill(fill_bulk, fill_async);
+  }
+  /* starts the pair DWT_STAGES-1 ahead, waits for pair t and returns its slot */
+  template <class Bulk, class Async>
+  __device__ __forceinline__ const uint8_t* acquire(int t, const Bulk& fill_bulk, const Async& fill_async)
+  {
+    if(Stage::COOPERATIVE || bulk)
+      __syncwarp(); /* every lane has read the slot that is refilled next */
+    refill(fill_bulk, fill_async);
+    const int k = t - tfirst;
+    if(bulk)
+      mbar_wait(bars + k % DWT_STAGES, (unsigned)((k / DWT_STAGES) & 1));
+    else
+    {
+      cp_async_wait<DWT_STAGES - 1>();
+      if(Stage::COOPERATIVE)
+        __syncwarp();
+    }
+    return slots + (size_t)(k % DWT_STAGES) * Stage::PAIRB;
+  }
+  __device__ __forceinline__ void drain() const { cp_async_wait<0>(); }
+};
+
+/* staged row fetch for the forward kernels: a slot holds the NC warp-rows of the two rows of a
+   pair (odd row, next even row), the 8 samples of lane L at bytes [32L, 32L+32) of each */
+template <int NC>
 struct RowStage
 {
-  static constexpr int ROWB = U16 ? 512 : 1024; /* bytes of one warp-row of one component */
-  static constexpr int PAIRB = 2 * NC * ROWB;   /* one row pair, all components */
-  /* 16-byte chunk k of a 32-bit warp-row (lane L owns chunks 2L, 2L+1) is stored at chunk slot
+  static constexpr int ROWB = 1024;           /* bytes of one warp-row of one component */
+  static constexpr int PAIRB = 2 * NC * ROWB; /* one row pair, all components */
+  static constexpr bool COOPERATIVE = true;
+  /* 16-byte chunk k of a warp-row (lane L owns chunks 2L, 2L+1) is stored at chunk slot
      k ^ ((k >> 3) & 1): the two 128-bit reads of a lane then hit disjoint banks per quarter warp */
   static __device__ __forceinline__ int swz(int k) { return k ^ ((k >> 3) & 1); }
 
-  /* fill slot `which` (0 = odd row, 1 = next even row) of a stage with canvas row v.
-     32-bit rows are copied COOPERATIVELY: one cp.async instruction moves 512 contiguous bytes
+  /* fill row `which` (0 = odd row, 1 = next even row) of a slot with canvas row v.
+     Rows are copied COOPERATIVELY: one cp.async instruction moves 512 contiguous bytes
      (lane L copies chunks L and L+32), so every 32-byte DRAM sector is requested once.
      fastmask: ballot of the lanes whose 8 columns are interior and aligned. */
   static __device__ __forceinline__ void fill(uint8_t* stage, int which, const DwtLevelDesc& D, const Job& J, int v,
@@ -465,76 +609,30 @@ struct RowStage
     for(int c = 0; c < NC; ++c)
     {
       uint8_t* dst = stage + (which * NC + c) * ROWB;
-      if(U16)
-      {
-        const uint16_t* row = reinterpret_cast<const uint16_t*>(D.in[c]) + (size_t)r * D.in_pitch;
-        if(fast)
-          cp_async16(dst + J.lane * 16, row + rel);
-        else if(J.need)
-        {
-          uint32_t w[4];
+      const int32_t* row = reinterpret_cast<const int32_t*>(D.in[c]) + (size_t)r * D.in_pitch;
+      const int rel0 = rel - 8 * J.lane; /* lane 0's first column */
 #pragma unroll
-          for(int i = 0; i < 4; ++i)
-            w[i] = (uint32_t)__ldg(row + mcol[2 * i]) | ((uint32_t)__ldg(row + mcol[2 * i + 1]) << 16);
-          *reinterpret_cast<uint4*>(dst + J.lane * 16) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
+      for(int h = 0; h < 2; ++h)
+      {
+        const int k = J.lane + 32 * h;
+        if((fastmask >> (k >> 1)) & 1u)
+          cp_async16(dst + swz(k) * 16, row + rel0 + 4 * k);
       }
-      else
-      {
-        const int32_t* row = reinterpret_cast<const int32_t*>(D.in[c]) + (size_t)r * D.in_pitch;
-        const int rel0 = rel - 8 * J.lane; /* lane 0's first column */
+      if(J.need && !fast)
+      { /* edge lane: mirrored columns, still asynchronous (4-byte copies) */
+        uint8_t* d0 = dst + swz(2 * J.lane) * 16;
+        uint8_t* d1 = dst + swz(2 * J.lane + 1) * 16;
 #pragma unroll
-        for(int h = 0; h < 2; ++h)
+        for(int i = 0; i < 4; ++i)
         {
-          const int k = J.lane + 32 * h;
-          if((fastmask >> (k >> 1)) & 1u)
-            cp_async16(dst + swz(k) * 16, row + rel0 + 4 * k);
-        }
-        if(J.need && !fast)
-        { /* edge lane: mirrored columns, still asynchronous (4-byte copies) */
-          uint8_t* d0 = dst + swz(2 * J.lane) * 16;
-          uint8_t* d1 = dst + swz(2 * J.lane + 1) * 16;
-#pragma unroll
-          for(int i = 0; i < 4; ++i)
-          {
-            cp_async4(d0 + 4 * i, row + mcol[i]);
-            cp_async4(d1 + 4 * i, row + mcol[4 + i]);
-          }
+          cp_async4(d0 + 4 * i, row + mcol[i]);
+          cp_async4(d1 + 4 * i, row + mcol[4 + i]);
         }
       }
     }
   }
-  static __device__ __forceinline__ void read(const uint8_t* stage, int which, const DwtLevelDesc& D, const Job& J,
-                                              int (&out)[NC][8])
-  {
-#pragma unroll
-    for(int c = 0; c < NC; ++c)
-    {
-      const uint8_t* src = stage + (which * NC + c) * ROWB;
-      if(U16)
-      {
-        const uint4 a = *reinterpret_cast<const uint4*>(src + J.lane * 16);
-        out[c][0] = a.x & 0xFFFF; out[c][1] = a.x >> 16; out[c][2] = a.y & 0xFFFF; out[c][3] = a.y >> 16;
-        out[c][4] = a.z & 0xFFFF; out[c][5] = a.z >> 16; out[c][6] = a.w & 0xFFFF; out[c][7] = a.w >> 16;
-        if(D.in_is_u16 == 2)
-        {
-#pragma unroll
-          for(int i = 0; i < 8; ++i)
-            out[c][i] = (int)(int16_t)out[c][i];
-        }
-      }
-      else
-      {
-        const int4 a = *reinterpret_cast<const int4*>(src + swz(2 * J.lane) * 16),
-                   b = *reinterpret_cast<const int4*>(src + swz(2 * J.lane + 1) * 16);
-        out[c][0] = a.x; out[c][1] = a.y; out[c][2] = a.z; out[c][3] = a.w;
-        out[c][4] = b.x; out[c][5] = b.y; out[c][6] = b.z; out[c][7] = b.w;
-      }
-      /* lanes beyond the right halo hold stale shared memory: nothing they compute is stored */
-    }
-  }
-  /* bulk path (32-bit samples, every lane fast): one lane asks the copy engine for the NC whole warp-rows of canvas
-     row v; they land linearly in the slot and complete on `bar` (the caller has armed it with expect_tx) */
+  /* bulk path (every lane fast): one lane asks the copy engine for the NC whole warp-rows of canvas
+     row v; they land linearly in the slot and complete on `bar` (armed with expect_tx) */
   static __device__ __forceinline__ void fill_bulk(uint8_t* stage, int which, const DwtLevelDesc& D, const Job& J, int v, uint64_t* bar)
   {
     const int r = mirror_rel(v - D.v0, J.hn);
@@ -543,123 +641,46 @@ struct RowStage
     for(int c = 0; c < NC; ++c)
       bulk_g2s(stage + (which * NC + c) * ROWB, reinterpret_cast<const int32_t*>(D.in[c]) + (size_t)r * D.in_pitch + rel0, ROWB, bar);
   }
-  static __device__ __forceinline__ void read_linear(const uint8_t* stage, int which, const Job& J, int (&out)[NC][8])
+  /* the lane's 8 samples of row `which`: linear after a bulk fill, swizzled after a cp.async one */
+  static __device__ __forceinline__ void read(const uint8_t* stage, int which, const Job& J, bool linear, int (&out)[NC][8])
   {
 #pragma unroll
     for(int c = 0; c < NC; ++c)
     {
-      const uint8_t* src = stage + (which * NC + c) * ROWB + J.lane * 32;
-      const int4 a = *reinterpret_cast<const int4*>(src), b = *reinterpret_cast<const int4*>(src + 16);
+      const uint8_t* row = stage + (which * NC + c) * ROWB;
+      int4 a, b;
+      if(linear)
+      {
+        a = *reinterpret_cast<const int4*>(row + J.lane * 32);
+        b = *reinterpret_cast<const int4*>(row + J.lane * 32 + 16);
+      }
+      else
+      {
+        a = *reinterpret_cast<const int4*>(row + swz(2 * J.lane) * 16);
+        b = *reinterpret_cast<const int4*>(row + swz(2 * J.lane + 1) * 16);
+      }
       out[c][0] = a.x; out[c][1] = a.y; out[c][2] = a.z; out[c][3] = a.w;
       out[c][4] = b.x; out[c][5] = b.y; out[c][6] = b.z; out[c][7] = b.w;
+      /* lanes beyond the right halo hold stale shared memory: nothing they compute is stored */
     }
   }
   /* lane can use 16-byte async copies: its 8 columns are inside the line and 16-byte aligned */
   static __device__ __forceinline__ bool lane_fast(const DwtLevelDesc& D, const Job& J)
   {
     const int rel = J.ulane - D.u0;
-    bool ok = J.need && rel >= 0 && rel + 8 <= J.wn && ((D.in_pitch * (U16 ? 2u : 4u)) & 15u) == 0;
+    bool ok = J.need && rel >= 0 && rel + 8 <= J.wn && (D.in_pitch & 3u) == 0;
 #pragma unroll
     for(int c = 0; c < NC; ++c)
-      ok = ok && (((reinterpret_cast<uintptr_t>(D.in[c]) + (size_t)rel * (U16 ? 2 : 4)) & 15) == 0);
+      ok = ok && (((reinterpret_cast<uintptr_t>(D.in[c]) + (size_t)rel * 4) & 15) == 0);
     return ok;
   }
 };
 
-/* integer samples of the finest level -> DC shift (+ RCT): mct.cpp L497-531 */
-template <int NC>
-__device__ __forceinline__ void rct_fwd_inplace(const DwtLevelDesc& D, int (&x)[NC][8])
-{
-  if(!D.first_level)
-    return;
-#pragma unroll
-  for(int i = 0; i < 8; ++i)
-  {
-    if(NC == 3)
-    {
-      const int r = x[0][i] + D.shift[0], g = x[NC > 1 ? 1 : 0][i] + D.shift[1], b = x[NC > 2 ? 2 : 0][i] + D.shift[2];
-      x[0][i] = ((g + g) + b + r) >> 2;
-      x[NC > 1 ? 1 : 0][i] = b - g;
-      x[NC > 2 ? 2 : 0][i] = r - g;
-    }
-    else
-      x[0][i] += D.shift[0];
-  }
-}
-
-/* per-lane constants of the sub-band stores */
-struct StoreCtx
-{
-  unsigned mlo, mhi;
-  bool vec_ll, vec_lo, vec_hi; /* all four samples valid and the 16-byte store is aligned */
-  int col_ll, col_lo, col_hi; /* column of the lane's first low sample in the LL plane / in the
-                                 Mallat buffer, and of its first high sample */
-};
-__device__ __forceinline__ StoreCtx store_ctx(const DwtLevelDesc& D, const Job& J, const BandGeom& g)
-{
-  StoreCtx s;
-  s.mlo = s.mhi = 0;
-  if(J.owner)
-  {
-#pragma unroll
-    for(int i = 0; i < 4; ++i)
-    {
-      const int ue = J.ulane + 2 * i;
-      if(ue >= D.u0 && ue < D.u1)
-        s.mlo |= 1u << i;
-      if(ue + 1 >= D.u0 && ue + 1 < D.u1)
-        s.mhi |= 1u << i;
-    }
-  }
-  const int k0 = J.ulane >> 1;
-  s.col_ll = k0 - g.x0l;
-  s.col_lo = k0 - g.x0l;
-  s.col_hi = g.snx + k0 - g.x0h;
-  /* row pitches are multiples of 4 elements (engine allocates 128-byte multiples) */
-  const bool pitch_ok = ((D.ll_pitch | D.c_pitch) & 3u) == 0;
-  s.vec_ll = pitch_ok && s.mlo == 0xF && (((reinterpret_cast<uintptr_t>(D.out_ll[0]) >> 2) + (unsigned)s.col_ll) & 3u) == 0;
-  s.vec_lo = pitch_ok && s.mlo == 0xF && (((reinterpret_cast<uintptr_t>(D.out_c[0]) >> 2) + (unsigned)s.col_lo) & 3u) == 0;
-  s.vec_hi = pitch_ok && s.mhi == 0xF && (((reinterpret_cast<uintptr_t>(D.out_c[0]) >> 2) + (unsigned)s.col_hi) & 3u) == 0;
-  return s;
-}
-__device__ __forceinline__ void store4v(int32_t* __restrict__ p, const int (&v)[4], unsigned mask, bool vec)
-{
-  if(vec)
-    *reinterpret_cast<int4*>(p) = make_int4(v[0], v[1], v[2], v[3]);
-  else
-  {
-#pragma unroll
-    for(int i = 0; i < 4; ++i)
-      if(mask & (1u << i))
-        p[i] = v[i];
-  }
-}
-__device__ __forceinline__ void store_rows_fast(const DwtLevelDesc& D, const BandGeom& g, const StoreCtx& S, int c, int j,
-                                                bool vhigh, const int (&lo)[4], const int (&hi)[4])
-{
-  const int v = 2 * j + (vhigh ? 1 : 0);
-  if(v < D.v0 || v >= D.v1 || (S.mlo | S.mhi) == 0)
-    return;
-  /* all components of a descriptor share the alignment of component 0 (planes are equally laid out) */
-  if(!vhigh)
-  {
-    const int r = j - g.y0l;
-    store4v(reinterpret_cast<int32_t*>(D.out_ll[c]) + (r * (int)D.ll_pitch + S.col_ll), lo, S.mlo, S.vec_ll);
-    store4v(reinterpret_cast<int32_t*>(D.out_c[c]) + (r * (int)D.c_pitch + S.col_hi), hi, S.mhi, S.vec_hi);
-  }
-  else
-  {
-    const int r = g.sny + j - g.y0h;
-    int32_t* crow = reinterpret_cast<int32_t*>(D.out_c[c]) + r * (int)D.c_pitch;
-    store4v(crow + S.col_lo, lo, S.mlo, S.vec_lo);
-    store4v(crow + S.col_hi, hi, S.mhi, S.vec_hi);
-  }
-}
-
-
 /* a tile component one sample wide or high at this level: straightforward, unpipelined path
-   (WaveletFwd.cpp L146-156, L289-300 special cases live here, not in the hot loop) */
-template <int NC, bool U16>
+   (WaveletFwd.cpp L146-156, L289-300 special cases live here, not in the hot loop).  The degenerate
+   jobs build their store context at every store instead of keeping it live across the loop: held in
+   registers it would raise the register count of the kernel that calls them. */
+template <int NC>
 __device__ __noinline__ void fwd53_degenerate_job(const DwtLevelDesc* __restrict__ dptr, const Job J)
 {
   const DwtLevelDesc& D = *dptr; /* re-read from global memory: this path is cold */
@@ -667,9 +688,9 @@ __device__ __noinline__ void fwd53_degenerate_job(const DwtLevelDesc* __restrict
   int E[NC][8], DP[NC][8];
   {
     int A[NC][8], B[NC][8];
-    fetch53<NC, U16>(D, J, 2 * J.jbeg - 2, A);
-    fetch53<NC, U16>(D, J, 2 * J.jbeg - 1, B);
-    fetch53<NC, U16>(D, J, 2 * J.jbeg, E);
+    fetch53<NC>(D, J, 2 * J.jbeg - 2, A);
+    fetch53<NC>(D, J, 2 * J.jbeg - 1, B);
+    fetch53<NC>(D, J, 2 * J.jbeg, E);
 #pragma unroll
     for(int c = 0; c < NC; ++c)
 #pragma unroll
@@ -679,8 +700,8 @@ __device__ __noinline__ void fwd53_degenerate_job(const DwtLevelDesc* __restrict
   for(int j = J.jbeg; j < J.jend; ++j)
   {
     int O[NC][8], E2[NC][8];
-    fetch53<NC, U16>(D, J, 2 * j + 1, O);
-    fetch53<NC, U16>(D, J, 2 * j + 2, E2);
+    fetch53<NC>(D, J, 2 * j + 1, O);
+    fetch53<NC>(D, J, 2 * j + 2, E2);
 #pragma unroll 1
     for(int c = 0; c < NC; ++c)
     {
@@ -700,9 +721,9 @@ __device__ __noinline__ void fwd53_degenerate_job(const DwtLevelDesc* __restrict
       }
       int lo[4], hi[4];
       hfwd53<true>(s, J.wn, lo, hi);
-      store_band_rows(D, J, g, c, j, false, lo, hi);
+      store_rows(D, g, store_ctx(D, J, g), c, j, false, lo, hi);
       hfwd53<true>(d, J.wn, lo, hi);
-      store_band_rows(D, J, g, c, j, true, lo, hi);
+      store_rows(D, g, store_ctx(D, J, g), c, j, true, lo, hi);
     }
   }
 }
@@ -710,75 +731,44 @@ __device__ __noinline__ void fwd53_degenerate_job(const DwtLevelDesc* __restrict
 /* =============================================================================================
  * forward 5/3
  * =========================================================================================== */
-template <int NC, bool U16, int STAGES>
+template <int NC>
 __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_fwd(const DwtLevelDesc* __restrict__ descs)
 {
   extern __shared__ __align__(16) uint8_t smem_dwt[];
-  typedef RowStage<NC, U16> RS;
+  typedef RowStage<NC> RS;
   const DwtLevelDesc D = descs[blockIdx.y]; /* by value: fields live in (uniform) registers, not re-read after every store */
   Job J;
   if(!decode_job(D, J))
     return;
   if(J.hn == 1 || J.wn == 1)
   {
-    fwd53_degenerate_job<NC, U16>(descs + blockIdx.y, J);
+    fwd53_degenerate_job<NC>(descs + blockIdx.y, J);
     return;
   }
   const BandGeom g = band_geom(D);
   const StoreCtx SC = store_ctx(D, J, g);
-  uint8_t* wsm = smem_dwt + (size_t)(threadIdx.x >> 5) * STAGES * RS::PAIRB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_dwt + (size_t)B2K_WARPS_PER_CTA * STAGES * RS::PAIRB) + (threadIdx.x >> 5) * STAGES;
   const bool fast = RS::lane_fast(D, J);
   const unsigned fastmask = __ballot_sync(0xffffffffu, fast);
-  /* interior strip: rows arrive by bulk copy (TMA engine) on per-slot mbarriers; edge strips keep the LDGSTS path */
-  const bool bulk = !U16 && fastmask == 0xffffffffu;
-  if(bulk)
-  {
-    if(J.lane == 0)
-    {
-#pragma unroll
-      for(int s = 0; s < STAGES; ++s)
-        mbar_init(bars + s, 1);
-      mbar_fence_init();
-    }
-    __syncwarp();
-  }
   int mcol[8]; /* mirrored column of each of the lane's samples: only edge lanes use them */
 #pragma unroll
   for(int i = 0; i < 8; ++i)
     mcol[i] = mirror_rel(J.ulane - D.u0 + i, J.wn);
 
-  /* pairs t = jbeg-1 .. jend-1 : rows (2t+1, 2t+2); the even row before them is fetched directly */
+  /* pairs t = jbeg-1 .. jend-1 : rows (2t+1, 2t+2); the even row before them is fetched directly.
+     Interior strip: rows arrive by bulk copy (TMA engine); edge strips keep the LDGSTS path */
   const int tfirst = J.jbeg - 1, tlast = J.jend - 1;
-  int tfill = tfirst;
-  auto fill_pair = [&](int tf) {
-    const int slot = (tf - tfirst) % STAGES;
-    uint8_t* st = wsm + (size_t)slot * RS::PAIRB;
-    if(bulk)
-    {
-      if(J.lane == 0)
-      {
-        mbar_expect_tx(bars + slot, RS::PAIRB);
-        RS::fill_bulk(st, 0, D, J, 2 * tf + 1, bars + slot);
-        RS::fill_bulk(st, 1, D, J, 2 * tf + 2, bars + slot);
-      }
-    }
-    else
-    {
-      RS::fill(st, 0, D, J, 2 * tf + 1, fast, fastmask, mcol);
-      RS::fill(st, 1, D, J, 2 * tf + 2, fast, fastmask, mcol);
-    }
+  WarpPipe<RS> pipe(smem_dwt, fastmask == 0xffffffffu, tfirst, tlast);
+  auto fill_bulk = [&](uint8_t* st, int tf, uint64_t* bar) {
+    RS::fill_bulk(st, 0, D, J, 2 * tf + 1, bar);
+    RS::fill_bulk(st, 1, D, J, 2 * tf + 2, bar);
   };
-#pragma unroll
-  for(int s = 0; s < STAGES - 1; ++s)
-  {
-    if(tfill <= tlast)
-      fill_pair(tfill);
-    cp_async_commit();
-    ++tfill;
-  }
+  auto fill_async = [&](uint8_t* st, int tf) {
+    RS::fill(st, 0, D, J, 2 * tf + 1, fast, fastmask, mcol);
+    RS::fill(st, 1, D, J, 2 * tf + 2, fast, fastmask, mcol);
+  };
+  pipe.prime(fill_bulk, fill_async);
   int E[NC][8], DP[NC][8];
-  fetch53<NC, U16>(D, J, 2 * tfirst, E);
+  fetch53<NC>(D, J, 2 * tfirst, E);
 #pragma unroll
   for(int c = 0; c < NC; ++c)
 #pragma unroll
@@ -787,28 +777,12 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_fwd(const DwtL
 
   for(int t = tfirst; t <= tlast; ++t)
   {
-    __syncwarp(); /* every lane has read the stage that is refilled next */
-    if(tfill <= tlast)
-      fill_pair(tfill);
-    cp_async_commit();
-    ++tfill;
-    const uint8_t* st = wsm + (size_t)((t - tfirst) % STAGES) * RS::PAIRB;
+    const uint8_t* st = pipe.acquire(t, fill_bulk, fill_async);
     int O[NC][8], E2[NC][8];
-    if(bulk)
-    {
-      mbar_wait(bars + (t - tfirst) % STAGES, (unsigned)(((t - tfirst) / STAGES) & 1));
-      RS::read_linear(st, 0, J, O);
-      RS::read_linear(st, 1, J, E2);
-    }
-    else
-    {
-      cp_async_wait<STAGES - 1>();
-      __syncwarp(); /* rows were copied cooperatively */
-      RS::read(st, 0, D, J, O);
-      RS::read(st, 1, D, J, E2);
-    }
-    rct_fwd_inplace<NC>(D, O);
-    rct_fwd_inplace<NC>(D, E2);
+    RS::read(st, 0, J, pipe.bulk, O);
+    RS::read(st, 1, J, pipe.bulk, E2);
+    to_coeffs53<NC>(D, O);
+    to_coeffs53<NC>(D, E2);
     const bool emit = t >= J.jbeg;
 #pragma unroll
     for(int c = 0; c < NC; ++c)
@@ -826,20 +800,20 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_fwd(const DwtL
       { /* warp-uniform */
         int lo[4], hi[4];
         hfwd53<false>(s, J.wn, lo, hi);
-        store_rows_fast(D, g, SC, c, t, false, lo, hi);
+        store_rows(D, g, SC, c, t, false, lo, hi);
         hfwd53<false>(d, J.wn, lo, hi);
-        store_rows_fast(D, g, SC, c, t, true, lo, hi);
+        store_rows(D, g, SC, c, t, true, lo, hi);
       }
     }
   }
-  cp_async_wait<0>();
+  pipe.drain();
 }
 
 /* =============================================================================================
  * forward 9/7: vertical pipeline  d1[t] -> s1[t] -> d2[t-1] -> s2[t-1]   (see DESIGN.md)
  * =========================================================================================== */
 /* unpipelined path for lines of one sample (cold) */
-template <int NC, bool U16>
+template <int NC>
 __device__ __noinline__ void fwd97_degenerate_job(const DwtLevelDesc* __restrict__ dptr, const Job J)
 {
   const DwtLevelDesc& D = *dptr;
@@ -848,7 +822,7 @@ __device__ __noinline__ void fwd97_degenerate_job(const DwtLevelDesc* __restrict
   const float deltaS = __fmul_rn(F97_DELTA, invK);
 
   float Ev[NC][8], D1[NC][8], S1[NC][8], D2[NC][8];
-  fetch97<NC, U16>(D, J, 2 * (J.jbeg - 2), Ev);
+  fetch97<NC>(D, J, 2 * (J.jbeg - 2), Ev);
 #pragma unroll
   for(int c = 0; c < NC; ++c)
 #pragma unroll
@@ -858,8 +832,8 @@ __device__ __noinline__ void fwd97_degenerate_job(const DwtLevelDesc* __restrict
   for(int t = J.jbeg - 2; t <= J.jend; ++t)
   {
     float O[NC][8], E2[NC][8];
-    fetch97<NC, U16>(D, J, 2 * t + 1, O);
-    fetch97<NC, U16>(D, J, 2 * t + 2, E2);
+    fetch97<NC>(D, J, 2 * t + 1, O);
+    fetch97<NC>(D, J, 2 * t + 2, E2);
     const bool emit = (t - 1) >= J.jbeg;
 #pragma unroll
     for(int c = 0; c < NC; ++c)
@@ -889,83 +863,32 @@ __device__ __noinline__ void fwd97_degenerate_job(const DwtLevelDesc* __restrict
       int lo[4], hi[4];
       hfwd97(lowrow, J.wn, invK, deltaS, lo, hi);
       if(emit)
-        store_band_rows(D, J, g, c, t - 1, false, lo, hi);
+        store_rows(D, g, store_ctx(D, J, g), c, t - 1, false, lo, hi);
       hfwd97(highrow, J.wn, invK, deltaS, lo, hi);
       if(emit)
-        store_band_rows(D, J, g, c, t - 1, true, lo, hi);
+        store_rows(D, g, store_ctx(D, J, g), c, t - 1, true, lo, hi);
     }
   }
 }
 
-
-/* float samples of a staged row: finest level = integers from the image (+DC shift, +ICT,
-   mct.cpp L584-636), other levels = float bits */
 template <int NC>
-__device__ __forceinline__ void ict_fwd_convert(const DwtLevelDesc& D, const int (&raw)[NC][8], float (&out)[NC][8])
-{
-  if(D.first_level)
-  {
-    const float a_r = 0.299f, a_g = 0.587f, a_b = 0.114f;
-    const float cb = __fdiv_rn(0.5f, __fsub_rn(1.0f, a_b)), cr = __fdiv_rn(0.5f, __fsub_rn(1.0f, a_r));
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-    {
-      if(NC == 3)
-      {
-        const float r = (float)(raw[0][i] + D.shift[0]), g = (float)(raw[NC > 1 ? 1 : 0][i] + D.shift[1]),
-                    b = (float)(raw[NC > 2 ? 2 : 0][i] + D.shift[2]);
-        /* the reference build contracts a_r*r + a_g*g + a_b*b into two FMAs (pinned against libgrokj2k, tests/test_interop.py) */
-        const float y = __fmaf_rn(a_b, b, __fmaf_rn(a_g, g, __fmul_rn(a_r, r)));
-        out[0][i] = y;
-        out[NC > 1 ? 1 : 0][i] = __fmul_rn(cb, __fsub_rn(b, y));
-        out[NC > 2 ? 2 : 0][i] = __fmul_rn(cr, __fsub_rn(r, y));
-      }
-      else
-        out[0][i] = (float)(raw[0][i] + D.shift[0]);
-    }
-  }
-  else
-  {
-#pragma unroll
-    for(int c = 0; c < NC; ++c)
-#pragma unroll
-      for(int i = 0; i < 8; ++i)
-        out[c][i] = __int_as_float(raw[c][i]);
-  }
-}
-
-template <int NC, bool U16, int STAGES>
 __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_fwd(const DwtLevelDesc* __restrict__ descs)
 {
   extern __shared__ __align__(16) uint8_t smem_dwt[];
-  typedef RowStage<NC, U16> RS;
+  typedef RowStage<NC> RS;
   const DwtLevelDesc D = descs[blockIdx.y]; /* by value */
   Job J;
   if(!decode_job(D, J))
     return;
   if(J.hn == 1 || J.wn == 1)
   {
-    fwd97_degenerate_job<NC, U16>(descs + blockIdx.y, J);
+    fwd97_degenerate_job<NC>(descs + blockIdx.y, J);
     return;
   }
   const BandGeom g = band_geom(D);
   const StoreCtx SC = store_ctx(D, J, g);
-  uint8_t* wsm = smem_dwt + (size_t)(threadIdx.x >> 5) * STAGES * RS::PAIRB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_dwt + (size_t)B2K_WARPS_PER_CTA * STAGES * RS::PAIRB) + (threadIdx.x >> 5) * STAGES;
   const bool fast = RS::lane_fast(D, J);
   const unsigned fastmask = __ballot_sync(0xffffffffu, fast);
-  const bool bulk = !U16 && fastmask == 0xffffffffu; /* interior strip: rows by bulk copy (TMA engine), see k_dwt53_fwd */
-  if(bulk)
-  {
-    if(J.lane == 0)
-    {
-#pragma unroll
-      for(int s = 0; s < STAGES; ++s)
-        mbar_init(bars + s, 1);
-      mbar_fence_init();
-    }
-    __syncwarp();
-  }
   int mcol[8];
 #pragma unroll
   for(int i = 0; i < 8; ++i)
@@ -973,37 +896,21 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_fwd(const DwtL
   const float invK = (float)(1.0 / 1.230174105);
   const float deltaS = __fmul_rn(F97_DELTA, invK);
 
-  /* pairs t = jbeg-2 .. jend : rows (2t+1, 2t+2); output pair t-1 from t = jbeg+1 on */
+  /* pairs t = jbeg-2 .. jend : rows (2t+1, 2t+2); output pair t-1 from t = jbeg+1 on.
+     Interior strip: rows by bulk copy (TMA engine), see k_dwt53_fwd */
   const int tfirst = J.jbeg - 2, tlast = J.jend;
-  int tfill = tfirst;
-  auto fill_pair = [&](int tf) {
-    const int slot = (tf - tfirst) % STAGES;
-    uint8_t* st = wsm + (size_t)slot * RS::PAIRB;
-    if(bulk)
-    {
-      if(J.lane == 0)
-      {
-        mbar_expect_tx(bars + slot, RS::PAIRB);
-        RS::fill_bulk(st, 0, D, J, 2 * tf + 1, bars + slot);
-        RS::fill_bulk(st, 1, D, J, 2 * tf + 2, bars + slot);
-      }
-    }
-    else
-    {
-      RS::fill(st, 0, D, J, 2 * tf + 1, fast, fastmask, mcol);
-      RS::fill(st, 1, D, J, 2 * tf + 2, fast, fastmask, mcol);
-    }
+  WarpPipe<RS> pipe(smem_dwt, fastmask == 0xffffffffu, tfirst, tlast);
+  auto fill_bulk = [&](uint8_t* st, int tf, uint64_t* bar) {
+    RS::fill_bulk(st, 0, D, J, 2 * tf + 1, bar);
+    RS::fill_bulk(st, 1, D, J, 2 * tf + 2, bar);
   };
-#pragma unroll
-  for(int s = 0; s < STAGES - 1; ++s)
-  {
-    if(tfill <= tlast)
-      fill_pair(tfill);
-    cp_async_commit();
-    ++tfill;
-  }
+  auto fill_async = [&](uint8_t* st, int tf) {
+    RS::fill(st, 0, D, J, 2 * tf + 1, fast, fastmask, mcol);
+    RS::fill(st, 1, D, J, 2 * tf + 2, fast, fastmask, mcol);
+  };
+  pipe.prime(fill_bulk, fill_async);
   float Ev[NC][8], D1[NC][8], S1[NC][8], D2[NC][8];
-  fetch97<NC, U16>(D, J, 2 * tfirst, Ev);
+  fetch97<NC>(D, J, 2 * tfirst, Ev);
 #pragma unroll
   for(int c = 0; c < NC; ++c)
 #pragma unroll
@@ -1012,32 +919,14 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_fwd(const DwtL
 
   for(int t = tfirst; t <= tlast; ++t)
   {
-    __syncwarp();
-    if(tfill <= tlast)
-      fill_pair(tfill);
-    cp_async_commit();
-    ++tfill;
-    if(bulk)
-      mbar_wait(bars + (t - tfirst) % STAGES, (unsigned)(((t - tfirst) / STAGES) & 1));
-    else
-    {
-      cp_async_wait<STAGES - 1>();
-      __syncwarp();
-    }
-    const uint8_t* st = wsm + (size_t)((t - tfirst) % STAGES) * RS::PAIRB;
+    const uint8_t* st = pipe.acquire(t, fill_bulk, fill_async);
     float O[NC][8], E2[NC][8];
     {
       int raw[NC][8];
-      if(bulk)
-        RS::read_linear(st, 0, J, raw);
-      else
-        RS::read(st, 0, D, J, raw);
-      ict_fwd_convert<NC>(D, raw, O);
-      if(bulk)
-        RS::read_linear(st, 1, J, raw);
-      else
-        RS::read(st, 1, D, J, raw);
-      ict_fwd_convert<NC>(D, raw, E2);
+      RS::read(st, 0, J, pipe.bulk, raw);
+      to_coeffs97<NC>(D, raw, O);
+      RS::read(st, 1, J, pipe.bulk, raw);
+      to_coeffs97<NC>(D, raw, E2);
     }
     const bool emit = (t - 1) >= J.jbeg;
 #pragma unroll
@@ -1062,13 +951,13 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_fwd(const DwtL
       { /* warp-uniform */
         int lo[4], hi[4];
         hfwd97(lowrow, 2, invK, deltaS, lo, hi);
-        store_rows_fast(D, g, SC, c, t - 1, false, lo, hi);
+        store_rows(D, g, SC, c, t - 1, false, lo, hi);
         hfwd97(highrow, 2, invK, deltaS, lo, hi);
-        store_rows_fast(D, g, SC, c, t - 1, true, lo, hi);
+        store_rows(D, g, SC, c, t - 1, true, lo, hi);
       }
     }
   }
-  cp_async_wait<0>();
+  pipe.drain();
 }
 
 /* =============================================================================================
@@ -1111,6 +1000,7 @@ __device__ __forceinline__ void fetch_band_rows(const DwtLevelDesc& D, const Job
 }
 
 /* inverse horizontal 5/3: WaveletReverse.cpp L879-1072 */
+template <bool DEGEN = true>
 __device__ __forceinline__ void hinv53(const int (&lo)[4], const int (&hi)[4], int wn, int (&r)[8])
 {
   const int dm = __shfl_up_sync(0xffffffffu, hi[3], 1);
@@ -1126,7 +1016,7 @@ __device__ __forceinline__ void hinv53(const int (&lo)[4], const int (&hi)[4], i
     r[2 * i] = e[i];
     r[2 * i + 1] = hi[i] + ((e[i] + e[i + 1]) >> 1);
   }
-  if(wn == 1)
+  if(DEGEN && wn == 1)
   {
 #pragma unroll
     for(int i = 0; i < 4; ++i)
@@ -1180,75 +1070,69 @@ __device__ __forceinline__ void hinv97(const int (&loi)[4], const int (&hii)[4],
   }
 }
 
-/* write one reconstructed sample row (canvas row v) of NC components */
-template <int NC>
-__device__ __forceinline__ void store_rows53(const DwtLevelDesc& D, const Job& J, int v, int (&x)[NC][8])
+/* per-lane constants of the reconstructed-row stores */
+struct OutCtx
 {
-  if(!J.owner || v < D.v0 || v >= D.v1)
-    return;
-  unsigned m = 0;
-#pragma unroll
-  for(int i = 0; i < 8; ++i)
-    if(J.ulane + i >= D.u0 && J.ulane + i < D.u1)
-      m |= 1u << i;
-  if(D.first_level)
+  unsigned m;
+  bool vec;
+  int col;
+};
+__device__ __forceinline__ OutCtx out_ctx(const DwtLevelDesc& D, const Job& J)
+{
+  OutCtx o;
+  o.m = 0;
+  if(J.owner)
   {
 #pragma unroll
     for(int i = 0; i < 8; ++i)
-    {
-      if(NC == 3)
-      { /* mct.cpp L201-256 */
-        const int y = x[0][i], u = x[1][i], w = x[2][i];
-        const int gg = y - ((u + w) >> 2);
-        x[0][i] = w + gg;
-        x[1][i] = gg;
-        x[2][i] = u + gg;
-      }
-#pragma unroll
-      for(int c = 0; c < NC; ++c)
-        x[c][i] = min(max(x[c][i] - D.shift[c], D.lo[c]), D.hi[c]);
-    }
+      if(J.ulane + i >= D.u0 && J.ulane + i < D.u1)
+        o.m |= 1u << i;
   }
+  o.col = J.ulane - D.u0;
+  o.vec = o.m == 0xFF && (D.in_pitch & 3u) == 0 && (((reinterpret_cast<uintptr_t>(D.in[0]) >> 2) + (unsigned)o.col) & 3u) == 0;
+  return o;
+}
+/* write one reconstructed row (canvas row v) of NC components, already in its output form */
+template <int NC>
+__device__ __forceinline__ void store_out_rows(const DwtLevelDesc& D, const OutCtx& O, int v, const int (&x)[NC][8])
+{
 #pragma unroll
   for(int c = 0; c < NC; ++c)
   {
-    int32_t* row = reinterpret_cast<int32_t*>(const_cast<void*>(D.in[c])) + (size_t)(v - D.v0) * D.in_pitch;
-    store8(row, J.ulane - D.u0, x[c], m);
-  }
-}
-template <int NC>
-__device__ __forceinline__ void store_rows97(const DwtLevelDesc& D, const Job& J, int v, float (&x)[NC][8])
-{
-  if(!J.owner || v < D.v0 || v >= D.v1)
-    return;
-  unsigned m = 0;
-#pragma unroll
-  for(int i = 0; i < 8; ++i)
-    if(J.ulane + i >= D.u0 && J.ulane + i < D.u1)
-      m |= 1u << i;
-  int o[NC][8];
-  if(D.first_level)
-  {
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
+    int32_t* p = reinterpret_cast<int32_t*>(const_cast<void*>(D.in[c])) + ((v - D.v0) * (int)D.in_pitch + O.col);
+    if(O.vec)
     {
-      float f[NC];
-      if(NC == 3)
-      { /* mct.cpp L318-391 */
-        const float y = x[0][i], u = x[1][i], w = x[2][i];
-        f[0] = __fmaf_rn(w, 1.402f, y); /* FMA / FNMA as the reference build contracts them (tests/test_interop.py) */
-        if(NC > 1)
-          f[NC > 1 ? 1 : 0] = __fmaf_rn(-w, 0.71414f, __fmaf_rn(-u, 0.34413f, y));
-        if(NC > 2)
-          f[NC > 2 ? 2 : 0] = __fmaf_rn(u, 1.772f, y);
-      }
-      else
-        f[0] = x[0][i];
+      reinterpret_cast<int4*>(p)[0] = make_int4(x[c][0], x[c][1], x[c][2], x[c][3]);
+      reinterpret_cast<int4*>(p)[1] = make_int4(x[c][4], x[c][5], x[c][6], x[c][7]);
+    }
+    else
+    {
 #pragma unroll
-      for(int c = 0; c < NC; ++c)
-        o[c][i] = min(max(__float2int_rn(f[c]) - D.shift[c], D.lo[c]), D.hi[c]);
+      for(int i = 0; i < 8; ++i)
+        if(O.m & (1u << i))
+          p[i] = x[c][i];
     }
   }
+}
+/* 5/3: at the finest level the samples go through the inverse RCT + DC shift + clamp (in place) */
+template <int NC>
+__device__ __forceinline__ void store_rows53(const DwtLevelDesc& D, const OutCtx& O, int v, int (&x)[NC][8])
+{
+  if(v < D.v0 || v >= D.v1 || O.m == 0)
+    return;
+  if(D.first_level)
+    rct_inv<NC>(D, x);
+  store_out_rows<NC>(D, O, v, x);
+}
+/* 9/7: at the finest level inverse ICT + rounding + DC shift + clamp, elsewhere the float bits */
+template <int NC>
+__device__ __forceinline__ void store_rows97(const DwtLevelDesc& D, const OutCtx& O, int v, const float (&x)[NC][8])
+{
+  if(v < D.v0 || v >= D.v1 || O.m == 0)
+    return;
+  int o[NC][8];
+  if(D.first_level)
+    ict_inv<NC>(D, x, o);
   else
   {
 #pragma unroll
@@ -1257,12 +1141,7 @@ __device__ __forceinline__ void store_rows97(const DwtLevelDesc& D, const Job& J
       for(int i = 0; i < 8; ++i)
         o[c][i] = __float_as_int(x[c][i]);
   }
-#pragma unroll
-  for(int c = 0; c < NC; ++c)
-  {
-    int32_t* row = reinterpret_cast<int32_t*>(const_cast<void*>(D.in[c])) + (size_t)(v - D.v0) * D.in_pitch;
-    store8(row, J.ulane - D.u0, o[c], m);
-  }
+  store_out_rows<NC>(D, O, v, o);
 }
 
 /* a resolution one sample wide or high: straightforward, unpipelined path (cold) */
@@ -1312,14 +1191,14 @@ __device__ __noinline__ void inv53_degenerate_job(const DwtLevelDesc* __restrict
 #pragma unroll
           for(int i = 0; i < 8; ++i)
             hv[c][i] = dv[c][i] >> 1;
-        store_rows53<NC>(D, J, 2 * t, sv);
-        store_rows53<NC>(D, J, 2 * t + 1, hv);
+        store_rows53<NC>(D, out_ctx(D, J), 2 * t, sv);
+        store_rows53<NC>(D, out_ctx(D, J), 2 * t + 1, hv);
       }
     }
     else if(t - 1 >= J.jbeg)
     {
-      store_rows53<NC>(D, J, 2 * (t - 1), Er);
-      store_rows53<NC>(D, J, 2 * (t - 1) + 1, Or);
+      store_rows53<NC>(D, out_ctx(D, J), 2 * (t - 1), Er);
+      store_rows53<NC>(D, out_ctx(D, J), 2 * (t - 1) + 1, Or);
     }
   }
 }
@@ -1333,6 +1212,7 @@ struct BandStage
 {
   static constexpr int ROWB = 512;
   static constexpr int PAIRB = 4 * NC * ROWB;
+  static constexpr bool COOPERATIVE = false;
   struct Lane
   {
     bool need;
@@ -1422,108 +1302,7 @@ struct BandStage
   }
 };
 
-/* per-lane constants of the reconstructed-row stores */
-struct OutCtx
-{
-  unsigned m;
-  bool vec;
-  int col;
-};
-template <bool OUT16 = false>
-__device__ __forceinline__ OutCtx out_ctx(const DwtLevelDesc& D, const Job& J)
-{
-  OutCtx o;
-  o.m = 0;
-  if(J.owner)
-  {
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-      if(J.ulane + i >= D.u0 && J.ulane + i < D.u1)
-        o.m |= 1u << i;
-  }
-  o.col = J.ulane - D.u0;
-  if(OUT16)
-    o.vec = o.m == 0xFF && (D.in_pitch & 7u) == 0 && (((reinterpret_cast<uintptr_t>(D.in[0]) >> 1) + (unsigned)o.col) & 7u) == 0;
-  else
-    o.vec = o.m == 0xFF && (D.in_pitch & 3u) == 0 && (((reinterpret_cast<uintptr_t>(D.in[0]) >> 2) + (unsigned)o.col) & 3u) == 0;
-  return o;
-}
-template <int NC, bool OUT16 = false>
-__device__ __forceinline__ void store_rows53_fast(const DwtLevelDesc& D, const OutCtx& O, int v, int (&x)[NC][8])
-{
-  if(v < D.v0 || v >= D.v1 || O.m == 0)
-    return;
-  if(D.first_level)
-  {
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-    {
-      if(NC == 3)
-      { /* mct.cpp L201-256 */
-        const int y = x[0][i], u = x[NC > 1 ? 1 : 0][i], w = x[NC > 2 ? 2 : 0][i];
-        const int gg = y - ((u + w) >> 2);
-        x[0][i] = w + gg;
-        x[NC > 1 ? 1 : 0][i] = gg;
-        x[NC > 2 ? 2 : 0][i] = u + gg;
-      }
-#pragma unroll
-      for(int c = 0; c < NC; ++c)
-        x[c][i] = min(max(x[c][i] - D.shift[c], D.lo[c]), D.hi[c]);
-    }
-  }
-#pragma unroll
-  for(int c = 0; c < NC; ++c)
-  {
-    if(OUT16)
-    { /* 16-bit sample containers: the clamped value fits, two's complement for signed data */
-      uint16_t* q = reinterpret_cast<uint16_t*>(const_cast<void*>(D.in[c])) + ((v - D.v0) * (int)D.in_pitch + O.col);
-      if(O.vec)
-        *reinterpret_cast<uint4*>(q) = make_uint4((x[c][0] & 0xFFFF) | (x[c][1] << 16), (x[c][2] & 0xFFFF) | (x[c][3] << 16),
-                                                  (x[c][4] & 0xFFFF) | (x[c][5] << 16), (x[c][6] & 0xFFFF) | (x[c][7] << 16));
-      else
-      {
-#pragma unroll
-        for(int i = 0; i < 8; ++i)
-          if(O.m & (1u << i))
-            q[i] = (uint16_t)x[c][i];
-      }
-      continue;
-    }
-    int32_t* p = reinterpret_cast<int32_t*>(const_cast<void*>(D.in[c])) + ((v - D.v0) * (int)D.in_pitch + O.col);
-    if(O.vec)
-    {
-      reinterpret_cast<int4*>(p)[0] = make_int4(x[c][0], x[c][1], x[c][2], x[c][3]);
-      reinterpret_cast<int4*>(p)[1] = make_int4(x[c][4], x[c][5], x[c][6], x[c][7]);
-    }
-    else
-    {
-#pragma unroll
-      for(int i = 0; i < 8; ++i)
-        if(O.m & (1u << i))
-          p[i] = x[c][i];
-    }
-  }
-}
-
-template <bool DEGEN = true>
-__device__ __forceinline__ void hinv53t(const int (&lo)[4], const int (&hi)[4], int (&r)[8])
-{
-  const int dm = __shfl_up_sync(0xffffffffu, hi[3], 1);
-  int e[5];
-  e[0] = lo[0] - ((dm + hi[0] + 2) >> 2);
-  e[1] = lo[1] - ((hi[0] + hi[1] + 2) >> 2);
-  e[2] = lo[2] - ((hi[1] + hi[2] + 2) >> 2);
-  e[3] = lo[3] - ((hi[2] + hi[3] + 2) >> 2);
-  e[4] = __shfl_down_sync(0xffffffffu, e[0], 1);
-#pragma unroll
-  for(int i = 0; i < 4; ++i)
-  {
-    r[2 * i] = e[i];
-    r[2 * i + 1] = hi[i] + ((e[i] + e[i + 1]) >> 1);
-  }
-}
-
-template <int NC, int STAGES, bool OUT16>
+template <int NC>
 __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtLevelDesc* __restrict__ descs)
 {
   extern __shared__ __align__(16) uint8_t smem_dwt[];
@@ -1532,7 +1311,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtL
   Job J;
   if(!decode_job(D, J))
     return;
-  if((J.hn == 1 || J.wn == 1) && !OUT16)
+  if(J.hn == 1 || J.wn == 1)
   {
     inv53_degenerate_job<NC>(descs + blockIdx.y, J);
     return;
@@ -1540,46 +1319,14 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtL
   const BandGeom g = band_geom(D);
   typename BS::Lane L;
   BS::setup(D, J, g, L);
-  const OutCtx OC = out_ctx<OUT16>(D, J);
-  uint8_t* wsm = smem_dwt + (size_t)(threadIdx.x >> 5) * STAGES * BS::PAIRB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_dwt + (size_t)B2K_WARPS_PER_CTA * STAGES * BS::PAIRB) + (threadIdx.x >> 5) * STAGES;
-  const bool bulk = BS::all_fast(L); /* interior strip: band rows by bulk copy (TMA engine) on per-slot mbarriers */
-  if(bulk)
-  {
-    if(J.lane == 0)
-    {
-#pragma unroll
-      for(int s = 0; s < STAGES; ++s)
-        mbar_init(bars + s, 1);
-      mbar_fence_init();
-    }
-    __syncwarp();
-  }
+  const OutCtx OC = out_ctx(D, J);
 
+  /* interior strip: band rows by bulk copy (TMA engine) on per-slot mbarriers */
   const int tfirst = J.jbeg - 1, tlast = J.jend;
-  auto fill_pair = [&](int tf) {
-    const int slot = (tf - tfirst) % STAGES;
-    uint8_t* st = wsm + (size_t)slot * BS::PAIRB;
-    if(bulk)
-    {
-      if(J.lane == 0)
-      {
-        mbar_expect_tx(bars + slot, BS::PAIRB);
-        BS::fill_bulk(st, D, J, g, L, tf, bars + slot);
-      }
-    }
-    else
-      BS::fill(st, D, J, g, L, tf);
-  };
-  int tfill = tfirst;
-#pragma unroll
-  for(int s = 0; s < STAGES - 1; ++s)
-  {
-    if(tfill <= tlast)
-      fill_pair(tfill);
-    cp_async_commit();
-    ++tfill;
-  }
+  WarpPipe<BS> pipe(smem_dwt, BS::all_fast(L), tfirst, tlast);
+  auto fill_bulk = [&](uint8_t* st, int tf, uint64_t* bar) { BS::fill_bulk(st, D, J, g, L, tf, bar); };
+  auto fill_async = [&](uint8_t* st, int tf) { BS::fill(st, D, J, g, L, tf); };
+  pipe.prime(fill_bulk, fill_async);
   int DV[NC][8], EP[NC][8];
 #pragma unroll
   for(int c = 0; c < NC; ++c)
@@ -1589,17 +1336,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtL
 
   for(int t = tfirst; t <= tlast; ++t)
   {
-    if(bulk)
-      __syncwarp(); /* every lane has read the slot that is refilled next */
-    if(tfill <= tlast)
-      fill_pair(tfill);
-    cp_async_commit();
-    ++tfill;
-    if(bulk)
-      mbar_wait(bars + (t - tfirst) % STAGES, (unsigned)(((t - tfirst) / STAGES) & 1));
-    else
-      cp_async_wait<STAGES - 1>();
-    const uint8_t* st = wsm + (size_t)((t - tfirst) % STAGES) * BS::PAIRB;
+    const uint8_t* st = pipe.acquire(t, fill_bulk, fill_async);
     int Er[NC][8], Or[NC][8];
 #pragma unroll
     for(int c = 0; c < NC; ++c)
@@ -1607,10 +1344,10 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtL
       int lo[4], hi[4], sv[8], dv[8];
       BS::read(st, J, 0, c, lo);
       BS::read(st, J, 1, c, hi);
-      hinv53t<false>(lo, hi, sv);
+      hinv53<false>(lo, hi, J.wn, sv);
       BS::read(st, J, 2, c, lo);
       BS::read(st, J, 3, c, hi);
-      hinv53t<false>(lo, hi, dv);
+      hinv53<false>(lo, hi, J.wn, dv);
 #pragma unroll
       for(int i = 0; i < 8; ++i)
       {
@@ -1623,11 +1360,11 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtL
     }
     if(t - 1 >= J.jbeg)
     {
-      store_rows53_fast<NC, OUT16>(D, OC, 2 * (t - 1), Er);
-      store_rows53_fast<NC, OUT16>(D, OC, 2 * (t - 1) + 1, Or);
+      store_rows53<NC>(D, OC, 2 * (t - 1), Er);
+      store_rows53<NC>(D, OC, 2 * (t - 1) + 1, Or);
     }
   }
-  cp_async_wait<0>();
+  pipe.drain();
 }
 
 /* unpipelined path for lines of one sample (cold) */
@@ -1679,73 +1416,19 @@ __device__ __noinline__ void inv97_degenerate_job(const DwtLevelDesc* __restrict
     {
       if(t >= J.jbeg && t < J.jend)
       {
-        store_rows97<NC>(D, J, 2 * t, sv);
-        store_rows97<NC>(D, J, 2 * t + 1, dv);
+        store_rows97<NC>(D, out_ctx(D, J), 2 * t, sv);
+        store_rows97<NC>(D, out_ctx(D, J), 2 * t + 1, dv);
       }
     }
     else if(t - 2 >= J.jbeg)
     {
-      store_rows97<NC>(D, J, 2 * (t - 2), Er);
-      store_rows97<NC>(D, J, 2 * (t - 2) + 1, Or);
+      store_rows97<NC>(D, out_ctx(D, J), 2 * (t - 2), Er);
+      store_rows97<NC>(D, out_ctx(D, J), 2 * (t - 2) + 1, Or);
     }
   }
 }
-
 
 template <int NC>
-__device__ __forceinline__ void store_rows97_fast(const DwtLevelDesc& D, const OutCtx& O, int v, float (&x)[NC][8])
-{
-  if(v < D.v0 || v >= D.v1 || O.m == 0)
-    return;
-  int o[NC][8];
-  if(D.first_level)
-  {
-#pragma unroll
-    for(int i = 0; i < 8; ++i)
-    {
-      float f[NC];
-      if(NC == 3)
-      { /* mct.cpp L318-391 */
-        const float y = x[0][i], u = x[NC > 1 ? 1 : 0][i], w = x[NC > 2 ? 2 : 0][i];
-        f[0] = __fmaf_rn(w, 1.402f, y); /* FMA / FNMA as the reference build contracts them (tests/test_interop.py) */
-        f[NC > 1 ? 1 : 0] = __fmaf_rn(-w, 0.71414f, __fmaf_rn(-u, 0.34413f, y));
-        f[NC > 2 ? 2 : 0] = __fmaf_rn(u, 1.772f, y);
-      }
-      else
-        f[0] = x[0][i];
-#pragma unroll
-      for(int c = 0; c < NC; ++c)
-        o[c][i] = min(max(__float2int_rn(f[c]) - D.shift[c], D.lo[c]), D.hi[c]);
-    }
-  }
-  else
-  {
-#pragma unroll
-    for(int c = 0; c < NC; ++c)
-#pragma unroll
-      for(int i = 0; i < 8; ++i)
-        o[c][i] = __float_as_int(x[c][i]);
-  }
-#pragma unroll
-  for(int c = 0; c < NC; ++c)
-  {
-    int32_t* p = reinterpret_cast<int32_t*>(const_cast<void*>(D.in[c])) + ((v - D.v0) * (int)D.in_pitch + O.col);
-    if(O.vec)
-    {
-      reinterpret_cast<int4*>(p)[0] = make_int4(o[c][0], o[c][1], o[c][2], o[c][3]);
-      reinterpret_cast<int4*>(p)[1] = make_int4(o[c][4], o[c][5], o[c][6], o[c][7]);
-    }
-    else
-    {
-#pragma unroll
-      for(int i = 0; i < 8; ++i)
-        if(O.m & (1u << i))
-          p[i] = o[c][i];
-    }
-  }
-}
-
-template <int NC, int STAGES>
 __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_inv(const DwtLevelDesc* __restrict__ descs)
 {
   extern __shared__ __align__(16) uint8_t smem_dwt[];
@@ -1762,47 +1445,15 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_inv(const DwtL
   const BandGeom g = band_geom(D);
   typename BS::Lane L;
   BS::setup(D, J, g, L);
-  const OutCtx OC = out_ctx<false>(D, J);
-  uint8_t* wsm = smem_dwt + (size_t)(threadIdx.x >> 5) * STAGES * BS::PAIRB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_dwt + (size_t)B2K_WARPS_PER_CTA * STAGES * BS::PAIRB) + (threadIdx.x >> 5) * STAGES;
-  const bool bulk = BS::all_fast(L); /* interior strip: band rows by bulk copy (TMA engine) on per-slot mbarriers */
-  if(bulk)
-  {
-    if(J.lane == 0)
-    {
-#pragma unroll
-      for(int s = 0; s < STAGES; ++s)
-        mbar_init(bars + s, 1);
-      mbar_fence_init();
-    }
-    __syncwarp();
-  }
+  const OutCtx OC = out_ctx(D, J);
   const float K = 1.230174105f, twice_invK = 1.625732422f;
 
+  /* interior strip: band rows by bulk copy (TMA engine) on per-slot mbarriers */
   const int tfirst = J.jbeg - 2, tlast = J.jend + 1;
-  auto fill_pair = [&](int tf) {
-    const int slot = (tf - tfirst) % STAGES;
-    uint8_t* st = wsm + (size_t)slot * BS::PAIRB;
-    if(bulk)
-    {
-      if(J.lane == 0)
-      {
-        mbar_expect_tx(bars + slot, BS::PAIRB);
-        BS::fill_bulk(st, D, J, g, L, tf, bars + slot);
-      }
-    }
-    else
-      BS::fill(st, D, J, g, L, tf);
-  };
-  int tfill = tfirst;
-#pragma unroll
-  for(int s = 0; s < STAGES - 1; ++s)
-  {
-    if(tfill <= tlast)
-      fill_pair(tfill);
-    cp_async_commit();
-    ++tfill;
-  }
+  WarpPipe<BS> pipe(smem_dwt, BS::all_fast(L), tfirst, tlast);
+  auto fill_bulk = [&](uint8_t* st, int tf, uint64_t* bar) { BS::fill_bulk(st, D, J, g, L, tf, bar); };
+  auto fill_async = [&](uint8_t* st, int tf) { BS::fill(st, D, J, g, L, tf); };
+  pipe.prime(fill_bulk, fill_async);
   /* state: d0[t-1], s1[t-1], d1[t-2], s2[t-2] */
   float D0[NC][8], S1[NC][8], D1[NC][8], S2[NC][8];
 #pragma unroll
@@ -1813,17 +1464,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_inv(const DwtL
 
   for(int t = tfirst; t <= tlast; ++t)
   {
-    if(bulk)
-      __syncwarp(); /* every lane has read the slot that is refilled next */
-    if(tfill <= tlast)
-      fill_pair(tfill);
-    cp_async_commit();
-    ++tfill;
-    if(bulk)
-      mbar_wait(bars + (t - tfirst) % STAGES, (unsigned)(((t - tfirst) / STAGES) & 1));
-    else
-      cp_async_wait<STAGES - 1>();
-    const uint8_t* st = wsm + (size_t)((t - tfirst) % STAGES) * BS::PAIRB;
+    const uint8_t* st = pipe.acquire(t, fill_bulk, fill_async);
     float Er[NC][8], Or[NC][8];
 #pragma unroll
     for(int c = 0; c < NC; ++c)
@@ -1854,11 +1495,11 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_inv(const DwtL
     }
     if(t - 2 >= J.jbeg)
     {
-      store_rows97_fast<NC>(D, OC, 2 * (t - 2), Er);
-      store_rows97_fast<NC>(D, OC, 2 * (t - 2) + 1, Or);
+      store_rows97<NC>(D, OC, 2 * (t - 2), Er);
+      store_rows97<NC>(D, OC, 2 * (t - 2) + 1, Or);
     }
   }
-  cp_async_wait<0>();
+  pipe.drain();
 }
 
 /* 16-bit sample containers <-> the engine's 32-bit planes: one rectangle (a merged tile row) per
@@ -1997,91 +1638,40 @@ void b2k_launch_narrow16(const int32_t* src, uint32_t spitch, uint16_t* dst, uin
   b2k_count_launch();
 }
 
-constexpr int FWD_STAGES = 3;
-template <int NC, bool U16, int STAGES>
-static void launch_fwd53(dim3 grid, dim3 block, cudaStream_t st, const DwtLevelDesc* d)
+/* one launch of a DWT kernel whose warps stage through WarpPipe<Stage>; the shared-memory limit it needs is raised once
+   per device for each kernel */
+template <class Stage, void (*KERNEL)(const DwtLevelDesc*)>
+static void launch_dwt(dim3 grid, dim3 block, cudaStream_t st, const DwtLevelDesc* d)
 {
-  const size_t smem = (size_t)B2K_WARPS_PER_CTA * STAGES * RowStage<NC, U16>::PAIRB + (size_t)B2K_WARPS_PER_CTA * STAGES * sizeof(uint64_t);
+  const size_t smem = WarpPipe<Stage>::SMEM_BYTES;
   static DeviceOnce once; /* function attributes are per device */
-  once.run([&] {
-    cudaFuncSetAttribute(k_dwt53_fwd<NC, U16, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  });
-  k_dwt53_fwd<NC, U16, STAGES><<<grid, block, smem, st>>>(d);
+  once.run([&] { cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); });
+  KERNEL<<<grid, block, smem, st>>>(d);
 }
 
-template <int NC, bool U16, int STAGES>
-static void launch_fwd97(dim3 grid, dim3 block, cudaStream_t st, const DwtLevelDesc* d)
-{
-  const size_t smem = (size_t)B2K_WARPS_PER_CTA * STAGES * RowStage<NC, U16>::PAIRB + (size_t)B2K_WARPS_PER_CTA * STAGES * sizeof(uint64_t);
-  static DeviceOnce once; /* function attributes are per device */
-  once.run([&] {
-    cudaFuncSetAttribute(k_dwt97_fwd<NC, U16, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  });
-  k_dwt97_fwd<NC, U16, STAGES><<<grid, block, smem, st>>>(d);
-}
-
-void b2k_launch_dwt_fwd(const DwtLevelDesc* d, int ndesc, int max_jobs, int nc, bool irreversible, bool in_u16,
-                        cudaStream_t st)
+void b2k_launch_dwt_fwd(const DwtLevelDesc* d, int ndesc, int max_jobs, int nc, bool irreversible, cudaStream_t st)
 {
   if(ndesc <= 0 || max_jobs <= 0)
     return;
   dim3 grid((max_jobs + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA, ndesc), block(B2K_WARPS_PER_CTA * 32);
   if(!irreversible)
   {
-    if(nc == 3)
-    {
-      if(in_u16) launch_fwd53<3, true, FWD_STAGES>(grid, block, st, d);
-      else launch_fwd53<3, false, FWD_STAGES>(grid, block, st, d);
-    }
-    else
-    {
-      if(in_u16) launch_fwd53<1, true, FWD_STAGES>(grid, block, st, d);
-      else launch_fwd53<1, false, FWD_STAGES>(grid, block, st, d);
-    }
+    if(nc == 3) launch_dwt<RowStage<3>, k_dwt53_fwd<3>>(grid, block, st, d);
+    else launch_dwt<RowStage<1>, k_dwt53_fwd<1>>(grid, block, st, d);
   }
   else
   {
-    if(nc == 3)
-    {
-      if(in_u16) launch_fwd97<3, true, FWD_STAGES>(grid, block, st, d);
-      else launch_fwd97<3, false, FWD_STAGES>(grid, block, st, d);
-    }
-    else
-    {
-      if(in_u16) launch_fwd97<1, true, FWD_STAGES>(grid, block, st, d);
-      else launch_fwd97<1, false, FWD_STAGES>(grid, block, st, d);
-    }
+    if(nc == 3) launch_dwt<RowStage<3>, k_dwt97_fwd<3>>(grid, block, st, d);
+    else launch_dwt<RowStage<1>, k_dwt97_fwd<1>>(grid, block, st, d);
   }
   b2k_count_launch();
 }
 
-template <int NC, int STAGES, bool OUT16>
-static void launch_inv53(dim3 grid, dim3 block, cudaStream_t st, const DwtLevelDesc* d)
-{
-  const size_t smem = (size_t)B2K_WARPS_PER_CTA * STAGES * BandStage<NC>::PAIRB + (size_t)B2K_WARPS_PER_CTA * STAGES * sizeof(uint64_t);
-  static DeviceOnce once; /* function attributes are per device */
-  once.run([&] {
-    cudaFuncSetAttribute(k_dwt53_inv<NC, STAGES, OUT16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  });
-  k_dwt53_inv<NC, STAGES, OUT16><<<grid, block, smem, st>>>(d);
-}
-
-template <int NC, int STAGES>
-static void launch_inv97(dim3 grid, dim3 block, cudaStream_t st, const DwtLevelDesc* d)
-{
-  const size_t smem = (size_t)B2K_WARPS_PER_CTA * STAGES * BandStage<NC>::PAIRB + (size_t)B2K_WARPS_PER_CTA * STAGES * sizeof(uint64_t);
-  static DeviceOnce once; /* function attributes are per device */
-  once.run([&] {
-    cudaFuncSetAttribute(k_dwt97_inv<NC, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  });
-  k_dwt97_inv<NC, STAGES><<<grid, block, smem, st>>>(d);
-}
-
 /* ---- tiles with NO wavelet level (numres = 1): what is left of the stage is the point transform -- DC shift + RCT / ICT
- * forwards, its inverse + rounding + clamp backwards (mct.cpp L497-636 / L201-391; with one resolution the tile itself is the
- * LL band, TileProcessor.cpp L366-425).  The arithmetic is the level-1 kernels' own (rct_fwd_inplace / ict_fwd_convert,
- * store_rows53 / store_rows97), one sample per thread; the descriptors reuse DwtLevelDesc: in = image samples of the tile
- * component(s), out_c = the tile's place in the coefficient planes. */
+ * forwards, its inverse + rounding + clamp backwards (with one resolution the tile itself is the LL band,
+ * TileProcessor.cpp L366-425).  The arithmetic is the level-1 kernels' own (rct_fwd / ict_fwd, rct_inv / ict_inv), one
+ * sample per thread; the descriptors reuse DwtLevelDesc: in = image samples of the tile component(s), out_c = the tile's
+ * place in the coefficient planes. */
 template <int NC, bool IRREV, bool FWD>
 __global__ void k_point_transform(const DwtLevelDesc* __restrict__ descs, int ndesc)
 {
@@ -2097,84 +1687,47 @@ __global__ void k_point_transform(const DwtLevelDesc* __restrict__ descs, int nd
   const size_t ii = (size_t)y * D.in_pitch + x, oi = (size_t)y * D.c_pitch + x;
   if(FWD)
   {
-    int v[3];
+    int v[NC][1];
 #pragma unroll
     for(int c = 0; c < NC; ++c)
-      v[c] = static_cast<const int32_t*>(D.in[c])[ii] + D.shift[c];
+      v[c][0] = static_cast<const int32_t*>(D.in[c])[ii];
     if(!IRREV)
     {
-      if(NC == 3)
-      {
-        const int r = v[0], g = v[NC > 1 ? 1 : 0], b = v[NC > 2 ? 2 : 0];
-        v[0] = ((g + g) + b + r) >> 2;
-        v[NC > 1 ? 1 : 0] = b - g;
-        v[NC > 2 ? 2 : 0] = r - g;
-      }
+      rct_fwd<NC>(D, v);
 #pragma unroll
       for(int c = 0; c < NC; ++c)
-        static_cast<int32_t*>(D.out_c[c])[oi] = v[c];
+        static_cast<int32_t*>(D.out_c[c])[oi] = v[c][0];
     }
     else
     {
-      float f[3];
-      if(NC == 3)
-      {
-        const float a_r = 0.299f, a_g = 0.587f, a_b = 0.114f;
-        const float cb = __fdiv_rn(0.5f, __fsub_rn(1.0f, a_b)), cr = __fdiv_rn(0.5f, __fsub_rn(1.0f, a_r));
-        const float r = (float)v[0], g = (float)v[NC > 1 ? 1 : 0], b = (float)v[NC > 2 ? 2 : 0];
-        const float yy = __fmaf_rn(a_b, b, __fmaf_rn(a_g, g, __fmul_rn(a_r, r)));
-        f[0] = yy;
-        f[NC > 1 ? 1 : 0] = __fmul_rn(cb, __fsub_rn(b, yy));
-        f[NC > 2 ? 2 : 0] = __fmul_rn(cr, __fsub_rn(r, yy));
-      }
-      else
-        f[0] = (float)v[0];
+      float f[NC][1];
+      ict_fwd<NC>(D, v, f);
 #pragma unroll
       for(int c = 0; c < NC; ++c)
-        static_cast<float*>(D.out_c[c])[oi] = f[c];
+        static_cast<float*>(D.out_c[c])[oi] = f[c][0];
     }
   }
   else
   {
-    int o[3];
+    int o[NC][1];
     if(!IRREV)
     {
-      int v[3];
 #pragma unroll
       for(int c = 0; c < NC; ++c)
-        v[c] = static_cast<const int32_t*>(D.out_c[c])[oi];
-      if(NC == 3)
-      {
-        const int yy = v[0], u = v[NC > 1 ? 1 : 0], ww = v[NC > 2 ? 2 : 0];
-        const int gg = yy - ((u + ww) >> 2);
-        v[0] = ww + gg;
-        v[NC > 1 ? 1 : 0] = gg;
-        v[NC > 2 ? 2 : 0] = u + gg;
-      }
-#pragma unroll
-      for(int c = 0; c < NC; ++c)
-        o[c] = v[c];
+        o[c][0] = static_cast<const int32_t*>(D.out_c[c])[oi];
+      rct_inv<NC>(D, o);
     }
     else
     {
-      float f[3];
+      float f[NC][1];
 #pragma unroll
       for(int c = 0; c < NC; ++c)
-        f[c] = static_cast<const float*>(D.out_c[c])[oi];
-      if(NC == 3)
-      {
-        const float yy = f[0], u = f[NC > 1 ? 1 : 0], ww = f[NC > 2 ? 2 : 0];
-        f[0] = __fmaf_rn(ww, 1.402f, yy);
-        f[NC > 1 ? 1 : 0] = __fmaf_rn(-ww, 0.71414f, __fmaf_rn(-u, 0.34413f, yy));
-        f[NC > 2 ? 2 : 0] = __fmaf_rn(u, 1.772f, yy);
-      }
-#pragma unroll
-      for(int c = 0; c < NC; ++c)
-        o[c] = __float2int_rn(f[c]);
+        f[c][0] = static_cast<const float*>(D.out_c[c])[oi];
+      ict_inv<NC>(D, f, o);
     }
 #pragma unroll
     for(int c = 0; c < NC; ++c)
-      static_cast<int32_t*>(const_cast<void*>(D.in[c]))[ii] = min(max(o[c] - D.shift[c], D.lo[c]), D.hi[c]);
+      static_cast<int32_t*>(const_cast<void*>(D.in[c]))[ii] = o[c][0];
   }
   } /* rows */
   } /* descriptors */
@@ -2201,29 +1754,20 @@ void b2k_launch_point_transform(const DwtLevelDesc* d, int ndesc, uint32_t max_w
   b2k_count_launch();
 }
 
-void b2k_launch_dwt_inv(const DwtLevelDesc* d, int ndesc, int max_jobs, int nc, bool irreversible, bool out_u16,
-                        cudaStream_t st)
+void b2k_launch_dwt_inv(const DwtLevelDesc* d, int ndesc, int max_jobs, int nc, bool irreversible, cudaStream_t st)
 {
   if(ndesc <= 0 || max_jobs <= 0)
     return;
   dim3 grid((max_jobs + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA, ndesc), block(B2K_WARPS_PER_CTA * 32);
   if(!irreversible)
   {
-    if(out_u16)
-    { /* finest level straight into 16-bit containers (widths of 1 are not supported there: the engine checks) */
-      if(nc == 3) launch_inv53<3, FWD_STAGES, true>(grid, block, st, d);
-      else launch_inv53<1, FWD_STAGES, true>(grid, block, st, d);
-    }
-    else
-    {
-      if(nc == 3) launch_inv53<3, FWD_STAGES, false>(grid, block, st, d);
-      else launch_inv53<1, FWD_STAGES, false>(grid, block, st, d);
-    }
+    if(nc == 3) launch_dwt<BandStage<3>, k_dwt53_inv<3>>(grid, block, st, d);
+    else launch_dwt<BandStage<1>, k_dwt53_inv<1>>(grid, block, st, d);
   }
   else
   {
-    if(nc == 3) launch_inv97<3, FWD_STAGES>(grid, block, st, d);
-    else launch_inv97<1, FWD_STAGES>(grid, block, st, d);
+    if(nc == 3) launch_dwt<BandStage<3>, k_dwt97_inv<3>>(grid, block, st, d);
+    else launch_dwt<BandStage<1>, k_dwt97_inv<1>>(grid, block, st, d);
   }
   b2k_count_launch();
 }

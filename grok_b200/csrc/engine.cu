@@ -607,7 +607,6 @@ static int build_dwt_plan(b2k_device_job* J)
           DwtLevelDesc d{};
           d.u0 = (int32_t)r.x0; d.v0 = (int32_t)r.y0; d.u1 = (int32_t)r.x1; d.v1 = (int32_t)r.y1;
           d.first_level = lvl == 1;
-          d.in_is_u16 = 0;
           d.comp0 = (uint8_t)c;
           const uint32_t llx = (r.x0 + 1) >> 1, lly = (r.y0 + 1) >> 1;
           for(int k = 0; k < nc; ++k)
@@ -1331,7 +1330,7 @@ static int ring_download_all(b2k_device_job* J, void* const* user, const uint32_
 
 /* ---- stages ----------------------------------------------------------------------------------- */
 static int enqueue_forward(b2k_device_job* J, cudaStream_t st, bool time_level1, size_t t0 = 0, size_t t1 = (size_t)-1,
-                           bool use16 = false, cudaEvent_t l1_begin = nullptr, cudaEvent_t l1_end = nullptr)
+                           cudaEvent_t l1_begin = nullptr, cudaEvent_t l1_end = nullptr)
 {
   if(!l1_begin) l1_begin = J->ev[4];
   if(!l1_end) l1_end = J->ev[5];
@@ -1339,8 +1338,6 @@ static int enqueue_forward(b2k_device_job* J, cudaStream_t st, bool time_level1,
   bool first = true;
   for(size_t li = 0; li < J->fwd.size(); ++li)
   {
-    const bool l16 = false;
-    (void)use16;
     LevelLaunch& L = J->fwd[li];
     const uint32_t d0 = L.tile_first[t0], d1 = L.tile_first[t1];
     if(first && time_level1)
@@ -1348,7 +1345,7 @@ static int enqueue_forward(b2k_device_job* J, cudaStream_t st, bool time_level1,
     if(d1 > d0 && L.point)
       b2k_launch_point_transform(L.d_descs + d0, (int)(d1 - d0), L.max_w, L.max_h, L.nc, J->cp.irreversible, true, st);
     else if(d1 > d0)
-      b2k_launch_dwt_fwd(L.d_descs + d0, (int)(d1 - d0), L.max_jobs, L.nc, J->cp.irreversible, l16, st);
+      b2k_launch_dwt_fwd(L.d_descs + d0, (int)(d1 - d0), L.max_jobs, L.nc, J->cp.irreversible, st);
     if(first && time_level1)
     {
       CUDA_TRY(cudaEventRecord(l1_end, st));
@@ -1360,19 +1357,17 @@ static int enqueue_forward(b2k_device_job* J, cudaStream_t st, bool time_level1,
   return 0;
 }
 
-static int enqueue_inverse(b2k_device_job* J, cudaStream_t st, size_t t0 = 0, size_t t1 = (size_t)-1, bool use16 = false)
+static int enqueue_inverse(b2k_device_job* J, cudaStream_t st, size_t t0 = 0, size_t t1 = (size_t)-1)
 {
   t1 = std::min(t1, J->tiles.size());
   for(size_t li = 0; li < J->inv.size(); ++li)
   {
-    const bool l16 = false;
-    (void)use16;
     LevelLaunch& L = J->inv[li];
     const uint32_t d0 = L.tile_first[t0], d1 = L.tile_first[t1];
     if(d1 > d0 && L.point)
       b2k_launch_point_transform(L.d_descs + d0, (int)(d1 - d0), L.max_w, L.max_h, L.nc, J->cp.irreversible, false, st);
     else if(d1 > d0)
-      b2k_launch_dwt_inv(L.d_descs + d0, (int)(d1 - d0), L.max_jobs, L.nc, J->cp.irreversible, l16, st);
+      b2k_launch_dwt_inv(L.d_descs + d0, (int)(d1 - d0), L.max_jobs, L.nc, J->cp.irreversible, st);
   }
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -1675,7 +1670,7 @@ extern "C" int32_t b2k_job_roundtrip_n(b2k_device_job* J, uint32_t steps, float*
   {
     cudaEvent_t* e = J->q_ev.data() + per * s;
     CUDA_TRY(cudaEventRecord(e[0], st));
-    if(enqueue_forward(J, st, true, 0, (size_t)-1, false, e[1], e[2])) return -1;
+    if(enqueue_forward(J, st, true, 0, (size_t)-1, e[1], e[2])) return -1;
     CUDA_TRY(cudaEventRecord(e[3], st));
     if(enqueue_t1_encode(J, st)) return -1;
     b2k_launch_ht_gather(J->d_enc_desc, J->d_out, J->d_offsets, J->d_scratch, J->d_bytes, n, J->bytes_cap, st);
@@ -1781,7 +1776,7 @@ extern "C" int32_t b2k_job_roundtrip_pipelined_n(b2k_device_job* J, uint32_t ste
   {
     cudaEvent_t* e = J->q_ev.data() + per * s;
     CUDA_TRY(cudaEventRecord(e[0], st));
-    if(enqueue_forward(J, st, true, 0, (size_t)-1, false, e[1], e[2])) return -1;
+    if(enqueue_forward(J, st, true, 0, (size_t)-1, e[1], e[2])) return -1;
     CUDA_TRY(cudaEventRecord(e[3], st));
     for(uint32_t k = 0; k < streams && k < nch; ++k)
       CUDA_TRY(cudaStreamWaitEvent(J->p_streams[k], e[3], 0));

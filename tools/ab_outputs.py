@@ -1,0 +1,101 @@
+"""Byte-for-byte A/B check of two library builds on seeded inputs.
+
+    B2K_LIB=<build A> python tools/ab_outputs.py OUT_A
+    B2K_LIB=<build B> python tools/ab_outputs.py OUT_B
+    python tools/ab_outputs.py --compare OUT_A OUT_B
+
+Each run writes, per case, the forward coefficients, the coded bytes and block lengths and the planes that inverse()
+rebuilds from them, as .npy files under OUT.  Cases: tests/test_gpu.py's GEOMS, reversible and irreversible (shapes whose
+coding the engine refuses are skipped), the 9/7 degenerate-geometry shapes, a 2048^2 single-tile 9/7 image, and one
+b2k_encode16 / b2k_decode16 round trip.  --compare exits 1 when any array differs; tolerances would hide a drift of
+one rounding step in the 9/7 inverse, so there are none."""
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+
+
+def cases():
+    import test_gpu
+    degenerate = next(m.args[1] for m in test_gpu.test_irreversible_degenerate_geometry.pytestmark if m.name == "parametrize")
+    out = [("geom%02d_%s" % (i, "irrev" if irr else "rev"), dict(g, irreversible=irr))
+           for irr in (False, True) for i, g in enumerate(test_gpu.GEOMS)]
+    out += [("degen97_%d" % i, dict(g, irreversible=True)) for i, g in enumerate(degenerate)]
+    out.append(("single_tile_97_2048", dict(width=2048, height=2048, numcomps=3, prec=12, irreversible=True)))
+    return out
+
+
+def one_case(G, P, eng, args):
+    planes = P.synthetic_image(args["width"], args["height"], args["numcomps"], args["prec"], seed=42,
+                               origin=args.get("origin", (0, 0)))
+    if args.get("sgnd"):
+        planes = [p - (1 << (args["prec"] - 1)) for p in planes]
+    job = eng.job(G.make_coding(**args))
+    try:
+        job.upload(planes)
+        job.forward()
+        coef = [np.zeros_like(p) for p in planes]
+        job.download_coeffs(coef)
+        arrs = {"coef%d" % c: a for c, a in enumerate(coef)}
+        job.t1_encode()
+        res = job.fetch_result()
+        arrs["bytes"], arrs["lengths"] = res.bytes.copy(), res.blocks["length"].copy()
+        res.free()
+        job.t1_decode()
+        job.inverse()
+        rec = [np.zeros_like(p) for p in planes]
+        job.download(rec)
+        arrs.update(("rec%d" % c, a) for c, a in enumerate(rec))
+        return arrs
+    finally:
+        job.close()
+
+
+def run(outdir):
+    import grok_b200 as G
+    import oracle_pipeline as P
+    os.makedirs(outdir, exist_ok=True)
+    eng = G.Engine()
+    for name, args in cases():
+        try:
+            arrs = one_case(G, P, eng, args)
+        except G.EngineError as e:
+            print("skip %s: %s" % (name, e))
+            continue
+        for k, a in arrs.items():
+            np.save(os.path.join(outdir, "%s.%s.npy" % (name, k)), a)
+    # 16-bit containers: b2k_encode16 / b2k_decode16
+    cp = G.make_coding(600, 300, 3, 12, numres=5, tile=(256, 128), origin=(8, 0))
+    p16 = [p.astype(np.uint16) for p in P.synthetic_image(600, 300, 3, 12, seed=77)]
+    res = eng.encode(cp, p16)
+    rec = [np.zeros_like(p) for p in p16]
+    eng.decode(cp, res.blocks.copy(), res.bytes.copy(), rec)
+    arrs = {"bytes": res.bytes.copy(), "lengths": res.blocks["length"].copy()}
+    arrs.update(("rec%d" % c, a) for c, a in enumerate(rec))
+    res.free()
+    for k, a in arrs.items():
+        np.save(os.path.join(outdir, "u16.%s.npy" % k), a)
+    eng.close()
+    print("wrote %d arrays to %s" % (len(os.listdir(outdir)), outdir))
+
+
+def compare(a, b):
+    fa, fb = sorted(os.listdir(a)), sorted(os.listdir(b))
+    bad = sorted(set(fa) ^ set(fb))
+    for f in sorted(set(fa) & set(fb)):
+        x, y = np.load(os.path.join(a, f)), np.load(os.path.join(b, f))
+        if x.dtype != y.dtype or x.shape != y.shape or x.tobytes() != y.tobytes():
+            bad.append(f)
+    for f in bad:
+        print("DIFFERS:", f)
+    print("%d arrays compared, %d differ" % (len(set(fa) | set(fb)), len(bad)))
+    return 1 if bad else 0
+
+
+if __name__ == "__main__":
+    if sys.argv[1] == "--compare":
+        sys.exit(compare(sys.argv[2], sys.argv[3]))
+    run(sys.argv[1])
