@@ -11,6 +11,7 @@ calls raise.  (The CPU oracle lives under ``oracle/`` and is test infrastructure
 """
 import ctypes as C
 import os
+import sys
 
 import numpy as np
 
@@ -49,6 +50,12 @@ class Result(C.Structure):
                 ("ms_total", C.c_double)]
 
 
+class DevicePlanes(C.Structure):
+    """b2k_device_planes: an image in the engine GPU's memory (component c of pixel (x, y) at
+    comp[c] + (y * row_pitch[c] + x * col_step[c]) * sample_bytes)."""
+    _fields_ = [("comp", C.c_void_p * 4), ("row_pitch", C.c_uint32 * 4), ("col_step", C.c_uint32 * 4), ("sample_bytes", C.c_uint32)]
+
+
 BLOCK_DTYPE = np.dtype([("tile", "<u4"), ("comp", "<u2"), ("resno", "u1"), ("band_index", "u1"), ("orient", "u1"),
                         ("kmax", "u1"), ("numbps", "u1"), ("numpasses", "u1"), ("precno", "<u4"), ("cblkno", "<u4"),
                         ("x0", "<u4"), ("y0", "<u4"), ("x1", "<u4"), ("y1", "<u4"), ("buf_x", "<u4"), ("buf_y", "<u4"),
@@ -59,7 +66,7 @@ assert BLOCK_DTYPE.itemsize == C.sizeof(Block), (BLOCK_DTYPE.itemsize, C.sizeof(
 # plugin_decompress (C++-ABI callback struct) is declared in csrc/plugin_decode_abi.h, not in the C header
 EXPORTS = ["minpf_post_load_plugin", "plugin_init", "plugin_get_debug_state", "gpup_encode_mem", "gpup_tile_free",
            "b2k_engine_create", "b2k_engine_destroy", "b2k_last_error", "b2k_host_alloc", "b2k_host_free",
-           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_enumerate",
+           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_enumerate",
            "b2k_result_to_gpup_tile", "b2k_job_create", "b2k_job_destroy", "b2k_job_upload", "b2k_job_forward",
            "b2k_job_t1_encode", "b2k_job_t1_decode", "b2k_job_t1_decode_blocks", "b2k_job_inverse", "b2k_job_roundtrip", "b2k_job_roundtrip_n", "b2k_job_roundtrip_pipelined_n", "b2k_job_download",
            "b2k_job_download_coeffs", "b2k_job_upload_coeffs", "b2k_job_fetch_result", "b2k_job_num_blocks",
@@ -99,6 +106,9 @@ def lib():
     L.b2k_decode.argtypes = [vp, C.POINTER(Coding), vp, u64, vp, u64, pp, C.POINTER(u32), u32, u32,
                              C.POINTER(C.c_double)]
     L.b2k_decode16.argtypes = L.b2k_decode.argtypes
+    L.b2k_encode_device.argtypes = [vp, C.POINTER(Coding), C.POINTER(DevicePlanes), u32, u32, vp, C.POINTER(C.POINTER(Result))]
+    L.b2k_decode_device.argtypes = [vp, C.POINTER(Coding), vp, u64, vp, u64, C.POINTER(DevicePlanes), C.POINTER(u32), u32, u32, vp,
+                                    C.POINTER(C.c_double)]
     L.b2k_enumerate.argtypes = [C.POINTER(Coding), u32, u32, vp, u64]
     L.b2k_enumerate.restype = C.c_int64
     L.b2k_result_to_gpup_tile.argtypes = [C.POINTER(Coding), C.POINTER(Result), u32]
@@ -179,6 +189,99 @@ def _plane_ptrs(planes):
     return arr, strides
 
 
+# ------------------------------------------------------------------------------------------------
+# images in device memory: anything with __cuda_array_interface__ (torch CUDA tensors, CuPy, ...)
+# ------------------------------------------------------------------------------------------------
+DEVICE_DTYPES = ("u1", "i1", "u2", "i2", "i4", "u4")
+
+
+def _cuda_array(a):
+    try:
+        iface = a.__cuda_array_interface__
+    except AttributeError:
+        raise TypeError("%s has no __cuda_array_interface__: a CUDA array is needed (e.g. a torch tensor on a GPU)"
+                        % type(a).__name__) from None
+    t = iface["typestr"]
+    if t[1:] not in DEVICE_DTYPES or (t[0] == ">" and t[2:] != "1"):
+        raise ValueError("dtype %r is not one of the sample containers %s (little-endian)" % (t, ", ".join(DEVICE_DTYPES)))
+    size = int(t[2:])
+    shape = tuple(int(n) for n in iface["shape"])
+    strides = iface.get("strides")
+    if strides is None:  # C-contiguous
+        strides, acc = [], size
+        for n in reversed(shape):
+            strides.insert(0, acc)
+            acc *= n
+    for s in strides:
+        if s < 0:
+            raise ValueError("negative strides %s are not supported" % (tuple(strides),))
+        if s % size:
+            raise ValueError("strides %s (bytes) are not whole %d-byte samples" % (tuple(strides), size))
+    ptr, readonly = iface["data"]
+    return dict(ptr=int(ptr or 0), shape=shape, steps=[s // size for s in strides], size=size, typestr=t[1:], readonly=bool(readonly))
+
+
+def device_planes(image, numcomps, height, width, layout="CHW", writable=False):
+    """b2k_device_planes for `image`: one array of shape (C, H, W) (layout "CHW") or (H, W, C) ("HWC"), an (H, W) array
+    for one component, or a list of C arrays of shape (H, W).  Pointers, row pitches and column steps come from the
+    arrays' __cuda_array_interface__ strides, so padded rows, slices of larger tensors and views such as t[..., :3] of
+    an RGBA tensor need no copy.  Raises on a shape that is not (numcomps, height, width), a dtype that is not a
+    sample container, or strides that are negative or not whole samples.  Returns the DevicePlanes."""
+    if layout not in ("CHW", "HWC"):
+        raise ValueError("layout must be 'CHW' or 'HWC', not %r" % (layout,))
+    arrays = list(image) if isinstance(image, (list, tuple)) else [image]
+    descs = [_cuda_array(a) for a in arrays]
+    if len({d["typestr"] for d in descs}) != 1:
+        raise ValueError("the components have different dtypes: %s" % [d["typestr"] for d in descs])
+    if writable and any(d["readonly"] for d in descs):
+        raise ValueError("the image is read-only")
+    if numcomps > 4:
+        raise ValueError("a device image holds at most 4 components, not %d" % numcomps)
+    img = DevicePlanes()
+    img.sample_bytes = descs[0]["size"]
+    comps = []  # (address, row pitch, column step) per component, in samples
+    if isinstance(image, (list, tuple)) or len(descs[0]["shape"]) == 2:
+        want = [(height, width)] * numcomps
+        got = [d["shape"] for d in descs]
+        if got != want:
+            raise ValueError("shape %s does not match the image: %d component(s) of %s"
+                             % (got if len(got) > 1 else got[0], numcomps, (height, width)))
+        comps = [(d["ptr"], d["steps"][0], d["steps"][1]) for d in descs]
+    else:
+        d = descs[0]
+        want = (numcomps, height, width) if layout == "CHW" else (height, width, numcomps)
+        if d["shape"] != want:
+            raise ValueError("shape %s does not match the image: %s for layout %s" % (d["shape"], want, layout))
+        cstep, rstep, xstep = (d["steps"][0], d["steps"][1], d["steps"][2]) if layout == "CHW" else \
+            (d["steps"][2], d["steps"][0], d["steps"][1])
+        comps = [(d["ptr"] + c * cstep * d["size"], rstep, xstep) for c in range(numcomps)]
+    for c, (ptr, pitch, step) in enumerate(comps):
+        if pitch >= 1 << 32 or step >= 1 << 32:
+            raise ValueError("component %d: row pitch %d / column step %d samples do not fit 32 bits" % (c, pitch, step))
+        img.comp[c], img.row_pitch[c], img.col_step[c] = ptr, pitch, step
+    return img
+
+
+def _stream_handle(stream, image):
+    """cudaStream_t for `stream`: None = torch's current stream of a torch tensor's device, else the legacy default stream
+    (as the CUDA Array Interface assumes); an int handle; or anything with .cuda_stream (torch / CuPy streams)."""
+    if stream is None:
+        torch = sys.modules.get("torch")
+        first = image[0] if isinstance(image, (list, tuple)) else image
+        if torch is not None and isinstance(first, torch.Tensor) and first.is_cuda:
+            return torch.cuda.current_stream(first.device).cuda_stream or None
+        return None
+    if isinstance(stream, int):
+        return stream or None
+    return int(stream.cuda_stream) or None
+
+
+def _check_handled(rc, what):
+    if rc == 1:
+        raise NotHandled("%s -> 1: %s" % (what, (lib().b2k_last_error() or b"").decode()))
+    _check(rc, what)
+
+
 def set_host_threads(n):
     """Host threads that narrow/widen int32 planes to 16-bit PCIe containers (0 = off, <0 = default)."""
     return int(lib().b2k_set_host_threads(int(n)))
@@ -221,6 +324,31 @@ def codestream_write(cp, blocks, data, flags=CS_TLM | CS_PLT, num_tiles=None, ou
     n2 = lib().b2k_codestream_write(C.byref(cp), C.byref(r), flags, out.ctypes.data, n)
     assert n2 == n
     return out
+
+
+def codestream_parse_window(cs, window=None, reduce=0):
+    """b2k_codestream_parse_window -> (virtual Coding, block table, rect): rect = (x0, y0, x1, y1) of the window's pixels
+    at 1 / 2**reduce resolution on the virtual coding's canvas (the whole virtual image when window is None)."""
+    cs = np.ascontiguousarray(cs, dtype=np.uint8)
+    L = lib()
+    L.b2k_codestream_parse_window.restype = C.c_int64
+    L.b2k_codestream_parse_window.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(Coding), C.c_void_p, C.c_uint64]
+    win = (C.c_uint32 * 4)(*window) if window is not None else None
+    cp = Coding()
+    n = L.b2k_codestream_parse_window(cs.ctypes.data, len(cs), win, reduce, C.byref(cp), None, 0)
+    if n <= 1:
+        raise EngineError("b2k_codestream_parse_window: %d %s" % (n, (L.b2k_last_error() or b"").decode()))
+    blocks = np.zeros(n, BLOCK_DTYPE)
+    m = L.b2k_codestream_parse_window(cs.ctypes.data, len(cs), win, reduce, C.byref(cp), blocks.ctypes.data, n)
+    if m != n:
+        raise EngineError("b2k_codestream_parse_window: %d %s" % (m, (L.b2k_last_error() or b"").decode()))
+    if window is None:
+        rect = (cp.x0, cp.y0, cp.x1, cp.y1)
+    else:
+        sh = (1 << reduce) - 1
+        x0, y0, x1, y1 = [(v + sh) >> reduce for v in window]
+        rect = (max(x0, cp.x0), max(y0, cp.y0), min(x1, cp.x1), min(y1, cp.y1))
+    return cp, blocks, rect
 
 
 def codestream_parse(cs):
@@ -380,6 +508,7 @@ class Engine:
 
     def __init__(self, device=0):
         self._h = C.c_void_p()
+        self.device = device
         _check(lib().b2k_engine_create(device, C.byref(self._h)), "b2k_engine_create")
 
     def close(self):
@@ -429,23 +558,8 @@ class Engine:
         reuses for later windows of the same tile-box shape: copy them to keep them."""
         cs = np.ascontiguousarray(cs, dtype=np.uint8)
         L = lib()
-        L.b2k_codestream_parse_window.restype = C.c_int64
-        L.b2k_codestream_parse_window.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(Coding), C.c_void_p, C.c_uint64]
-        win = (C.c_uint32 * 4)(*window) if window is not None else None
-        cp = Coding()
-        n = L.b2k_codestream_parse_window(cs.ctypes.data, len(cs), win, reduce, C.byref(cp), None, 0)
-        if n <= 1:
-            raise EngineError("b2k_codestream_parse_window: %d %s" % (n, (L.b2k_last_error() or b"").decode()))
-        blocks = np.zeros(n, BLOCK_DTYPE)
-        m = L.b2k_codestream_parse_window(cs.ctypes.data, len(cs), win, reduce, C.byref(cp), blocks.ctypes.data, n)
-        if m != n:
-            raise EngineError("b2k_codestream_parse_window: %d %s" % (m, (L.b2k_last_error() or b"").decode()))
-        if window is None:
-            rect = (cp.x0, cp.y0, cp.x1, cp.y1)
-        else:
-            sh = (1 << reduce) - 1
-            x0, y0, x1, y1 = [(v + sh) >> reduce for v in window]
-            rect = (max(x0, cp.x0), max(y0, cp.y0), min(x1, cp.x1), min(y1, cp.y1))
+        cp, blocks, rect = codestream_parse_window(cs, window, reduce)
+        n = len(blocks)
         # pinned landing planes of the WINDOW's size, kept per shape: only the window's pixels come back over PCIe
         cache = self.__dict__.setdefault("_win_planes", {})
         key = (rect[3] - rect[1], rect[2] - rect[0], cp.numcomps, np.dtype(dtype).str)
@@ -472,6 +586,61 @@ class Engine:
         _check(getattr(lib(), fn)(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), data.ctypes.data, len(data),
                                   ptrs, strides, tile_mod, tile_rem, C.byref(ms)), fn)
         return ms.value
+
+    # ---- images in device memory (b2k_encode_device / b2k_decode_device) ----
+    def encode_device(self, cp, image, layout="CHW", stream=None, tile_mod=1, tile_rem=0):
+        """Encode an image that is already on the engine's GPU: any object (or list of per-component objects) with
+        __cuda_array_interface__ -- see device_planes() for the shapes.  Samples are read where they are, ordered after
+        the work queued on `stream` (None: torch's current stream for a torch tensor, else the legacy default stream);
+        the result equals encode() of the same samples."""
+        img = device_planes(image, cp.numcomps, cp.y1 - cp.y0, cp.x1 - cp.x0, layout)
+        out = C.POINTER(Result)()
+        _check_handled(lib().b2k_encode_device(self._h, C.byref(cp), C.byref(img), tile_mod, tile_rem, _stream_handle(stream, image),
+                                               C.byref(out)), "b2k_encode_device")
+        return EncodeResult(out)
+
+    def decode_device(self, cp, blocks, data, out, layout="CHW", window=None, stream=None, tile_mod=1, tile_rem=0):
+        """Decode into `out` on the engine's GPU (shapes as for encode_device; a window (x0, y0, x1, y1) in cp's canvas
+        coordinates makes `out` the window's pixels).  The block table and coded bytes stay in host memory.  Work queued
+        on `stream` after the call sees the pixels.  Returns the device ms of the call."""
+        if window is None:
+            h, w = cp.y1 - cp.y0, cp.x1 - cp.x0
+        else:
+            h, w = window[3] - window[1], window[2] - window[0]
+        img = device_planes(out, cp.numcomps, h, w, layout, writable=True)
+        blocks = np.ascontiguousarray(blocks, dtype=BLOCK_DTYPE)
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        win = (C.c_uint32 * 4)(*window) if window is not None else None
+        ms = C.c_double()
+        _check_handled(lib().b2k_decode_device(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), data.ctypes.data, len(data),
+                                               C.byref(img), win, tile_mod, tile_rem, _stream_handle(stream, out), C.byref(ms)),
+                       "b2k_decode_device")
+        return ms.value
+
+    def encode_codestream_device(self, cp, image, flags=CS_TLM | CS_PLT, layout="CHW", stream=None):
+        """An image on the GPU -> a complete HTJ2K codestream (numpy uint8): b2k_encode_device + b2k_codestream_write."""
+        res = self.encode_device(cp, image, layout=layout, stream=stream)
+        try:
+            return codestream_write(cp, res.blocks, res.bytes, flags, num_tiles=res.num_tiles)
+        finally:
+            res.free()
+
+    def decode_codestream_device(self, cs, out=None, dtype=None, layout="CHW", window=None, reduce=0, stream=None):
+        """HTJ2K codestream -> (Coding, image on the GPU).  window (x0, y0, x1, y1 on the full-resolution canvas) and
+        reduce work as in decode_window (the Coding is then the virtual one).  out: a CUDA array of the (window's) shape
+        in `layout`, or None for a new torch tensor of `dtype` (default torch.uint16) on the engine's GPU."""
+        cs = np.ascontiguousarray(cs, dtype=np.uint8)
+        if window is not None or reduce:
+            cp, blocks, rect = codestream_parse_window(cs, window, reduce)
+        else:
+            (cp, blocks), rect = codestream_parse(cs), None
+        x0, y0, x1, y1 = rect if rect is not None else (cp.x0, cp.y0, cp.x1, cp.y1)
+        if out is None:
+            import torch
+            shape = (cp.numcomps, y1 - y0, x1 - x0) if layout == "CHW" else (y1 - y0, x1 - x0, cp.numcomps)
+            out = torch.empty(shape, dtype=torch.uint16 if dtype is None else dtype, device="cuda:%d" % self.device)
+        self.decode_device(cp, blocks, cs, out, layout=layout, window=rect, stream=stream)
+        return cp, out
 
     def job(self, cp, tile_mod=1, tile_rem=0):
         return Job(self, cp, tile_mod, tile_rem)

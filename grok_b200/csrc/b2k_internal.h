@@ -105,6 +105,13 @@ void b2k_launch_ht_decode_magsgn(const HtBlockDesc* d_blocks, const uint8_t* d_b
                                  int any_refinement, cudaStream_t st);
 void b2k_launch_build_dec_desc(const HtBlockDesc* d_enc, const HtBlockOut* d_out, const uint64_t* d_offsets,
                                const float* d_dec_quant, HtBlockDesc* d_dec, uint32_t n, cudaStream_t st);
+/* sample containers (sample_bytes 1, 2 or 4) <-> int32 planes.  Component c of pixel (x, y) of the container is at
+   base + y * pitch + x * step + c samples; the nc components go to / come from dst[c] / src[c] + y * plane pitch + x */
+void b2k_launch_container_to_planes(const void* src, uint32_t spitch, uint32_t step, uint32_t sample_bytes, int32_t* const* dst, int nc,
+                                    uint32_t dpitch, uint32_t w, uint32_t h, int sgnd, cudaStream_t st);
+void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t spitch, void* dst, uint32_t dpitch, uint32_t step,
+                                    uint32_t sample_bytes, uint32_t w, uint32_t h, cudaStream_t st);
+/* the 16-bit instances of the two */
 void b2k_launch_widen16_interleaved(const uint16_t* src, uint32_t spitch, int32_t* const* dst, int nc, uint32_t dpitch, uint32_t w,
                                     uint32_t h, int sgnd, cudaStream_t st);
 void b2k_launch_widen16(const uint16_t* src, uint32_t spitch, int32_t* dst, uint32_t dpitch, uint32_t w, uint32_t h, int sgnd,

@@ -1502,140 +1502,260 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_inv(const DwtL
   pipe.drain();
 }
 
-/* 16-bit sample containers <-> the engine's 32-bit planes: one rectangle (a merged tile row) per
-   launch, 8 samples per thread, 128-bit accesses.  Costs 6 B/sample of HBM traffic -- noise next to
-   the PCIe transfer it halves. */
-__global__ void k_widen16(const uint16_t* __restrict__ src, uint32_t spitch, int32_t* __restrict__ dst, uint32_t dpitch,
-                          uint32_t w, uint32_t h, int sgnd)
+/* ---- sample containers <-> the engine's 32-bit planes ----------------------------------------------------------------
+   A container holds S-byte samples (S = 1, 2 or 4); component c of pixel (x, y) is at  base + y * pitch + x * step + c
+   samples.  Planar containers (step 1) take one launch per component; NC components that sit side by side in every pixel
+   take one launch together (step == NC: RGB / RGBA rows; step > NC: e.g. the RGB of an RGBA buffer).  One rectangle (a
+   merged tile row) per launch, 8 pixels per thread.  When the thread's 8 pixels are whole, step == NC and the addresses
+   are aligned, the container side moves as one group of 8 * NC * S bytes in 128-bit accesses (64-bit ones when the group
+   is not a multiple of 16 bytes: 8-bit samples with NC odd) and every plane as two 128-bit accesses; anything else goes
+   sample by sample.  HBM traffic is S + 4 bytes per sample, which bounds these kernels.
+   Widening sign-extends from the container width when the samples are signed; narrowing truncates (the inverse
+   transforms have already clamped to the precision). */
+template <int S> struct Sample;
+template <> struct Sample<1> { typedef uint8_t U; typedef int8_t I; };
+template <> struct Sample<2> { typedef uint16_t U; typedef int16_t I; };
+template <> struct Sample<4> { typedef uint32_t U; typedef int32_t I; };
+
+template <int S>
+__device__ __forceinline__ int widen_sample(uint32_t u, int sgnd)
 {
-  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8, y = blockIdx.y;
-  if(x8 >= w || y >= h)
-    return;
-  const uint16_t* s = src + (size_t)y * spitch + x8;
-  int32_t* d = dst + (size_t)y * dpitch + x8;
-  if(x8 + 8 <= w && ((reinterpret_cast<uintptr_t>(s) & 15) == 0) && ((reinterpret_cast<uintptr_t>(d) & 15) == 0))
+  if constexpr(S == 4)
+    return (int)u;
+  else
   {
-    const uint4 a = __ldg(reinterpret_cast<const uint4*>(s));
-    int v[8] = {(int)(a.x & 0xFFFF), (int)(a.x >> 16), (int)(a.y & 0xFFFF), (int)(a.y >> 16),
-                (int)(a.z & 0xFFFF), (int)(a.z >> 16), (int)(a.w & 0xFFFF), (int)(a.w >> 16)};
-    if(sgnd)
-    {
+    u &= (1u << (8 * S)) - 1;
+    return sgnd ? (int)(typename Sample<S>::I)u : (int)u;
+  }
+}
+
+/* a group of BYTES bytes (a multiple of 8) as 32-bit words, in 128-bit pieces when BYTES allows, else 64-bit ones */
+template <int BYTES>
+__device__ __forceinline__ void load_group(const void* p, uint32_t (&wd)[BYTES / 4])
+{
+  if constexpr(BYTES % 16 == 0)
+  {
 #pragma unroll
-      for(int i = 0; i < 8; ++i)
-        v[i] = (int)(int16_t)v[i];
+    for(int i = 0; i < BYTES / 16; ++i)
+    {
+      const uint4 a = __ldg(reinterpret_cast<const uint4*>(p) + i);
+      wd[4 * i] = a.x; wd[4 * i + 1] = a.y; wd[4 * i + 2] = a.z; wd[4 * i + 3] = a.w;
     }
-    reinterpret_cast<int4*>(d)[0] = make_int4(v[0], v[1], v[2], v[3]);
-    reinterpret_cast<int4*>(d)[1] = make_int4(v[4], v[5], v[6], v[7]);
   }
   else
-    for(uint32_t i = 0; i < 8 && x8 + i < w; ++i)
-      d[i] = sgnd ? (int)(int16_t)s[i] : (int)s[i];
+  {
+#pragma unroll
+    for(int i = 0; i < BYTES / 8; ++i)
+    {
+      const uint2 a = __ldg(reinterpret_cast<const uint2*>(p) + i);
+      wd[2 * i] = a.x; wd[2 * i + 1] = a.y;
+    }
+  }
 }
+template <int BYTES>
+__device__ __forceinline__ void store_group(void* p, const uint32_t (&wd)[BYTES / 4])
+{
+  if constexpr(BYTES % 16 == 0)
+  {
+#pragma unroll
+    for(int i = 0; i < BYTES / 16; ++i)
+      reinterpret_cast<uint4*>(p)[i] = make_uint4(wd[4 * i], wd[4 * i + 1], wd[4 * i + 2], wd[4 * i + 3]);
+  }
+  else
+  {
+#pragma unroll
+    for(int i = 0; i < BYTES / 8; ++i)
+      reinterpret_cast<uint2*>(p)[i] = make_uint2(wd[2 * i], wd[2 * i + 1]);
+  }
+}
+
 struct Ptr4
 {
   int32_t* p[4];
 };
-/* pixel-interleaved 16-bit samples (RGB48LE rows, the packed frames of gpup_batch_memory_submit: grok.cpp L1806-1836)
-   -> NC int32 planes.  A thread takes 8 pixels: NC 128-bit loads, 2*NC 128-bit stores. */
-template <int NC>
-__global__ void k_widen16_interleaved(const uint16_t* __restrict__ src, uint32_t spitch, Ptr4 dst, uint32_t dpitch, uint32_t w,
-                                      uint32_t h, int sgnd)
+struct CPtr4
 {
-  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8, y = blockIdx.y;
-  if(x8 >= w || y >= h)
+  const int32_t* p[4];
+};
+
+/* container -> NC int32 planes (b2k_encode16 / b2k_encode16_interleaved after the upload, b2k_encode_device) */
+template <int S, int NC>
+__global__ void __launch_bounds__(128) k_container_to_planes(const void* __restrict__ src, uint32_t spitch, uint32_t step, Ptr4 dst,
+                                                             uint32_t dpitch, uint32_t w, uint32_t h, int sgnd)
+{
+  typedef typename Sample<S>::U U;
+  constexpr int BYTES = 8 * NC * S, V = BYTES % 16 == 0 ? 16 : 8;
+  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  if(x8 >= w)
     return;
-  const uint16_t* s = src + (size_t)y * spitch + (size_t)x8 * NC;
-  const size_t doff = (size_t)y * dpitch + x8;
-  if(x8 + 8 <= w && ((reinterpret_cast<uintptr_t>(s) & 15) == 0) && ((doff & 3) == 0))
+  for(uint32_t y = blockIdx.y; y < h; y += gridDim.y)
   {
-    uint32_t wd[4 * NC];
-#pragma unroll
-    for(int i = 0; i < NC; ++i)
-    {
-      const uint4 a = __ldg(reinterpret_cast<const uint4*>(s) + i);
-      wd[4 * i] = a.x; wd[4 * i + 1] = a.y; wd[4 * i + 2] = a.z; wd[4 * i + 3] = a.w;
-    }
+    const U* s = static_cast<const U*>(src) + (size_t)y * spitch + (size_t)x8 * step;
+    const size_t doff = (size_t)y * dpitch + x8;
+    bool vec = x8 + 8 <= w && step == NC && (reinterpret_cast<uintptr_t>(s) & (V - 1)) == 0;
 #pragma unroll
     for(int c = 0; c < NC; ++c)
+      vec = vec && (reinterpret_cast<uintptr_t>(dst.p[c] + doff) & 15) == 0;
+    if(vec)
     {
-      int v[8];
-#pragma unroll
-      for(int i = 0; i < 8; ++i)
-      {
-        const int e = i * NC + c; /* 16-bit element index within the 8-pixel group */
-        const uint32_t u = (wd[e >> 1] >> ((e & 1) * 16)) & 0xFFFF;
-        v[i] = sgnd ? (int)(int16_t)u : (int)u;
-      }
-      int4* d = reinterpret_cast<int4*>(dst.p[c] + doff);
-      d[0] = make_int4(v[0], v[1], v[2], v[3]);
-      d[1] = make_int4(v[4], v[5], v[6], v[7]);
-    }
-  }
-  else
-    for(uint32_t i = 0; i < 8 && x8 + i < w; ++i)
+      uint32_t wd[BYTES / 4];
+      load_group<BYTES>(s, wd);
 #pragma unroll
       for(int c = 0; c < NC; ++c)
       {
-        const uint16_t u = s[i * NC + c];
-        dst.p[c][doff + i] = sgnd ? (int)(int16_t)u : (int)u;
+        int v[8];
+#pragma unroll
+        for(int i = 0; i < 8; ++i)
+        {
+          const int e = (i * NC + c) * S; /* byte of the sample within the group */
+          v[i] = widen_sample<S>(wd[e >> 2] >> ((e & 3) * 8), sgnd);
+        }
+        int4* d = reinterpret_cast<int4*>(dst.p[c] + doff);
+        d[0] = make_int4(v[0], v[1], v[2], v[3]);
+        d[1] = make_int4(v[4], v[5], v[6], v[7]);
       }
-}
-__global__ void k_narrow16(const int32_t* __restrict__ src, uint32_t spitch, uint16_t* __restrict__ dst, uint32_t dpitch,
-                           uint32_t w, uint32_t h)
-{
-  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8, y = blockIdx.y;
-  if(x8 >= w || y >= h)
-    return;
-  const int32_t* s = src + (size_t)y * spitch + x8;
-  uint16_t* d = dst + (size_t)y * dpitch + x8;
-  if(x8 + 8 <= w && ((reinterpret_cast<uintptr_t>(s) & 15) == 0) && ((reinterpret_cast<uintptr_t>(d) & 15) == 0))
-  {
-    const int4 a = __ldg(reinterpret_cast<const int4*>(s)), b = __ldg(reinterpret_cast<const int4*>(s) + 1);
-    *reinterpret_cast<uint4*>(d) = make_uint4((a.x & 0xFFFF) | (a.y << 16), (a.z & 0xFFFF) | (a.w << 16),
-                                              (b.x & 0xFFFF) | (b.y << 16), (b.z & 0xFFFF) | (b.w << 16));
+    }
+    else
+    { /* a row's last pixels, or an unaligned / strided container */
+      const uint32_t n = w - x8 < 8 ? w - x8 : 8;
+#pragma unroll 1
+      for(uint32_t i = 0; i < n; ++i)
+#pragma unroll
+        for(int c = 0; c < NC; ++c)
+          dst.p[c][doff + i] = widen_sample<S>(s[(size_t)i * step + c], sgnd);
+    }
   }
-  else
-    for(uint32_t i = 0; i < 8 && x8 + i < w; ++i)
-      d[i] = (uint16_t)s[i];
+}
+
+/* NC int32 planes -> container (b2k_decode16 before the download, b2k_decode_device) */
+template <int S, int NC>
+__global__ void __launch_bounds__(128) k_planes_to_container(CPtr4 src, uint32_t spitch, void* __restrict__ dst, uint32_t dpitch,
+                                                             uint32_t step, uint32_t w, uint32_t h)
+{
+  typedef typename Sample<S>::U U;
+  constexpr int BYTES = 8 * NC * S, V = BYTES % 16 == 0 ? 16 : 8;
+  constexpr uint32_t MASK = S == 4 ? 0xFFFFFFFFu : (1u << (8 * S)) - 1;
+  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  if(x8 >= w)
+    return;
+  for(uint32_t y = blockIdx.y; y < h; y += gridDim.y)
+  {
+    const size_t soff = (size_t)y * spitch + x8;
+    U* d = static_cast<U*>(dst) + (size_t)y * dpitch + (size_t)x8 * step;
+    bool vec = x8 + 8 <= w && step == NC && (reinterpret_cast<uintptr_t>(d) & (V - 1)) == 0;
+#pragma unroll
+    for(int c = 0; c < NC; ++c)
+      vec = vec && (reinterpret_cast<uintptr_t>(src.p[c] + soff) & 15) == 0;
+    if(vec)
+    {
+      uint32_t wd[BYTES / 4];
+#pragma unroll
+      for(int k = 0; k < BYTES / 4; ++k)
+        wd[k] = 0;
+#pragma unroll
+      for(int c = 0; c < NC; ++c)
+      {
+        const int4 a = __ldg(reinterpret_cast<const int4*>(src.p[c] + soff)), b = __ldg(reinterpret_cast<const int4*>(src.p[c] + soff) + 1);
+        const int v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+        for(int i = 0; i < 8; ++i)
+        {
+          const int e = (i * NC + c) * S;
+          wd[e >> 2] |= ((uint32_t)v[i] & MASK) << ((e & 3) * 8);
+        }
+      }
+      store_group<BYTES>(d, wd);
+    }
+    else
+    { /* a row's last pixels, or an unaligned / strided container */
+      const uint32_t n = w - x8 < 8 ? w - x8 : 8;
+#pragma unroll 1
+      for(uint32_t i = 0; i < n; ++i)
+#pragma unroll
+        for(int c = 0; c < NC; ++c)
+          d[(size_t)i * step + c] = (U)src.p[c][soff + i];
+    }
+  }
+}
+
+dim3 convert_grid(uint32_t w, uint32_t h) { return dim3((w + 8 * 128 - 1) / (8 * 128), h < 65535u ? h : 65535u); }
+
+template <int S>
+void launch_container_to_planes(const void* src, uint32_t spitch, uint32_t step, const Ptr4& P, int nc, uint32_t dpitch, uint32_t w,
+                                uint32_t h, int sgnd, cudaStream_t st)
+{
+  const dim3 grid = convert_grid(w, h), block(128);
+  switch(nc)
+  {
+    case 1: k_container_to_planes<S, 1><<<grid, block, 0, st>>>(src, spitch, step, P, dpitch, w, h, sgnd); break;
+    case 2: k_container_to_planes<S, 2><<<grid, block, 0, st>>>(src, spitch, step, P, dpitch, w, h, sgnd); break;
+    case 3: k_container_to_planes<S, 3><<<grid, block, 0, st>>>(src, spitch, step, P, dpitch, w, h, sgnd); break;
+    default: k_container_to_planes<S, 4><<<grid, block, 0, st>>>(src, spitch, step, P, dpitch, w, h, sgnd); break;
+  }
+}
+template <int S>
+void launch_planes_to_container(const CPtr4& P, int nc, uint32_t spitch, void* dst, uint32_t dpitch, uint32_t step, uint32_t w,
+                                uint32_t h, cudaStream_t st)
+{
+  const dim3 grid = convert_grid(w, h), block(128);
+  switch(nc)
+  {
+    case 1: k_planes_to_container<S, 1><<<grid, block, 0, st>>>(P, spitch, dst, dpitch, step, w, h); break;
+    case 2: k_planes_to_container<S, 2><<<grid, block, 0, st>>>(P, spitch, dst, dpitch, step, w, h); break;
+    case 3: k_planes_to_container<S, 3><<<grid, block, 0, st>>>(P, spitch, dst, dpitch, step, w, h); break;
+    default: k_planes_to_container<S, 4><<<grid, block, 0, st>>>(P, spitch, dst, dpitch, step, w, h); break;
+  }
 }
 
 } /* namespace */
 
-void b2k_launch_widen16(const uint16_t* src, uint32_t spitch, int32_t* dst, uint32_t dpitch, uint32_t w, uint32_t h, int sgnd,
-                        cudaStream_t st)
-{
-  if(!w || !h)
-    return;
-  dim3 grid((w + 8 * 128 - 1) / (8 * 128), h), block(128);
-  k_widen16<<<grid, block, 0, st>>>(src, spitch, dst, dpitch, w, h, sgnd);
-  b2k_count_launch();
-}
-void b2k_launch_widen16_interleaved(const uint16_t* src, uint32_t spitch, int32_t* const* dst, int nc, uint32_t dpitch, uint32_t w,
-                                    uint32_t h, int sgnd, cudaStream_t st)
+void b2k_launch_container_to_planes(const void* src, uint32_t spitch, uint32_t step, uint32_t sample_bytes, int32_t* const* dst, int nc,
+                                    uint32_t dpitch, uint32_t w, uint32_t h, int sgnd, cudaStream_t st)
 {
   if(!w || !h)
     return;
   Ptr4 P{};
   for(int c = 0; c < nc && c < 4; ++c)
     P.p[c] = dst[c];
-  dim3 grid((w + 8 * 128 - 1) / (8 * 128), h), block(128);
-  switch(nc)
+  switch(sample_bytes)
   {
-    case 1: k_widen16_interleaved<1><<<grid, block, 0, st>>>(src, spitch, P, dpitch, w, h, sgnd); break;
-    case 2: k_widen16_interleaved<2><<<grid, block, 0, st>>>(src, spitch, P, dpitch, w, h, sgnd); break;
-    case 3: k_widen16_interleaved<3><<<grid, block, 0, st>>>(src, spitch, P, dpitch, w, h, sgnd); break;
-    default: k_widen16_interleaved<4><<<grid, block, 0, st>>>(src, spitch, P, dpitch, w, h, sgnd); break;
+    case 1: launch_container_to_planes<1>(src, spitch, step, P, nc, dpitch, w, h, sgnd, st); break;
+    case 2: launch_container_to_planes<2>(src, spitch, step, P, nc, dpitch, w, h, sgnd, st); break;
+    default: launch_container_to_planes<4>(src, spitch, step, P, nc, dpitch, w, h, sgnd, st); break;
   }
   b2k_count_launch();
+}
+void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t spitch, void* dst, uint32_t dpitch, uint32_t step,
+                                    uint32_t sample_bytes, uint32_t w, uint32_t h, cudaStream_t st)
+{
+  if(!w || !h)
+    return;
+  CPtr4 P{};
+  for(int c = 0; c < nc && c < 4; ++c)
+    P.p[c] = src[c];
+  switch(sample_bytes)
+  {
+    case 1: launch_planes_to_container<1>(P, nc, spitch, dst, dpitch, step, w, h, st); break;
+    case 2: launch_planes_to_container<2>(P, nc, spitch, dst, dpitch, step, w, h, st); break;
+    default: launch_planes_to_container<4>(P, nc, spitch, dst, dpitch, step, w, h, st); break;
+  }
+  b2k_count_launch();
+}
+/* the 16-bit containers of b2k_encode16 / b2k_decode16 / b2k_encode16_interleaved */
+void b2k_launch_widen16(const uint16_t* src, uint32_t spitch, int32_t* dst, uint32_t dpitch, uint32_t w, uint32_t h, int sgnd,
+                        cudaStream_t st)
+{
+  b2k_launch_container_to_planes(src, spitch, 1, 2, &dst, 1, dpitch, w, h, sgnd, st);
+}
+void b2k_launch_widen16_interleaved(const uint16_t* src, uint32_t spitch, int32_t* const* dst, int nc, uint32_t dpitch, uint32_t w,
+                                    uint32_t h, int sgnd, cudaStream_t st)
+{
+  b2k_launch_container_to_planes(src, spitch, (uint32_t)nc, 2, dst, nc, dpitch, w, h, sgnd, st);
 }
 void b2k_launch_narrow16(const int32_t* src, uint32_t spitch, uint16_t* dst, uint32_t dpitch, uint32_t w, uint32_t h,
                          cudaStream_t st)
 {
-  if(!w || !h)
-    return;
-  dim3 grid((w + 8 * 128 - 1) / (8 * 128), h), block(128);
-  k_narrow16<<<grid, block, 0, st>>>(src, spitch, dst, dpitch, w, h);
-  b2k_count_launch();
+  b2k_launch_planes_to_container(&src, 1, spitch, dst, dpitch, 1, 2, w, h, st);
 }
 
 /* one launch of a DWT kernel whose warps stage through WarpPipe<Stage>; the shared-memory limit it needs is raised once

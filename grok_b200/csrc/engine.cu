@@ -61,6 +61,7 @@ struct b2k_engine
      belong to the engine: calls on one engine are serialised, engines (one per GPU) run side by side */
   std::mutex mu;
   b2k_device_job* cached = nullptr;
+  cudaEvent_t caller_ev = nullptr; /* b2k_encode_device / b2k_decode_device: orders the engine's streams after the caller's */
 };
 
 /* ---- device memory cache --------------------------------------------------------------------------------------
@@ -422,6 +423,7 @@ extern "C" int32_t b2k_engine_create(int32_t device, b2k_engine** out)
   CUDA_TRY(cudaStreamCreateWithFlags(&eng->h2d_stream, cudaStreamNonBlocking));
   for(cudaStream_t& a : eng->aux)
     CUDA_TRY(cudaStreamCreateWithFlags(&a, cudaStreamNonBlocking));
+  CUDA_TRY(cudaEventCreateWithFlags(&eng->caller_ev, cudaEventDisableTiming));
   *out = eng;
   return 0;
 }
@@ -445,6 +447,8 @@ extern "C" void b2k_engine_destroy(b2k_engine* e)
   for(cudaStream_t a : e->aux)
     if(a)
       cudaStreamDestroy(a);
+  if(e->caller_ev)
+    cudaEventDestroy(e->caller_ev);
   delete e;
 }
 
@@ -884,10 +888,14 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
 
 extern "C" uint64_t b2k_job_num_blocks(const b2k_device_job* J) { return J ? J->blocks.size() : 0; }
 
-/* ---- host <-> device plane copies, per selected tile ---------------------------------------- */
+/* ---- copies between the caller's int32 planes and the engine's, per selected tile -------------
+   to_device: into the engine's planes.  user_on_device: the caller's planes are device memory too (b2k_encode_device /
+   b2k_decode_device), so the copy stays on the device */
 static int copy_planes(b2k_device_job* J, const Planes& P, void* const* host, const uint32_t* strides, bool to_device,
-                       cudaStream_t st, size_t t0 = 0, size_t t1 = (size_t)-1)
+                       cudaStream_t st, size_t t0 = 0, size_t t1 = (size_t)-1, bool user_on_device = false)
 {
+  const cudaMemcpyKind in = user_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  const cudaMemcpyKind out = user_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   const b2k_coding& cp = J->cp;
   t1 = std::min(t1, J->tiles.size());
   for(size_t ti = t0; ti < t1;)
@@ -917,11 +925,9 @@ static int copy_planes(b2k_device_job* J, const Planes& P, void* const* host, co
       int32_t* dev = P.at(c, r.x0, r.y0);
       int32_t* hst = reinterpret_cast<int32_t*>(host[c]) + (size_t)(r.y0 - oy) * strides[c] + (r.x0 - ox);
       if(to_device)
-        CUDA_TRY(cudaMemcpy2DAsync(dev, (size_t)P.pitch * 4, hst, (size_t)strides[c] * 4, (size_t)r.w() * 4, r.h(),
-                                   cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpy2DAsync(dev, (size_t)P.pitch * 4, hst, (size_t)strides[c] * 4, (size_t)r.w() * 4, r.h(), in, st));
       else
-        CUDA_TRY(cudaMemcpy2DAsync(hst, (size_t)strides[c] * 4, dev, (size_t)P.pitch * 4, (size_t)r.w() * 4, r.h(),
-                                   cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpy2DAsync(hst, (size_t)strides[c] * 4, dev, (size_t)P.pitch * 4, (size_t)r.w() * 4, r.h(), out, st));
     }
     ti = tj;
   }
@@ -1116,6 +1122,109 @@ static int split_interleaved(b2k_device_job* J, cudaStream_t st, size_t t0, size
       dst[c] = J->img.at(c, r.x0, r.y0);
     b2k_launch_widen16_interleaved(J->d_ileave + (size_t)(r.y0 - cp.y0) * J->ileave_pitch + (size_t)(r.x0 - cp.x0) * cp.numcomps,
                                    J->ileave_pitch, dst, cp.numcomps, J->img.pitch, r.w(), r.h(), cp.sgnd, st);
+  });
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+/* ---- images the caller keeps in device memory (b2k_encode_device / b2k_decode_device) ------------------------------ */
+/* 0 usable, 1 not handled, -1 bad input; b2k_last_error says why */
+static int check_device_planes(const b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img)
+{
+  if(!img)
+  {
+    g_err = "no device image";
+    return -1;
+  }
+  if(img->sample_bytes != 1 && img->sample_bytes != 2 && img->sample_bytes != 4)
+  {
+    g_err = "sample_bytes must be 1, 2 or 4";
+    return -1;
+  }
+  if(cp->numcomps > 4)
+  {
+    g_err = "a device image holds at most 4 components";
+    return 1;
+  }
+  if(img->sample_bytes * 8 < cp->prec)
+  {
+    g_err = std::to_string(img->sample_bytes * 8) + "-bit containers cannot hold " + std::to_string(cp->prec) + "-bit samples";
+    return 1;
+  }
+  for(int c = 0; c < cp->numcomps; ++c)
+  {
+    const std::string comp = "device image component " + std::to_string(c) + ": ";
+    cudaPointerAttributes a{};
+    const cudaError_t err = img->comp[c] ? cudaPointerGetAttributes(&a, img->comp[c]) : cudaErrorInvalidValue;
+    if(err != cudaSuccess)
+      (void)cudaGetLastError();
+    if(err != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != e->device)
+    {
+      g_err = comp + "not device or managed memory of the engine's device (" + std::to_string(e->device) + ")";
+      return -1;
+    }
+    if(reinterpret_cast<uintptr_t>(img->comp[c]) % img->sample_bytes)
+    {
+      g_err = comp + "address not a multiple of sample_bytes";
+      return -1;
+    }
+    if(!img->col_step[c])
+    {
+      g_err = comp + "col_step is 0";
+      return -1;
+    }
+  }
+  return 0;
+}
+
+/* components one conversion launch covers: all of them when they are pixel-interleaved (comp[c] = comp[0] + c samples, one
+   pitch and one step), else one */
+static int device_group(const b2k_device_planes& img, int nc)
+{
+  const uint8_t* base = static_cast<const uint8_t*>(img.comp[0]);
+  for(int c = 1; c < nc; ++c)
+    if(static_cast<const uint8_t*>(img.comp[c]) != base + (size_t)c * img.sample_bytes || img.row_pitch[c] != img.row_pitch[0] ||
+       img.col_step[c] != img.col_step[0])
+      return 1;
+  return nc;
+}
+
+/* the caller's device image -> the engine's planes (to_planes) or back, selected tiles [t0, t1), on stream st.  On the way
+   back a windowed decode writes only the crop, which the image then holds */
+static int device_convert(b2k_device_job* J, const b2k_device_planes& img, bool to_planes, cudaStream_t st, size_t t0, size_t t1)
+{
+  const b2k_coding& cp = J->cp;
+  const int nc = cp.numcomps;
+  bool planar32 = img.sample_bytes == 4;
+  for(int c = 0; c < nc; ++c)
+    planar32 = planar32 && img.col_step[c] == 1;
+  if(planar32) /* int32 planes: nothing to convert, a device-to-device copy */
+    return copy_planes(J, J->img, img.comp, img.row_pitch, to_planes, st, t0, t1, true);
+  const int group = device_group(img, nc);
+  for_tile_row_runs(J, t0, t1, [&](Rect r) {
+    uint32_t ox = cp.x0, oy = cp.y0; /* canvas position of the image's first sample */
+    if(!to_planes && J->has_crop)
+    {
+      r.x0 = std::max(r.x0, J->crop.x0); r.y0 = std::max(r.y0, J->crop.y0);
+      r.x1 = std::min(r.x1, J->crop.x1); r.y1 = std::min(r.y1, J->crop.y1);
+      ox = J->crop.x0; oy = J->crop.y0;
+      if(r.x1 <= r.x0 || r.y1 <= r.y0)
+        return;
+    }
+    for(int c = 0; c < nc; c += group)
+    {
+      uint8_t* base = static_cast<uint8_t*>(img.comp[c]) +
+                      ((size_t)(r.y0 - oy) * img.row_pitch[c] + (size_t)(r.x0 - ox) * img.col_step[c]) * img.sample_bytes;
+      int32_t* planes[4];
+      for(int k = 0; k < group; ++k)
+        planes[k] = J->img.at(c + k, r.x0, r.y0);
+      if(to_planes)
+        b2k_launch_container_to_planes(base, img.row_pitch[c], img.col_step[c], img.sample_bytes, planes, group, J->img.pitch, r.w(),
+                                       r.h(), cp.sgnd, st);
+      else
+        b2k_launch_planes_to_container(planes, group, J->img.pitch, base, img.row_pitch[c], img.col_step[c], img.sample_bytes, r.w(),
+                                       r.h(), st);
+    }
   });
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -2115,10 +2224,12 @@ static b2k_device_job* cached_job(b2k_engine* e, const b2k_coding* cp, uint32_t 
   return J;
 }
 
+/* dev: the samples are the caller's device image (b2k_encode_device), ordered after the work queued on `caller` */
 static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* planes, const uint32_t* strides,
-                             uint32_t mod, uint32_t rem, b2k_result** out, bool u16, bool interleaved = false)
+                             uint32_t mod, uint32_t rem, b2k_result** out, bool u16, bool interleaved = false,
+                             const b2k_device_planes* dev = nullptr, cudaStream_t caller = nullptr)
 {
-  if(!e || !cp || !planes || !strides || !out)
+  if(!e || !cp || !out || (!dev && (!planes || !strides)))
     return -1;
   std::lock_guard<std::mutex> lock(e->mu);
   int rc = 0;
@@ -2132,10 +2243,10 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* p
   uint32_t stage_strides[4];
   /* several ranks on one host share its DRAM and CPU quota: measured (DESIGN.md section 4) packing loses there,
      so the automatic policy only considers it for a process that has the host to itself */
-  const bool tuned = !u16 && host_pack_eligible(J) && g_pack_policy.load() < 0 && b2k_host_local_peers() == 1;
-  const bool pack = !u16 && host_pack_eligible(J) && (tuned ? J->tune_enc.next_mode() : g_pack_policy.load() > 0);
+  const bool tuned = !dev && !u16 && host_pack_eligible(J) && g_pack_policy.load() < 0 && b2k_host_local_peers() == 1;
+  const bool pack = !dev && !u16 && host_pack_eligible(J) && (tuned ? J->tune_enc.next_mode() : g_pack_policy.load() > 0);
   const auto wall0 = std::chrono::steady_clock::now();
-  if(!u16)
+  if(!dev && !u16)
     g_last_pack[0].store(pack ? 1 : 0);
   const bool ring = pack && ring_geom(false).slot_mb > 0;
   uint64_t ring_counter = 0;
@@ -2163,6 +2274,11 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* p
   /* software pipeline over tile chunks: chunk k+1 crosses PCIe on the copy stream while chunk k
      is transformed and block-coded on the compute stream */
   cudaStream_t cs = e->copy_stream;
+  if(dev)
+  { /* what the caller queued before the call (the kernel that made the frame) comes first */
+    CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
+    CUDA_TRY(cudaStreamWaitEvent(st, e->caller_ev, 0));
+  }
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   CUDA_TRY(cudaStreamWaitEvent(cs, J->ev[0], 0));
   const size_t nchunks = J->chunk_tile.size() - 1;
@@ -2222,21 +2338,28 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* p
   for(size_t k = 0; k < nchunks; ++k)
   {
     const size_t t0 = J->chunk_tile[k], t1 = J->chunk_tile[k + 1];
-    if(ring)
-    {
-      if(ring_upload_chunk(J, user_planes, user_strides, (uint32_t)k, cs, ring_counter, [&] { return return_chunks(false); })) return -1;
+    if(dev)
+    { /* the samples are on the device already: chunk k's conversion on the compute stream replaces its upload */
+      if(device_convert(J, *dev, true, st, t0, t1)) return -1;
     }
     else
     {
-      if(pack)
-        host_convert_chunk(J, user_planes, user_strides, false, t0, t1); /* overlaps chunk k-1's H2D */
-      if(interleaved ? upload_interleaved(J, static_cast<const uint16_t*>(planes[0]), strides[0], cs, t0, t1)
-         : u16       ? copy_planes16(J, planes, strides, true, cs, t0, t1)
-                     : copy_planes(J, J->img, planes, strides, true, cs, t0, t1))
-        return -1;
+      if(ring)
+      {
+        if(ring_upload_chunk(J, user_planes, user_strides, (uint32_t)k, cs, ring_counter, [&] { return return_chunks(false); })) return -1;
+      }
+      else
+      {
+        if(pack)
+          host_convert_chunk(J, user_planes, user_strides, false, t0, t1); /* overlaps chunk k-1's H2D */
+        if(interleaved ? upload_interleaved(J, static_cast<const uint16_t*>(planes[0]), strides[0], cs, t0, t1)
+           : u16       ? copy_planes16(J, planes, strides, true, cs, t0, t1)
+                       : copy_planes(J, J->img, planes, strides, true, cs, t0, t1))
+          return -1;
+      }
+      CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, k)], cs));
+      CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(0, k)], 0));
     }
-    CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, k)], cs));
-    CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(0, k)], 0));
     if(k == nchunks - 1)
       CUDA_TRY(cudaEventRecord(J->ev[1], st)); /* all planes on the device */
     if(u16 && (interleaved ? split_interleaved(J, st, t0, t1) : convert_planes16(J, true, st, t0, t1))) return -1;
@@ -2258,6 +2381,11 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* p
     }
   }
   CUDA_TRY(cudaEventRecord(J->ev[2], st));
+  if(dev)
+  { /* the caller's stream goes on once every chunk of its image has been read */
+    CUDA_TRY(cudaEventRecord(e->caller_ev, st));
+    CUDA_TRY(cudaStreamWaitEvent(caller, e->caller_ev, 0));
+  }
   DBG_T("encode: chunks enqueued");
   b2k_result* R = nullptr;
   const uint32_t nb_all = (uint32_t)J->h_enc_desc.size();
@@ -2337,7 +2465,8 @@ extern "C" int32_t b2k_encode16_interleaved(b2k_engine* e, const b2k_coding* cp,
 
 static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
                              const uint8_t* bytes, uint64_t num_bytes, void* const* planes, const uint32_t* strides,
-                             uint32_t tile_mod, uint32_t tile_rem, double* ms_total, bool u16, const uint32_t* crop = nullptr);
+                             uint32_t tile_mod, uint32_t tile_rem, double* ms_total, bool u16, const uint32_t* crop = nullptr,
+                             const b2k_device_planes* dev = nullptr, cudaStream_t caller = nullptr);
 
 extern "C" int32_t b2k_decode(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
                               const uint8_t* bytes, uint64_t num_bytes, int32_t* const* planes, const uint32_t* strides,
@@ -2366,11 +2495,42 @@ extern "C" int32_t b2k_decode_window(b2k_engine* e, const b2k_coding* cp, const 
   return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, planes, strides, 1, 0, ms_total, sample_bytes == 2, window);
 }
 
+/* NULL is the legacy default stream, as the CUDA Array Interface assumes */
+static cudaStream_t caller_stream(void* s) { return s ? static_cast<cudaStream_t>(s) : cudaStreamLegacy; }
+
+extern "C" int32_t b2k_encode_device(b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img, uint32_t tile_mod,
+                                     uint32_t tile_rem, void* cuda_stream, b2k_result** out)
+{
+  if(!e || !cp || !out)
+    return -1;
+  if(int rc = check_device_planes(e, cp, img))
+    return rc;
+  return encode_common(e, cp, nullptr, nullptr, tile_mod, tile_rem, out, false, false, img, caller_stream(cuda_stream));
+}
+
+extern "C" int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
+                                     const uint8_t* bytes, uint64_t num_bytes, const b2k_device_planes* img, const uint32_t* window,
+                                     uint32_t tile_mod, uint32_t tile_rem, void* cuda_stream, double* ms_total)
+{
+  if(!e || !cp)
+    return -1;
+  if(window && tile_mod != 1)
+  {
+    g_err = "a windowed decode takes every tile: tile_mod must be 1";
+    return -1;
+  }
+  if(int rc = check_device_planes(e, cp, img))
+    return rc;
+  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, nullptr, nullptr, tile_mod, tile_rem, ms_total, false, window, img,
+                       caller_stream(cuda_stream));
+}
+
 static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
                              const uint8_t* bytes, uint64_t num_bytes, void* const* planes, const uint32_t* strides,
-                             uint32_t tile_mod, uint32_t tile_rem, double* ms_total, bool u16, const uint32_t* crop)
+                             uint32_t tile_mod, uint32_t tile_rem, double* ms_total, bool u16, const uint32_t* crop,
+                             const b2k_device_planes* dev, cudaStream_t caller)
 {
-  if(!e || !cp || !blocks || !planes || !strides)
+  if(!e || !cp || !blocks || (!dev && (!planes || !strides)))
     return -1;
   if(crop && (crop[0] >= crop[2] || crop[1] >= crop[3] || crop[0] < cp->x0 || crop[1] < cp->y0 || crop[2] > cp->x1 || crop[3] > cp->y1))
   {
@@ -2398,10 +2558,10 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
   uint32_t stage_strides[4];
   /* several ranks on one host share its DRAM and CPU quota: measured (DESIGN.md section 4) packing loses there,
      so the automatic policy only considers it for a process that has the host to itself */
-  const bool tuned = !crop && !u16 && host_pack_eligible(J) && g_pack_policy.load() < 0 && b2k_host_local_peers() == 1;
-  const bool pack = !crop && !u16 && host_pack_eligible(J) && (tuned ? J->tune_dec.next_mode() : g_pack_policy.load() > 0);
+  const bool tuned = !dev && !crop && !u16 && host_pack_eligible(J) && g_pack_policy.load() < 0 && b2k_host_local_peers() == 1;
+  const bool pack = !dev && !crop && !u16 && host_pack_eligible(J) && (tuned ? J->tune_dec.next_mode() : g_pack_policy.load() > 0);
   const auto wall0 = std::chrono::steady_clock::now();
-  if(!u16)
+  if(!dev && !u16)
     g_last_pack[1].store(pack ? 1 : 0);
   const bool ring = pack && ring_geom(true).slot_mb > 0;
   if(pack)
@@ -2430,6 +2590,11 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
     cudaFree(J->d_bytes);
     J->bytes_cap = num_bytes + 4096;
     CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
+  }
+  if(dev)
+  { /* what the caller queued before the call (e.g. the last reader of its buffer) comes first */
+    CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
+    CUDA_TRY(cudaStreamWaitEvent(st, e->caller_ev, 0));
   }
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
@@ -2498,6 +2663,11 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
                                     (J->cp.cblk_sty & 0x08) != 0, st);
     }
     if(enqueue_inverse(J, st, t0, t1)) return -1;
+    if(dev)
+    { /* into the caller's device image instead of down to the host */
+      if(device_convert(J, *dev, false, st, t0, t1)) return -1;
+      continue;
+    }
     if(u16 && convert_planes16(J, false, st, t0, t1)) return -1;
     CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, k)], st));
     if(ring)
@@ -2522,6 +2692,11 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
   CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, nchunks)], cs));
   CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(0, nchunks)], 0));
   CUDA_TRY(cudaEventRecord(J->ev[1], st));
+  if(dev)
+  { /* the caller's stream goes on once its image is written */
+    CUDA_TRY(cudaEventRecord(e->caller_ev, st));
+    CUDA_TRY(cudaStreamWaitEvent(caller, e->caller_ev, 0));
+  }
   CUDA_TRY(cudaEventSynchronize(J->ev[1]));
   CUDA_TRY(cudaGetLastError());
   DBG_T("decode: done");

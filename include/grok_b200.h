@@ -469,6 +469,41 @@ B2K_API int32_t b2k_decode16(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
                              uint16_t* const* planes, const uint32_t* strides, uint32_t tile_mod,
                              uint32_t tile_rem, double* ms_total);
 
+/* ---- images in device memory: encode from / decode into a buffer the caller keeps on the engine's GPU ---------------
+ * A renderer's frame, a video pipeline's surface or a CUDA tensor need not cross PCIe: only the coded bytes do.  The image
+ * is described per component; component c of pixel (x, y) (counted from the image's, or the window's, first pixel) is at
+ *   (char*)comp[c] + (y * row_pitch[c] + x * col_step[c]) * sample_bytes
+ * so planar buffers (col_step 1), pixel-interleaved ones (col_step = numcomps, comp[c] = comp[0] + c samples) and views
+ * such as the RGB of an RGBA buffer (col_step 4) all fit.  Samples are sample_bytes wide, signed when cp->sgnd. */
+typedef struct b2k_device_planes
+{
+  void* comp[4];          /* device address of component c's first sample (canvas x0, y0 of the image, or of the window) */
+  uint32_t row_pitch[4];  /* samples between the starts of two rows */
+  uint32_t col_step[4];   /* samples between two pixels of a row: 1 planar, numcomps pixel-interleaved, 4 for RGB of RGBA */
+  uint32_t sample_bytes;  /* 1, 2 or 4; signedness is cp->sgnd */
+} b2k_device_planes;
+/* b2k_encode_device gives exactly what b2k_encode gives for the same samples; b2k_decode_device writes exactly what
+ * b2k_decode writes, cast to the container (the decoder clamps to cp->prec, so narrowing only truncates).  Only the
+ * selected tiles (tile % tile_mod == tile_rem) are read or written.  window works as in b2k_decode_window: img then holds
+ * the window, and tile_mod must be 1.  The coded data (`bytes`, the result's arena) stay in host memory: T2 is host code.
+ * Samples are converted between the container and the engine's int32 planes on the device, chunk by chunk in place of the
+ * host calls' PCIe copies (int32 planar images are copied device to device).
+ * Stream order: the call first records an event on cuda_stream (NULL = the legacy default stream) and the engine's
+ * streams wait for it, so work the caller queued before the call (the kernel that produced the frame) is finished before
+ * the engine reads the buffer; before returning, it makes cuda_stream wait for the engine's last access to the buffer.
+ * Like the host calls it returns once its work is done (the encode result is in host memory; decode reports HT decoder
+ * errors as b2k_decode does, -2).
+ * Returns 0 handled; 1 not handled (a container narrower than cp->prec, more than 4 components); -1 bad input (a comp[c]
+ * that cudaPointerGetAttributes does not report as device or managed memory of the engine's device, one that is not a
+ * multiple of sample_bytes, col_step 0, a window outside the image).  b2k_last_error says which.
+ * These calls share the engine's cached job with b2k_encode / b2k_decode and leave the host-packing policy alone
+ * (b2k_host_pack_last keeps reporting the last host call). */
+B2K_API int32_t b2k_encode_device(b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img, uint32_t tile_mod,
+                                  uint32_t tile_rem, void* cuda_stream, b2k_result** out);
+B2K_API int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
+                                  const uint8_t* bytes, uint64_t num_bytes, const b2k_device_planes* img, const uint32_t* window,
+                                  uint32_t tile_mod, uint32_t tile_rem, void* cuda_stream, double* ms_total);
+
 /* Geometry only (host): enumerate the blocks of the selected tiles, lengths zero.  Returns the
  * count; fills at most cap entries. */
 B2K_API int64_t b2k_enumerate(const b2k_coding* cp, uint32_t tile_mod, uint32_t tile_rem,
