@@ -111,13 +111,6 @@ void b2k_launch_container_to_planes(const void* src, uint32_t spitch, uint32_t s
                                     uint32_t dpitch, uint32_t w, uint32_t h, int sgnd, cudaStream_t st);
 void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t spitch, void* dst, uint32_t dpitch, uint32_t step,
                                     uint32_t sample_bytes, uint32_t w, uint32_t h, cudaStream_t st);
-/* the 16-bit instances of the two */
-void b2k_launch_widen16_interleaved(const uint16_t* src, uint32_t spitch, int32_t* const* dst, int nc, uint32_t dpitch, uint32_t w,
-                                    uint32_t h, int sgnd, cudaStream_t st);
-void b2k_launch_widen16(const uint16_t* src, uint32_t spitch, int32_t* dst, uint32_t dpitch, uint32_t w, uint32_t h, int sgnd,
-                        cudaStream_t st);
-void b2k_launch_narrow16(const int32_t* src, uint32_t spitch, uint16_t* dst, uint32_t dpitch, uint32_t w, uint32_t h,
-                         cudaStream_t st);
 void b2k_count_launch(void);
 
 /* host_pack.cpp: container conversion on a small host thread pool (int32 planes <-> pinned 16-bit staging) */

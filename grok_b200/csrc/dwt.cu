@@ -1741,22 +1741,6 @@ void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t 
   }
   b2k_count_launch();
 }
-/* the 16-bit containers of b2k_encode16 / b2k_decode16 / b2k_encode16_interleaved */
-void b2k_launch_widen16(const uint16_t* src, uint32_t spitch, int32_t* dst, uint32_t dpitch, uint32_t w, uint32_t h, int sgnd,
-                        cudaStream_t st)
-{
-  b2k_launch_container_to_planes(src, spitch, 1, 2, &dst, 1, dpitch, w, h, sgnd, st);
-}
-void b2k_launch_widen16_interleaved(const uint16_t* src, uint32_t spitch, int32_t* const* dst, int nc, uint32_t dpitch, uint32_t w,
-                                    uint32_t h, int sgnd, cudaStream_t st)
-{
-  b2k_launch_container_to_planes(src, spitch, (uint32_t)nc, 2, dst, nc, dpitch, w, h, sgnd, st);
-}
-void b2k_launch_narrow16(const int32_t* src, uint32_t spitch, uint16_t* dst, uint32_t dpitch, uint32_t w, uint32_t h,
-                         cudaStream_t st)
-{
-  b2k_launch_planes_to_container(&src, 1, spitch, dst, dpitch, 1, 2, w, h, st);
-}
 
 /* one launch of a DWT kernel whose warps stage through WarpPipe<Stage>; the shared-memory limit it needs is raised once
    per device for each kernel */

@@ -256,15 +256,6 @@ static int alloc_planes(Planes& p, int n, uint32_t cx0, uint32_t cy0, uint32_t c
   return 0;
 }
 
-struct Planes16
-{
-  uint16_t* base = nullptr;
-  uint32_t pitch = 0, rows = 0, X0 = 0, Y0 = 0;
-  int n = 0;
-  size_t plane_elems() const { return (size_t)pitch * rows; }
-  uint16_t* at(int c, uint32_t x, uint32_t y) const { return base + (size_t)c * plane_elems() + (size_t)(y - Y0) * pitch + (x - X0); }
-};
-
 struct LevelLaunch
 {
   std::vector<DwtLevelDesc> descs;
@@ -282,7 +273,7 @@ struct LevelLaunch
    ranks share a socket's DRAM.  Default policy: time both ways on the first calls, keep the faster,
    look at the other one again every 64 calls. */
 /* pipeline chunks per call (tile granular) and their events: purpose 0 chunk done on its stream, 1 chunk's
-   upload done, 2 side-stream / scan done, 3 chunk's download done, 4 misc */
+   upload done, 2 side-stream / scan done, 3 misc */
 #define B2K_MAX_CHUNKS 32
 #define CEV(purpose, k) ((purpose) * (B2K_MAX_CHUNKS + 1) + (int)(k))
 
@@ -342,24 +333,19 @@ struct b2k_device_job
   std::vector<float> dec_quant;        /* per coded block: decoder step / 2^(31-Kmax) */
   std::vector<uint32_t> coded_first;   /* coded blocks of selected tile ti are [coded_first[ti], coded_first[ti+1]) */
   std::vector<uint32_t> chunk_tile;    /* pipeline chunks: selected tiles [chunk_tile[k], chunk_tile[k+1]) */
-  cudaEvent_t chunk_ev[5 * (B2K_MAX_CHUNKS + 1)]{}; /* [purpose][chunk], see CEV() */
+  cudaEvent_t chunk_ev[4 * (B2K_MAX_CHUNKS + 1)]{}; /* [purpose][chunk], see CEV() */
   uint32_t max_cblk_w = 0;
   HtEncodeLimits enc_limits{0, 0};     /* shared-memory sizing of the HT encoder launches */
 
   Planes img, coef, ll[2];
-  Planes16 img16;                      /* 16-bit sample containers (b2k_encode16 / b2k_decode16), lazily */
-  uint16_t* d_ileave = nullptr;        /* pixel-interleaved 16-bit frame (b2k_encode16_interleaved), lazily */
-  uint32_t ileave_pitch = 0;           /* in samples: numcomps * width, rounded up to 8 */
+  uint16_t* d_stage = nullptr;         /* 16-bit containers crossing PCIe, planar or pixel-interleaved (stage_container), lazily */
   std::vector<LevelLaunch> fwd, inv;   /* launch order */
-  std::vector<LevelLaunch> fwd16, inv16; /* finest-level launches re-pointed at img16 (parallel to fwd / inv) */
   HtBlockDesc* d_enc_desc = nullptr;
   HtBlockDesc* d_dec_desc = nullptr;
   std::vector<HtBlockDesc> h_enc_desc;
   HtBlockDesc* h_dec_desc = nullptr;   /* pinned staging */
   HtBlockOut* d_out = nullptr;
   uint64_t* d_offsets = nullptr;
-  bool has_crop = false;           /* b2k_decode_window: only this rectangle of the pixels goes back to the host, */
-  Rect crop{};                     /* and the host planes are the rectangle's (row 0 / column 0 = crop.y0 / crop.x0) */
   uint32_t* d_recs = nullptr;     /* decode: per-quad records between the two decode phases */
   float* d_dec_quant = nullptr;
   HtBlockOut* d_dec_status = nullptr;
@@ -375,11 +361,8 @@ struct b2k_device_job
   cudaEvent_t ev[8]{};
   float last_level1_ms = 0.f, last_inv_level1_ms = 0.f;
   uint64_t level1_alg_bytes = 0;
-  bool img_is_u16 = false;
-  uint16_t* h_stage16 = nullptr;  /* pinned 16-bit staging for the int32 entry points (host_pack.cpp) */
-  uint64_t stage16_elems = 0;
-  /* ring staging (B2K_STAGE_RING_MB > 0): a few MB-sized pinned slots that are narrowed into / widened out of
-     while still cache-resident, instead of one image-sized staging buffer that round-trips through DRAM */
+  /* host packing (host_pack.cpp): a few MB-sized pinned slots, narrowed into / widened out of while still cache-resident,
+     so that the 16-bit copy of the image never round-trips through host DRAM */
   uint16_t* h_ring = nullptr;
   uint32_t ring_slots = 0;
   uint64_t ring_slot_elems = 0, ring_elems = 0;
@@ -844,10 +827,7 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
   cudaSetDevice(J->eng->device);
   cudaStreamSynchronize(J->eng->stream);
   cudaFree(J->img.base);
-  cudaFree(J->img16.base);
-  cudaFree(J->d_ileave);
-  for(LevelLaunch& L : J->fwd16) cudaFree(L.d_descs);
-  for(LevelLaunch& L : J->inv16) cudaFree(L.d_descs);
+  cudaFree(J->d_stage);
   cudaFree(J->coef.base);
   cudaFree(J->ll[0].base);
   cudaFree(J->ll[1].base);
@@ -866,7 +846,6 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
   cudaFreeHost(J->h_out);
   cudaFreeHost(J->h_dec_desc);
   cudaFreeHost(J->h_offsets);
-  cudaFreeHost(J->h_stage16);
   cudaFreeHost(J->h_ring);
   for(cudaEvent_t ev : J->q_ev)
     cudaEventDestroy(ev);
@@ -888,19 +867,107 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
 
 extern "C" uint64_t b2k_job_num_blocks(const b2k_device_job* J) { return J ? J->blocks.size() : 0; }
 
-/* ---- copies between the caller's int32 planes and the engine's, per selected tile -------------
-   to_device: into the engine's planes.  user_on_device: the caller's planes are device memory too (b2k_encode_device /
-   b2k_decode_device), so the copy stays on the device */
-static int copy_planes(b2k_device_job* J, const Planes& P, void* const* host, const uint32_t* strides, bool to_device,
-                       cudaStream_t st, size_t t0 = 0, size_t t1 = (size_t)-1, bool user_on_device = false)
+/* ---- sample transport: the caller's containers <-> the engine's int32 planes ---------------------------------------
+   Every container samples cross is described as a b2k_device_planes: component c of canvas pixel (x, y) is at
+   comp[c] + ((y - oy) * row_pitch[c] + (x - ox) * col_step[c]) * sample_bytes, (ox, oy) being the canvas position of its
+   first sample (the image's, the window's, or the staging's own origin). */
+struct Container
 {
-  const cudaMemcpyKind in = user_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-  const cudaMemcpyKind out = user_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  b2k_device_planes d{};
+  uint32_t ox = 0, oy = 0;
+  bool device = false;      /* device memory (the engine's buffers, the caller's device image), else host memory */
+  bool interleaved = false; /* pixel-interleaved: comp[c] = comp[0] + c samples, col_step = numcomps */
+  uint8_t* at(int c, uint32_t x, uint32_t y) const
+  {
+    return static_cast<uint8_t*>(d.comp[c]) +
+           ((size_t)(y - oy) * d.row_pitch[c] + (size_t)(x - ox) * d.col_step[c]) * d.sample_bytes;
+  }
+};
+
+/* planar: the caller's host planes, or the engine's int32 planes */
+static Container planar_container(int nc, void* const* comp, const uint32_t* pitch, uint32_t sample_bytes, uint32_t ox, uint32_t oy,
+                                  bool device)
+{
+  Container C;
+  for(int c = 0; c < nc && c < 4; ++c)
+  {
+    C.d.comp[c] = comp[c];
+    C.d.row_pitch[c] = pitch[c];
+    C.d.col_step[c] = 1;
+  }
+  C.d.sample_bytes = sample_bytes;
+  C.ox = ox;
+  C.oy = oy;
+  C.device = device;
+  return C;
+}
+static Container interleaved_container(int nc, void* base, uint32_t pitch, uint32_t sample_bytes, uint32_t ox, uint32_t oy, bool device)
+{
+  Container C;
+  for(int c = 0; c < nc && c < 4; ++c)
+  {
+    C.d.comp[c] = static_cast<uint8_t*>(base) + (size_t)c * sample_bytes;
+    C.d.row_pitch[c] = pitch;
+    C.d.col_step[c] = (uint32_t)nc;
+  }
+  C.d.sample_bytes = sample_bytes;
+  C.ox = ox;
+  C.oy = oy;
+  C.device = device;
+  C.interleaved = true;
+  return C;
+}
+static Container plane_container(const Planes& P)
+{
+  void* comp[4];
+  uint32_t pitch[4];
+  for(int c = 0; c < P.n && c < 4; ++c)
+  {
+    comp[c] = P.at(c, P.X0, P.Y0);
+    pitch[c] = P.pitch;
+  }
+  return planar_container(P.n, comp, pitch, 4, P.X0, P.Y0, true);
+}
+
+/* The 16-bit containers that cross PCIe land in (and leave from) one device buffer, J->d_stage, in one of two layouts:
+   planar, canvas column x0 & ~63 at column 0, rows of the image's width rounded up to 8 samples (a full-width tile row is one
+   contiguous block) and two rows of slack; or pixel-interleaved, the image's rows as they are, rounded up to 8 samples. */
+static uint32_t stage_pitch(const b2k_coding& cp, bool interleaved)
+{
+  return interleaved ? ((cp.x1 - cp.x0) * cp.numcomps + 7u) & ~7u : ((cp.x1 - (cp.x0 & ~63u)) + 7u) & ~7u;
+}
+static size_t stage_plane_elems(const b2k_coding& cp) { return (size_t)stage_pitch(cp, false) * (cp.y1 - cp.y0 + 2); }
+static Container stage_container(const b2k_device_job* J, bool interleaved)
+{
   const b2k_coding& cp = J->cp;
+  const uint32_t pitch = stage_pitch(cp, interleaved);
+  if(interleaved)
+    return interleaved_container(cp.numcomps, J->d_stage, pitch, 2, cp.x0, cp.y0, true);
+  void* comp[4];
+  const uint32_t pitches[4] = {pitch, pitch, pitch, pitch};
+  for(int c = 0; c < cp.numcomps; ++c)
+    comp[c] = J->d_stage + c * stage_plane_elems(cp);
+  return planar_container(cp.numcomps, comp, pitches, 2, cp.x0 & ~63u, cp.y0, true);
+}
+static int ensure_stage(b2k_device_job* J)
+{
+  if(J->d_stage)
+    return 0;
+  const b2k_coding& cp = J->cp;
+  const size_t bytes = std::max(cp.numcomps * stage_plane_elems(cp), (size_t)stage_pitch(cp, true) * (cp.y1 - cp.y0)) * sizeof(uint16_t);
+  CUDA_TRY(cudaMalloc(&J->d_stage, bytes));
+  CUDA_TRY(cudaMemset(J->d_stage, 0, bytes));
+  return 0;
+}
+
+/* fn(r) for every run of horizontally adjacent selected tiles of [t0, t1) in one tile row, merged into one rectangle; with a
+   window, r is clipped to it and runs outside it are skipped */
+template <typename F>
+static void for_tile_row_runs(const b2k_device_job* J, size_t t0, size_t t1, const Rect* window, F&& fn)
+{
   t1 = std::min(t1, J->tiles.size());
   for(size_t ti = t0; ti < t1;)
   {
-    /* merge horizontally adjacent selected tiles of one tile row into a single rectangle */
     Rect r = J->tile_rects[ti];
     size_t tj = ti + 1;
     while(tj < t1 && J->tile_rects[tj].y0 == r.y0 && J->tile_rects[tj].y1 == r.y1 && J->tile_rects[tj].x0 == r.x1)
@@ -908,29 +975,46 @@ static int copy_planes(b2k_device_job* J, const Planes& P, void* const* host, co
       r.x1 = J->tile_rects[tj].x1;
       ++tj;
     }
-    uint32_t ox = cp.x0, oy = cp.y0; /* canvas position of the host planes' first sample */
-    if(!to_device && J->has_crop)
-    {
-      r.x0 = std::max(r.x0, J->crop.x0); r.y0 = std::max(r.y0, J->crop.y0);
-      r.x1 = std::min(r.x1, J->crop.x1); r.y1 = std::min(r.y1, J->crop.y1);
-      ox = J->crop.x0; oy = J->crop.y0;
-      if(r.x1 <= r.x0 || r.y1 <= r.y0)
-      {
-        ti = tj;
-        continue;
-      }
-    }
-    for(int c = 0; c < cp.numcomps; ++c)
-    {
-      int32_t* dev = P.at(c, r.x0, r.y0);
-      int32_t* hst = reinterpret_cast<int32_t*>(host[c]) + (size_t)(r.y0 - oy) * strides[c] + (r.x0 - ox);
-      if(to_device)
-        CUDA_TRY(cudaMemcpy2DAsync(dev, (size_t)P.pitch * 4, hst, (size_t)strides[c] * 4, (size_t)r.w() * 4, r.h(), in, st));
-      else
-        CUDA_TRY(cudaMemcpy2DAsync(hst, (size_t)strides[c] * 4, dev, (size_t)P.pitch * 4, (size_t)r.w() * 4, r.h(), out, st));
-    }
     ti = tj;
+    if(window)
+    {
+      r.x0 = std::max(r.x0, window->x0); r.y0 = std::max(r.y0, window->y0);
+      r.x1 = std::min(r.x1, window->x1); r.y1 = std::min(r.y1, window->y1);
+      if(r.empty())
+        continue;
+    }
+    fn(r);
   }
+}
+
+/* `rows` rows of `row` bytes: one linear copy where they abut on both sides, else one 2-D copy */
+static cudaError_t copy_rows(void* dst, size_t dpitch, const void* src, size_t spitch, size_t row, uint32_t rows, cudaMemcpyKind kind,
+                             cudaStream_t st)
+{
+  if(dpitch == row && spitch == row)
+    return cudaMemcpyAsync(dst, src, row * rows, kind, st);
+  return cudaMemcpy2DAsync(dst, dpitch, src, spitch, row, rows, kind, st);
+}
+
+/* the selected tiles [t0, t1), clipped to `window`, from one container to another of the same sample size and layout: host to
+   device, device to host or device to device, per run one copy per component, or one for all of them when pixel-interleaved */
+static int copy_runs(const b2k_device_job* J, const Container& dst, const Container& src, cudaStream_t st, size_t t0, size_t t1,
+                     const Rect* window)
+{
+  const int nc = J->cp.numcomps, group = src.interleaved ? nc : 1;
+  const size_t sb = src.d.sample_bytes;
+  const cudaMemcpyKind kind = !src.device ? cudaMemcpyHostToDevice : dst.device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  cudaError_t err = cudaSuccess;
+  for_tile_row_runs(J, t0, t1, window, [&](const Rect& r) {
+    for(int c = 0; c < nc; c += group)
+    {
+      const cudaError_t e = copy_rows(dst.at(c, r.x0, r.y0), dst.d.row_pitch[c] * sb, src.at(c, r.x0, r.y0), src.d.row_pitch[c] * sb,
+                                      (size_t)r.w() * group * sb, r.h(), kind, st);
+      if(e != cudaSuccess)
+        err = e;
+    }
+  });
+  CUDA_TRY(err);
   return 0;
 }
 
@@ -938,7 +1022,8 @@ extern "C" int32_t b2k_job_upload(b2k_device_job* J, const int32_t* const* plane
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  if(copy_planes(J, J->img, (void* const*)planes, strides, true, J->eng->stream)) return -1;
+  const Container host = planar_container(J->cp.numcomps, (void* const*)planes, strides, 4, J->cp.x0, J->cp.y0, false);
+  if(copy_runs(J, plane_container(J->img), host, J->eng->stream, 0, J->tiles.size(), nullptr)) return -1;
   CUDA_TRY(cudaStreamSynchronize(J->eng->stream));
   return 0;
 }
@@ -946,7 +1031,8 @@ extern "C" int32_t b2k_job_download(b2k_device_job* J, int32_t* const* planes, c
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  if(copy_planes(J, J->img, (void* const*)planes, strides, false, J->eng->stream)) return -1;
+  const Container host = planar_container(J->cp.numcomps, (void* const*)planes, strides, 4, J->cp.x0, J->cp.y0, false);
+  if(copy_runs(J, host, plane_container(J->img), J->eng->stream, 0, J->tiles.size(), nullptr)) return -1;
   CUDA_TRY(cudaStreamSynchronize(J->eng->stream));
   return 0;
 }
@@ -954,7 +1040,8 @@ extern "C" int32_t b2k_job_download_coeffs(b2k_device_job* J, int32_t* const* pl
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  if(copy_planes(J, J->coef, (void* const*)planes, strides, false, J->eng->stream)) return -1;
+  const Container host = planar_container(J->cp.numcomps, (void* const*)planes, strides, 4, J->cp.x0, J->cp.y0, false);
+  if(copy_runs(J, host, plane_container(J->coef), J->eng->stream, 0, J->tiles.size(), nullptr)) return -1;
   CUDA_TRY(cudaStreamSynchronize(J->eng->stream));
   return 0;
 }
@@ -962,168 +1049,9 @@ extern "C" int32_t b2k_job_upload_coeffs(b2k_device_job* J, const int32_t* const
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  if(copy_planes(J, J->coef, (void* const*)planes, strides, true, J->eng->stream)) return -1;
+  const Container host = planar_container(J->cp.numcomps, (void* const*)planes, strides, 4, J->cp.x0, J->cp.y0, false);
+  if(copy_runs(J, plane_container(J->coef), host, J->eng->stream, 0, J->tiles.size(), nullptr)) return -1;
   CUDA_TRY(cudaStreamSynchronize(J->eng->stream));
-  return 0;
-}
-
-
-/* ---- 16-bit sample containers ---------------------------------------------------------------- */
-static int ensure_u16(b2k_device_job* J)
-{
-  if(J->img16.base)
-    return 0;
-  const b2k_coding& cp = J->cp;
-  Planes16& P = J->img16;
-  P.n = cp.numcomps;
-  P.X0 = cp.x0 & ~63u;
-  P.Y0 = cp.y0;
-  P.pitch = ((cp.x1 - P.X0) + 7u) & ~7u; /* no slack: a full-width tile row is one contiguous block */
-  P.rows = (cp.y1 - cp.y0) + 2;
-  CUDA_TRY(cudaMalloc(&P.base, (size_t)P.n * P.plane_elems() * sizeof(uint16_t)));
-  CUDA_TRY(cudaMemset(P.base, 0, (size_t)P.n * P.plane_elems() * sizeof(uint16_t)));
-  return 0;
-}
-
-/* widen (after H2D) or narrow (before D2H) the rectangles of selected tiles [t0, t1) */
-static int convert_planes16(b2k_device_job* J, bool widen, cudaStream_t st, size_t t0, size_t t1)
-{
-  const b2k_coding& cp = J->cp;
-  t1 = std::min(t1, J->tiles.size());
-  for(size_t ti = t0; ti < t1;)
-  {
-    Rect r = J->tile_rects[ti];
-    size_t tj = ti + 1;
-    while(tj < t1 && J->tile_rects[tj].y0 == r.y0 && J->tile_rects[tj].y1 == r.y1 && J->tile_rects[tj].x0 == r.x1)
-    {
-      r.x1 = J->tile_rects[tj].x1;
-      ++tj;
-    }
-    for(int c = 0; c < cp.numcomps; ++c)
-    {
-      if(widen)
-        b2k_launch_widen16(J->img16.at(c, r.x0, r.y0), J->img16.pitch, J->img.at(c, r.x0, r.y0), J->img.pitch, r.w(), r.h(),
-                           cp.sgnd, st);
-      else
-        b2k_launch_narrow16(J->img.at(c, r.x0, r.y0), J->img.pitch, J->img16.at(c, r.x0, r.y0), J->img16.pitch, r.w(), r.h(), st);
-    }
-    ti = tj;
-  }
-  CUDA_TRY(cudaGetLastError());
-  return 0;
-}
-
-static int copy_planes16(b2k_device_job* J, void* const* host, const uint32_t* strides, bool to_device, cudaStream_t st,
-                         size_t t0, size_t t1)
-{
-  const b2k_coding& cp = J->cp;
-  const Planes16& P = J->img16;
-  t1 = std::min(t1, J->tiles.size());
-  for(size_t ti = t0; ti < t1;)
-  {
-    Rect r = J->tile_rects[ti];
-    size_t tj = ti + 1;
-    while(tj < t1 && J->tile_rects[tj].y0 == r.y0 && J->tile_rects[tj].y1 == r.y1 && J->tile_rects[tj].x0 == r.x1)
-    {
-      r.x1 = J->tile_rects[tj].x1;
-      ++tj;
-    }
-    uint32_t ox = cp.x0, oy = cp.y0;
-    if(!to_device && J->has_crop)
-    {
-      r.x0 = std::max(r.x0, J->crop.x0); r.y0 = std::max(r.y0, J->crop.y0);
-      r.x1 = std::min(r.x1, J->crop.x1); r.y1 = std::min(r.y1, J->crop.y1);
-      ox = J->crop.x0; oy = J->crop.y0;
-      if(r.x1 <= r.x0 || r.y1 <= r.y0)
-      {
-        ti = tj;
-        continue;
-      }
-    }
-    for(int c = 0; c < cp.numcomps; ++c)
-    {
-      uint16_t* dev = P.at(c, r.x0, r.y0);
-      uint16_t* hst = reinterpret_cast<uint16_t*>(host[c]) + (size_t)(r.y0 - oy) * strides[c] + (r.x0 - ox);
-      if(strides[c] == P.pitch && r.w() == P.pitch)
-      { /* contiguous on both sides: one linear copy */
-        if(to_device)
-          CUDA_TRY(cudaMemcpyAsync(dev, hst, (size_t)r.w() * r.h() * 2, cudaMemcpyHostToDevice, st));
-        else
-          CUDA_TRY(cudaMemcpyAsync(hst, dev, (size_t)r.w() * r.h() * 2, cudaMemcpyDeviceToHost, st));
-        continue;
-      }
-      if(to_device)
-        CUDA_TRY(cudaMemcpy2DAsync(dev, (size_t)P.pitch * 2, hst, (size_t)strides[c] * 2, (size_t)r.w() * 2, r.h(),
-                                   cudaMemcpyHostToDevice, st));
-      else
-        CUDA_TRY(cudaMemcpy2DAsync(hst, (size_t)strides[c] * 2, dev, (size_t)P.pitch * 2, (size_t)r.w() * 2, r.h(),
-                                   cudaMemcpyDeviceToHost, st));
-    }
-    ti = tj;
-  }
-  return 0;
-}
-
-/* ---- pixel-interleaved 16-bit frames: the rows cross PCIe as they are, the planes are made on the device ---- */
-static int ensure_ileave(b2k_device_job* J)
-{
-  if(J->d_ileave)
-    return 0;
-  const b2k_coding& cp = J->cp;
-  J->ileave_pitch = ((cp.x1 - cp.x0) * cp.numcomps + 7u) & ~7u;
-  CUDA_TRY(cudaMalloc(&J->d_ileave, (size_t)J->ileave_pitch * (cp.y1 - cp.y0) * sizeof(uint16_t)));
-  return 0;
-}
-
-template <typename F>
-static void for_tile_row_runs(const b2k_device_job* J, size_t t0, size_t t1, F&& fn)
-{
-  t1 = std::min(t1, J->tiles.size());
-  for(size_t ti = t0; ti < t1;)
-  {
-    Rect r = J->tile_rects[ti];
-    size_t tj = ti + 1;
-    while(tj < t1 && J->tile_rects[tj].y0 == r.y0 && J->tile_rects[tj].y1 == r.y1 && J->tile_rects[tj].x0 == r.x1)
-    {
-      r.x1 = J->tile_rects[tj].x1;
-      ++tj;
-    }
-    fn(r);
-    ti = tj;
-  }
-}
-
-static int upload_interleaved(b2k_device_job* J, const uint16_t* host, uint32_t stride, cudaStream_t st, size_t t0, size_t t1)
-{
-  const b2k_coding& cp = J->cp;
-  const uint32_t nc = cp.numcomps;
-  cudaError_t err = cudaSuccess;
-  for_tile_row_runs(J, t0, t1, [&](const Rect& r) {
-    uint16_t* dev = J->d_ileave + (size_t)(r.y0 - cp.y0) * J->ileave_pitch + (size_t)(r.x0 - cp.x0) * nc;
-    const uint16_t* hst = host + (size_t)(r.y0 - cp.y0) * stride + (size_t)(r.x0 - cp.x0) * nc;
-    const size_t row_bytes = (size_t)r.w() * nc * 2;
-    cudaError_t e = (stride == J->ileave_pitch && r.w() == cp.x1 - cp.x0)
-                        ? cudaMemcpyAsync(dev, hst, (size_t)stride * 2 * (r.h() - 1) + row_bytes, cudaMemcpyHostToDevice, st)
-                        : cudaMemcpy2DAsync(dev, (size_t)J->ileave_pitch * 2, hst, (size_t)stride * 2, row_bytes, r.h(),
-                                            cudaMemcpyHostToDevice, st);
-    if(e != cudaSuccess)
-      err = e;
-  });
-  CUDA_TRY(err);
-  return 0;
-}
-
-static int split_interleaved(b2k_device_job* J, cudaStream_t st, size_t t0, size_t t1)
-{
-  const b2k_coding& cp = J->cp;
-  for_tile_row_runs(J, t0, t1, [&](const Rect& r) {
-    int32_t* dst[4] = {nullptr, nullptr, nullptr, nullptr};
-    for(int c = 0; c < cp.numcomps; ++c)
-      dst[c] = J->img.at(c, r.x0, r.y0);
-    b2k_launch_widen16_interleaved(J->d_ileave + (size_t)(r.y0 - cp.y0) * J->ileave_pitch + (size_t)(r.x0 - cp.x0) * cp.numcomps,
-                                   J->ileave_pitch, dst, cp.numcomps, J->img.pitch, r.w(), r.h(), cp.sgnd, st);
-  });
-  CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
@@ -1189,41 +1117,34 @@ static int device_group(const b2k_device_planes& img, int nc)
   return nc;
 }
 
-/* the caller's device image -> the engine's planes (to_planes) or back, selected tiles [t0, t1), on stream st.  On the way
-   back a windowed decode writes only the crop, which the image then holds */
-static int device_convert(b2k_device_job* J, const b2k_device_planes& img, bool to_planes, cudaStream_t st, size_t t0, size_t t1)
+/* a device container -> the engine's planes (to_planes) or back, selected tiles [t0, t1) clipped to `window`, on stream st:
+   conversion launches, or device-to-device copies for int32 planes */
+static int device_convert(b2k_device_job* J, const Container& img, bool to_planes, cudaStream_t st, size_t t0, size_t t1,
+                          const Rect* window)
 {
   const b2k_coding& cp = J->cp;
   const int nc = cp.numcomps;
-  bool planar32 = img.sample_bytes == 4;
+  bool planar32 = img.d.sample_bytes == 4;
   for(int c = 0; c < nc; ++c)
-    planar32 = planar32 && img.col_step[c] == 1;
-  if(planar32) /* int32 planes: nothing to convert, a device-to-device copy */
-    return copy_planes(J, J->img, img.comp, img.row_pitch, to_planes, st, t0, t1, true);
-  const int group = device_group(img, nc);
-  for_tile_row_runs(J, t0, t1, [&](Rect r) {
-    uint32_t ox = cp.x0, oy = cp.y0; /* canvas position of the image's first sample */
-    if(!to_planes && J->has_crop)
-    {
-      r.x0 = std::max(r.x0, J->crop.x0); r.y0 = std::max(r.y0, J->crop.y0);
-      r.x1 = std::min(r.x1, J->crop.x1); r.y1 = std::min(r.y1, J->crop.y1);
-      ox = J->crop.x0; oy = J->crop.y0;
-      if(r.x1 <= r.x0 || r.y1 <= r.y0)
-        return;
-    }
+    planar32 = planar32 && img.d.col_step[c] == 1;
+  if(planar32) /* int32 planes: nothing to convert */
+  {
+    const Container planes = plane_container(J->img);
+    return to_planes ? copy_runs(J, planes, img, st, t0, t1, window) : copy_runs(J, img, planes, st, t0, t1, window);
+  }
+  const int group = device_group(img.d, nc);
+  for_tile_row_runs(J, t0, t1, window, [&](const Rect& r) {
     for(int c = 0; c < nc; c += group)
     {
-      uint8_t* base = static_cast<uint8_t*>(img.comp[c]) +
-                      ((size_t)(r.y0 - oy) * img.row_pitch[c] + (size_t)(r.x0 - ox) * img.col_step[c]) * img.sample_bytes;
       int32_t* planes[4];
       for(int k = 0; k < group; ++k)
         planes[k] = J->img.at(c + k, r.x0, r.y0);
       if(to_planes)
-        b2k_launch_container_to_planes(base, img.row_pitch[c], img.col_step[c], img.sample_bytes, planes, group, J->img.pitch, r.w(),
-                                       r.h(), cp.sgnd, st);
+        b2k_launch_container_to_planes(img.at(c, r.x0, r.y0), img.d.row_pitch[c], img.d.col_step[c], img.d.sample_bytes, planes, group,
+                                       J->img.pitch, r.w(), r.h(), cp.sgnd, st);
       else
-        b2k_launch_planes_to_container(planes, group, J->img.pitch, base, img.row_pitch[c], img.col_step[c], img.sample_bytes, r.w(),
-                                       r.h(), st);
+        b2k_launch_planes_to_container(planes, group, J->img.pitch, img.at(c, r.x0, r.y0), img.d.row_pitch[c], img.d.col_step[c],
+                                       img.d.sample_bytes, r.w(), r.h(), st);
     }
   });
   CUDA_TRY(cudaGetLastError());
@@ -1239,59 +1160,6 @@ static bool host_pack_eligible(const b2k_device_job* J)
   return cp.prec <= 16 && samples >= (1u << 22) && J->chunk_tile.size() > 2 && b2k_host_threads() > 0;
 }
 
-static int ensure_stage16(b2k_device_job* J)
-{
-  if(J->h_stage16)
-    return 0;
-  const b2k_coding& cp = J->cp;
-  J->stage16_elems = (uint64_t)(cp.x1 - cp.x0) * (cp.y1 - cp.y0);
-  CUDA_TRY(cudaHostAlloc(&J->h_stage16, J->stage16_elems * cp.numcomps * sizeof(uint16_t), cudaHostAllocDefault));
-  return 0;
-}
-/* staging planes are image-shaped, stride = image width */
-static void stage16_views(const b2k_device_job* J, void** planes, uint32_t* strides)
-{
-  for(int c = 0; c < J->cp.numcomps; ++c)
-  {
-    planes[c] = J->h_stage16 + (uint64_t)c * J->stage16_elems;
-    strides[c] = J->cp.x1 - J->cp.x0;
-  }
-}
-static void host_convert_chunk(const b2k_device_job* J, void* const* user, const uint32_t* strides, bool widen, size_t t0,
-                               size_t t1)
-{
-  const b2k_coding& cp = J->cp;
-  const uint32_t W = cp.x1 - cp.x0;
-  std::vector<b2k_host_rect> rects;
-  t1 = std::min(t1, J->tiles.size());
-  for(size_t ti = t0; ti < t1;)
-  {
-    Rect r = J->tile_rects[ti];
-    size_t tj = ti + 1;
-    while(tj < t1 && J->tile_rects[tj].y0 == r.y0 && J->tile_rects[tj].y1 == r.y1 && J->tile_rects[tj].x0 == r.x1)
-    {
-      r.x1 = J->tile_rects[tj].x1;
-      ++tj;
-    }
-    for(int c = 0; c < cp.numcomps; ++c)
-    {
-      int32_t* u = reinterpret_cast<int32_t*>(user[c]) + (size_t)(r.y0 - cp.y0) * strides[c] + (r.x0 - cp.x0);
-      uint16_t* s = J->h_stage16 + (uint64_t)c * J->stage16_elems + (size_t)(r.y0 - cp.y0) * W + (r.x0 - cp.x0);
-      if(widen)
-        rects.push_back({s, u, W, strides[c], r.w(), r.h()});
-      else
-        rects.push_back({u, s, strides[c], W, r.w(), r.h()});
-    }
-    ti = tj;
-  }
-  static const bool dbg = getenv("B2K_DEBUG_TIMING") != nullptr;
-  const auto t_a = std::chrono::steady_clock::now();
-  b2k_host_convert(rects.data(), rects.size(), widen, cp.sgnd != 0);
-  if(dbg)
-    fprintf(stderr, "[b2k] host %s tiles [%zu,%zu): %.3f ms\n", widen ? "widen" : "narrow", t0, t1,
-            std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_a).count());
-}
-
 /* ---- ring staging ---------------------------------------------------------------------------- */
 struct StagePiece
 {
@@ -1301,29 +1169,19 @@ struct RingGeom
 {
   uint32_t slot_mb, slots;
 };
-/* B2K_RING_ENC / B2K_RING_DEC = "<slot MB>,<slots>" ("0" = image-sized staging instead of a ring) */
+/* B2K_RING_ENC / B2K_RING_DEC = "<slot MB>,<slots>": slots of at least 1 MB, 2 to 16 of them */
 static RingGeom ring_geom(bool decode)
 {
-  static const RingGeom g[2] = {[] {
-                                  RingGeom r{8, 4};
-                                  if(const char* e = getenv("B2K_RING_ENC"))
-                                  {
-                                    r.slot_mb = (uint32_t)std::max(0, atoi(e));
-                                    if(const char* c = strchr(e, ','))
-                                      r.slots = (uint32_t)std::max(2, std::min(16, atoi(c + 1)));
-                                  }
-                                  return r;
-                                }(),
-                                [] {
-                                  RingGeom r{16, 4};
-                                  if(const char* e = getenv("B2K_RING_DEC"))
-                                  {
-                                    r.slot_mb = (uint32_t)std::max(0, atoi(e));
-                                    if(const char* c = strchr(e, ','))
-                                      r.slots = (uint32_t)std::max(2, std::min(16, atoi(c + 1)));
-                                  }
-                                  return r;
-                                }()};
+  auto parse = [](const char* name, RingGeom r) {
+    if(const char* e = getenv(name))
+    {
+      r.slot_mb = (uint32_t)std::max(1, atoi(e));
+      if(const char* c = strchr(e, ','))
+        r.slots = (uint32_t)std::max(2, std::min(16, atoi(c + 1)));
+    }
+    return r;
+  };
+  static const RingGeom g[2] = {parse("B2K_RING_ENC", {8, 4}), parse("B2K_RING_DEC", {16, 4})};
   return g[decode ? 1 : 0];
 }
 static int ensure_ring(b2k_device_job* J, bool decode)
@@ -1349,29 +1207,17 @@ static int ensure_ring(b2k_device_job* J, bool decode)
 }
 static void chunk_pieces(const b2k_device_job* J, uint32_t chunk, std::vector<StagePiece>& out)
 {
-  const b2k_coding& cp = J->cp;
-  const size_t t0 = J->chunk_tile[chunk], t1 = std::min<size_t>(J->chunk_tile[chunk + 1], J->tiles.size());
-  for(size_t ti = t0; ti < t1;)
-  {
-    Rect r = J->tile_rects[ti];
-    size_t tj = ti + 1;
-    while(tj < t1 && J->tile_rects[tj].y0 == r.y0 && J->tile_rects[tj].y1 == r.y1 && J->tile_rects[tj].x0 == r.x1)
-    {
-      r.x1 = J->tile_rects[tj].x1;
-      ++tj;
-    }
+  for_tile_row_runs(J, J->chunk_tile[chunk], J->chunk_tile[chunk + 1], nullptr, [&](const Rect& r) {
     const uint32_t rows_per = (uint32_t)std::max<uint64_t>(1, J->ring_slot_elems / r.w());
     for(uint32_t y = r.y0; y < r.y1; y += rows_per)
-      for(uint32_t c = 0; c < cp.numcomps; ++c)
+      for(uint32_t c = 0; c < J->cp.numcomps; ++c)
         out.push_back({chunk, c, r.x0, y, r.w(), std::min(rows_per, r.y1 - y)});
-    ti = tj;
-  }
+  });
 }
-/* narrow one chunk piece by piece into the ring and send each piece on its way */
-static int ring_upload_chunk(b2k_device_job* J, void* const* user, const uint32_t* strides, uint32_t chunk, cudaStream_t cs,
+/* narrow one chunk of the caller's int32 planes piece by piece into the ring and send each piece on its way to the staging */
+static int ring_upload_chunk(b2k_device_job* J, const Container& user, const Container& stage, uint32_t chunk, cudaStream_t cs,
                              uint64_t& counter, const std::function<int()>& between_pieces)
 {
-  const b2k_coding& cp = J->cp;
   std::vector<StagePiece> pcs;
   chunk_pieces(J, chunk, pcs);
   for(const StagePiece& pc : pcs)
@@ -1380,15 +1226,10 @@ static int ring_upload_chunk(b2k_device_job* J, void* const* user, const uint32_
     if(counter >= J->ring_slots)
       CUDA_TRY(cudaEventSynchronize(J->ring_ev[slot])); /* the slot's previous piece has left */
     uint16_t* sp = J->h_ring + (uint64_t)slot * J->ring_slot_elems;
-    const int32_t* u = reinterpret_cast<const int32_t*>(user[pc.comp]) + (size_t)(pc.y0 - cp.y0) * strides[pc.comp] + (pc.x0 - cp.x0);
-    const b2k_host_rect hr{u, sp, strides[pc.comp], pc.w, pc.w, pc.rows};
-    b2k_host_convert(&hr, 1, false, cp.sgnd != 0, true);
-    uint16_t* dev = J->img16.at(pc.comp, pc.x0, pc.y0);
-    if(J->img16.pitch == pc.w)
-      CUDA_TRY(cudaMemcpyAsync(dev, sp, (size_t)pc.w * pc.rows * 2, cudaMemcpyHostToDevice, cs));
-    else
-      CUDA_TRY(cudaMemcpy2DAsync(dev, (size_t)J->img16.pitch * 2, sp, (size_t)pc.w * 2, (size_t)pc.w * 2, pc.rows,
-                                 cudaMemcpyHostToDevice, cs));
+    const b2k_host_rect hr{user.at(pc.comp, pc.x0, pc.y0), sp, user.d.row_pitch[pc.comp], pc.w, pc.w, pc.rows};
+    b2k_host_convert(&hr, 1, false, J->cp.sgnd != 0, true);
+    CUDA_TRY(copy_rows(stage.at(pc.comp, pc.x0, pc.y0), (size_t)stage.d.row_pitch[pc.comp] * 2, sp, (size_t)pc.w * 2,
+                       (size_t)pc.w * 2, pc.rows, cudaMemcpyHostToDevice, cs));
     CUDA_TRY(cudaEventRecord(J->ring_ev[slot], cs));
     ++counter;
     if(between_pieces())
@@ -1396,11 +1237,10 @@ static int ring_upload_chunk(b2k_device_job* J, void* const* user, const uint32_
   }
   return 0;
 }
-/* bring every chunk's pixels down through the ring and widen them into the caller's planes; chunk k's pixels are
-   ready on the device when chunk_ev[CEV(0, k)] fires */
-static int ring_download_all(b2k_device_job* J, void* const* user, const uint32_t* strides, cudaStream_t cs)
+/* bring every chunk's pixels down from the staging through the ring and widen them into the caller's int32 planes; chunk
+   k's pixels are ready on the device when chunk_ev[CEV(0, k)] fires */
+static int ring_download_all(b2k_device_job* J, const Container& user, const Container& stage, cudaStream_t cs)
 {
-  const b2k_coding& cp = J->cp;
   std::vector<StagePiece> pcs;
   for(uint32_t k = 0; k + 1 < J->chunk_tile.size(); ++k)
     chunk_pieces(J, k, pcs);
@@ -1411,12 +1251,8 @@ static int ring_download_all(b2k_device_job* J, void* const* user, const uint32_
     uint16_t* sp = J->h_ring + (uint64_t)slot * J->ring_slot_elems;
     if(p == 0 || pcs[p - 1].chunk != pc.chunk)
       CUDA_TRY(cudaStreamWaitEvent(cs, J->chunk_ev[CEV(0, pc.chunk)], 0));
-    const uint16_t* dev = J->img16.at(pc.comp, pc.x0, pc.y0);
-    if(J->img16.pitch == pc.w)
-      CUDA_TRY(cudaMemcpyAsync(sp, dev, (size_t)pc.w * pc.rows * 2, cudaMemcpyDeviceToHost, cs));
-    else
-      CUDA_TRY(cudaMemcpy2DAsync(sp, (size_t)pc.w * 2, dev, (size_t)J->img16.pitch * 2, (size_t)pc.w * 2, pc.rows,
-                                 cudaMemcpyDeviceToHost, cs));
+    CUDA_TRY(copy_rows(sp, (size_t)pc.w * 2, stage.at(pc.comp, pc.x0, pc.y0), (size_t)stage.d.row_pitch[pc.comp] * 2,
+                       (size_t)pc.w * 2, pc.rows, cudaMemcpyDeviceToHost, cs));
     CUDA_TRY(cudaEventRecord(J->ring_ev[slot], cs));
     return 0;
   };
@@ -1428,13 +1264,93 @@ static int ring_download_all(b2k_device_job* J, void* const* user, const uint32_
     const uint32_t slot = (uint32_t)(p % S);
     CUDA_TRY(cudaEventSynchronize(J->ring_ev[slot]));
     const uint16_t* sp = J->h_ring + (uint64_t)slot * J->ring_slot_elems;
-    int32_t* u = reinterpret_cast<int32_t*>(user[pc.comp]) + (size_t)(pc.y0 - cp.y0) * strides[pc.comp] + (pc.x0 - cp.x0);
-    const b2k_host_rect hr{sp, u, pc.w, strides[pc.comp], pc.w, pc.rows};
-    b2k_host_convert(&hr, 1, true, cp.sgnd != 0);
+    const b2k_host_rect hr{sp, user.at(pc.comp, pc.x0, pc.y0), pc.w, user.d.row_pitch[pc.comp], pc.w, pc.rows};
+    b2k_host_convert(&hr, 1, true, J->cp.sgnd != 0);
     if(p + S < N)
       if(issue(p + S)) return -1;
   }
   return 0;
+}
+
+/* ---- one call's transport -------------------------------------------------------------------------------------- */
+/* How the samples of one b2k_encode* / b2k_decode* call travel between the caller and the engine's planes; settled before the
+   chunk pipeline starts (resolve_transport), so that the pipeline only asks for chunk k to be brought in or sent out */
+struct Transport
+{
+  Container user;               /* the caller's samples: host planes or pixels, or a device image */
+  const Rect* window = nullptr; /* b2k_decode_window / b2k_decode_device: only these pixels go back, and `user` holds them */
+  Container stage;              /* the 16-bit staging, when `staged` */
+  bool staged = false;          /* host copies go to / come from the staging, converted to / from the planes on the device */
+  bool ring = false;            /* int32 host planes packed on host threads, through the pinned ring into the staging */
+  uint64_t ring_pieces = 0;     /* pieces sent through the ring so far */
+  PackTuner* tuner = nullptr;   /* the tuner chose whether to pack; it hears how long the call took */
+  Transport() = default;
+  Transport(const Transport&) = delete;
+  ~Transport()
+  {
+    if(ring)
+      b2k_host_session(false);
+  }
+};
+
+/* T.user (and T.window) given: whether the call packs on host threads, by policy or tuner, and whether it goes through the
+   staging, which 16-bit host samples and packed ones do */
+static int resolve_transport(b2k_device_job* J, Transport& T, bool decode)
+{
+  if(T.user.device)
+    return 0;
+  if(T.user.d.sample_bytes == 4)
+  { /* several ranks on one host share its DRAM and CPU quota: measured (DESIGN.md section 4) packing loses there,
+       so the automatic policy only considers it for a process that has the host to itself */
+    const bool eligible = !T.window && host_pack_eligible(J);
+    const bool tuned = eligible && g_pack_policy.load() < 0 && b2k_host_local_peers() == 1;
+    PackTuner& tuner = decode ? J->tune_dec : J->tune_enc;
+    const bool pack = eligible && (tuned ? tuner.next_mode() : g_pack_policy.load() > 0);
+    g_last_pack[decode ? 1 : 0].store(pack ? 1 : 0);
+    T.tuner = tuned ? &tuner : nullptr;
+    if(!pack)
+      return 0;
+    if(ensure_ring(J, decode))
+      return -1;
+    T.ring = true;
+    b2k_host_session(true);
+  }
+  if(ensure_stage(J))
+    return -1;
+  T.stage = stage_container(J, T.user.interleaved);
+  T.staged = true;
+  return 0;
+}
+
+/* chunk k of the caller's host samples onto the device on the copy stream cs, and the compute stream st waits for it: packed
+   through the ring, or copied as they are into the staging or the planes.  between_pieces: host work slotted in between ring
+   pieces */
+static int upload_chunk(b2k_device_job* J, Transport& T, size_t k, cudaStream_t st, cudaStream_t cs,
+                        const std::function<int()>& between_pieces)
+{
+  if(T.ring ? ring_upload_chunk(J, T.user, T.stage, (uint32_t)k, cs, T.ring_pieces, between_pieces)
+            : copy_runs(J, T.staged ? T.stage : plane_container(J->img), T.user, cs, J->chunk_tile[k], J->chunk_tile[k + 1], nullptr))
+    return -1;
+  CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, k)], cs));
+  CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(0, k)], 0));
+  return 0;
+}
+
+/* chunk k's pixels out of the planes, once the compute stream st has them: into a device image by conversion on st; to the
+   host narrowed into the staging on st (when staged), then copied on the copy stream cs, or through the ring once every chunk
+   is queued (ring_download_all) */
+static int download_chunk(b2k_device_job* J, const Transport& T, size_t k, cudaStream_t st, cudaStream_t cs)
+{
+  const size_t t0 = J->chunk_tile[k], t1 = J->chunk_tile[k + 1];
+  if(T.user.device)
+    return device_convert(J, T.user, false, st, t0, t1, T.window);
+  if(T.staged && device_convert(J, T.stage, false, st, t0, t1, T.window))
+    return -1;
+  CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, k)], st));
+  if(T.ring)
+    return 0;
+  CUDA_TRY(cudaStreamWaitEvent(cs, J->chunk_ev[CEV(0, k)], 0));
+  return copy_runs(J, T.user, T.staged ? T.stage : plane_container(J->img), cs, t0, t1, T.window);
 }
 
 /* ---- stages ----------------------------------------------------------------------------------- */
@@ -2224,12 +2140,11 @@ static b2k_device_job* cached_job(b2k_engine* e, const b2k_coding* cp, uint32_t 
   return J;
 }
 
-/* dev: the samples are the caller's device image (b2k_encode_device), ordered after the work queued on `caller` */
-static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* planes, const uint32_t* strides,
-                             uint32_t mod, uint32_t rem, b2k_result** out, bool u16, bool interleaved = false,
-                             const b2k_device_planes* dev = nullptr, cudaStream_t caller = nullptr)
+/* T.user: the caller's samples.  A device image (b2k_encode_device) is read after the work queued on `caller` */
+static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, uint32_t rem, b2k_result** out, Transport& T,
+                             cudaStream_t caller = nullptr)
 {
-  if(!e || !cp || !out || (!dev && (!planes || !strides)))
+  if(!e || !cp || !out)
     return -1;
   std::lock_guard<std::mutex> lock(e->mu);
   int rc = 0;
@@ -2237,39 +2152,10 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* p
   if(rc)
     return rc;
   CUDA_TRY(cudaSetDevice(e->device));
-  void* const* user_planes = planes;
-  const uint32_t* user_strides = strides;
-  void* stage_planes[4];
-  uint32_t stage_strides[4];
-  /* several ranks on one host share its DRAM and CPU quota: measured (DESIGN.md section 4) packing loses there,
-     so the automatic policy only considers it for a process that has the host to itself */
-  const bool tuned = !dev && !u16 && host_pack_eligible(J) && g_pack_policy.load() < 0 && b2k_host_local_peers() == 1;
-  const bool pack = !dev && !u16 && host_pack_eligible(J) && (tuned ? J->tune_enc.next_mode() : g_pack_policy.load() > 0);
   const auto wall0 = std::chrono::steady_clock::now();
-  if(!dev && !u16)
-    g_last_pack[0].store(pack ? 1 : 0);
-  const bool ring = pack && ring_geom(false).slot_mb > 0;
-  uint64_t ring_counter = 0;
-  if(pack)
-  {
-    if(ring ? ensure_ring(J, false) : ensure_stage16(J)) return -1;
-    if(!ring)
-    {
-      stage16_views(J, stage_planes, stage_strides);
-      planes = stage_planes;
-      strides = stage_strides;
-    }
-    u16 = true;
-    b2k_host_session(true);
-  }
-  struct SessionEnd
-  {
-    bool on;
-    ~SessionEnd() { if(on) b2k_host_session(false); }
-  } session_end{pack};
-  if(u16)
-    if(int urc = interleaved ? ensure_ileave(J) : ensure_u16(J))
-      return urc;
+  if(resolve_transport(J, T, false))
+    return -1;
+  const bool dev = T.user.device;
   cudaStream_t st = e->stream;
   /* software pipeline over tile chunks: chunk k+1 crosses PCIe on the copy stream while chunk k
      is transformed and block-coded on the compute stream */
@@ -2338,31 +2224,12 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* p
   for(size_t k = 0; k < nchunks; ++k)
   {
     const size_t t0 = J->chunk_tile[k], t1 = J->chunk_tile[k + 1];
-    if(dev)
-    { /* the samples are on the device already: chunk k's conversion on the compute stream replaces its upload */
-      if(device_convert(J, *dev, true, st, t0, t1)) return -1;
-    }
-    else
-    {
-      if(ring)
-      {
-        if(ring_upload_chunk(J, user_planes, user_strides, (uint32_t)k, cs, ring_counter, [&] { return return_chunks(false); })) return -1;
-      }
-      else
-      {
-        if(pack)
-          host_convert_chunk(J, user_planes, user_strides, false, t0, t1); /* overlaps chunk k-1's H2D */
-        if(interleaved ? upload_interleaved(J, static_cast<const uint16_t*>(planes[0]), strides[0], cs, t0, t1)
-           : u16       ? copy_planes16(J, planes, strides, true, cs, t0, t1)
-                       : copy_planes(J, J->img, planes, strides, true, cs, t0, t1))
-          return -1;
-      }
-      CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, k)], cs));
-      CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(0, k)], 0));
-    }
+    /* a device image's chunk is converted on the compute stream in place of its upload */
+    if(dev ? device_convert(J, T.user, true, st, t0, t1, nullptr) : upload_chunk(J, T, k, st, cs, [&] { return return_chunks(false); }))
+      return -1;
     if(k == nchunks - 1)
       CUDA_TRY(cudaEventRecord(J->ev[1], st)); /* all planes on the device */
-    if(u16 && (interleaved ? split_interleaved(J, st, t0, t1) : convert_planes16(J, true, st, t0, t1))) return -1;
+    if(T.staged && device_convert(J, T.stage, true, st, t0, t1, nullptr)) return -1;
     if(enqueue_forward(J, st, k == 0, t0, t1)) return -1;
     if(enqueue_t1_blocks(J, st, t0, t1)) return -1;
     if(streamed)
@@ -2393,8 +2260,8 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* p
   if(streamed)
   {
     if(return_chunks(true)) return -1;
-    CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(4, 0)], ds));
-    CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(4, 0)], 0));
+    CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(3, 0)], ds));
+    CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(3, 0)], 0));
     DBG_T("encode: last chunk coded");
     J->bytes_used = total;
     if(overflow)
@@ -2435,22 +2302,46 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, void* const* p
   cudaEventElapsedTime(&d, J->ev[3], J->ev[6]);
   cudaEventElapsedTime(&J->last_level1_ms, J->ev[4], J->ev[5]);
   R->ms_h2d = a; R->ms_dwt = b; R->ms_t1 = c; R->ms_d2h = d; R->ms_total = a + b + c + d;
-  if(tuned)
-    J->tune_enc.record(pack, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count());
+  if(T.tuner)
+    T.tuner->record(T.ring, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count());
   *out = R;
   return 0;
+}
+
+/* the caller's planes in host memory, samples of 4 or 2 bytes, the first one at canvas (x0, y0) */
+static int32_t host_samples(Transport& T, const b2k_coding* cp, const void* const* planes, const uint32_t* strides, uint32_t sample_bytes,
+                            uint32_t x0, uint32_t y0)
+{
+  if(!planes || !strides)
+    return -1;
+  T.user = planar_container(cp->numcomps, const_cast<void* const*>(planes), strides, sample_bytes, x0, y0, false);
+  return 0;
+}
+/* the caller's device image, the first sample at canvas (x0, y0) */
+static void device_samples(Transport& T, const b2k_device_planes& img, uint32_t x0, uint32_t y0)
+{
+  T.user.d = img;
+  T.user.ox = x0;
+  T.user.oy = y0;
+  T.user.device = true;
 }
 
 extern "C" int32_t b2k_encode(b2k_engine* e, const b2k_coding* cp, const int32_t* const* planes, const uint32_t* strides,
                               uint32_t tile_mod, uint32_t tile_rem, b2k_result** out)
 {
-  return encode_common(e, cp, (void* const*)planes, strides, tile_mod, tile_rem, out, false);
+  Transport T;
+  if(!cp || host_samples(T, cp, (const void* const*)planes, strides, 4, cp->x0, cp->y0))
+    return -1;
+  return encode_common(e, cp, tile_mod, tile_rem, out, T);
 }
 
 extern "C" int32_t b2k_encode16(b2k_engine* e, const b2k_coding* cp, const uint16_t* const* planes, const uint32_t* strides,
                                 uint32_t tile_mod, uint32_t tile_rem, b2k_result** out)
 {
-  return encode_common(e, cp, (void* const*)planes, strides, tile_mod, tile_rem, out, true);
+  Transport T;
+  if(!cp || host_samples(T, cp, (const void* const*)planes, strides, 2, cp->x0, cp->y0))
+    return -1;
+  return encode_common(e, cp, tile_mod, tile_rem, out, T);
 }
 
 extern "C" int32_t b2k_encode16_interleaved(b2k_engine* e, const b2k_coding* cp, const uint16_t* pixels, uint32_t stride,
@@ -2458,29 +2349,32 @@ extern "C" int32_t b2k_encode16_interleaved(b2k_engine* e, const b2k_coding* cp,
 {
   if(!cp || !pixels || stride < (uint32_t)(cp->x1 - cp->x0) * cp->numcomps)
     return -1;
-  void* planes[4] = {const_cast<uint16_t*>(pixels), nullptr, nullptr, nullptr};
-  const uint32_t strides[4] = {stride, 0, 0, 0};
-  return encode_common(e, cp, planes, strides, tile_mod, tile_rem, out, true, true);
+  Transport T;
+  T.user = interleaved_container(cp->numcomps, const_cast<uint16_t*>(pixels), stride, 2, cp->x0, cp->y0, false);
+  return encode_common(e, cp, tile_mod, tile_rem, out, T);
 }
 
 static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
-                             const uint8_t* bytes, uint64_t num_bytes, void* const* planes, const uint32_t* strides,
-                             uint32_t tile_mod, uint32_t tile_rem, double* ms_total, bool u16, const uint32_t* crop = nullptr,
-                             const b2k_device_planes* dev = nullptr, cudaStream_t caller = nullptr);
+                             const uint8_t* bytes, uint64_t num_bytes, uint32_t tile_mod, uint32_t tile_rem, double* ms_total,
+                             Transport& T, const uint32_t* window = nullptr, cudaStream_t caller = nullptr);
 
 extern "C" int32_t b2k_decode(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
                               const uint8_t* bytes, uint64_t num_bytes, int32_t* const* planes, const uint32_t* strides,
                               uint32_t tile_mod, uint32_t tile_rem, double* ms_total)
 {
-  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, (void* const*)planes, strides, tile_mod, tile_rem,
-                       ms_total, false);
+  Transport T;
+  if(!cp || host_samples(T, cp, (const void* const*)planes, strides, 4, cp->x0, cp->y0))
+    return -1;
+  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, tile_mod, tile_rem, ms_total, T);
 }
 extern "C" int32_t b2k_decode16(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
                                 const uint8_t* bytes, uint64_t num_bytes, uint16_t* const* planes, const uint32_t* strides,
                                 uint32_t tile_mod, uint32_t tile_rem, double* ms_total)
 {
-  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, (void* const*)planes, strides, tile_mod, tile_rem,
-                       ms_total, true);
+  Transport T;
+  if(!cp || host_samples(T, cp, (const void* const*)planes, strides, 2, cp->x0, cp->y0))
+    return -1;
+  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, tile_mod, tile_rem, ms_total, T);
 }
 
 /* b2k_decode / b2k_decode16 with only `window` (x0, y0, x1, y1 in cp's canvas coordinates) of the pixels returned: planes[c]
@@ -2490,9 +2384,11 @@ extern "C" int32_t b2k_decode_window(b2k_engine* e, const b2k_coding* cp, const 
                                      const uint8_t* bytes, uint64_t num_bytes, void* const* planes, const uint32_t* strides,
                                      const uint32_t* window, uint32_t sample_bytes, double* ms_total)
 {
-  if(!window || (sample_bytes != 2 && sample_bytes != 4))
+  Transport T;
+  if(!cp || !window || (sample_bytes != 2 && sample_bytes != 4) ||
+     host_samples(T, cp, (const void* const*)planes, strides, sample_bytes, window[0], window[1]))
     return -1;
-  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, planes, strides, 1, 0, ms_total, sample_bytes == 2, window);
+  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, 1, 0, ms_total, T, window);
 }
 
 /* NULL is the legacy default stream, as the CUDA Array Interface assumes */
@@ -2505,7 +2401,9 @@ extern "C" int32_t b2k_encode_device(b2k_engine* e, const b2k_coding* cp, const 
     return -1;
   if(int rc = check_device_planes(e, cp, img))
     return rc;
-  return encode_common(e, cp, nullptr, nullptr, tile_mod, tile_rem, out, false, false, img, caller_stream(cuda_stream));
+  Transport T;
+  device_samples(T, *img, cp->x0, cp->y0);
+  return encode_common(e, cp, tile_mod, tile_rem, out, T, caller_stream(cuda_stream));
 }
 
 extern "C" int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
@@ -2521,18 +2419,21 @@ extern "C" int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const 
   }
   if(int rc = check_device_planes(e, cp, img))
     return rc;
-  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, nullptr, nullptr, tile_mod, tile_rem, ms_total, false, window, img,
-                       caller_stream(cuda_stream));
+  Transport T;
+  device_samples(T, *img, window ? window[0] : cp->x0, window ? window[1] : cp->y0);
+  return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, tile_mod, tile_rem, ms_total, T, window, caller_stream(cuda_stream));
 }
 
+/* T.user: the caller's samples, which hold only `window` (x0, y0, x1, y1) of the pixels when there is one.  A device image
+   (b2k_decode_device) is written after the work queued on `caller` */
 static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
-                             const uint8_t* bytes, uint64_t num_bytes, void* const* planes, const uint32_t* strides,
-                             uint32_t tile_mod, uint32_t tile_rem, double* ms_total, bool u16, const uint32_t* crop,
-                             const b2k_device_planes* dev, cudaStream_t caller)
+                             const uint8_t* bytes, uint64_t num_bytes, uint32_t tile_mod, uint32_t tile_rem, double* ms_total,
+                             Transport& T, const uint32_t* window, cudaStream_t caller)
 {
-  if(!e || !cp || !blocks || (!dev && (!planes || !strides)))
+  if(!e || !cp || !blocks)
     return -1;
-  if(crop && (crop[0] >= crop[2] || crop[1] >= crop[3] || crop[0] < cp->x0 || crop[1] < cp->y0 || crop[2] > cp->x1 || crop[3] > cp->y1))
+  if(window &&
+     (window[0] >= window[2] || window[1] >= window[3] || window[0] < cp->x0 || window[1] < cp->y0 || window[2] > cp->x1 || window[3] > cp->y1))
   {
     g_err = "window outside the image";
     return -1;
@@ -2543,47 +2444,12 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
   if(rc)
     return rc;
   CUDA_TRY(cudaSetDevice(e->device));
-  /* a window: only its pixels cross PCIe on the way back, into planes of the window's size (copy_planes / copy_planes16) */
-  J->has_crop = crop != nullptr;
-  if(crop)
-    J->crop = Rect{crop[0], crop[1], crop[2], crop[3]};
-  struct CropEnd
-  {
-    b2k_device_job* j;
-    ~CropEnd() { j->has_crop = false; }
-  } crop_end{J};
-  void* const* user_planes = planes;
-  const uint32_t* user_strides = strides;
-  void* stage_planes[4];
-  uint32_t stage_strides[4];
-  /* several ranks on one host share its DRAM and CPU quota: measured (DESIGN.md section 4) packing loses there,
-     so the automatic policy only considers it for a process that has the host to itself */
-  const bool tuned = !dev && !crop && !u16 && host_pack_eligible(J) && g_pack_policy.load() < 0 && b2k_host_local_peers() == 1;
-  const bool pack = !dev && !crop && !u16 && host_pack_eligible(J) && (tuned ? J->tune_dec.next_mode() : g_pack_policy.load() > 0);
+  const Rect win = window ? Rect{window[0], window[1], window[2], window[3]} : Rect{};
+  T.window = window ? &win : nullptr;
   const auto wall0 = std::chrono::steady_clock::now();
-  if(!dev && !u16)
-    g_last_pack[1].store(pack ? 1 : 0);
-  const bool ring = pack && ring_geom(true).slot_mb > 0;
-  if(pack)
-  {
-    if(ring ? ensure_ring(J, true) : ensure_stage16(J)) return -1;
-    if(!ring)
-    {
-      stage16_views(J, stage_planes, stage_strides);
-      planes = stage_planes;
-      strides = stage_strides;
-    }
-    u16 = true;
-    b2k_host_session(true);
-  }
-  struct SessionEnd
-  {
-    bool on;
-    ~SessionEnd() { if(on) b2k_host_session(false); }
-  } session_end{pack};
-  if(u16)
-    if(int urc = ensure_u16(J))
-      return urc;
+  if(resolve_transport(J, T, true))
+    return -1;
+  const bool dev = T.user.device;
   cudaStream_t st = e->stream;
   if(num_bytes + 64 > J->bytes_cap)
   {
@@ -2663,32 +2529,10 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
                                     (J->cp.cblk_sty & 0x08) != 0, st);
     }
     if(enqueue_inverse(J, st, t0, t1)) return -1;
-    if(dev)
-    { /* into the caller's device image instead of down to the host */
-      if(device_convert(J, *dev, false, st, t0, t1)) return -1;
-      continue;
-    }
-    if(u16 && convert_planes16(J, false, st, t0, t1)) return -1;
-    CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, k)], st));
-    if(ring)
-      continue; /* pixels come down piece by piece below */
-    CUDA_TRY(cudaStreamWaitEvent(cs, J->chunk_ev[CEV(0, k)], 0));
-    if(u16 ? copy_planes16(J, planes, strides, false, cs, t0, t1) : copy_planes(J, J->img, planes, strides, false, cs, t0, t1))
-      return -1;
-    if(pack)
-      CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(3, k)], cs));
+    if(download_chunk(J, T, k, st, cs)) return -1;
   }
   DBG_T("decode: chunks enqueued");
-  if(ring)
-  {
-    if(ring_download_all(J, user_planes, user_strides, cs)) return -1;
-  }
-  else if(pack) /* widen chunk k into the caller's planes while chunk k+1 is still coming down */
-    for(size_t k = 0; k < nchunks; ++k)
-    {
-      CUDA_TRY(cudaEventSynchronize(J->chunk_ev[CEV(3, k)]));
-      host_convert_chunk(J, user_planes, user_strides, true, J->chunk_tile[k], J->chunk_tile[k + 1]);
-    }
+  if(T.ring && ring_download_all(J, T.user, T.stage, cs)) return -1;
   CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, nchunks)], cs));
   CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(0, nchunks)], 0));
   CUDA_TRY(cudaEventRecord(J->ev[1], st));
@@ -2703,8 +2547,8 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
   float t = 0;
   cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
   if(ms_total) *ms_total = t;
-  if(tuned)
-    J->tune_dec.record(pack, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count());
+  if(T.tuner)
+    T.tuner->record(T.ring, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count());
   int herr = 0;
   CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
   if(herr)

@@ -567,12 +567,29 @@ def test_corrupt_streams_are_rejected_or_decoded_never_fatal(engine):
         assert np.array_equal(a, s)
 
 
-@pytest.mark.parametrize("sgnd", [False, True])
-def test_host_packing_matches_direct_copies(engine, sgnd):
+@pytest.mark.parametrize("sgnd, ring", [(False, None), (True, None), (False, "1,2"), (True, "1,2")],
+                         ids=["False", "True", "False-ring", "True-ring"])
+def test_host_packing_matches_direct_copies(engine, sgnd, ring):
     """int32 entry points with host packing forced on (16-bit PCIe containers through the pinned ring, host
     thread pool) against the same calls with packing off: same coded bytes, same pixels, lossless -- on a
     geometry with ragged tiles, an odd canvas origin and (second case) signed samples, large enough
-    (>= 4 Msamples, several pipeline chunks) for the packed path to be taken, with unpinned caller planes."""
+    (>= 4 Msamples, several pipeline chunks) for the packed path to be taken, with unpinned caller planes.
+    ring: B2K_RING_ENC / B2K_RING_DEC set to two 1 MB slots, so that every chunk row travels in many pieces; the
+    library reads them once per process, so that case runs in a subprocess."""
+    if ring is None:
+        _host_packing_case(engine, sgnd)
+        return
+    import os, subprocess, sys
+    here = os.path.dirname(os.path.abspath(__file__))
+    env = dict(os.environ, B2K_RING_ENC=ring, B2K_RING_DEC=ring,
+               PYTHONPATH=os.pathsep.join([os.path.dirname(here), here, os.environ.get("PYTHONPATH", "")]))
+    code = "import grok_b200 as G, test_gpu\ne = G.Engine(0)\ntest_gpu._host_packing_case(e, %r)\ne.close()\n" % sgnd
+    p = subprocess.run([sys.executable, "-c", code], env=env, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True,
+                       timeout=900)
+    assert p.returncode == 0, p.stdout[-3000:] + p.stderr[-3000:]
+
+
+def _host_packing_case(engine, sgnd):
     w, h, prec = 2501, 1803, (16 if sgnd else 12)
     cp = G.make_coding(w, h, 3, prec, sgnd=sgnd, numres=5, tile=(700, 500), origin=(3, 5), numgbits=2 if sgnd else 1)
     planes = P.synthetic_image(w, h, 3, prec, seed=11, origin=(3, 5))
@@ -601,6 +618,27 @@ def test_host_packing_matches_direct_copies(engine, sgnd):
         G.set_host_threads(-1)
     assert np.array_equal(results["direct"][1], results["packed"][1])
     assert np.array_equal(results["direct"][0]["length"], results["packed"][0]["length"])
+
+
+@pytest.mark.parametrize("irreversible", [False, True])
+def test_decode_window_16bit_matches_int32(engine, irreversible):
+    """b2k_decode_window into 16-bit planes returns exactly the samples of the same window in int32 planes: the whole
+    image, one pixel, and windows that start and end inside tiles or on tile edges, on a tiled image with an odd origin,
+    at full and half resolution."""
+    w, h, origin = 700, 500, (5, 11)      # the tile grid starts at 0, so that reduce=1 windows may span several tiles
+    cp = G.make_coding(w, h, 3, 12, numres=5, tile=(256, 192), origin=origin, tile_origin=(0, 0), irreversible=irreversible)
+    planes = P.synthetic_image(w, h, 3, 12, seed=23, origin=origin)
+    cs = engine.encode_codestream(cp, planes)
+    windows = [(5, 11, 705, 511), (100, 50, 101, 51), (37, 200, 650, 333), (256, 192, 512, 384), (261, 11, 517, 203),
+               (300, 300, 705, 511), (6, 12, 704, 510)]
+    for reduce in (0, 1):
+        for win in windows:
+            _, want = engine.decode_window(cs, win, reduce)
+            want = [p.copy() for p in want]
+            _, got = engine.decode_window(cs, win, reduce, dtype=np.uint16)
+            for g, r in zip(got, want):
+                assert g.dtype == np.uint16 and g.shape == r.shape, (win, reduce)
+                assert np.array_equal(g.astype(np.int32), r), (win, reduce)
 
 
 @pytest.mark.parametrize("irreversible", [False, True])

@@ -6,9 +6,12 @@
 
 Each run writes, per case, the forward coefficients, the coded bytes and block lengths and the planes that inverse()
 rebuilds from them, as .npy files under OUT.  Cases: tests/test_gpu.py's GEOMS, reversible and irreversible (shapes whose
-coding the engine refuses are skipped), the 9/7 degenerate-geometry shapes, a 2048^2 single-tile 9/7 image, and one
-b2k_encode16 / b2k_decode16 round trip.  --compare exits 1 when any array differs; tolerances would hide a drift of
-one rounding step in the 9/7 inverse, so there are none."""
+coding the engine refuses are skipped), the 9/7 degenerate-geometry shapes, a 2048^2 single-tile 9/7 image, and the
+sample transports of the one-call entry points: a b2k_encode16 / b2k_decode16 round trip, b2k_encode16_interleaved,
+b2k_encode / b2k_decode with host packing forced on, 16-bit windowed decodes (b2k_decode_window), and, where torch has
+CUDA, b2k_encode_device / b2k_decode_device with uint16 tensors.  Every one-call entry point except the windowed decode
+also stores b2k_launch_count() before and after the call.  --compare exits 1 when any array differs; tolerances would
+hide a drift of one rounding step in the 9/7 inverse, so there are none."""
 import os
 import sys
 
@@ -67,17 +70,69 @@ def run(outdir):
             continue
         for k, a in arrs.items():
             np.save(os.path.join(outdir, "%s.%s.npy" % (name, k)), a)
-    # 16-bit containers: b2k_encode16 / b2k_decode16
+    arrs = {}
+
+    def counted(name, fn):
+        before = int(G.lib().b2k_launch_count())
+        r = fn()
+        arrs[name + "_launches"] = np.array([before, int(G.lib().b2k_launch_count())], np.uint64)
+        return r
+
+    def keep(name, res):
+        arrs[name + "_bytes"], arrs[name + "_lengths"] = res.bytes.copy(), res.blocks["length"].copy()
+        res.free()
+
+    # 16-bit containers: b2k_encode16 / b2k_decode16, and the same pixels interleaved (b2k_encode16_interleaved)
     cp = G.make_coding(600, 300, 3, 12, numres=5, tile=(256, 128), origin=(8, 0))
     p16 = [p.astype(np.uint16) for p in P.synthetic_image(600, 300, 3, 12, seed=77)]
-    res = eng.encode(cp, p16)
+    res = counted("u16_enc", lambda: eng.encode(cp, p16))
+    blocks, data = res.blocks.copy(), res.bytes.copy()
+    keep("u16", res)
     rec = [np.zeros_like(p) for p in p16]
-    eng.decode(cp, res.blocks.copy(), res.bytes.copy(), rec)
-    arrs = {"bytes": res.bytes.copy(), "lengths": res.blocks["length"].copy()}
-    arrs.update(("rec%d" % c, a) for c, a in enumerate(rec))
-    res.free()
+    counted("u16_dec", lambda: eng.decode(cp, blocks, data, rec))
+    arrs.update(("u16_rec%d" % c, a) for c, a in enumerate(rec))
+    keep("u16_interleaved", counted("u16_interleaved", lambda: eng.encode_interleaved(cp, np.ascontiguousarray(np.stack(p16, -1)))))
+    # int32 planes through the host-packing ring: large enough (>= 4 Msamples, several chunks) to be packed
+    w, h = 2501, 1803
+    cp = G.make_coding(w, h, 3, 12, numres=5, tile=(700, 500), origin=(3, 5))
+    planes = P.synthetic_image(w, h, 3, 12, seed=11, origin=(3, 5))
+    G.set_host_threads(3)
+    try:
+        res = counted("packed_enc", lambda: eng.encode(cp, planes))
+        blocks, data = res.blocks.copy(), res.bytes.copy()
+        keep("packed", res)
+        rec = [np.zeros_like(p) for p in planes]
+        counted("packed_dec", lambda: eng.decode(cp, blocks, data, rec))
+        arrs["packed_used"] = np.array(G.host_pack_last())
+        arrs.update(("packed_rec%d" % c, a) for c, a in enumerate(rec))
+    finally:
+        G.set_host_threads(-1)
+    # b2k_encode_device / b2k_decode_device from and into uint16 tensors, planar and pixel-interleaved
+    try:
+        import torch
+        cuda = torch.cuda.is_available()
+    except ImportError:
+        cuda = False
+    if cuda:
+        cp = G.make_coding(600, 300, 3, 12, numres=5, tile=(256, 128), origin=(8, 0))
+        chw = torch.from_numpy(np.stack(p16)).cuda()
+        for layout, img in (("CHW", chw), ("HWC", chw.permute(1, 2, 0).contiguous())):
+            res = counted("dev_%s_enc" % layout, lambda: eng.encode_device(cp, img, layout=layout))
+            blocks, data = res.blocks.copy(), res.bytes.copy()
+            keep("dev_%s" % layout, res)
+            out = torch.zeros_like(img)
+            counted("dev_%s_dec" % layout, lambda: eng.decode_device(cp, blocks, data, out, layout=layout))
+            torch.cuda.synchronize()
+            arrs["dev_%s_rec" % layout] = out.cpu().numpy()
+    # 16-bit windowed decodes of a tiled image with an odd origin, at full and half resolution
+    cp = G.make_coding(700, 500, 3, 12, numres=5, tile=(256, 192), origin=(5, 11), tile_origin=(0, 0), irreversible=True)
+    cs = eng.encode_codestream(cp, P.synthetic_image(700, 500, 3, 12, seed=23, origin=(5, 11)))
+    for i, win in enumerate([(5, 11, 705, 511), (37, 200, 650, 333), (261, 11, 517, 203)]):
+        for reduce in (0, 1):
+            _, got = eng.decode_window(cs, win, reduce, dtype=np.uint16)
+            arrs.update(("win%d_r%d_rec%d" % (i, reduce, c), g.copy()) for c, g in enumerate(got))
     for k, a in arrs.items():
-        np.save(os.path.join(outdir, "u16.%s.npy" % k), a)
+        np.save(os.path.join(outdir, "transport.%s.npy" % k), a)
     eng.close()
     print("wrote %d arrays to %s" % (len(os.listdir(outdir)), outdir))
 
