@@ -957,6 +957,9 @@ static int ensure_stage(b2k_device_job* J)
   const size_t bytes = std::max(cp.numcomps * stage_plane_elems(cp), (size_t)stage_pitch(cp, true) * (cp.y1 - cp.y0)) * sizeof(uint16_t);
   CUDA_TRY(cudaMalloc(&J->d_stage, bytes));
   CUDA_TRY(cudaMemset(J->d_stage, 0, bytes));
+  /* cudaMemset runs on the legacy default stream, which the engine's non-blocking streams do not wait for: without this
+     wait the zeroing could land after the first chunk of the call that allocated the staging had been copied into it */
+  CUDA_TRY(cudaStreamSynchronize(0));
   return 0;
 }
 

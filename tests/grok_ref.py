@@ -70,15 +70,15 @@ def init(threads=0, plugin_path=None, device_id=0):
 
 
 def compress(planes, prec, sgnd=False, tile=None, numres=6, irreversible=False, mct=None, ht=True, tlm=False, plt=False,
-             cblk=(64, 64), device_id=-1, precinct=None, out=None):
-    """-> (codestream bytes as np.uint8 array, seconds inside grk_compress())"""
+             cblk=(64, 64), device_id=-1, precinct=None, numgbits=0, out=None):
+    """-> (codestream bytes as np.uint8 array, seconds inside grk_compress()).  numgbits 0: the mode's default"""
     planes = [np.ascontiguousarray(p, dtype=np.int32) for p in planes]
     h, w = planes[0].shape
     n = len(planes)
     p = Params(w=w, h=h, ncomp=n, prec=prec, sgnd=int(sgnd), tile_w=tile[0] if tile else 0, tile_h=tile[1] if tile else 0,
                numres=numres, cblk_w=cblk[0], cblk_h=cblk[1], irreversible=int(irreversible),
                mct=int(n >= 3 if mct is None else mct), ht=int(ht), tlm=int(tlm), plt=int(plt), device_id=device_id,
-               numgbits=0, prc_w=precinct[0] if precinct else 0, prc_h=precinct[1] if precinct else 0)
+               numgbits=numgbits, prc_w=precinct[0] if precinct else 0, prc_h=precinct[1] if precinct else 0)
     cap = w * h * n * 4 + (1 << 20)
     if out is None or out.size < cap:
         out = np.empty(cap, np.uint8)
