@@ -374,7 +374,7 @@ def _run_pipeline_job(job, cp, planes, ref, lo, hi):
     wide = inverse97_unclamped(cp, dec)
     checked = 0
     for c, (g, r, u, s) in enumerate(zip(rec, oracle_rec, wide, planes)):
-        assert np.abs(g - r).max() <= 1, "component %d" % c
+        assert np.array_equal(g, r), "component %d: %d samples differ from the oracle's inverse" % (c, int((g != r).sum()))
         assert g.min() >= lo and g.max() <= hi, "component %d outside [%d, %d]" % (c, lo, hi)
         over, under = u >= hi + 1, u <= lo - 1
         assert np.all(g[over] == hi) and np.all(g[under] == lo), "component %d: the clamp is off" % c
