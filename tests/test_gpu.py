@@ -518,8 +518,18 @@ def test_corrupt_streams_are_rejected_or_decoded_never_fatal(engine):
     """Damaged block tables / byte arenas (flipped bytes, garbage Scup, wrong lengths, impossible bit-plane
     counts, bogus refinement segments): b2k_decode either decodes or reports rejected blocks (-2) or a bad
     table (-1); it never faults, and the engine decodes a clean stream right afterwards."""
+    _corrupt_streams_case(engine, (64, 64))
+
+
+def test_corrupt_streams_in_wide_blocks_are_rejected_or_decoded_never_fatal(engine):
+    """The same damage with 1024x4 code blocks: the image's bands give blocks up to 128 wide, so the damaged
+    tables and arenas reach the parse of blocks wider than 64 (k_ht_decode_vlc<true>)."""
+    _corrupt_streams_case(engine, (1024, 4))
+
+
+def _corrupt_streams_case(engine, cblk):
     w, h = 256, 192
-    cp = G.make_coding(w, h, 3, 12, numres=4)
+    cp = G.make_coding(w, h, 3, 12, numres=4, cblk=cblk)
     planes = P.synthetic_image(w, h, 3, 12, seed=5)
     res = engine.encode(cp, planes)
     blocks, data = res.blocks.copy(), res.bytes.copy()
