@@ -11,7 +11,7 @@
  *             DecompressRev / DecompressIrrev         point_transform/mct.cpp L201-256, L318-391
  *
  * Design (not a port of the column-strip SIMD loops):
- *   - one warp = one job = (tile component(s), 8*strip_w-column strip, row segment).  Each lane
+ *   - one warp = one job = (tile component(s), column strip, row segment).  Each lane
  *     owns 8 consecutive canvas columns (two 128-bit loads per row).  The reference's
  *     "all columns, then all rows" double pass is fused: rows stream through a register
  *     sliding window for the vertical lifting, every finished vertical row is lifted
@@ -19,8 +19,10 @@
  *     sub-bands are written once, de-interleaved, with 128-bit stores.  HBM traffic per level is
  *     one read + one write of every coefficient: the algorithmic minimum.
  *   - symmetric extension is implemented in the LOADS (mirrored addresses), so the lifting
- *     code has no boundary cases; lanes 0 and 31 are halo lanes (recompute instead of
- *     cross-warp exchange), row segments recompute 3 (5/3) or 7 (9/7) halo rows.
+ *     code has no boundary cases.  Neighbours outside the warp are recomputed instead of
+ *     exchanged: 5/3 strips are 256 columns wide, all 32 lanes own, and the few columns the
+ *     edge lanes need from outside arrive as ghost columns (GhostCol / GhostBand); 9/7 strips
+ *     keep lanes 0 and 31 as halo lanes.  Row segments recompute 3 (5/3) or 7 (9/7) halo rows.
  *   - integer maths is bit-exact with the reference; 9/7 uses fmaf() where the reference build
  *     contracts to FMA (see oracle/j2k_oracle.c fwd97_line) and explicit _rn intrinsics elsewhere.
  */
@@ -102,6 +104,10 @@ struct Job
   int lane, ulane, jbeg, jend, wn, hn, nvalid;
   bool owner, need;
 };
+/* WHOLE (5/3): whole-warp strips of 256 columns, lane L owns columns x0 + 8L .. x0 + 8L + 7 and the neighbours outside the
+   warp arrive as ghost columns.  Otherwise (9/7): lane 0 is the left halo lane, lanes 1 .. strip_w/8 own, the next is the
+   right halo.  `need`: the lane's samples feed an owner (its own, or the right neighbour of the line's last owner). */
+template <bool WHOLE>
 __device__ __forceinline__ bool decode_job(const DwtLevelDesc& D, Job& J)
 {
   J.lane = threadIdx.x & 31;
@@ -109,12 +115,13 @@ __device__ __forceinline__ bool decode_job(const DwtLevelDesc& D, Job& J)
   if(job >= (int)D.nstrips * (int)D.nsegs)
     return false;
   const int strip = job % D.nstrips, seg = job / D.nstrips;
+  constexpr int halo = WHOLE ? 0 : 1;
   J.wn = D.u1 - D.u0;
   J.hn = D.v1 - D.v0;
   J.nvalid = D.strip_w >> 3;
-  J.ulane = (D.u0 & ~7) + strip * (int)D.strip_w + (J.lane - 1) * 8;
-  J.owner = J.lane >= 1 && J.lane <= J.nvalid && J.ulane < D.u1;
-  J.need = J.lane <= J.nvalid + 1 && J.ulane < D.u1 + 8;
+  J.ulane = (D.u0 & ~7) + strip * (int)D.strip_w + (J.lane - halo) * 8;
+  J.owner = J.lane >= halo && J.lane < J.nvalid + halo && J.ulane < D.u1;
+  J.need = J.lane <= J.nvalid + halo && J.ulane < D.u1 + 8;
   const int jlo = D.v0 >> 1, jhi = (D.v1 - 1) >> 1;
   J.jbeg = jlo + seg * (int)D.pairs_per_seg;
   J.jend = min(J.jbeg + (int)D.pairs_per_seg, jhi + 1);
@@ -237,11 +244,11 @@ __device__ __forceinline__ void fetch_int_rows(const DwtLevelDesc& D, const Job&
 }
 
 /* a fetched row -> the values the 5/3 lifting starts from */
-template <int NC>
-__device__ __forceinline__ void to_coeffs53(const DwtLevelDesc& D, int (&x)[NC][8])
+template <int NC, int N>
+__device__ __forceinline__ void to_coeffs53(const DwtLevelDesc& D, int (&x)[NC][N])
 {
   if(D.first_level)
-    rct_fwd<NC>(D, x);
+    rct_fwd<NC, N>(D, x);
 }
 
 /* a fetched row -> the values the 9/7 lifting starts from; the float conversion of the finest level
@@ -265,6 +272,36 @@ template <int NC>
 __device__ __forceinline__ void fetch53(const DwtLevelDesc& D, const Job& J, int v, int (&out)[NC][8])
 {
   fetch_int_rows<NC>(D, J, v, out);
+  to_coeffs53<NC>(D, out);
+}
+
+/* ---- ghost columns of a whole-warp 5/3 strip (forward) ----------------------------------------------------------------
+ * The horizontal lifting of lane 0 needs the vertically lifted columns x0-2 and x0-1, lane 31 needs x0+256 (x0 = the
+ * strip's first column).  Lane 0 carries column x0-1, lane 1 column x0-2 and lane 31 column x0+256 through the same
+ * vertical lifting as its body (one extra column per lane, mirrored address: the extension stays in the loads); a
+ * shuffle hands lane 1's result to lane 0.  The other lanes carry a copy of their own first column, which nobody uses. */
+struct GhostCol
+{
+  int col;    /* mirrored column, relative to u0 */
+  int slot;   /* 0, 1, 2 for lanes 0, 1, 31; -1: no ghost */
+};
+__device__ __forceinline__ GhostCol ghost_col(const DwtLevelDesc& D, const Job& J)
+{
+  const int x0 = J.ulane - 8 * J.lane;
+  GhostCol G;
+  G.slot = J.lane == 0 ? 0 : J.lane == 1 ? 1 : J.lane == 31 ? 2 : -1;
+  const int x = J.lane == 0 ? x0 - 1 : J.lane == 1 ? x0 - 2 : J.lane == 31 ? x0 + 256 : J.ulane;
+  G.col = mirror_rel(x - D.u0, J.wn);
+  return G;
+}
+/* the ghost column of canvas row v, unstaged (degenerate jobs and the first even row of a segment) */
+template <int NC>
+__device__ __forceinline__ void fetch_ghost53(const DwtLevelDesc& D, const Job& J, const GhostCol& G, int v, int (&out)[NC][1])
+{
+  const int r = mirror_rel(v - D.v0, J.hn);
+#pragma unroll
+  for(int c = 0; c < NC; ++c)
+    out[c][0] = __ldg(reinterpret_cast<const int32_t*>(D.in[c]) + (size_t)r * D.in_pitch + G.col);
   to_coeffs53<NC>(D, out);
 }
 
@@ -365,15 +402,21 @@ __device__ __forceinline__ void store_rows(const DwtLevelDesc& D, const BandGeom
 }
 
 /* ---- horizontal lifting of one row held as 8 values per lane -------------------------------- */
+/* g: the lane's ghost column of the same row (see GhostCol); lanes 0 and 31 take their outer neighbours from the ghosts
+   by selects, so every lane runs the same instructions */
 template <bool DEGEN = true>
-__device__ __forceinline__ void hfwd53(const int (&r)[8], int wn, int (&lo)[4], int (&hi)[4])
+__device__ __forceinline__ void hfwd53(const int (&r)[8], int g, int wn, int (&lo)[4], int (&hi)[4])
 {
-  const int en = __shfl_down_sync(0xffffffffu, r[0], 1);
+  const int lane = threadIdx.x & 31;
+  const int g2 = __shfl_down_sync(0xffffffffu, g, 1); /* lane 0: column x0-2 */
+  const int rn = __shfl_down_sync(0xffffffffu, r[0], 1);
+  const int en = lane == 31 ? g : rn;
   hi[0] = r[1] - ((r[0] + r[2]) >> 1);
   hi[1] = r[3] - ((r[2] + r[4]) >> 1);
   hi[2] = r[5] - ((r[4] + r[6]) >> 1);
   hi[3] = r[7] - ((r[6] + en) >> 1);
-  const int dp = __shfl_up_sync(0xffffffffu, hi[3], 1);
+  const int hp = __shfl_up_sync(0xffffffffu, hi[3], 1);
+  const int dp = lane == 0 ? g - ((g2 + r[0]) >> 1) : hp;
   lo[0] = r[0] + ((dp + hi[0] + 2) >> 2);
   lo[1] = r[2] + ((hi[0] + hi[1] + 2) >> 2);
   lo[2] = r[4] + ((hi[1] + hi[2] + 2) >> 2);
@@ -495,8 +538,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity)
  * the per-warp staging pipeline of all four DWT kernels: each warp owns DWT_STAGES shared-memory
  * slots of one row pair (Stage::PAIRB bytes), plus one mbarrier per slot, so DWT_STAGES-1 row pairs
  * are in flight while one is lifted, without holding registers.  Pair t sits in slot
- * (t - tfirst) % DWT_STAGES.  A warp whose lanes are all interior (`bulk`) has lane 0 fill a slot
- * with bulk copies that complete on the slot's mbarrier; any other warp fills it with cp.async.
+ * (t - tfirst) % DWT_STAGES.  A warp whose lanes are all interior (`bulk`) has lane 0 fill the
+ * slot's body (its first Stage::BODYB bytes) with bulk copies that complete on the slot's mbarrier;
+ * any other warp fills it with cp.async.  Stages with ghost columns (Stage::GHOSTS, the whole-warp
+ * 5/3 strips) keep them after the body; every lane fills its own ghost words with cp.async
+ * (fill_side) on both paths, and the bulk path waits for those too.
  * A commit group is closed on every step, filled or not, so that wait_group DWT_STAGES-1 always
  * leaves exactly the pair about to be read complete.
  * Stage::COOPERATIVE: the cp.async fill has each lane copy samples other lanes read, so the warp
@@ -504,6 +550,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, unsigned parity)
  * slot is private and only the bulk path (lane 0 writes every lane's samples) syncs before a refill.
  * =========================================================================================== */
 constexpr int DWT_STAGES = 3;
+
+struct NoSideFill
+{
+  __device__ __forceinline__ void operator()(uint8_t*, int) const {}
+};
 
 template <class Stage>
 struct WarpPipe
@@ -523,9 +574,9 @@ struct WarpPipe
         tlast(tlast_), tfill(tfirst_), bulk(bulk_)
   {
   }
-  /* fill_bulk(slot, t, bar) runs on lane 0 only; fill_async(slot, t) on every lane */
-  template <class Bulk, class Async>
-  __device__ __forceinline__ void refill(const Bulk& fill_bulk, const Async& fill_async)
+  /* fill_bulk(slot, t, bar) runs on lane 0 only; fill_async(slot, t) and fill_side(slot, t) on every lane */
+  template <class Bulk, class Async, class Side = NoSideFill>
+  __device__ __forceinline__ void refill(const Bulk& fill_bulk, const Async& fill_async, const Side& fill_side = Side())
   {
     if(tfill <= tlast)
     {
@@ -535,18 +586,19 @@ struct WarpPipe
       {
         if((threadIdx.x & 31) == 0)
         {
-          mbar_expect_tx(bars + slot, Stage::PAIRB);
+          mbar_expect_tx(bars + slot, Stage::BODYB);
           fill_bulk(st, tfill, bars + slot);
         }
       }
       else
         fill_async(st, tfill);
+      fill_side(st, tfill);
     }
     cp_async_commit();
     ++tfill;
   }
-  template <class Bulk, class Async>
-  __device__ __forceinline__ void prime(const Bulk& fill_bulk, const Async& fill_async)
+  template <class Bulk, class Async, class Side = NoSideFill>
+  __device__ __forceinline__ void prime(const Bulk& fill_bulk, const Async& fill_async, const Side& fill_side = Side())
   {
     if(bulk)
     {
@@ -561,18 +613,23 @@ struct WarpPipe
     }
 #pragma unroll
     for(int s = 0; s < DWT_STAGES - 1; ++s)
-      refill(fill_bulk, fill_async);
+      refill(fill_bulk, fill_async, fill_side);
   }
   /* starts the pair DWT_STAGES-1 ahead, waits for pair t and returns its slot */
-  template <class Bulk, class Async>
-  __device__ __forceinline__ const uint8_t* acquire(int t, const Bulk& fill_bulk, const Async& fill_async)
+  template <class Bulk, class Async, class Side = NoSideFill>
+  __device__ __forceinline__ const uint8_t* acquire(int t, const Bulk& fill_bulk, const Async& fill_async,
+                                                    const Side& fill_side = Side())
   {
     if(Stage::COOPERATIVE || bulk)
       __syncwarp(); /* every lane has read the slot that is refilled next */
-    refill(fill_bulk, fill_async);
+    refill(fill_bulk, fill_async, fill_side);
     const int k = t - tfirst;
     if(bulk)
+    {
       mbar_wait(bars + k % DWT_STAGES, (unsigned)((k / DWT_STAGES) & 1));
+      if(Stage::GHOSTS)
+        cp_async_wait<DWT_STAGES - 1>(); /* the lane's own ghost words: read by this lane only */
+    }
     else
     {
       cp_async_wait<DWT_STAGES - 1>();
@@ -585,12 +642,16 @@ struct WarpPipe
 };
 
 /* staged row fetch for the forward kernels: a slot holds the NC warp-rows of the two rows of a
-   pair (odd row, next even row), the 8 samples of lane L at bytes [32L, 32L+32) of each */
-template <int NC>
+   pair (odd row, next even row), the 8 samples of lane L at bytes [32L, 32L+32) of each.
+   GHOSTS_ (whole-warp 5/3 strips): then a 16-byte group per row and component, whose words 0, 1, 2
+   hold the ghost samples of lanes 0, 1, 31 (GhostCol) */
+template <int NC, bool GHOSTS_ = false>
 struct RowStage
 {
   static constexpr int ROWB = 1024;           /* bytes of one warp-row of one component */
-  static constexpr int PAIRB = 2 * NC * ROWB; /* one row pair, all components */
+  static constexpr int BODYB = 2 * NC * ROWB; /* one row pair, all components */
+  static constexpr bool GHOSTS = GHOSTS_;
+  static constexpr int PAIRB = BODYB + (GHOSTS ? 2 * NC * 16 : 0);
   static constexpr bool COOPERATIVE = true;
   /* 16-byte chunk k of a warp-row (lane L owns chunks 2L, 2L+1) is stored at chunk slot
      k ^ ((k >> 3) & 1): the two 128-bit reads of a lane then hit disjoint banks per quarter warp */
@@ -599,9 +660,11 @@ struct RowStage
   /* fill row `which` (0 = odd row, 1 = next even row) of a slot with canvas row v.
      Rows are copied COOPERATIVELY: one cp.async instruction moves 512 contiguous bytes
      (lane L copies chunks L and L+32), so every 32-byte DRAM sector is requested once.
-     fastmask: ballot of the lanes whose 8 columns are interior and aligned. */
+     fastmask: ballot of the lanes whose 8 columns are interior and aligned.
+     mcol(i): mirrored column of the lane's sample i (edge lanes only). */
+  template <class MCol>
   static __device__ __forceinline__ void fill(uint8_t* stage, int which, const DwtLevelDesc& D, const Job& J, int v,
-                                              bool fast, unsigned fastmask, const int (&mcol)[8])
+                                              bool fast, unsigned fastmask, const MCol& mcol)
   {
     const int r = mirror_rel(v - D.v0, J.hn);
     const int rel = J.ulane - D.u0;
@@ -625,11 +688,35 @@ struct RowStage
 #pragma unroll
         for(int i = 0; i < 4; ++i)
         {
-          cp_async4(d0 + 4 * i, row + mcol[i]);
-          cp_async4(d1 + 4 * i, row + mcol[4 + i]);
+          cp_async4(d0 + 4 * i, row + mcol(i));
+          cp_async4(d1 + 4 * i, row + mcol(4 + i));
         }
       }
     }
+  }
+  /* the lane's ghost sample of canvas row v into word G.slot of the row's ghost group (lanes 0, 1, 31) */
+  static __device__ __forceinline__ void fill_ghost(uint8_t* stage, int which, const DwtLevelDesc& D, const Job& J, int v,
+                                                    const GhostCol& G)
+  {
+    static_assert(GHOSTS, "stage without ghost columns");
+    const int r = mirror_rel(v - D.v0, J.hn);
+#pragma unroll
+    for(int c = 0; c < NC; ++c)
+      if(G.slot >= 0)
+        cp_async4(stage + BODYB + (which * NC + c) * 16 + 4 * G.slot,
+                  reinterpret_cast<const int32_t*>(D.in[c]) + (size_t)r * D.in_pitch + G.col);
+  }
+  /* byte offset, relative to row `which` = 0, component 0, and stride per (row, component) of the lane's ghost sample;
+     a lane without a ghost reads its own first sample instead */
+  static __device__ __forceinline__ int2 ghost_at(const Job& J, const GhostCol& G)
+  {
+    return G.slot >= 0 ? make_int2(BODYB + 4 * G.slot, 16) : make_int2(32 * J.lane, ROWB);
+  }
+  static __device__ __forceinline__ void read_ghost(const uint8_t* stage, int which, int2 at, int (&out)[NC][1])
+  {
+#pragma unroll
+    for(int c = 0; c < NC; ++c)
+      out[c][0] = *reinterpret_cast<const int*>(stage + at.x + (which * NC + c) * at.y);
   }
   /* bulk path (every lane fast): one lane asks the copy engine for the NC whole warp-rows of canvas
      row v; they land linearly in the slot and complete on `bar` (armed with expect_tx) */
@@ -685,29 +772,44 @@ __device__ __noinline__ void fwd53_degenerate_job(const DwtLevelDesc* __restrict
 {
   const DwtLevelDesc& D = *dptr; /* re-read from global memory: this path is cold */
   const BandGeom g = band_geom(D);
-  int E[NC][8], DP[NC][8];
+  const GhostCol G = ghost_col(D, J);
+  /* column 8 of each row is the lane's ghost column */
+  int E[NC][9], DP[NC][9];
+  auto fetch = [&](int v, int (&x)[NC][9]) {
+    int b[NC][8], gh[NC][1];
+    fetch53<NC>(D, J, v, b);
+    fetch_ghost53<NC>(D, J, G, v, gh);
+#pragma unroll
+    for(int c = 0; c < NC; ++c)
+    {
+#pragma unroll
+      for(int i = 0; i < 8; ++i)
+        x[c][i] = b[c][i];
+      x[c][8] = gh[c][0];
+    }
+  };
   {
-    int A[NC][8], B[NC][8];
-    fetch53<NC>(D, J, 2 * J.jbeg - 2, A);
-    fetch53<NC>(D, J, 2 * J.jbeg - 1, B);
-    fetch53<NC>(D, J, 2 * J.jbeg, E);
+    int A[NC][9], B[NC][9];
+    fetch(2 * J.jbeg - 2, A);
+    fetch(2 * J.jbeg - 1, B);
+    fetch(2 * J.jbeg, E);
 #pragma unroll
     for(int c = 0; c < NC; ++c)
 #pragma unroll
-      for(int i = 0; i < 8; ++i)
+      for(int i = 0; i < 9; ++i)
         DP[c][i] = B[c][i] - ((A[c][i] + E[c][i]) >> 1);
   }
   for(int j = J.jbeg; j < J.jend; ++j)
   {
-    int O[NC][8], E2[NC][8];
-    fetch53<NC>(D, J, 2 * j + 1, O);
-    fetch53<NC>(D, J, 2 * j + 2, E2);
+    int O[NC][9], E2[NC][9];
+    fetch(2 * j + 1, O);
+    fetch(2 * j + 2, E2);
 #pragma unroll 1
     for(int c = 0; c < NC; ++c)
     {
-      int s[8], d[8];
+      int s[9], d[9];
 #pragma unroll
-      for(int i = 0; i < 8; ++i)
+      for(int i = 0; i < 9; ++i)
       {
         d[i] = O[c][i] - ((E[c][i] + E2[c][i]) >> 1);
         s[i] = E[c][i] + ((DP[c][i] + d[i] + 2) >> 2);
@@ -719,10 +821,16 @@ __device__ __noinline__ void fwd53_degenerate_job(const DwtLevelDesc* __restrict
         DP[c][i] = d[i];
         E[c][i] = E2[c][i];
       }
-      int lo[4], hi[4];
-      hfwd53<true>(s, J.wn, lo, hi);
+      int s8[8], d8[8], lo[4], hi[4];
+#pragma unroll
+      for(int i = 0; i < 8; ++i)
+      {
+        s8[i] = s[i];
+        d8[i] = d[i];
+      }
+      hfwd53<true>(s8, s[8], J.wn, lo, hi);
       store_rows(D, g, store_ctx(D, J, g), c, j, false, lo, hi);
-      hfwd53<true>(d, J.wn, lo, hi);
+      hfwd53<true>(d8, d[8], J.wn, lo, hi);
       store_rows(D, g, store_ctx(D, J, g), c, j, true, lo, hi);
     }
   }
@@ -731,14 +839,15 @@ __device__ __noinline__ void fwd53_degenerate_job(const DwtLevelDesc* __restrict
 /* =============================================================================================
  * forward 5/3
  * =========================================================================================== */
+/* 3 CTAs (12 warps) per SM, as the shared memory allows: at most 168 registers per thread, without spills */
 template <int NC>
-__global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_fwd(const DwtLevelDesc* __restrict__ descs)
+__global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32, 3) k_dwt53_fwd(const DwtLevelDesc* __restrict__ descs)
 {
   extern __shared__ __align__(16) uint8_t smem_dwt[];
-  typedef RowStage<NC> RS;
+  typedef RowStage<NC, true> RS;
   const DwtLevelDesc D = descs[blockIdx.y]; /* by value: fields live in (uniform) registers, not re-read after every store */
   Job J;
-  if(!decode_job(D, J))
+  if(!decode_job<true>(D, J))
     return;
   if(J.hn == 1 || J.wn == 1)
   {
@@ -749,40 +858,53 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_fwd(const DwtL
   const StoreCtx SC = store_ctx(D, J, g);
   const bool fast = RS::lane_fast(D, J);
   const unsigned fastmask = __ballot_sync(0xffffffffu, fast);
-  int mcol[8]; /* mirrored column of each of the lane's samples: only edge lanes use them */
-#pragma unroll
-  for(int i = 0; i < 8; ++i)
-    mcol[i] = mirror_rel(J.ulane - D.u0 + i, J.wn);
+  const GhostCol G = ghost_col(D, J);
+  const int2 gat = RS::ghost_at(J, G);
 
   /* pairs t = jbeg-1 .. jend-1 : rows (2t+1, 2t+2); the even row before them is fetched directly.
-     Interior strip: rows arrive by bulk copy (TMA engine); edge strips keep the LDGSTS path */
+     A strip whose 256 columns lie inside the line gets its rows by bulk copy (TMA engine), any other (the ragged last
+     strip, a first strip that starts left of the line) by LDGSTS with mirrored columns for the lanes at the line's ends
+     (computed at the copy: only those strips pay for them).  The ghost columns always arrive by LDGSTS. */
   const int tfirst = J.jbeg - 1, tlast = J.jend - 1;
   WarpPipe<RS> pipe(smem_dwt, fastmask == 0xffffffffu, tfirst, tlast);
   auto fill_bulk = [&](uint8_t* st, int tf, uint64_t* bar) {
     RS::fill_bulk(st, 0, D, J, 2 * tf + 1, bar);
     RS::fill_bulk(st, 1, D, J, 2 * tf + 2, bar);
   };
+  auto mcol = [&](int i) { return mirror_rel(J.ulane - D.u0 + i, J.wn); };
   auto fill_async = [&](uint8_t* st, int tf) {
     RS::fill(st, 0, D, J, 2 * tf + 1, fast, fastmask, mcol);
     RS::fill(st, 1, D, J, 2 * tf + 2, fast, fastmask, mcol);
   };
-  pipe.prime(fill_bulk, fill_async);
-  int E[NC][8], DP[NC][8];
+  auto fill_ghost = [&](uint8_t* st, int tf) {
+    RS::fill_ghost(st, 0, D, J, 2 * tf + 1, G);
+    RS::fill_ghost(st, 1, D, J, 2 * tf + 2, G);
+  };
+  pipe.prime(fill_bulk, fill_async, fill_ghost);
+  int E[NC][8], DP[NC][8], gE[NC][1], gDP[NC];
   fetch53<NC>(D, J, 2 * tfirst, E);
+  fetch_ghost53<NC>(D, J, G, 2 * tfirst, gE);
 #pragma unroll
   for(int c = 0; c < NC; ++c)
+  {
 #pragma unroll
     for(int i = 0; i < 8; ++i)
       DP[c][i] = 0;
+    gDP[c] = 0;
+  }
 
   for(int t = tfirst; t <= tlast; ++t)
   {
-    const uint8_t* st = pipe.acquire(t, fill_bulk, fill_async);
-    int O[NC][8], E2[NC][8];
+    const uint8_t* st = pipe.acquire(t, fill_bulk, fill_async, fill_ghost);
+    int O[NC][8], E2[NC][8], gO[NC][1], gE2[NC][1];
     RS::read(st, 0, J, pipe.bulk, O);
     RS::read(st, 1, J, pipe.bulk, E2);
+    RS::read_ghost(st, 0, gat, gO);
+    RS::read_ghost(st, 1, gat, gE2);
     to_coeffs53<NC>(D, O);
     to_coeffs53<NC>(D, E2);
+    to_coeffs53<NC>(D, gO);
+    to_coeffs53<NC>(D, gE2);
     const bool emit = t >= J.jbeg;
 #pragma unroll
     for(int c = 0; c < NC; ++c)
@@ -796,12 +918,16 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_fwd(const DwtL
         DP[c][i] = d[i];
         E[c][i] = E2[c][i];
       }
+      const int gd = gO[c][0] - ((gE[c][0] + gE2[c][0]) >> 1);
+      const int gs = gE[c][0] + ((gDP[c] + gd + 2) >> 2);
+      gDP[c] = gd;
+      gE[c][0] = gE2[c][0];
       if(emit)
       { /* warp-uniform */
         int lo[4], hi[4];
-        hfwd53<false>(s, J.wn, lo, hi);
+        hfwd53<false>(s, gs, J.wn, lo, hi);
         store_rows(D, g, SC, c, t, false, lo, hi);
-        hfwd53<false>(d, J.wn, lo, hi);
+        hfwd53<false>(d, gd, J.wn, lo, hi);
         store_rows(D, g, SC, c, t, true, lo, hi);
       }
     }
@@ -878,7 +1004,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_fwd(const DwtL
   typedef RowStage<NC> RS;
   const DwtLevelDesc D = descs[blockIdx.y]; /* by value */
   Job J;
-  if(!decode_job(D, J))
+  if(!decode_job<false>(D, J))
     return;
   if(J.hn == 1 || J.wn == 1)
   {
@@ -904,9 +1030,10 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_fwd(const DwtL
     RS::fill_bulk(st, 0, D, J, 2 * tf + 1, bar);
     RS::fill_bulk(st, 1, D, J, 2 * tf + 2, bar);
   };
+  auto mc = [&](int i) { return mcol[i]; };
   auto fill_async = [&](uint8_t* st, int tf) {
-    RS::fill(st, 0, D, J, 2 * tf + 1, fast, fastmask, mcol);
-    RS::fill(st, 1, D, J, 2 * tf + 2, fast, fastmask, mcol);
+    RS::fill(st, 0, D, J, 2 * tf + 1, fast, fastmask, mc);
+    RS::fill(st, 1, D, J, 2 * tf + 2, fast, fastmask, mc);
   };
   pipe.prime(fill_bulk, fill_async);
   float Ev[NC][8], D1[NC][8], S1[NC][8], D2[NC][8];
@@ -999,17 +1126,64 @@ __device__ __forceinline__ void fetch_band_rows(const DwtLevelDesc& D, const Job
   }
 }
 
-/* inverse horizontal 5/3: WaveletReverse.cpp L879-1072 */
-template <bool DEGEN = true>
-__device__ __forceinline__ void hinv53(const int (&lo)[4], const int (&hi)[4], int wn, int (&r)[8])
+/* ---- ghost samples of a whole-warp 5/3 strip (inverse) ------------------------------------------------------------------
+ * Lane 0's synthesis needs the high-band sample at column x0-1, lane 31's the low-band sample at x0+256 and the high-band
+ * sample at x0+257, from each of the two band-row pairs (LL|HL, LH|HH) of a row pair; mirrored addresses, as for the body.
+ * `a`: the high-band sample's column in the row that holds HL (or HH) at snx; `b`: the low-band sample's column in the row
+ * of LL (or LH).  a is lane 0's x0-1 and lane 31's x0+257, b is lane 31's x0+256; other lanes use neither. */
+struct GhostBand
 {
-  const int dm = __shfl_up_sync(0xffffffffu, hi[3], 1);
+  int a, b;
+};
+__device__ __forceinline__ GhostBand ghost_band(const DwtLevelDesc& D, const Job& J, const BandGeom& g)
+{
+  const int x0 = J.ulane - 8 * J.lane;
+  const int ua = J.lane == 0 ? x0 - 1 : J.lane == 31 ? x0 + 257 : J.ulane + 1;
+  const int ub = J.lane == 31 ? x0 + 256 : J.ulane;
+  /* symmetric extension keeps a column's parity (wn >= 2) */
+  const int uam = D.u0 + mirror_rel(ua - D.u0, J.wn), ubm = D.u0 + mirror_rel(ub - D.u0, J.wn);
+  GhostBand G;
+  G.a = g.snx + (uam >> 1) - g.x0h;
+  G.b = (ubm >> 1) - g.x0l;
+  return G;
+}
+/* the lane's ghost samples of the band rows of pair j (vertical low or high), unstaged (degenerate jobs; a line one
+   sample wide has no horizontal lifting and no ghosts) */
+template <int NC>
+__device__ __forceinline__ void fetch_band_ghosts(const DwtLevelDesc& D, const Job& J, const BandGeom& g, const GhostBand& G,
+                                                  int j, bool vhigh, int (&ga)[NC], int (&gb)[NC])
+{
+  const int vm = D.v0 + mirror_rel(2 * j + (vhigh ? 1 : 0) - D.v0, J.hn);
+  const int jm = vm >> 1;
+#pragma unroll
+  for(int c = 0; c < NC; ++c)
+  {
+    ga[c] = gb[c] = 0;
+    if(J.wn == 1 || (vm & 1) != (vhigh ? 1 : 0))
+      continue;
+    const int32_t* lrow = !vhigh ? reinterpret_cast<const int32_t*>(D.out_ll[c]) + (size_t)(jm - g.y0l) * D.ll_pitch
+                                 : reinterpret_cast<const int32_t*>(D.out_c[c]) + (size_t)(g.sny + jm - g.y0h) * D.c_pitch;
+    const int32_t* hrow = !vhigh ? reinterpret_cast<const int32_t*>(D.out_c[c]) + (size_t)(jm - g.y0l) * D.c_pitch : lrow;
+    ga[c] = __ldg(hrow + G.a);
+    gb[c] = __ldg(lrow + G.b);
+  }
+}
+
+/* inverse horizontal 5/3: WaveletReverse.cpp L879-1072.  ga, gb: the lane's ghost samples of the same band row pair (see
+   GhostBand); lanes 0 and 31 take their outer neighbours from them by selects */
+template <bool DEGEN = true>
+__device__ __forceinline__ void hinv53(const int (&lo)[4], const int (&hi)[4], int ga, int gb, int wn, int (&r)[8])
+{
+  const int lane = threadIdx.x & 31;
+  const int hp = __shfl_up_sync(0xffffffffu, hi[3], 1);
+  const int dm = lane == 0 ? ga : hp;
   int e[5];
   e[0] = lo[0] - ((dm + hi[0] + 2) >> 2);
   e[1] = lo[1] - ((hi[0] + hi[1] + 2) >> 2);
   e[2] = lo[2] - ((hi[1] + hi[2] + 2) >> 2);
   e[3] = lo[3] - ((hi[2] + hi[3] + 2) >> 2);
-  e[4] = __shfl_down_sync(0xffffffffu, e[0], 1);
+  const int en = __shfl_down_sync(0xffffffffu, e[0], 1);
+  e[4] = lane == 31 ? gb - ((hi[3] + ga + 2) >> 2) : en;
 #pragma unroll
   for(int i = 0; i < 4; ++i)
   {
@@ -1150,6 +1324,7 @@ __device__ __noinline__ void inv53_degenerate_job(const DwtLevelDesc* __restrict
 {
   const DwtLevelDesc& D = *dptr;
   const BandGeom g = band_geom(D);
+  const GhostBand G = ghost_band(D, J, g);
   int DV[NC][8], EP[NC][8];
 #pragma unroll
   for(int c = 0; c < NC; ++c)
@@ -1159,16 +1334,18 @@ __device__ __noinline__ void inv53_degenerate_job(const DwtLevelDesc* __restrict
 
   for(int t = J.jbeg - 1; t <= J.jend; ++t)
   {
-    int lo[NC][4], hi[NC][4];
+    int lo[NC][4], hi[NC][4], ga[NC], gb[NC];
     int sv[NC][8], dv[NC][8];
     fetch_band_rows<NC>(D, J, g, t, false, lo, hi);
+    fetch_band_ghosts<NC>(D, J, g, G, t, false, ga, gb);
 #pragma unroll
     for(int c = 0; c < NC; ++c)
-      hinv53(lo[c], hi[c], J.wn, sv[c]);
+      hinv53(lo[c], hi[c], ga[c], gb[c], J.wn, sv[c]);
     fetch_band_rows<NC>(D, J, g, t, true, lo, hi);
+    fetch_band_ghosts<NC>(D, J, g, G, t, true, ga, gb);
 #pragma unroll
     for(int c = 0; c < NC; ++c)
-      hinv53(lo[c], hi[c], J.wn, dv[c]);
+      hinv53(lo[c], hi[c], ga[c], gb[c], J.wn, dv[c]);
     int Er[NC][8], Or[NC][8];
 #pragma unroll
     for(int c = 0; c < NC; ++c)
@@ -1206,30 +1383,43 @@ __device__ __noinline__ void inv53_degenerate_job(const DwtLevelDesc* __restrict
 
 /* staged band-row fetch for the inverse kernels: per row pair four band rows (LL|HL, LH|HH) x NC,
    each lane owning 4 consecutive samples (16 bytes) of each -> one cp.async per lane per band row,
-   512 contiguous bytes per instruction, private slots (no barrier) */
-template <int NC>
+   512 contiguous bytes per instruction, private slots (no barrier).
+   WHOLE (whole-warp 5/3 strips): a 16-byte group per band-row pair and component follows the body, word 0 holding lane 0's
+   ghost sample a, words 2, 3 lane 31's a and b (GhostBand); the mirrored columns of edge lanes are computed at the copy
+   instead of being held in registers */
+template <int NC, bool WHOLE = false>
 struct BandStage
 {
   static constexpr int ROWB = 512;
-  static constexpr int PAIRB = 4 * NC * ROWB;
+  static constexpr int BODYB = 4 * NC * ROWB;
+  static constexpr bool GHOSTS = WHOLE;
+  static constexpr int PAIRB = BODYB + (GHOSTS ? 2 * NC * 16 : 0);
   static constexpr bool COOPERATIVE = false;
   struct Lane
   {
     bool need;
     bool fast[4];   /* LL, HL, LH, HH source: 4 samples interior and 16-byte aligned */
     int col[4];     /* band-relative column of the lane's first sample (low, high) per source */
-    int mlo[4], mhi[4]; /* mirrored band-relative columns for edge lanes */
+    int mlo[4], mhi[4]; /* mirrored band-relative columns for edge lanes (!WHOLE) */
   };
+  /* mirrored band-relative column of the lane's low (odd = 0) or high (odd = 1) sample i */
+  static __device__ __forceinline__ int mirrored(const DwtLevelDesc& D, const Job& J, const BandGeom& g, int i, int odd)
+  {
+    const int u = D.u0 + mirror_rel(2 * ((J.ulane >> 1) + i) + odd - D.u0, J.wn);
+    return (u >> 1) - (odd ? g.x0h : g.x0l);
+  }
   static __device__ __forceinline__ void setup(const DwtLevelDesc& D, const Job& J, const BandGeom& g, Lane& L)
   {
     const int k0 = J.ulane >> 1;
     L.need = J.need;
-#pragma unroll
-    for(int i = 0; i < 4; ++i)
+    if(!WHOLE)
     {
-      const int ul = D.u0 + mirror_rel(2 * (k0 + i) - D.u0, J.wn), uh = D.u0 + mirror_rel(2 * (k0 + i) + 1 - D.u0, J.wn);
-      L.mlo[i] = (ul >> 1) - g.x0l;
-      L.mhi[i] = (uh >> 1) - g.x0h;
+#pragma unroll
+      for(int i = 0; i < 4; ++i)
+      {
+        L.mlo[i] = mirrored(D, J, g, i, 0);
+        L.mhi[i] = mirrored(D, J, g, i, 1);
+      }
     }
     const bool in_lo = 2 * k0 >= D.u0 && 2 * k0 + 6 < D.u1, in_hi = 2 * k0 + 1 >= D.u0 && 2 * k0 + 7 < D.u1;
     const int clo = k0 - g.x0l, chi = k0 - g.x0h;
@@ -1266,10 +1456,49 @@ struct BandStage
           const int base = (b & 1) ? g.snx : 0;
 #pragma unroll
           for(int i = 0; i < 4; ++i)
-            cp_async4(dst + 4 * i, src[b] + base + ((b & 1) ? L.mhi[i] : L.mlo[i]));
+          {
+            const int m = WHOLE ? mirrored(D, J, g, i, b & 1) : ((b & 1) ? L.mhi[i] : L.mlo[i]);
+            cp_async4(dst + 4 * i, src[b] + base + m);
+          }
         }
       }
     }
+  }
+  /* the ghost samples of pair t: lane 0's a, lane 31's a and b, of both band-row pairs */
+  static __device__ __forceinline__ void fill_ghost(uint8_t* stage, const DwtLevelDesc& D, const Job& J, const BandGeom& g,
+                                                    const GhostBand& G, int t)
+  {
+    static_assert(GHOSTS, "stage without ghost samples");
+    const int jl = ((D.v0 + mirror_rel(2 * t - D.v0, J.hn)) >> 1), jh = ((D.v0 + mirror_rel(2 * t + 1 - D.v0, J.hn)) >> 1);
+    const bool right = J.lane == 31, on = J.lane == 0 || right;
+#pragma unroll
+    for(int c = 0; c < NC; ++c)
+    {
+      const int32_t* lsrc[2];
+      const int32_t* hsrc[2];
+      lsrc[0] = reinterpret_cast<const int32_t*>(D.out_ll[c]) + (jl - g.y0l) * (int)D.ll_pitch;
+      hsrc[0] = reinterpret_cast<const int32_t*>(D.out_c[c]) + (jl - g.y0l) * (int)D.c_pitch;
+      lsrc[1] = hsrc[1] = reinterpret_cast<const int32_t*>(D.out_c[c]) + (g.sny + jh - g.y0h) * (int)D.c_pitch;
+#pragma unroll
+      for(int v = 0; v < 2; ++v)
+      {
+        uint8_t* dst = stage + BODYB + (v * NC + c) * 16;
+        if(on)
+          cp_async4(dst + (right ? 8 : 0), hsrc[v] + G.a);
+        if(right)
+          cp_async4(dst + 12, lsrc[v] + G.b);
+      }
+    }
+  }
+  /* byte offset, relative to band-row pair 0, component 0, and stride per (band-row pair, component) of the lane's
+     ghost samples; a lane without them reads two of its own body samples instead */
+  static __device__ __forceinline__ int2 ghost_at(const Job& J)
+  {
+    return J.lane == 0 ? make_int2(BODYB, 16) : J.lane == 31 ? make_int2(BODYB + 8, 16) : make_int2(16 * J.lane, ROWB);
+  }
+  static __device__ __forceinline__ int2 read_ghost(const uint8_t* stage, int2 at, int v, int c)
+  {
+    return *reinterpret_cast<const int2*>(stage + at.x + (v * NC + c) * at.y);
   }
   /* bulk path: every lane of the warp is `fast` on all four sources, so each band row of the pair is 512 contiguous,
      16-byte aligned bytes starting at lane 0's column: lane 0 asks the copy engine (TMA, UBLKCP) for the 4 x NC rows,
@@ -1302,14 +1531,15 @@ struct BandStage
   }
 };
 
+/* 3 CTAs per SM, as k_dwt53_fwd */
 template <int NC>
-__global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtLevelDesc* __restrict__ descs)
+__global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32, 3) k_dwt53_inv(const DwtLevelDesc* __restrict__ descs)
 {
   extern __shared__ __align__(16) uint8_t smem_dwt[];
-  typedef BandStage<NC> BS;
+  typedef BandStage<NC, true> BS;
   const DwtLevelDesc D = descs[blockIdx.y]; /* by value: fields live in (uniform) registers */
   Job J;
-  if(!decode_job(D, J))
+  if(!decode_job<true>(D, J))
     return;
   if(J.hn == 1 || J.wn == 1)
   {
@@ -1320,13 +1550,17 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtL
   typename BS::Lane L;
   BS::setup(D, J, g, L);
   const OutCtx OC = out_ctx(D, J);
+  const GhostBand G = ghost_band(D, J, g);
+  const int2 gat = BS::ghost_at(J);
 
-  /* interior strip: band rows by bulk copy (TMA engine) on per-slot mbarriers */
+  /* a strip whose band quads all lie inside the line and are 16-byte aligned: band rows by bulk copy (TMA engine) on
+     per-slot mbarriers; the ghost samples always arrive by LDGSTS */
   const int tfirst = J.jbeg - 1, tlast = J.jend;
   WarpPipe<BS> pipe(smem_dwt, BS::all_fast(L), tfirst, tlast);
   auto fill_bulk = [&](uint8_t* st, int tf, uint64_t* bar) { BS::fill_bulk(st, D, J, g, L, tf, bar); };
   auto fill_async = [&](uint8_t* st, int tf) { BS::fill(st, D, J, g, L, tf); };
-  pipe.prime(fill_bulk, fill_async);
+  auto fill_ghost = [&](uint8_t* st, int tf) { BS::fill_ghost(st, D, J, g, G, tf); };
+  pipe.prime(fill_bulk, fill_async, fill_ghost);
   int DV[NC][8], EP[NC][8];
 #pragma unroll
   for(int c = 0; c < NC; ++c)
@@ -1336,7 +1570,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtL
 
   for(int t = tfirst; t <= tlast; ++t)
   {
-    const uint8_t* st = pipe.acquire(t, fill_bulk, fill_async);
+    const uint8_t* st = pipe.acquire(t, fill_bulk, fill_async, fill_ghost);
     int Er[NC][8], Or[NC][8];
 #pragma unroll
     for(int c = 0; c < NC; ++c)
@@ -1344,10 +1578,12 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt53_inv(const DwtL
       int lo[4], hi[4], sv[8], dv[8];
       BS::read(st, J, 0, c, lo);
       BS::read(st, J, 1, c, hi);
-      hinv53<false>(lo, hi, J.wn, sv);
+      int2 gh = BS::read_ghost(st, gat, 0, c);
+      hinv53<false>(lo, hi, gh.x, gh.y, J.wn, sv);
       BS::read(st, J, 2, c, lo);
       BS::read(st, J, 3, c, hi);
-      hinv53<false>(lo, hi, J.wn, dv);
+      gh = BS::read_ghost(st, gat, 1, c);
+      hinv53<false>(lo, hi, gh.x, gh.y, J.wn, dv);
 #pragma unroll
       for(int i = 0; i < 8; ++i)
       {
@@ -1435,7 +1671,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32) k_dwt97_inv(const DwtL
   typedef BandStage<NC> BS;
   const DwtLevelDesc D = descs[blockIdx.y]; /* by value */
   Job J;
-  if(!decode_job(D, J))
+  if(!decode_job<false>(D, J))
     return;
   if(J.hn == 1 || J.wn == 1)
   {
@@ -1760,8 +1996,8 @@ void b2k_launch_dwt_fwd(const DwtLevelDesc* d, int ndesc, int max_jobs, int nc, 
   dim3 grid((max_jobs + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA, ndesc), block(B2K_WARPS_PER_CTA * 32);
   if(!irreversible)
   {
-    if(nc == 3) launch_dwt<RowStage<3>, k_dwt53_fwd<3>>(grid, block, st, d);
-    else launch_dwt<RowStage<1>, k_dwt53_fwd<1>>(grid, block, st, d);
+    if(nc == 3) launch_dwt<RowStage<3, true>, k_dwt53_fwd<3>>(grid, block, st, d);
+    else launch_dwt<RowStage<1, true>, k_dwt53_fwd<1>>(grid, block, st, d);
   }
   else
   {
@@ -1865,8 +2101,8 @@ void b2k_launch_dwt_inv(const DwtLevelDesc* d, int ndesc, int max_jobs, int nc, 
   dim3 grid((max_jobs + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA, ndesc), block(B2K_WARPS_PER_CTA * 32);
   if(!irreversible)
   {
-    if(nc == 3) launch_dwt<BandStage<3>, k_dwt53_inv<3>>(grid, block, st, d);
-    else launch_dwt<BandStage<1>, k_dwt53_inv<1>>(grid, block, st, d);
+    if(nc == 3) launch_dwt<BandStage<3, true>, k_dwt53_inv<3>>(grid, block, st, d);
+    else launch_dwt<BandStage<1, true>, k_dwt53_inv<1>>(grid, block, st, d);
   }
   else
   {

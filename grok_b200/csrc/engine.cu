@@ -478,11 +478,14 @@ extern "C" int64_t b2k_enumerate(const b2k_coding* cp, uint32_t tile_mod, uint32
 }
 
 /* -------------------------------------------------------------------------------------------- */
-static void fill_strips(DwtLevelDesc& d, int pairs_per_seg)
+/* Column strips of one warp job each.  5/3 (whole_warp): 256 columns, all 32 lanes own 8 of them and the neighbours
+   outside the warp arrive as ghost columns (dwt.cu); only the last strip may be narrower.  9/7: lanes 0 and 31 are
+   halo lanes, so a strip owns at most 240 columns, and the span is cut into strips of equal width. */
+static void fill_strips(DwtLevelDesc& d, int pairs_per_seg, bool whole_warp)
 {
   const int span = d.u1 - (d.u0 & ~7);
-  const int nstrips = std::max(1, (span + 239) / 240);
-  int sw = (span + nstrips - 1) / nstrips;
+  const int nstrips = std::max(1, whole_warp ? (span + 255) / 256 : (span + 239) / 240);
+  int sw = whole_warp ? 256 : (span + nstrips - 1) / nstrips;
   sw = (sw + 7) & ~7;
   d.nstrips = (uint16_t)nstrips;
   d.strip_w = (uint16_t)sw;
@@ -620,7 +623,7 @@ static int build_dwt_plan(b2k_device_job* J)
             d.lo[k] = lo;
             d.hi[k] = hi;
           }
-          fill_strips(d, P);
+          fill_strips(d, P, !cp.irreversible);
           (group ? mctL : sglL).descs.push_back(d);
           const uint64_t samples = (uint64_t)r.w() * r.h() * nc;
           (group ? mctL : sglL).alg_bytes += samples * 8;
@@ -646,7 +649,7 @@ static int build_dwt_plan(b2k_device_job* J)
         {
           Pl >>= 1;
           for(DwtLevelDesc& d : LL->descs)
-            fill_strips(d, Pl);
+            fill_strips(d, Pl, !cp.irreversible);
         }
       }
       if(dir == 0)
