@@ -704,35 +704,28 @@ class Job:
                "b2k_job_t1_decode_blocks")
         return ms.value
 
+    # The round trips raise EngineError on return code 2 (the coded size of a 9/7 step outgrew the byte arena): the arena
+    # has been grown, but the image planes then hold a partial decode's reconstruction, so upload() again before a retry.
     def roundtrip_n(self, steps):
         """`steps` round trips queued back to back, one synchronisation.  Returns (total ms, [fwd, enc, dec, inv] ms
         summed over the steps, level-1 DWT kernel ms summed, coded bytes)."""
         ms, st, l1, nb = C.c_float(), (C.c_float * 4)(), C.c_float(), C.c_uint64()
-        rc = lib().b2k_job_roundtrip_n(self._h, steps, C.byref(ms), st, C.byref(l1), C.byref(nb))
-        if rc == 2:
-            rc = lib().b2k_job_roundtrip_n(self._h, steps, C.byref(ms), st, C.byref(l1), C.byref(nb))
-        _check(rc, "b2k_job_roundtrip_n")
+        _check(lib().b2k_job_roundtrip_n(self._h, steps, C.byref(ms), st, C.byref(l1), C.byref(nb)), "b2k_job_roundtrip_n")
         return ms.value, [float(v) for v in st], l1.value, int(nb.value)
 
     def roundtrip_pipelined_n(self, steps, chunks=0, streams=0):
         """`steps` round trips with the block-coder stage pipelined over block ranges on side streams
         (b2k_job_roundtrip_pipelined_n).  Returns (total ms, [fwd, block coder, inv] ms summed, level-1 kernel ms summed, bytes)."""
         ms, st, l1, nb = C.c_float(), (C.c_float * 3)(), C.c_float(), C.c_uint64()
-        args = (self._h, steps, chunks, streams, C.byref(ms), st, C.byref(l1), C.byref(nb))
-        rc = lib().b2k_job_roundtrip_pipelined_n(*args)
-        if rc == 2:
-            rc = lib().b2k_job_roundtrip_pipelined_n(*args)
-        _check(rc, "b2k_job_roundtrip_pipelined_n")
+        _check(lib().b2k_job_roundtrip_pipelined_n(self._h, steps, chunks, streams, C.byref(ms), st, C.byref(l1), C.byref(nb)),
+               "b2k_job_roundtrip_pipelined_n")
         return ms.value, [float(v) for v in st], l1.value, int(nb.value)
 
     def roundtrip(self):
         """forward -> block encode -> block decode -> inverse, device-resident, one synchronisation.
         Returns (total ms, [fwd, enc, dec, inv] ms, coded bytes)."""
         ms, st, nb = C.c_float(), (C.c_float * 4)(), C.c_uint64()
-        rc = lib().b2k_job_roundtrip(self._h, C.byref(ms), st, C.byref(nb))
-        if rc == 2:
-            rc = lib().b2k_job_roundtrip(self._h, C.byref(ms), st, C.byref(nb))
-        _check(rc, "b2k_job_roundtrip")
+        _check(lib().b2k_job_roundtrip(self._h, C.byref(ms), st, C.byref(nb)), "b2k_job_roundtrip")
         return ms.value, list(st), nb.value
 
     def fetch_result(self):

@@ -104,7 +104,7 @@ void b2k_launch_ht_decode_magsgn(const HtBlockDesc* d_blocks, const uint8_t* d_b
                                  const HtBlockOut* d_status, uint32_t nblocks, uint32_t max_w, int* d_err, int irreversible,
                                  int any_refinement, cudaStream_t st);
 void b2k_launch_build_dec_desc(const HtBlockDesc* d_enc, const HtBlockOut* d_out, const uint64_t* d_offsets,
-                               const float* d_dec_quant, HtBlockDesc* d_dec, uint32_t n, cudaStream_t st);
+                               const float* d_dec_quant, HtBlockDesc* d_dec, uint32_t n, uint64_t cap, cudaStream_t st);
 /* sample containers (sample_bytes 1, 2 or 4) <-> int32 planes.  Component c of pixel (x, y) of the container is at
    base + y * pitch + x * step + c samples; the nc components go to / come from dst[c] / src[c] + y * plane pitch + x */
 void b2k_launch_container_to_planes(const void* src, uint32_t spitch, uint32_t step, uint32_t sample_bytes, int32_t* const* dst, int nc,

@@ -354,6 +354,9 @@ struct b2k_device_job
   uint64_t scratch_bytes = 0;
   uint8_t* d_bytes = nullptr;
   uint64_t bytes_cap = 0, bytes_used = 0;
+  /* the arena was sized from a coding of the image the job holds: the round trips skip their sizing pass.  A new image
+     (b2k_job_upload, or b2k_job_inverse of the coefficient planes) or a caller's arena (b2k_job_t1_decode_blocks) clears it */
+  bool arena_sized = false;
   int* d_err = nullptr;
   /* pinned host staging for results */
   HtBlockOut* h_out = nullptr;
@@ -1029,6 +1032,7 @@ extern "C" int32_t b2k_job_upload(b2k_device_job* J, const int32_t* const* plane
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
   const Container host = planar_container(J->cp.numcomps, (void* const*)planes, strides, 4, J->cp.x0, J->cp.y0, false);
+  J->arena_sized = false;
   if(copy_runs(J, plane_container(J->img), host, J->eng->stream, 0, J->tiles.size(), nullptr)) return -1;
   CUDA_TRY(cudaStreamSynchronize(J->eng->stream));
   return 0;
@@ -1439,6 +1443,7 @@ static int finish_t1_encode(b2k_device_job* J, cudaStream_t st)
     CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
   }
   J->bytes_used = total;
+  J->arena_sized = true;
   b2k_launch_ht_gather(J->d_enc_desc, J->d_out, J->d_offsets, J->d_scratch, J->d_bytes, n, J->bytes_cap, st);
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -1465,6 +1470,7 @@ extern "C" int32_t b2k_job_inverse(b2k_device_job* J, float* ms)
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
   cudaStream_t st = J->eng->stream;
+  J->arena_sized = false; /* the image planes now hold whatever the coefficient planes make */
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   if(enqueue_inverse(J, st)) return -1;
   CUDA_TRY(cudaEventRecord(J->ev[1], st));
@@ -1533,7 +1539,7 @@ static int prepare_decode(b2k_device_job* J, const b2k_block* blocks, uint64_t n
 static int enqueue_t1_decode_own(b2k_device_job* J, cudaStream_t st)
 {
   const uint32_t n = (uint32_t)J->h_enc_desc.size();
-  b2k_launch_build_dec_desc(J->d_enc_desc, J->d_out, J->d_offsets, J->d_dec_quant, J->d_dec_desc, n, st);
+  b2k_launch_build_dec_desc(J->d_enc_desc, J->d_out, J->d_offsets, J->d_dec_quant, J->d_dec_desc, n, J->bytes_cap, st);
   b2k_launch_ht_decode(J->d_dec_desc, J->d_bytes, J->d_recs, J->d_dec_status, n, J->max_cblk_w, J->d_err, J->cp.irreversible, 0, st);
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -1570,6 +1576,7 @@ extern "C" int32_t b2k_job_t1_decode_blocks(b2k_device_job* J, const b2k_block* 
   if(!J || !blocks || (!bytes && num_bytes)) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
   cudaStream_t st = J->eng->stream;
+  J->arena_sized = false;
   if(num_bytes + 64 > J->bytes_cap)
   {
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -1612,15 +1619,18 @@ extern "C" int32_t b2k_job_t1_decode_blocks(b2k_device_job* J, const b2k_block* 
 
 /* One device-resident round trip, enqueued back to back with a single synchronisation at the end:
    forward (DC shift + MCT + DWT) -> block encode -> scan + compact -> block decode -> inverse.
-   stage_ms[4] (optional) = forward, encode (incl. scan/compact), decode, inverse from CUDA events. */
+   stage_ms[4] (optional) = forward, encode (incl. scan/compact), decode, inverse from CUDA events.  The arena is sized by
+   one synchronising pass over each newly uploaded image; a 9/7 step codes the previous step's reconstruction, whose size
+   can drift past that estimate's slack: then the call returns 2 with the arena grown, and the image planes hold the
+   reconstruction of a partial decode, so the caller uploads the image again before calling again. */
 extern "C" int32_t b2k_job_roundtrip(b2k_device_job* J, float* ms_total, float* stage_ms, uint64_t* total_bytes)
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
   cudaStream_t st = J->eng->stream;
   const uint32_t n = (uint32_t)J->h_enc_desc.size();
-  if(J->bytes_cap == 0)
-  { /* first use: size the arena (one synchronising pass) */
+  if(!J->arena_sized)
+  { /* a new image: size the arena from a coding of it (one synchronising pass) */
     float t;
     uint64_t b;
     if(int rc = b2k_job_forward(J, &t)) return rc;
@@ -1641,14 +1651,15 @@ extern "C" int32_t b2k_job_roundtrip(b2k_device_job* J, float* ms_total, float* 
   CUDA_TRY(cudaEventSynchronize(J->ev[6]));
   CUDA_TRY(cudaGetLastError());
   if(J->h_offsets[n] > J->bytes_cap)
-  { /* arena estimate too small (content changed): grow and let the caller repeat */
+  { /* arena estimate too small (a 9/7 step drifted past its slack): grow; the caller uploads again and repeats */
     cudaFree(J->d_bytes);
     J->bytes_cap = J->h_offsets[n] + J->h_offsets[n] / 8 + 4096;
     CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
-    g_err = "coded size grew past the arena: arena resized, call again";
+    g_err = "coded size grew past the arena: arena resized; the image planes hold a partial decode, upload again";
     return 2;
   }
   J->bytes_used = J->h_offsets[n];
+  J->arena_sized = true;
   float t[5] = {0, 0, 0, 0, 0};
   cudaEventElapsedTime(&t[0], J->ev[0], J->ev[1]);
   cudaEventElapsedTime(&t[1], J->ev[1], J->ev[2]);
@@ -1674,7 +1685,8 @@ extern "C" int32_t b2k_job_roundtrip(b2k_device_job* J, float* ms_total, float* 
 /* n device-resident round trips queued back to back on the stream, ONE synchronisation after the last: what a
    benchmark step loop should cost when the host is not in the way (several ranks on one box).  Times come from
    events recorded per step: ms_total = first step's start to last step's end; stage_ms[4] and level1_ms are sums
-   over the steps.  Returns 2 once if the coded size outgrew the arena (it has been resized: call again). */
+   over the steps.  Returns 2 if the coded size outgrew the arena, as b2k_job_roundtrip does (arena resized, image planes
+   no longer the input: upload again before calling again). */
 extern "C" int32_t b2k_job_roundtrip_n(b2k_device_job* J, uint32_t steps, float* ms_total, float* stage_ms, float* level1_ms,
                                        uint64_t* total_bytes)
 {
@@ -1682,8 +1694,8 @@ extern "C" int32_t b2k_job_roundtrip_n(b2k_device_job* J, uint32_t steps, float*
   CUDA_TRY(cudaSetDevice(J->eng->device));
   cudaStream_t st = J->eng->stream;
   const uint32_t n = (uint32_t)J->h_enc_desc.size();
-  if(J->bytes_cap == 0)
-  { /* first use: size the arena (one synchronising pass) */
+  if(!J->arena_sized)
+  { /* a new image: size the arena from a coding of it (one synchronising pass) */
     float t;
     uint64_t b;
     if(int rc = b2k_job_forward(J, &t)) return rc;
@@ -1720,10 +1732,11 @@ extern "C" int32_t b2k_job_roundtrip_n(b2k_device_job* J, uint32_t steps, float*
     cudaFree(J->d_bytes);
     J->bytes_cap = J->h_offsets[n] + J->h_offsets[n] / 8 + 4096;
     CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
-    g_err = "coded size grew past the arena: arena resized, call again";
+    g_err = "coded size grew past the arena: arena resized; the image planes hold a partial decode, upload again";
     return 2;
   }
   J->bytes_used = J->h_offsets[n];
+  J->arena_sized = true;
   float sums[4] = {0, 0, 0, 0}, l1 = 0, tot = 0;
   for(uint32_t s = 0; s < steps; ++s)
   {
@@ -1760,7 +1773,7 @@ extern "C" int32_t b2k_job_roundtrip_n(b2k_device_job* J, uint32_t steps, float*
    per block, the scan a single CTA) run under the issue-bound kernels of its neighbours; the inverse transform again
    runs alone after all ranges have joined.  Ranges are independent except for the byte offsets of the compacted arena,
    which chain from one range's scan to the next (event per range).  stage_ms[3] = forward, block coder (encode + decode
-   together), inverse.  Same results as b2k_job_roundtrip_n, byte for byte. */
+   together), inverse.  Same results as b2k_job_roundtrip_n, byte for byte, return code 2 included. */
 extern "C" int32_t b2k_job_roundtrip_pipelined_n(b2k_device_job* J, uint32_t steps, uint32_t chunks, uint32_t streams, float* ms_total,
                                                  float* stage_ms, float* level1_ms, uint64_t* total_bytes)
 {
@@ -1768,8 +1781,8 @@ extern "C" int32_t b2k_job_roundtrip_pipelined_n(b2k_device_job* J, uint32_t ste
   CUDA_TRY(cudaSetDevice(J->eng->device));
   cudaStream_t st = J->eng->stream;
   const uint32_t n = (uint32_t)J->h_enc_desc.size();
-  if(J->bytes_cap == 0)
-  { /* first use: size the arena (one synchronising pass) */
+  if(!J->arena_sized)
+  { /* a new image: size the arena from a coding of it (one synchronising pass) */
     float t;
     uint64_t b;
     if(int rc = b2k_job_forward(J, &t)) return rc;
@@ -1821,7 +1834,8 @@ extern "C" int32_t b2k_job_roundtrip_pipelined_n(b2k_device_job* J, uint32_t ste
       b2k_launch_scan_lengths(J->d_out + b0, J->d_offsets + b0, nb, ps);
       CUDA_TRY(cudaEventRecord(J->p_ev[2 * c], ps));
       b2k_launch_ht_gather(J->d_enc_desc + b0, J->d_out + b0, J->d_offsets + b0, J->d_scratch, J->d_bytes, nb, J->bytes_cap, ps);
-      b2k_launch_build_dec_desc(J->d_enc_desc + b0, J->d_out + b0, J->d_offsets + b0, J->d_dec_quant + b0, J->d_dec_desc + b0, nb, ps);
+      b2k_launch_build_dec_desc(J->d_enc_desc + b0, J->d_out + b0, J->d_offsets + b0, J->d_dec_quant + b0, J->d_dec_desc + b0, nb,
+                                J->bytes_cap, ps);
       b2k_launch_ht_decode(J->d_dec_desc + b0, J->d_bytes, J->d_recs, J->d_dec_status + b0, nb, J->max_cblk_w, J->d_err,
                            J->cp.irreversible, 0, ps);
       CUDA_TRY(cudaEventRecord(J->p_ev[2 * c + 1], ps));
@@ -1842,10 +1856,11 @@ extern "C" int32_t b2k_job_roundtrip_pipelined_n(b2k_device_job* J, uint32_t ste
     cudaFree(J->d_bytes);
     J->bytes_cap = J->h_offsets[n] + J->h_offsets[n] / 8 + 4096;
     CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
-    g_err = "coded size grew past the arena: arena resized, call again";
+    g_err = "coded size grew past the arena: arena resized; the image planes hold a partial decode, upload again";
     return 2;
   }
   J->bytes_used = J->h_offsets[n];
+  J->arena_sized = true;
   float sums[3] = {0, 0, 0}, l1 = 0, tot = 0;
   for(uint32_t s = 0; s < steps; ++s)
   {

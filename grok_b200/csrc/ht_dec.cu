@@ -921,18 +921,20 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32)
 } /* namespace */
 
 /* decode descriptors of the engine's OWN last encode, built on the device (device-resident round trip):
-   length/offset from the encoder's outputs, numbps = 1 as the encoder signals (CoderOJPH.cpp L203-206) */
+   length/offset from the encoder's outputs, numbps = 1 as the encoder signals (CoderOJPH.cpp L203-206).  A block that does
+   not fit the arena of `cap` bytes was not compacted (k_ht_gather): it decodes as an empty block, so that no decode reads
+   past the arena when the coded size outgrew it */
 namespace {
 __global__ void k_build_dec_desc(const HtBlockDesc* __restrict__ enc, const HtBlockOut* __restrict__ outs,
                                  const uint64_t* __restrict__ offsets, const float* __restrict__ dec_quant,
-                                 HtBlockDesc* __restrict__ dec, uint32_t n)
+                                 HtBlockDesc* __restrict__ dec, uint32_t n, uint64_t cap)
 {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if(i >= n)
     return;
   HtBlockDesc d = enc[i];
   const uint32_t t = outs[i].total;
-  d.length = t == 0xFFFFFFFFu ? 0 : t;
+  d.length = (t == 0xFFFFFFFFu || offsets[i] + t > cap) ? 0 : t;
   d.slot_off = offsets[i];
   d.mmsbs = (uint8_t)(d.kmax - 1);
   d.passes = 1;
@@ -942,11 +944,11 @@ __global__ void k_build_dec_desc(const HtBlockDesc* __restrict__ enc, const HtBl
 }
 } // namespace
 void b2k_launch_build_dec_desc(const HtBlockDesc* d_enc, const HtBlockOut* d_out, const uint64_t* d_offsets,
-                               const float* d_dec_quant, HtBlockDesc* d_dec, uint32_t n, cudaStream_t st)
+                               const float* d_dec_quant, HtBlockDesc* d_dec, uint32_t n, uint64_t cap, cudaStream_t st)
 {
   if(!n)
     return;
-  k_build_dec_desc<<<(n + 255) / 256, 256, 0, st>>>(d_enc, d_out, d_offsets, d_dec_quant, d_dec, n);
+  k_build_dec_desc<<<(n + 255) / 256, 256, 0, st>>>(d_enc, d_out, d_offsets, d_dec_quant, d_dec, n, cap);
   b2k_count_launch();
 }
 

@@ -525,8 +525,11 @@ B2K_API int32_t b2k_job_forward(b2k_device_job* j, float* ms);  /* DC shift+MCT+
 B2K_API int32_t b2k_job_t1_encode(b2k_device_job* j, float* ms, uint64_t* total_bytes);
 B2K_API int32_t b2k_job_t1_decode(b2k_device_job* j, float* ms);/* from the job's own coded blocks */
 B2K_API int32_t b2k_job_inverse(b2k_device_job* j, float* ms);  /* inverse DWT+MCT into image */
-/* all four stages enqueued back to back, one synchronisation; stage_ms[4] optional; returns 2 once if the
- * coded size outgrew the arena (arena resized: call again) */
+/* all four stages enqueued back to back, one synchronisation; stage_ms[4] optional.  The first call after an upload
+ * (or after b2k_job_inverse) sizes the byte arena for the job's image (one extra synchronising pass).  Returns 2 if the coded size outgrew the
+ * arena (a 9/7 step codes the previous step's reconstruction): the arena has been resized, and the image planes hold
+ * the reconstruction of a partial decode, so upload the image again before calling again.  The same holds for
+ * b2k_job_roundtrip_n and b2k_job_roundtrip_pipelined_n. */
 B2K_API int32_t b2k_job_roundtrip(b2k_device_job* j, float* ms_total, float* stage_ms, uint64_t* total_bytes);
 /* `steps` round trips queued back to back with one synchronisation after the last (a benchmark loop without the
  * host in it); stage_ms[4] and level1_ms are sums over the steps, ms_total spans first start to last end. */
