@@ -66,7 +66,7 @@ assert BLOCK_DTYPE.itemsize == C.sizeof(Block), (BLOCK_DTYPE.itemsize, C.sizeof(
 # plugin_decompress (C++-ABI callback struct) is declared in csrc/plugin_decode_abi.h, not in the C header
 EXPORTS = ["minpf_post_load_plugin", "plugin_init", "plugin_get_debug_state", "gpup_encode_mem", "gpup_tile_free",
            "b2k_engine_create", "b2k_engine_destroy", "b2k_last_error", "b2k_host_alloc", "b2k_host_free",
-           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_enumerate",
+           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_enumerate",
            "b2k_result_to_gpup_tile", "b2k_job_create", "b2k_job_destroy", "b2k_job_upload", "b2k_job_forward",
            "b2k_job_t1_encode", "b2k_job_t1_decode", "b2k_job_t1_decode_blocks", "b2k_job_inverse", "b2k_job_roundtrip", "b2k_job_roundtrip_n", "b2k_job_roundtrip_pipelined_n", "b2k_job_download",
            "b2k_job_download_coeffs", "b2k_job_upload_coeffs", "b2k_job_fetch_result", "b2k_job_num_blocks",
@@ -260,6 +260,13 @@ def device_planes(image, numcomps, height, width, layout="CHW", writable=False):
             raise ValueError("component %d: row pitch %d / column step %d samples do not fit 32 bits" % (c, pitch, step))
         img.comp[c], img.row_pitch[c], img.col_step[c] = ptr, pitch, step
     return img
+
+
+class _DeviceBytes:
+    """A CUDA array interface over n bytes of device memory the engine owns (torch.as_tensor makes a view of it)."""
+
+    def __init__(self, ptr, n):
+        self.__cuda_array_interface__ = dict(shape=(n,), typestr="|u1", strides=None, data=(ptr, False), version=2)
 
 
 def _stream_handle(stream, image):
@@ -617,13 +624,36 @@ class Engine:
                        "b2k_decode_device")
         return ms.value
 
-    def encode_codestream_device(self, cp, image, flags=CS_TLM | CS_PLT, layout="CHW", stream=None):
-        """An image on the GPU -> a complete HTJ2K codestream (numpy uint8): b2k_encode_device + b2k_codestream_write."""
+    def encode_codestream_device(self, cp, image, flags=CS_TLM | CS_PLT, layout="CHW", stream=None, device_output=False):
+        """An image on the GPU -> a complete HTJ2K codestream (numpy uint8): b2k_encode_device + b2k_codestream_write.
+        device_output=True: the code stream is written on the GPU (b2k_encode_codestream_device, the same bytes) and
+        returned as a new torch.uint8 CUDA tensor, copied out of the engine's buffer on `stream`."""
+        if device_output:
+            return self._encode_codestream_on_device(cp, image, flags, layout, stream)
         res = self.encode_device(cp, image, layout=layout, stream=stream)
         try:
             return codestream_write(cp, res.blocks, res.bytes, flags, num_tiles=res.num_tiles)
         finally:
             res.free()
+
+    def _encode_codestream_on_device(self, cp, image, flags, layout, stream):
+        import torch
+        img = device_planes(image, cp.numcomps, cp.y1 - cp.y0, cp.x1 - cp.x0, layout)
+        handle = _stream_handle(stream, image)
+        L = lib()
+        L.b2k_encode_codestream_device.restype = C.c_int64
+        L.b2k_encode_codestream_device.argtypes = [C.c_void_p, C.POINTER(Coding), C.POINTER(DevicePlanes), C.c_uint32, C.c_void_p,
+                                                   C.POINTER(C.c_void_p)]
+        ptr = C.c_void_p()
+        n = L.b2k_encode_codestream_device(self._h, C.byref(cp), C.byref(img), flags, handle, C.byref(ptr))
+        if n <= 1:
+            _check_handled(n, "b2k_encode_codestream_device")
+        view = torch.as_tensor(_DeviceBytes(ptr.value, n), device="cuda:%d" % self.device)
+        s = torch.cuda.ExternalStream(handle, device=self.device) if handle else torch.cuda.default_stream(self.device)
+        with torch.cuda.stream(s):
+            out = torch.empty(n, dtype=torch.uint8, device="cuda:%d" % self.device)
+            out.copy_(view)
+        return out
 
     def decode_codestream_device(self, cs, out=None, dtype=None, layout="CHW", window=None, reduce=0, stream=None):
         """HTJ2K codestream -> (Coding, image on the GPU).  window (x0, y0, x1, y1 on the full-resolution canvas) and

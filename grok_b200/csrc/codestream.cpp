@@ -19,6 +19,8 @@
  */
 #include "geometry.h"
 #include "b2k_internal.h"
+#include "t2_packet.h"
+#include "t2_plan.h"
 
 #include <algorithm>
 #include <cstring>
@@ -26,6 +28,7 @@
 #include <vector>
 
 using namespace b2k;
+using t2::floorlog2;
 
 extern "C" const char* b2k_last_error(void);
 void b2k_set_error(const char* msg); /* engine.cu */
@@ -33,39 +36,8 @@ void b2k_set_error(const char* msg); /* engine.cu */
 namespace
 {
 
-/* ---- packet-header bit I/O: MSB first, the byte after 0xFF carries 7 bits (T.800 B.10.1) ---------------- */
-struct BitWriter
-{
-  std::vector<uint8_t>& out;
-  uint32_t acc = 0;
-  int cap = 8, room = 8; /* bits the current byte holds / still free */
-  explicit BitWriter(std::vector<uint8_t>& o) : out(o) {}
-  void put(uint32_t bit)
-  {
-    --room;
-    acc |= (bit & 1u) << room;
-    if(room == 0)
-      emit();
-  }
-  void put_bits(uint32_t v, int n)
-  {
-    for(int i = n - 1; i >= 0; --i)
-      put((v >> i) & 1u);
-  }
-  void emit()
-  {
-    out.push_back((uint8_t)acc);
-    cap = room = (acc == 0xFF) ? 7 : 8;
-    acc = 0;
-  }
-  void flush()
-  {
-    if(room != cap)
-      emit();
-    if(!out.empty() && out.back() == 0xFF)
-      emit(); /* a header must not end on 0xFF: the stuffed byte follows */
-  }
-};
+/* ---- packet-header bit reader: MSB first, the byte after 0xFF carries 7 bits (T.800 B.10.1); the writer is
+   t2::BitWriter ---------------------------------------------------------------------------------------------------- */
 struct BitReader
 {
   const uint8_t* p;
@@ -108,7 +80,7 @@ struct BitReader
   }
 };
 
-/* ---- tag tree (T.800 B.10.2) ---------------------------------------------------------------------------- */
+/* ---- tag-tree decoder (T.800 B.10.2); the encoder is t2::tag_encode ---------------------------------------- */
 struct TagTree
 {
   struct Node
@@ -148,45 +120,6 @@ struct TagTree
         for(uint32_t x = 0; x < dims[l].first; ++x)
           nodes[base[l] + (size_t)y * dims[l].first + x].parent = (int)(base[l + 1] + (size_t)(y / 2) * dims[l + 1].first + x / 2);
   }
-  void set_value(uint32_t leaf, uint32_t v)
-  { /* encoder: a node holds the minimum of its leaves */
-    int n = (int)leaf;
-    while(n >= 0 && nodes[n].value > v)
-    {
-      nodes[n].value = v;
-      n = nodes[n].parent;
-    }
-  }
-  void encode(BitWriter& bw, uint32_t leaf, uint32_t threshold)
-  {
-    int path[32], np = 0;
-    for(int n = (int)leaf; n >= 0; n = nodes[n].parent)
-      path[np++] = n;
-    uint32_t low = 0;
-    for(int i = np - 1; i >= 0; --i)
-    {
-      Node& nd = nodes[path[i]];
-      if(low > nd.low)
-        nd.low = low;
-      else
-        low = nd.low;
-      while(low < threshold)
-      {
-        if(low >= nd.value)
-        {
-          if(!nd.known)
-          {
-            bw.put(1);
-            nd.known = true;
-          }
-          break;
-        }
-        bw.put(0);
-        ++low;
-      }
-      nd.low = low;
-    }
-  }
   /* true if the leaf's value is < threshold (then nodes[leaf].value holds it) */
   bool decode(BitReader& br, uint32_t leaf, uint32_t threshold)
   {
@@ -214,29 +147,15 @@ struct TagTree
   }
 };
 
-inline int floorlog2(uint32_t v)
-{
-  int l = 0;
-  while(v > 1)
-  {
-    v >>= 1;
-    ++l;
-  }
-  return l;
-}
-
 /* ---- packets of a tile in LRCP order, with where their blocks sit in the tile's enumeration ---------------- */
-struct PacketBand
-{
-  uint32_t first = 0, gw = 0, gh = 0; /* first block (index into the tile's blocks), code-block grid of the precinct */
-};
+typedef t2::BandGrid PacketBand; /* first block (index into the tile's blocks), code-block grid of the precinct */
 struct Packet
 {
   uint16_t comp;
   uint8_t resno, nbands;
   uint32_t precno;
   uint32_t xpos, ypos; /* where the position-driven progressions meet this precinct on the reference grid (B.12.1.3-5) */
-  PacketBand band[3];
+  PacketBand band[3] = {};
 };
 /* mirrors enumerate_tile_blocks() (geometry.cpp): same loops, counts instead of blocks */
 /* prog: 0 LRCP, 1 RLCP, 2 RPCL, 3 PCRL, 4 CPRL (one layer, so the first two coincide) */
@@ -480,86 +399,36 @@ int plan_tile_packets(const b2k_coding& cp, const Rect& tile, const b2k_block* b
     err = "block table does not match the tile's enumeration";
     return -1;
   }
-  TagTree incl, imsb;
-  std::vector<uint8_t> hdr;
+  std::vector<t2::TagNode> tags;
+  auto code = [blk](uint32_t i) {
+    const b2k_block& B = blk[i];
+    return t2::BlockCode{B.length, B.length2, B.numpasses, B.numbps, B.kmax};
+  };
+  uint8_t kmax = 0;
+  for(uint32_t i = 0; i < nblk; ++i)
+    kmax = std::max(kmax, blk[i].kmax);
   for(const Packet& pk : pkts)
-  {
-    hdr.clear();
-    if(sop)
-    { /* SOP (A.8.1): marker, Lsop = 4, packet counter modulo 65536 (T2Compress.cpp L420-438) */
-      const uint8_t m[6] = {0xFF, 0x91, 0, 4, (uint8_t)(nsop >> 8), (uint8_t)nsop};
-      hdr.insert(hdr.end(), m, m + 6);
-      nsop = (nsop + 1) & 0xFFFF;
-    }
-    const size_t bits_at = hdr.size();
-    BitWriter bw(hdr);
-    bw.put(1); /* non-empty packet; like the reference also when it carries no block (T2Compress.cpp L304-307) */
-    for(int b = 0; b < pk.nbands; ++b)
+  { /* the header goes straight into plan.hdrs, grown to the bound first */
+    const size_t at = plan.hdrs.size();
+    plan.hdrs.resize(at + t2::packet_header_bound(pk.band, pk.nbands, kmax));
+    tags.resize(std::max<size_t>(tags.size(), t2::packet_tag_nodes(pk.band, pk.nbands)));
+    t2::BitWriter bw;
+    bw.init(plan.hdrs.data() + at, plan.hdrs.size() - at);
+    if(t2::packet_header(bw, pk.band, pk.nbands, code, tags.data(), nsop, sop, eph))
     {
-      const PacketBand& pb = pk.band[b];
-      const uint32_t n = pb.gw * pb.gh;
-      if(!n)
-        continue;
-      incl.init(pb.gw, pb.gh);
-      imsb.init(pb.gw, pb.gh);
-      for(uint32_t k = 0; k < n; ++k)
-      {
-        const b2k_block& B = blk[pb.first + k];
-        if(B.numpasses && B.length)
-        {
-          if(B.numbps > B.kmax || B.numpasses > 3)
-          {
-            err = "code block outside the writer's range (bit planes / passes)";
-            return -1;
-          }
-          incl.set_value(k, 0);
-          imsb.set_value(k, (uint32_t)B.kmax - B.numbps);
-        }
-        else
-          incl.set_value(k, 1); /* never included in the only layer */
-      }
-      for(uint32_t k = 0; k < n; ++k)
-      {
-        const b2k_block& B = blk[pb.first + k];
-        const bool in = B.numpasses && B.length;
-        incl.encode(bw, k, 1);
-        if(!in)
-          continue;
-        imsb.encode(bw, k, TagTree::INF);
-        /* number of passes (B.10.6): 1 -> 0, 2 -> 10, 3 -> 1100 */
-        if(B.numpasses == 1)
-          bw.put(0);
-        else if(B.numpasses == 2)
-          bw.put_bits(2, 2);
-        else
-          bw.put_bits(12, 4);
-        /* HT: cleanup segment, then one segment for the refinement passes (T.814 B.10.7) */
-        const uint32_t len1 = B.length, len2 = B.numpasses > 1 ? B.length2 : 0;
-        const int extra2 = B.numpasses > 1 ? floorlog2((uint32_t)B.numpasses - 1) : 0;
-        int lblock = 3, inc = 0;
-        inc = std::max(inc, floorlog2(len1) + 1 - lblock);
-        if(B.numpasses > 1)
-          inc = std::max(inc, floorlog2(std::max<uint32_t>(len2, 1)) + 1 - (lblock + extra2));
-        for(int i = 0; i < inc; ++i)
-          bw.put(1);
-        bw.put(0);
-        lblock += inc;
-        bw.put_bits(len1, lblock);
-        if(B.numpasses > 1)
-          bw.put_bits(len2, lblock + extra2);
-      }
+      err = "code block outside the writer's range (bit planes / passes)";
+      return -1;
     }
-    bw.flush();
-    (void)bits_at;
-    if(eph)
-    { /* EPH (A.8.2) */
-      hdr.push_back(0xFF);
-      hdr.push_back(0x92);
+    if(bw.n > bw.cap)
+    {
+      err = "packet header longer than its bound";
+      return -1;
     }
-    plan.hdrs.insert(plan.hdrs.end(), hdr.begin(), hdr.end());
-    plan.hdr_len.push_back((uint32_t)hdr.size());
+    nsop = (nsop + 1) & 0xFFFF;
+    plan.hdrs.resize(at + bw.n);
+    plan.hdr_len.push_back((uint32_t)bw.n);
     plan.res_of.push_back(pk.resno);
-    uint64_t plen = hdr.size();
+    uint64_t plen = bw.n;
     uint32_t ns = 0;
     for(int b = 0; b < pk.nbands; ++b)
     {
@@ -597,59 +466,50 @@ int plan_tile_packets(const b2k_coding& cp, const Rect& tile, const b2k_block* b
   return 0;
 }
 
-/* cut the planned packets into tile parts and build each part's PLT (A.7.3: 7 bits per byte, MSB = continuation) */
+/* where a tile's tile parts end (packet indices): one part for the whole tile, or one per run of packets of the same
+   resolution; a tile without packets still has one (empty) tile part */
+std::vector<size_t> tile_part_ends(const std::vector<uint8_t>& res_of, bool split_res)
+{
+  std::vector<size_t> ends;
+  const size_t np = res_of.size();
+  size_t p = 0;
+  do
+  {
+    const uint8_t r0 = np ? res_of[p] : 0;
+    while(p < np && (!split_res || res_of[p] == r0))
+      ++p;
+    ends.push_back(p);
+  } while(p < np);
+  return ends;
+}
+
+/* cut the planned packets into tile parts and build each part's PLT */
 void plan_tile_parts(TilePlan& P, bool split_res, bool want_plt)
 {
-  const size_t np = P.packet_len.size();
   size_t p = 0, h = 0, sg = 0;
-  do
+  for(const size_t end : tile_part_ends(P.res_of, split_res))
   {
     TilePlan::Part part;
     part.p0 = p;
     part.h0 = h;
     part.s0 = sg;
     uint64_t body = 0;
-    const uint8_t r0 = np ? P.res_of[p] : 0;
-    while(p < np && (!split_res || P.res_of[p] == r0))
+    for(; p < end; ++p)
     {
       body += P.packet_len[p];
       h += P.hdr_len[p];
       sg += P.nseg[p];
-      ++p;
     }
     part.p1 = p;
     if(want_plt)
     {
-      std::vector<uint8_t> seg;
-      uint8_t z = 0;
-      auto flush_seg = [&] {
-        put16(part.plt, 0xFF58);
-        put16(part.plt, (uint32_t)seg.size() + 3);
-        part.plt.push_back(z++);
-        part.plt.insert(part.plt.end(), seg.begin(), seg.end());
-        seg.clear();
-      };
-      for(size_t k = part.p0; k < part.p1; ++k)
-      {
-        uint32_t L = P.packet_len[k];
-        uint8_t tmp[5];
-        int nb = 0;
-        do
-        {
-          tmp[nb++] = (uint8_t)(L & 0x7F);
-          L >>= 7;
-        } while(L);
-        if(seg.size() + nb > 65535 - 3)
-          flush_seg();
-        for(int i = nb - 1; i >= 0; --i)
-          seg.push_back((uint8_t)(tmp[i] | (i ? 0x80 : 0)));
-      }
-      if(!seg.empty() || part.p0 == part.p1)
-        flush_seg();
+      auto len = [&P](uint64_t k) { return P.packet_len[k]; };
+      part.plt.resize(t2::plt_segments(len, part.p0, part.p1, nullptr));
+      t2::plt_segments(len, part.p0, part.p1, part.plt.data());
     }
     part.bytes = 12 + part.plt.size() + 2 + body;
     P.parts.push_back(std::move(part));
-  } while(p < np);
+  }
 }
 
 } // namespace
@@ -663,10 +523,7 @@ void emit_tile_parts(const TilePlan& P, uint32_t t, const uint8_t* arena, uint8_
   for(size_t pi = 0; pi < P.parts.size(); ++pi)
   {
     const TilePlan::Part& pt = P.parts[pi];
-    const uint32_t psot = (uint32_t)pt.bytes;
-    const uint8_t sot[12] = {0xFF, 0x90, 0, 10, (uint8_t)(t >> 8), (uint8_t)t, (uint8_t)(psot >> 24), (uint8_t)(psot >> 16),
-                             (uint8_t)(psot >> 8), (uint8_t)psot, (uint8_t)pi, (uint8_t)P.parts.size()}; /* SOT (A.4.2) */
-    memcpy(w, sot, 12);
+    t2::put_sot(w, t, (uint32_t)pt.bytes, (uint32_t)pi, (uint32_t)P.parts.size());
     w += 12;
     if(!pt.plt.empty())
     {
@@ -691,40 +548,34 @@ void emit_tile_parts(const TilePlan& P, uint32_t t, const uint8_t* arena, uint8_
   }
 }
 
-/* TLM (A.7.1): 16-bit tile index + 32-bit length per tile part, in codestream order; 10921 entries fit a segment */
+/* TLM segments (A.7.1) for n tile parts appended to head, their entries zero; returns where they start */
+size_t append_tlm_segments(std::vector<uint8_t>& head, uint64_t n)
+{
+  const size_t at = head.size();
+  head.resize(at + t2::tlm_bytes(n), 0);
+  for(uint64_t e0 = 0; e0 < n; e0 += t2::TLM_PER_SEGMENT)
+    t2::put_tlm_segment(head.data() + at, e0, std::min<uint64_t>(t2::TLM_PER_SEGMENT, n - e0));
+  return at;
+}
+/* TLM: 16-bit tile index + 32-bit length per tile part, in codestream order */
 void append_tlm(std::vector<uint8_t>& head, const std::vector<std::pair<uint32_t, uint32_t>>& ent)
 {
-  uint8_t z = 0;
-  for(size_t e0 = 0; e0 < ent.size(); e0 += 10000)
-  {
-    const size_t n = std::min<size_t>(10000, ent.size() - e0);
-    put16(head, 0xFF55);
-    put16(head, (uint32_t)(4 + 6 * n));
-    head.push_back(z++);
-    head.push_back(0x60); /* ST = 2 (16-bit Ttlm), SP = 1 (32-bit Ptlm) */
-    for(size_t e = e0; e < e0 + n; ++e)
-    {
-      put16(head, ent[e].first);
-      put32(head, ent[e].second);
-    }
-  }
+  const size_t at = append_tlm_segments(head, ent.size());
+  for(size_t e = 0; e < ent.size(); ++e)
+    t2::put_tlm_entry(head.data() + at, e, ent[e].first, ent[e].second);
 }
-} // namespace
 
-/* ============================================================================================================ */
-extern "C" __attribute__((visibility("default"))) int64_t b2k_codestream_write(const b2k_coding* cp, const b2k_result* r,
-                                                                                uint32_t flags, uint8_t* out, uint64_t cap)
+/* what b2k_codestream_write checks before it looks at a block: 0, or -1 with the error set */
+int check_whole_image(const b2k_coding& cp, uint32_t num_tiles, uint32_t flags)
 {
-  if(!cp || !r)
-    return -1;
-  if(const char* why = unsupported_reason(*cp))
+  if(const char* why = unsupported_reason(cp))
   {
     b2k_set_error(why);
     return -1;
   }
-  const TileGrid g = tile_grid(*cp);
+  const TileGrid g = tile_grid(cp);
   const uint32_t ntiles = g.nx * g.ny;
-  if(r->num_tiles != ntiles)
+  if(num_tiles != ntiles)
   {
     b2k_set_error("the result does not hold every tile of the image (gather the shards first)");
     return -1;
@@ -734,35 +585,54 @@ extern "C" __attribute__((visibility("default"))) int64_t b2k_codestream_write(c
     b2k_set_error("more than 65535 tiles");
     return -1;
   }
-  const std::vector<BandQuant> q = band_quant(*cp);
-  std::vector<uint8_t> head;
-  const int prog = (int)((flags >> 8) & 7);
-  if(prog > 4)
+  if(((flags >> 8) & 7) > 4)
   {
     b2k_set_error("unknown progression order");
     return -1;
   }
+  return 0;
+}
+
+/* blocks of tile t are [first[t], first[t + 1]); false if the table is not in tile order */
+bool tile_block_ranges(const b2k_block* blocks, uint64_t n, uint32_t ntiles, std::vector<uint64_t>& first)
+{
+  first.assign(ntiles + 1, 0);
+  uint64_t i = 0;
+  for(uint32_t t = 0; t < ntiles; ++t)
+  {
+    first[t] = i;
+    while(i < n && blocks[i].tile == t)
+      ++i;
+  }
+  first[ntiles] = i;
+  return i == n;
+}
+} // namespace
+
+/* ============================================================================================================ */
+extern "C" __attribute__((visibility("default"))) int64_t b2k_codestream_write(const b2k_coding* cp, const b2k_result* r,
+                                                                                uint32_t flags, uint8_t* out, uint64_t cap)
+{
+  if(!cp || !r)
+    return -1;
+  if(check_whole_image(*cp, r->num_tiles, flags))
+    return -1;
+  const TileGrid g = tile_grid(*cp);
+  const uint32_t ntiles = g.nx * g.ny;
+  const std::vector<BandQuant> q = band_quant(*cp);
+  std::vector<uint8_t> head;
+  const int prog = (int)((flags >> 8) & 7);
   const bool split_res = (flags & B2K_CS_TPARTS_R) != 0 && prog <= 2; /* a tile part per resolution needs a resolution-major order */
   const bool sop = (flags & B2K_CS_SOP) != 0, eph = (flags & B2K_CS_EPH) != 0;
   write_main_header(*cp, g, q, head, prog, sop, eph);
 
   /* plan every tile part (their lengths feed TLM), then lay the codestream out */
   std::vector<TilePlan> plans(ntiles);
-  std::vector<uint64_t> tile_first(ntiles + 1, 0);
+  std::vector<uint64_t> tile_first;
+  if(!tile_block_ranges(r->blocks, r->num_blocks, ntiles, tile_first))
   {
-    uint64_t i = 0;
-    for(uint32_t t = 0; t < ntiles; ++t)
-    {
-      tile_first[t] = i;
-      while(i < r->num_blocks && r->blocks[i].tile == t)
-        ++i;
-    }
-    tile_first[ntiles] = i;
-    if(i != r->num_blocks)
-    {
-      b2k_set_error("block table is not in tile order");
-      return -1;
-    }
+    b2k_set_error("block table is not in tile order");
+    return -1;
   }
   std::vector<std::string> errs(ntiles);
   b2k_host_parallel(ntiles, [&](size_t t) { /* tiles are independent: plan them on the host pool */
@@ -816,6 +686,79 @@ extern "C" __attribute__((visibility("default"))) int64_t b2k_codestream_write(c
   *w++ = 0xFF; /* EOC */
   *w++ = 0xD9;
   return (int64_t)(w - out);
+}
+
+int b2k_t2_plan(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks, uint64_t nblocks, uint32_t num_tiles, t2::Plan& plan)
+{
+  if(check_whole_image(cp, num_tiles, flags))
+    return -1;
+  const TileGrid g = tile_grid(cp);
+  const uint32_t ntiles = g.nx * g.ny;
+  const int prog = (int)((flags >> 8) & 7);
+  const bool split_res = (flags & B2K_CS_TPARTS_R) != 0 && prog <= 2;
+  plan = t2::Plan();
+  plan.flags = flags;
+  write_main_header(cp, g, band_quant(cp), plan.head, prog, (flags & B2K_CS_SOP) != 0, (flags & B2K_CS_EPH) != 0);
+  std::vector<uint64_t> tile_first;
+  if(!tile_block_ranges(blocks, nblocks, ntiles, tile_first))
+  {
+    b2k_set_error("block table is not in tile order");
+    return -1;
+  }
+  std::vector<Packet> pkts;
+  std::vector<uint8_t> res_of;
+  for(uint32_t t = 0; t < ntiles; ++t)
+  {
+    uint32_t expect = 0;
+    tile_packets(cp, tile_rect(cp, g, t), pkts, expect, prog);
+    if(expect != tile_first[t + 1] - tile_first[t])
+    {
+      b2k_set_error("block table does not match the tile's enumeration");
+      return -1;
+    }
+    uint8_t kmax = 0;
+    for(uint64_t i = tile_first[t]; i < tile_first[t + 1]; ++i)
+      kmax = std::max(kmax, blocks[i].kmax);
+    const uint64_t p_first = plan.packets.size();
+    res_of.clear();
+    for(size_t k = 0; k < pkts.size(); ++k)
+    {
+      const Packet& pk = pkts[k];
+      t2::DevPacket d{};
+      for(int b = 0; b < pk.nbands; ++b)
+        d.band[b] = t2::BandGrid{(uint32_t)tile_first[t] + pk.band[b].first, pk.band[b].gw, pk.band[b].gh};
+      d.nbands = pk.nbands;
+      d.sop = (uint32_t)(k & 0xFFFF);
+      const uint64_t cap = t2::packet_header_bound(pk.band, pk.nbands, kmax);
+      if(cap > 0xFFFFFFFFull)
+      {
+        b2k_set_error("packet longer than 4 GiB");
+        return -1;
+      }
+      d.hdr_cap = (uint32_t)cap;
+      d.hdr_at = plan.hdr_bytes;
+      d.tag_at = plan.tag_nodes;
+      plan.hdr_bytes += cap;
+      plan.tag_nodes += t2::packet_tag_nodes(pk.band, pk.nbands);
+      plan.packets.push_back(d);
+      res_of.push_back(pk.resno);
+    }
+    const std::vector<size_t> ends = tile_part_ends(res_of, split_res);
+    if(ends.size() > 255)
+    {
+      b2k_set_error("more than 255 tile parts");
+      return -1;
+    }
+    size_t p0 = 0;
+    for(size_t i = 0; i < ends.size(); ++i)
+    {
+      plan.parts.push_back(t2::DevPart{p_first + p0, p_first + ends[i], t, (uint32_t)i, (uint32_t)ends.size()});
+      p0 = ends[i];
+    }
+  }
+  if(flags & B2K_CS_TLM)
+    plan.tlm_at = append_tlm_segments(plan.head, plan.parts.size());
+  return 0;
 }
 
 /* ---- per-rank writers (SURVEY.md 8e: "T2 can itself be sharded per tile; the writer concatenates in index order") ------

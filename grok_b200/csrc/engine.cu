@@ -31,6 +31,7 @@
 
 #include "b2k_internal.h"
 #include "geometry.h"
+#include "t2_device.h"
 
 using namespace b2k;
 
@@ -62,6 +63,8 @@ struct b2k_engine
   std::mutex mu;
   b2k_device_job* cached = nullptr;
   cudaEvent_t caller_ev = nullptr; /* b2k_encode_device / b2k_decode_device: orders the engine's streams after the caller's */
+  uint8_t* d_cs = nullptr;         /* b2k_encode_codestream_device: the last code stream */
+  uint64_t cs_cap = 0;
 };
 
 /* ---- device memory cache --------------------------------------------------------------------------------------
@@ -375,6 +378,7 @@ struct b2k_device_job
   std::vector<cudaEvent_t> p_ev;   /* per-chunk events of b2k_job_roundtrip_pipelined_n (scan done, chunk done) */
   std::vector<cudaStream_t> p_streams; /* its block-coder streams */
   bool dec_has_refinement = false; /* the block table of the current decode carries SigProp / MagRef passes */
+  T2Job* t2 = nullptr;             /* b2k_encode_codestream_device: the code stream's plan for the flags of the last call */
 };
 
 /* -------------------------------------------------------------------------------------------- */
@@ -435,6 +439,7 @@ extern "C" void b2k_engine_destroy(b2k_engine* e)
       cudaStreamDestroy(a);
   if(e->caller_ev)
     cudaEventDestroy(e->caller_ev);
+  cudaFree(e->d_cs);
   delete e;
 }
 
@@ -832,6 +837,7 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
     return;
   cudaSetDevice(J->eng->device);
   cudaStreamSynchronize(J->eng->stream);
+  b2k_t2_destroy(J->t2);
   cudaFree(J->img.base);
   cudaFree(J->d_stage);
   cudaFree(J->coef.base);
@@ -2161,11 +2167,44 @@ static b2k_device_job* cached_job(b2k_engine* e, const b2k_coding* cp, uint32_t 
   return J;
 }
 
-/* T.user: the caller's samples.  A device image (b2k_encode_device) is read after the work queued on `caller` */
-static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, uint32_t rem, b2k_result** out, Transport& T,
-                             cudaStream_t caller = nullptr)
+/* b2k_encode_codestream_device: the code stream is written on the device (t2_device.cu) instead of a result coming home */
+struct DeviceCodestream
 {
-  if(!e || !cp || !out)
+  uint32_t flags;
+  int64_t length = 0;
+};
+
+/* T2 on the device after the block coder, into the engine's code-stream buffer (grown, and T2 run again, when the code
+   stream outgrows it).  The call's one synchronisation reads the length. */
+static int device_t2(b2k_engine* e, b2k_device_job* J, cudaStream_t st, DeviceCodestream& dc)
+{
+  for(;;)
+  {
+    if(b2k_t2_enqueue(J->t2, J->d_enc_desc, J->d_out, J->d_scratch, e->d_cs, e->cs_cap, st))
+      return -1;
+    CUDA_TRY(cudaStreamSynchronize(st));
+    const int64_t n = b2k_t2_result(J->t2);
+    if(n < 0)
+      return (int)n;
+    if((uint64_t)n <= e->cs_cap)
+    {
+      dc.length = n;
+      return 0;
+    }
+    cudaFree(e->d_cs);
+    e->d_cs = nullptr;
+    e->cs_cap = 0;
+    CUDA_TRY(cudaMalloc(&e->d_cs, (uint64_t)n + (uint64_t)n / 8 + 4096));
+    e->cs_cap = (uint64_t)n + (uint64_t)n / 8 + 4096;
+  }
+}
+
+/* T.user: the caller's samples.  A device image (b2k_encode_device) is read after the work queued on `caller`.  With dc the
+   code stream is written on the device and *out is not touched. */
+static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, uint32_t rem, b2k_result** out, Transport& T,
+                             cudaStream_t caller = nullptr, DeviceCodestream* dc = nullptr)
+{
+  if(!e || !cp || (!out && !dc))
     return -1;
   std::lock_guard<std::mutex> lock(e->mu);
   int rc = 0;
@@ -2173,6 +2212,14 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
   if(rc)
     return rc;
   CUDA_TRY(cudaSetDevice(e->device));
+  if(dc && (!J->t2 || b2k_t2_flags(J->t2) != dc->flags))
+  { /* geometry and flags only: planned once for every frame of this coding */
+    b2k_t2_destroy(J->t2);
+    J->t2 = nullptr;
+    if(b2k_t2_create(*cp, dc->flags, J->blocks.data(), J->blocks.size(), (uint32_t)J->tiles.size(), J->coded_index.data(),
+                     J->coded_index.size(), &J->t2))
+      return -1;
+  }
   const auto wall0 = std::chrono::steady_clock::now();
   if(resolve_transport(J, T, false))
     return -1;
@@ -2191,7 +2238,7 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
   const size_t nchunks = J->chunk_tile.size() - 1;
   /* the arena size of the previous call is the estimate: scan + compact + return every chunk's bytes while later
      chunks are still arriving (the D2H direction of PCIe is otherwise idle) */
-  const bool streamed = J->bytes_cap > 0 && nchunks > 1;
+  const bool streamed = !dc && J->bytes_cap > 0 && nchunks > 1;
   uint8_t* hb = nullptr;
   struct ArenaGuard /* the pinned arena goes back to the pool on every early return until a result owns it */
   {
@@ -2275,6 +2322,8 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
     CUDA_TRY(cudaStreamWaitEvent(caller, e->caller_ev, 0));
   }
   DBG_T("encode: chunks enqueued");
+  if(dc)
+    return device_t2(e, J, st, *dc);
   b2k_result* R = nullptr;
   const uint32_t nb_all = (uint32_t)J->h_enc_desc.size();
   b2k_result* shell = result_shell(J); /* host work while the device finishes the last chunks */
@@ -2425,6 +2474,22 @@ extern "C" int32_t b2k_encode_device(b2k_engine* e, const b2k_coding* cp, const 
   Transport T;
   device_samples(T, *img, cp->x0, cp->y0);
   return encode_common(e, cp, tile_mod, tile_rem, out, T, caller_stream(cuda_stream));
+}
+
+extern "C" int64_t b2k_encode_codestream_device(b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img, uint32_t flags,
+                                                void* cuda_stream, const uint8_t** cs)
+{
+  if(!e || !cp || !cs)
+    return -1;
+  if(int rc = check_device_planes(e, cp, img))
+    return rc;
+  Transport T;
+  device_samples(T, *img, cp->x0, cp->y0);
+  DeviceCodestream dc{flags};
+  if(int32_t rc = encode_common(e, cp, 1, 0, nullptr, T, caller_stream(cuda_stream), &dc))
+    return rc;
+  *cs = e->d_cs;
+  return dc.length;
 }
 
 extern "C" int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,

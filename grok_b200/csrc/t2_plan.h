@@ -1,0 +1,46 @@
+/*
+ * grok_b200/csrc/t2_plan.h -- what the device code-stream writer (t2_device.cu) needs to know about an image's code
+ * stream before any block is coded: its packets in code-stream order, its tile parts and its main header.  Geometry
+ * and flags only, so one plan serves every frame of a job.  Built on the host by b2k_t2_plan (codestream.cpp) from the
+ * same tile_packets() / tile-part rule / main header the host writer uses.
+ */
+#pragma once
+#include <stdint.h>
+#include <vector>
+#include "t2_packet.h"
+#include "../../include/grok_b200.h"
+
+namespace b2k
+{
+namespace t2
+{
+struct DevPacket /* one packet, in code-stream order */
+{
+  BandGrid band[3];  /* band[b].first: index into the image's block enumeration */
+  uint32_t nbands;
+  uint32_t sop;      /* SOP counter: the packet's index in its tile, modulo 65536 */
+  uint32_t hdr_cap;  /* header bytes reserved (packet_header_bound) */
+  uint64_t hdr_at;   /* where they are reserved in the header scratch */
+  uint64_t tag_at;   /* its tag-tree scratch, in nodes (packet_tag_nodes) */
+};
+struct DevPart /* one tile part, in code-stream order: packets [p0, p1) */
+{
+  uint64_t p0, p1;
+  uint32_t tile, index, count; /* tile index, index of the part in its tile, tile parts of the tile */
+};
+struct Plan
+{
+  uint32_t flags = 0;
+  std::vector<uint8_t> head; /* SOC .. QCD, then the TLM segments with their entries zero */
+  uint64_t tlm_at = 0;       /* where the TLM segments start in head */
+  std::vector<DevPacket> packets;
+  std::vector<DevPart> parts;
+  uint64_t hdr_bytes = 0, tag_nodes = 0;
+};
+} // namespace t2
+} // namespace b2k
+
+/* the plan of the code stream b2k_codestream_write(cp, r, flags) writes, for the block table `blocks` (every block of the
+   tiles of r, enumeration order) and r->num_tiles = num_tiles.  0, or -1 with b2k_last_error set in the cases, and with the
+   text, of b2k_codestream_write. */
+int b2k_t2_plan(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks, uint64_t nblocks, uint32_t num_tiles, b2k::t2::Plan& plan);

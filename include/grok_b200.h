@@ -503,6 +503,19 @@ B2K_API int32_t b2k_encode_device(b2k_engine* e, const b2k_coding* cp, const b2k
 B2K_API int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
                                   const uint8_t* bytes, uint64_t num_bytes, const b2k_device_planes* img, const uint32_t* window,
                                   uint32_t tile_mod, uint32_t tile_rem, void* cuda_stream, double* ms_total);
+/* An image in device memory -> a complete HTJ2K code stream assembled in device memory, byte-identical to
+ * b2k_encode_device + b2k_codestream_write(cp, result, flags) over the whole image; any flags b2k_codestream_write takes.
+ * *cs = device address of the code stream, in a buffer the engine owns; valid until the next call of this function on e,
+ * or b2k_engine_destroy.  Returns the length (> 1); 1 not handled (as b2k_encode_device); < 0 on error: -2 a block
+ * overflowed the coder (as b2k_encode_device), -1 otherwise, in the cases and with the b2k_last_error text of
+ * b2k_encode_device and b2k_codestream_write (a tile grid the writer declines, more than 65535 tiles, more than 255 tile
+ * parts in a tile, a tile part of 4 GiB or more, ...).
+ * Input ordering on cuda_stream as b2k_encode_device; returns once the code stream is written.  Packet headers, PLT, TLM
+ * and the tile-part layout are computed by kernels and the block bytes go from the coder's scratch to the file without
+ * leaving the GPU: no block table or arena crosses PCIe, only the final length does.  The plan of the code stream
+ * (geometry and flags) is made once per coding and flags and kept with the engine's cached job. */
+B2K_API int64_t b2k_encode_codestream_device(b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img,
+                                             uint32_t flags, void* cuda_stream, const uint8_t** cs);
 
 /* Geometry only (host): enumerate the blocks of the selected tiles, lengths zero.  Returns the
  * count; fills at most cap entries. */
