@@ -158,13 +158,15 @@ def to_sgnmag(coef, kmax):
 
 
 def enumerate_blocks(tc, numres, cbw_exp=6, cbh_exp=6, prcw_exp=None, prch_exp=None):
-    cap = 1 << 16
-    arr = (Block * cap)()
     pw = (C.c_uint8 * 33)(*prcw_exp) if prcw_exp is not None else None
     ph = (C.c_uint8 * 33)(*prch_exp) if prch_exp is not None else None
-    n = lib().orc_enumerate_blocks(tc[0], tc[1], tc[2], tc[3], numres, cbw_exp, cbh_exp, pw, ph, arr, cap)
-    assert n <= cap
-    return [arr[i] for i in range(n)]
+    cap = 256                          # orc_enumerate_blocks returns the whole count: grow and enumerate again
+    while True:
+        arr = (Block * cap)()
+        n = lib().orc_enumerate_blocks(tc[0], tc[1], tc[2], tc[3], numres, cbw_exp, cbh_exp, pw, ph, arr, cap)
+        if n <= cap:
+            return [arr[i] for i in range(n)]
+        cap = n
 
 
 def aligned_zeros(shape, dtype, align=64):
