@@ -66,7 +66,7 @@ assert BLOCK_DTYPE.itemsize == C.sizeof(Block), (BLOCK_DTYPE.itemsize, C.sizeof(
 # plugin_decompress (C++-ABI callback struct) is declared in csrc/plugin_decode_abi.h, not in the C header
 EXPORTS = ["minpf_post_load_plugin", "plugin_init", "plugin_get_debug_state", "gpup_encode_mem", "gpup_tile_free",
            "b2k_engine_create", "b2k_engine_destroy", "b2k_last_error", "b2k_host_alloc", "b2k_host_free",
-           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_enumerate",
+           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_decode_codestream_device", "b2k_codestream_parse_device", "b2k_codestream_parse_device_stats", "b2k_enumerate",
            "b2k_result_to_gpup_tile", "b2k_job_create", "b2k_job_destroy", "b2k_job_upload", "b2k_job_forward",
            "b2k_job_t1_encode", "b2k_job_t1_decode", "b2k_job_t1_decode_blocks", "b2k_job_inverse", "b2k_job_roundtrip", "b2k_job_roundtrip_n", "b2k_job_roundtrip_pipelined_n", "b2k_job_download",
            "b2k_job_download_coeffs", "b2k_job_upload_coeffs", "b2k_job_fetch_result", "b2k_job_num_blocks",
@@ -658,7 +658,13 @@ class Engine:
     def decode_codestream_device(self, cs, out=None, dtype=None, layout="CHW", window=None, reduce=0, stream=None):
         """HTJ2K codestream -> (Coding, image on the GPU).  window (x0, y0, x1, y1 on the full-resolution canvas) and
         reduce work as in decode_window (the Coding is then the virtual one).  out: a CUDA array of the (window's) shape
-        in `layout`, or None for a new torch tensor of `dtype` (default torch.uint16) on the engine's GPU."""
+        in `layout`, or None for a new torch tensor of `dtype` (default torch.uint16) on the engine's GPU.
+        cs may itself be on the engine's GPU (a 1-D contiguous uint8 CUDA array): it is then parsed there
+        (b2k_decode_codestream_device) and never crosses PCIe; window / reduce are not available on that path."""
+        if hasattr(cs, "__cuda_array_interface__"):
+            if window is not None or reduce:
+                raise NotHandled("decode_codestream_device: window / reduce are not available for a code stream in device memory")
+            return self._decode_device_codestream(cs, out, dtype, layout, stream)
         cs = np.ascontiguousarray(cs, dtype=np.uint8)
         if window is not None or reduce:
             cp, blocks, rect = codestream_parse_window(cs, window, reduce)
@@ -670,6 +676,65 @@ class Engine:
             shape = (cp.numcomps, y1 - y0, x1 - x0) if layout == "CHW" else (y1 - y0, x1 - x0, cp.numcomps)
             out = torch.empty(shape, dtype=torch.uint16 if dtype is None else dtype, device="cuda:%d" % self.device)
         self.decode_device(cp, blocks, cs, out, layout=layout, window=rect, stream=stream)
+        return cp, out
+
+    def _device_codestream_bytes(self, cs):
+        iface = cs.__cuda_array_interface__
+        shape = tuple(int(n) for n in iface["shape"])
+        if iface["typestr"][1:] != "u1" or len(shape) != 1:
+            raise ValueError("a device code stream is a 1-D uint8 CUDA array, not %s of shape %s" % (iface["typestr"], shape))
+        strides = iface.get("strides")
+        if strides is not None and shape[0] > 1 and int(strides[0]) != 1:
+            raise ValueError("a device code stream must be contiguous (strides %s)" % (tuple(strides),))
+        return int(iface["data"][0] or 0), shape[0]
+
+    def codestream_parse_device(self, cs, stream=None):
+        """b2k_codestream_parse_device: (Coding, block table) of a code stream on the engine's GPU, parsed there; the
+        same as codestream_parse of its bytes."""
+        ptr, n = self._device_codestream_bytes(cs)
+        L = lib()
+        L.b2k_codestream_parse_device.restype = C.c_int64
+        L.b2k_codestream_parse_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(Coding), C.c_void_p, C.c_uint64]
+        handle = _stream_handle(stream, cs)
+        cp = Coding()
+        nb = L.b2k_codestream_parse_device(self._h, ptr, n, handle, C.byref(cp), None, 0)
+        if nb < 0 or nb == 1:
+            raise (NotHandled if nb == 1 else EngineError)("b2k_codestream_parse_device: " + (L.b2k_last_error() or b"").decode())
+        blocks = np.zeros(nb, BLOCK_DTYPE)
+        m = L.b2k_codestream_parse_device(self._h, ptr, n, handle, C.byref(cp), blocks.ctypes.data, nb)
+        if m != nb:
+            raise (NotHandled if m == 1 else EngineError)("b2k_codestream_parse_device: " + (L.b2k_last_error() or b"").decode())
+        return cp, blocks
+
+    def codestream_parse_device_stats(self):
+        """(tiles parsed packet by packet from PLT, tiles walked) of the last device parse on this engine"""
+        ix, wk = C.c_uint32(), C.c_uint32()
+        L = lib()
+        L.b2k_codestream_parse_device_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+        _check(L.b2k_codestream_parse_device_stats(self._h, C.byref(ix), C.byref(wk)), "b2k_codestream_parse_device_stats")
+        return ix.value, wk.value
+
+    def _decode_device_codestream(self, cs, out, dtype, layout, stream):
+        ptr, n = self._device_codestream_bytes(cs)
+        L = lib()
+        L.b2k_codestream_parse_device.restype = C.c_int64
+        L.b2k_codestream_parse_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(Coding), C.c_void_p, C.c_uint64]
+        L.b2k_decode_codestream_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(DevicePlanes), C.c_void_p,
+                                                   C.POINTER(Coding), C.POINTER(C.c_double)]
+        handle = _stream_handle(stream, cs)
+        cp = Coding()
+        nb = L.b2k_codestream_parse_device(self._h, ptr, n, handle, C.byref(cp), None, 0)  # the main header: the image's shape
+        if nb < 0 or nb == 1:
+            raise (NotHandled if nb == 1 else EngineError)("b2k_codestream_parse_device: " + (L.b2k_last_error() or b"").decode())
+        h, w = cp.y1 - cp.y0, cp.x1 - cp.x0
+        if out is None:
+            import torch
+            shape = (cp.numcomps, h, w) if layout == "CHW" else (h, w, cp.numcomps)
+            out = torch.empty(shape, dtype=torch.uint16 if dtype is None else dtype, device="cuda:%d" % self.device)
+        img = device_planes(out, cp.numcomps, h, w, layout, writable=True)
+        ms = C.c_double()
+        _check_handled(L.b2k_decode_codestream_device(self._h, ptr, n, C.byref(img), handle, C.byref(cp), C.byref(ms)),
+                       "b2k_decode_codestream_device")
         return cp, out
 
     def job(self, cp, tile_mod=1, tile_rem=0):

@@ -1061,17 +1061,16 @@ struct Cursor
 };
 } // namespace
 
-/* window: x0,y0,x1,y1 on the full-resolution canvas, or NULL for the whole image; reduce: highest resolutions to drop.
-   *cp_out is the coding to DECODE WITH: for a window / reduced decode a virtual image that holds exactly the tiles the
-   window touches, at the reduced resolution (see b2k_codestream_parse_window below). */
-static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* window, uint32_t reduce, b2k_coding* cp_out,
-                          b2k_block* blocks, uint64_t cap_blocks)
+/* The main header of cs[0, len), SOC up to the first SOT: the coding, the progression order, SOP / EPH and where the first
+   SOT starts.  0, or b2k_codestream_parse's return code and text for a main header it declines; h.short_read says the
+   failure came from reaching `len`, so that a longer prefix of the same stream may parse (b2k_codestream_parse_device
+   reads the header from a prefix). */
+int b2k_parse_main_header(const uint8_t* cs, uint64_t len, t2::MainHeader& h)
 {
-  if(!cs || !cp_out)
-    return -1;
+  h = t2::MainHeader();
   auto fail = [&](const char* m, int rc) {
     b2k_set_error(m);
-    return (int64_t)rc;
+    return rc;
   };
   Cursor c{cs, cs + len};
   if(c.u16() != 0xFF4F)
@@ -1088,7 +1087,10 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
   {
     const uint32_t m = c.u16();
     if(!c.ok)
+    {
+      h.short_read = true;
       return fail("truncated main header", -1);
+    }
     if(m == 0xFF90)
     {
       c.p -= 2;
@@ -1096,7 +1098,10 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
     }
     const uint32_t L = c.u16();
     if(!c.ok || L < 2 || c.p + (L - 2) > c.end)
+    {
+      h.short_read = !c.ok || (L >= 2 && c.p + (L - 2) > c.end);
       return fail("bad marker segment length", -1);
+    }
     Cursor s{c.p, c.p + (L - 2)};
     c.p += L - 2;
     switch(m)
@@ -1253,7 +1258,6 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
   }
   if(const char* why = unsupported_reason(cp))
     return fail(why, 1);
-  const std::vector<BandQuant> q = band_quant(cp);
   /* SIZ sanity (A.5.1) and a bound on what a damaged header can make us enumerate */
   if(cp.tw == 0 || cp.th == 0 || cp.tx0 > cp.x0 || cp.ty0 > cp.y0 || (uint64_t)cp.tx0 + cp.tw <= cp.x0 ||
      (uint64_t)cp.ty0 + cp.th <= cp.y0)
@@ -1277,6 +1281,34 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
     if((((uint64_t)(cp.x1 - cp.x0) * (cp.y1 - cp.y0) * cp.numcomps) >> (cp.cblkw_exp + cp.cblkh_exp)) > (1ull << 26))
       return fail("more than 2^26 code blocks", 1);
   }
+  memcpy(&h.cp, &cp, sizeof(cp)); /* padding included: the engine compares codings bytewise */
+  h.progression = progression;
+  h.sop = use_sop;
+  h.eph = use_eph;
+  h.sot = (uint64_t)(c.p - cs);
+  return 0;
+}
+
+/* window: x0,y0,x1,y1 on the full-resolution canvas, or NULL for the whole image; reduce: highest resolutions to drop.
+   *cp_out is the coding to DECODE WITH: for a window / reduced decode a virtual image that holds exactly the tiles the
+   window touches, at the reduced resolution (see b2k_codestream_parse_window below). */
+static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* window, uint32_t reduce, b2k_coding* cp_out,
+                          b2k_block* blocks, uint64_t cap_blocks)
+{
+  if(!cs || !cp_out)
+    return -1;
+  auto fail = [&](const char* m, int rc) {
+    b2k_set_error(m);
+    return (int64_t)rc;
+  };
+  t2::MainHeader mh;
+  if(int rc = b2k_parse_main_header(cs, len, mh))
+    return rc;
+  Cursor c{cs + mh.sot, cs + len};
+  const b2k_coding cp = mh.cp;
+  const int progression = mh.progression;
+  const bool use_sop = mh.sop, use_eph = mh.eph;
+  const std::vector<BandQuant> q = band_quant(cp);
   const TileGrid g = tile_grid(cp);
   const uint32_t ntiles = g.nx * g.ny;
 

@@ -32,6 +32,8 @@
 #include "b2k_internal.h"
 #include "geometry.h"
 #include "t2_device.h"
+#include "t2_decode.h"
+#include "t2_plan.h"
 
 using namespace b2k;
 
@@ -379,6 +381,7 @@ struct b2k_device_job
   std::vector<cudaStream_t> p_streams; /* its block-coder streams */
   bool dec_has_refinement = false; /* the block table of the current decode carries SigProp / MagRef passes */
   T2Job* t2 = nullptr;             /* b2k_encode_codestream_device: the code stream's plan for the flags of the last call */
+  T2Parse* t2p = nullptr;          /* b2k_decode_codestream_device: the packet plan for the last stream's progression / SOP / EPH */
 };
 
 /* -------------------------------------------------------------------------------------------- */
@@ -838,6 +841,7 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
   cudaSetDevice(J->eng->device);
   cudaStreamSynchronize(J->eng->stream);
   b2k_t2_destroy(J->t2);
+  b2k_t2_parse_destroy(J->t2p);
   cudaFree(J->img.base);
   cudaFree(J->d_stage);
   cudaFree(J->coef.base);
@@ -2510,6 +2514,27 @@ extern "C" int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const 
   return decode_common(e, cp, blocks, num_blocks, bytes, num_bytes, tile_mod, tile_rem, ms_total, T, window, caller_stream(cuda_stream));
 }
 
+/* the block decoder over chunk k's coded blocks, from the descriptors in d_dec_desc and the bytes in d_bytes: phase A
+   (serial VLC/MEL parse, one thread per block) is latency-bound and leaves the SMs nearly empty, so the chunks' parses run
+   concurrently on side streams once `ready` (this chunk's descriptors + bytes are on the device) has happened, ahead of st */
+static int enqueue_block_decode(b2k_engine* e, b2k_device_job* J, size_t k, cudaEvent_t ready, cudaStream_t st)
+{
+  const uint32_t b0 = J->coded_first[J->chunk_tile[k]], b1 = J->coded_first[J->chunk_tile[k + 1]];
+  if(b1 <= b0)
+    return 0;
+  cudaStream_t ax = e->aux[k & 3];
+  if(ready)
+    CUDA_TRY(cudaStreamWaitEvent(ax, ready, 0));
+  b2k_launch_ht_decode_vlc(J->d_dec_desc + b0, J->d_bytes, J->d_recs, J->d_dec_status + b0, b1 - b0, J->max_cblk_w, ax);
+  CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(2, k)], ax));
+  CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(2, k)], 0));
+  b2k_launch_ht_decode_magsgn(J->d_dec_desc + b0, J->d_bytes, J->d_recs, J->d_dec_status + b0, b1 - b0, J->max_cblk_w, J->d_err,
+                              J->cp.irreversible, J->dec_has_refinement, st);
+  if(J->dec_has_refinement)
+    b2k_launch_ht_decode_refine(J->d_dec_desc + b0, J->d_bytes, J->d_dec_status + b0, b1 - b0, (J->cp.cblk_sty & 0x08) != 0, st);
+  return 0;
+}
+
 /* T.user: the caller's samples, which hold only `window` (x0, y0, x1, y1) of the pixels when there is one.  A device image
    (b2k_decode_device) is written after the work queued on `caller` */
 static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
@@ -2599,21 +2624,7 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
     }
     CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(1, k)], e->h2d_stream));
     CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(1, k)], 0));
-    if(b1 > b0)
-    {
-      /* phase A (serial VLC/MEL parse, one thread per block) is latency-bound and leaves the SMs
-         nearly empty: run the chunks' parses concurrently on side streams, ahead of the main stream */
-      cudaStream_t ax = e->aux[k & 3];
-      CUDA_TRY(cudaStreamWaitEvent(ax, J->chunk_ev[CEV(1, k)], 0)); /* this chunk's descriptors + bytes are up */
-      b2k_launch_ht_decode_vlc(J->d_dec_desc + b0, J->d_bytes, J->d_recs, J->d_dec_status + b0, b1 - b0, J->max_cblk_w, ax);
-      CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(2, k)], ax));
-      CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(2, k)], 0));
-      b2k_launch_ht_decode_magsgn(J->d_dec_desc + b0, J->d_bytes, J->d_recs, J->d_dec_status + b0, b1 - b0, J->max_cblk_w,
-                                  J->d_err, J->cp.irreversible, J->dec_has_refinement, st);
-      if(J->dec_has_refinement)
-        b2k_launch_ht_decode_refine(J->d_dec_desc + b0, J->d_bytes, J->d_dec_status + b0, b1 - b0,
-                                    (J->cp.cblk_sty & 0x08) != 0, st);
-    }
+    if(enqueue_block_decode(e, J, k, J->chunk_ev[CEV(1, k)], st)) return -1;
     if(enqueue_inverse(J, st, t0, t1)) return -1;
     if(download_chunk(J, T, k, st, cs)) return -1;
   }
@@ -2642,5 +2653,206 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
     g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
     return -2;
   }
+  return 0;
+}
+
+/* ---- code streams in device memory (b2k_decode_codestream_device / b2k_codestream_parse_device) ----------------------
+ * The main header is read on the host from a prefix of the stream, by b2k_codestream_parse's own code; the tile parts and
+ * packets are parsed on the device (t2_decode.cu) from a copy of the stream in the job's arena, which also gives the HT
+ * decoder the slack it reads past a block.  Synchronisations: the header, the parse status, the end of the decode. */
+static int check_device_bytes(const b2k_engine* e, const uint8_t* cs, uint64_t len)
+{
+  if(len == 0)
+  { /* no bytes, whatever the pointer (an empty tensor's is often NULL): what the host parser says of them */
+    g_err = "no SOC marker";
+    return -1;
+  }
+  cudaPointerAttributes a{};
+  const cudaError_t err = cs ? cudaPointerGetAttributes(&a, cs) : cudaErrorInvalidValue;
+  if(err != cudaSuccess)
+    (void)cudaGetLastError();
+  if(err != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != e->device)
+  {
+    g_err = "code stream: not device or managed memory of the engine's device (" + std::to_string(e->device) + ")";
+    return -1;
+  }
+  return 0;
+}
+
+/* the main header from a prefix of cs read on st: 64 KiB, doubled while the header runs past it (a large TLM) */
+static int read_device_main_header(const uint8_t* cs, uint64_t len, cudaStream_t st, b2k::t2::MainHeader& h)
+{
+  uint64_t n = std::min<uint64_t>(len, 64u << 10);
+  for(;;)
+  {
+    uint8_t* buf = pool_get(n);
+    if(!buf)
+    {
+      g_err = "no pinned memory for the main header";
+      return -1;
+    }
+    cudaError_t ce = cudaMemcpyAsync(buf, cs, n, cudaMemcpyDeviceToHost, st);
+    if(ce == cudaSuccess)
+      ce = cudaStreamSynchronize(st);
+    const int rc = ce == cudaSuccess ? b2k_parse_main_header(buf, n, h) : -1;
+    pool_put(buf);
+    if(ce != cudaSuccess)
+    {
+      g_err = std::string("code stream prefix to the host: ") + cudaGetErrorString(ce);
+      return -1;
+    }
+    if(rc && h.short_read && n < len)
+    {
+      n = std::min<uint64_t>(len, 2 * n);
+      continue;
+    }
+    return rc;
+  }
+}
+
+/* the header, the job of its coding, the stream in the job's arena and its parse on st, up to the status.  With dec the
+   decoder's descriptors are built too.  0, or b2k_codestream_parse's return code with its text. */
+static int parse_device_codestream(b2k_engine* e, const uint8_t* cs, uint64_t len, cudaStream_t caller, b2k::t2::MainHeader& h,
+                                   b2k_device_job** out, bool dec, bool* refinement, uint64_t cap_blocks = UINT64_MAX)
+{
+  cudaStream_t st = e->stream;
+  CUDA_TRY(cudaSetDevice(e->device));
+  /* what the caller queued before the call (the kernel, receive or read that produced cs) comes first */
+  CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
+  CUDA_TRY(cudaStreamWaitEvent(st, e->caller_ev, 0));
+  if(int rc = read_device_main_header(cs, len, st, h))
+    return rc;
+  int rc = 0;
+  b2k_device_job* J = cached_job(e, &h.cp, 1, 0, &rc);
+  if(rc)
+    return rc;
+  *out = J;
+  if(cap_blocks < J->blocks.size())
+  { /* the host parser checks the caller's table before it looks at a tile part */
+    g_err = "block table too small";
+    return -1;
+  }
+  const uint32_t flags = B2K_CS_PROG(h.progression) | (h.sop ? B2K_CS_SOP : 0u) | (h.eph ? B2K_CS_EPH : 0u);
+  if(!J->t2p || b2k_t2_parse_flags(J->t2p) != flags)
+  { /* geometry and progression only: planned once for every stream of this coding */
+    b2k_t2_parse_destroy(J->t2p);
+    J->t2p = nullptr;
+    if(b2k_t2_parse_create(h.cp, flags, J->blocks.data(), J->blocks.size(), (uint32_t)J->tiles.size(), J->coded_index.data(),
+                           J->coded_index.size(), &J->t2p))
+      return -1;
+  }
+  if(len + 64 > J->bytes_cap)
+  {
+    cudaFree(J->d_bytes);
+    J->d_bytes = nullptr;
+    J->bytes_cap = 0;
+    CUDA_TRY(cudaMalloc(&J->d_bytes, len + 4096));
+    J->bytes_cap = len + 4096;
+  }
+  J->arena_sized = false; /* the arena now holds a caller's stream, not this job's coding of its image */
+  CUDA_TRY(cudaEventRecord(J->ev[0], st));
+  CUDA_TRY(cudaMemcpyAsync(J->d_bytes, cs, len, cudaMemcpyDeviceToDevice, st));
+  if(b2k_t2_parse_enqueue(J->t2p, J->d_bytes, len, h.sot, J->d_enc_desc, J->d_dec_quant, dec ? J->d_dec_desc : nullptr, st))
+    return -1;
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return b2k_t2_parse_result(J->t2p, refinement);
+}
+
+extern "C" int64_t b2k_codestream_parse_device(b2k_engine* e, const uint8_t* cs, uint64_t len, void* cuda_stream, b2k_coding* cp_out,
+                                               b2k_block* blocks, uint64_t cap_blocks)
+{
+  if(!e || !cp_out)
+    return -1;
+  if(check_device_bytes(e, cs, len))
+    return -1;
+  std::lock_guard<std::mutex> lock(e->mu);
+  cudaStream_t caller = caller_stream(cuda_stream);
+  b2k::t2::MainHeader h;
+  if(!blocks)
+  {
+    CUDA_TRY(cudaSetDevice(e->device));
+    CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
+    CUDA_TRY(cudaStreamWaitEvent(e->stream, e->caller_ev, 0));
+    if(int rc = read_device_main_header(cs, len, e->stream, h))
+      return rc;
+    *cp_out = h.cp;
+    return b2k_enumerate(&h.cp, 1, 0, nullptr, 0);
+  }
+  b2k_device_job* J = nullptr;
+  int rc = parse_device_codestream(e, cs, len, caller, h, &J, false, nullptr, cap_blocks);
+  if(J)
+    *cp_out = h.cp;
+  if(rc)
+    return rc;
+  const uint64_t n = J->blocks.size();
+  if(b2k_t2_parse_blocks(J->t2p, blocks, e->stream))
+    return -1;
+  return (int64_t)n;
+}
+
+extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const b2k_device_planes* img,
+                                                void* cuda_stream, b2k_coding* cp_out, double* ms_total)
+{
+  if(!e || !cp_out)
+    return -1;
+  if(check_device_bytes(e, cs, len))
+    return -1;
+  std::lock_guard<std::mutex> lock(e->mu);
+  const auto wall0 = std::chrono::steady_clock::now();
+  cudaStream_t caller = caller_stream(cuda_stream);
+  b2k::t2::MainHeader h;
+  b2k_device_job* J = nullptr;
+  bool refinement = false;
+  if(int rc = parse_device_codestream(e, cs, len, caller, h, &J, true, &refinement))
+    return rc;
+  *cp_out = h.cp;
+  DBG_T("device decode: parsed");
+  if(int rc = check_device_planes(e, &h.cp, img))
+    return rc;
+  Transport T;
+  device_samples(T, *img, h.cp.x0, h.cp.y0);
+  if(resolve_transport(J, T, true))
+    return -1;
+  cudaStream_t st = e->stream;
+  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
+  J->dec_has_refinement = refinement;
+  const size_t nchunks = J->chunk_tile.size() - 1;
+  for(size_t k = 0; k < nchunks; ++k)
+  { /* the parse has finished (its status was read): the side streams need not wait for it */
+    if(enqueue_block_decode(e, J, k, nullptr, st)) return -1;
+    if(enqueue_inverse(J, st, J->chunk_tile[k], J->chunk_tile[k + 1])) return -1;
+    if(download_chunk(J, T, k, st, e->copy_stream)) return -1;
+  }
+  CUDA_TRY(cudaEventRecord(J->ev[1], st));
+  /* the caller's stream goes on once its image is written */
+  CUDA_TRY(cudaEventRecord(e->caller_ev, st));
+  CUDA_TRY(cudaStreamWaitEvent(caller, e->caller_ev, 0));
+  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
+  CUDA_TRY(cudaGetLastError());
+  DBG_T("device decode: done");
+  float t = 0;
+  cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
+  if(ms_total) *ms_total = t;
+  int herr = 0;
+  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
+  if(herr)
+  {
+    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
+    return -2;
+  }
+  return 0;
+}
+
+extern "C" int32_t b2k_codestream_parse_device_stats(b2k_engine* e, uint32_t* tiles_indexed, uint32_t* tiles_walked)
+{
+  if(!e || !tiles_indexed || !tiles_walked)
+    return -1;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if(!e->cached || !e->cached->t2p)
+  {
+    g_err = "no code stream has been parsed on the device";
+    return -1;
+  }
+  b2k_t2_parse_stats(e->cached->t2p, tiles_indexed, tiles_walked);
   return 0;
 }

@@ -1,0 +1,473 @@
+/*
+ * grok_b200/csrc/t2_parse.h -- reading the tile parts and packet headers of an HTJ2K code stream, as __host__ __device__
+ * code over a byte buffer: the tile-part walk (SOT / Psot / tile-part header segments up to SOD), the packet-header bit
+ * reader (7 bits after 0xFF), the tag-tree decoder, pass count, Lblock and the HT segment lengths, SOP / EPH.
+ * The device parser (t2_decode.cu) runs these functions in its kernels; tests/t2_parse_check.cpp runs them on the host in
+ * the same order and compares with b2k_codestream_parse.
+ *
+ * The verdicts are those of the host parser (codestream.cpp, parse_impl / parse_tile_packets) for every input: the same
+ * tile parts, the same blocks, the same first failure and its return code.  Written from ITU-T T.800 Annex A/B and T.814
+ * Annex B; the packets of a tile and their blocks come from the code-stream plan (t2_plan.h).
+ */
+#pragma once
+#include <stdint.h>
+#include "t2_packet.h"
+
+namespace b2k
+{
+namespace t2
+{
+
+/* why a parse failed; 0 = it did not */
+enum ParseReason : uint32_t
+{
+  PR_NONE = 0,
+  PR_EXPECTED_SOT,  /* -1 */
+  PR_BAD_SOT,       /* -1 */
+  PR_TP_ORDER,      /*  1 */
+  PR_PSOT,          /* -1 */
+  PR_TP_TRUNCATED,  /* -1 */
+  PR_TP_SEGMENT,    /* -1 */
+  PR_TP_MARKER,     /*  1 */
+  PR_ZBP,           /* -1 */
+  PR_PASSES,        /*  1 */
+  PR_LBLOCK,        /* -1 */
+  PR_ZBP_KMAX,      /* -1 */
+  PR_SHORT_CLEANUP, /* -1 */
+  PR_HEADER_RUN,    /* -1 */
+  PR_EPH,           /* -1 */
+  PR_BODY_RUN,      /* -1 */
+  PR_PART_TABLE,    /* -1: more tile parts than the table holds (cannot happen: each takes at least 12 bytes) */
+  PR_COUNT
+};
+B2K_HD int parse_reason_rc(uint32_t r) { return (r == PR_TP_ORDER || r == PR_TP_MARKER || r == PR_PASSES) ? 1 : -1; }
+/* the host parser's text for each reason */
+inline const char* parse_reason_text(uint32_t r)
+{
+  switch(r)
+  {
+    case PR_EXPECTED_SOT: return "expected SOT or EOC";
+    case PR_BAD_SOT: return "bad SOT";
+    case PR_TP_ORDER: return "tile parts out of order";
+    case PR_PSOT: return "Psot exceeds the codestream";
+    case PR_TP_TRUNCATED: return "truncated tile-part header";
+    case PR_TP_SEGMENT: return "bad tile-part marker segment";
+    case PR_TP_MARKER: return "tile-part COD / COC / QCD / QCC / RGN / POC / PPT are not handled";
+    case PR_ZBP: return "corrupt packet header (zero bit planes)";
+    case PR_PASSES: return "HT code blocks with placeholder passes or several HT sets are not handled";
+    case PR_LBLOCK: return "corrupt packet header (Lblock)";
+    case PR_ZBP_KMAX: return "more zero bit planes than the band has bit planes";
+    case PR_SHORT_CLEANUP: return "HT cleanup segment shorter than 2 bytes";
+    case PR_HEADER_RUN: return "packet header runs past the tile part";
+    case PR_EPH: return "EPH marker missing after a packet header";
+    case PR_BODY_RUN: return "packet body runs past the tile part";
+    case PR_PART_TABLE: return "internal: tile-part table too small";
+    default: return "";
+  }
+}
+
+constexpr uint32_t PART_NONE = 0xFFFFFFFFu;
+/* one tile part, in stream order: where its header starts, its packet data [begin, end) (offsets into the code stream; begin may exceed end when
+   a tile-part header runs past Psot, exactly as on the host), its tile, the next tile part of the same tile */
+struct PartRange
+{
+  uint64_t hdr;        /* the tile-part header's first segment (just after SOT) */
+  uint64_t begin, end;
+  uint32_t tile, next;
+};
+/* what the parse gives a block: the fields b2k_codestream_parse fills in (offset into the code stream) */
+struct ParsedBlock
+{
+  uint64_t offset;
+  uint32_t length, length2;
+  uint8_t numbps, numpasses, pad[6];
+};
+
+/* big-endian reads with the host parser's sticky failure: a read past `end` fails and reads nothing */
+struct ByteCursor
+{
+  const uint8_t* cs;
+  uint64_t p, end;
+  bool ok;
+  B2K_HD uint32_t u8()
+  {
+    if(p + 1 > end)
+    {
+      ok = false;
+      return 0;
+    }
+    return cs[p++];
+  }
+  B2K_HD uint32_t u16()
+  {
+    if(p + 2 > end)
+    {
+      ok = false;
+      return 0;
+    }
+    const uint32_t v = ((uint32_t)cs[p] << 8) | cs[p + 1];
+    p += 2;
+    return v;
+  }
+  B2K_HD uint32_t u32()
+  {
+    const uint32_t a = u16();
+    return (a << 16) | u16();
+  }
+};
+
+/* The tile parts from the first SOT (at sot) to EOC or the end of the stream, in stream order, as the host parser walks
+ * them (A.4.2): SOT, Psot hop, tile-part header segments up to SOD.  head[t] / last[t] / count[t] (ntiles each) are
+ * scratch the walk initialises; parts holds cap entries.  Returns PR_NONE or the first failure in stream order. */
+B2K_HD uint32_t locate_tile_parts(const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t ntiles, PartRange* parts, uint64_t cap,
+                                  uint32_t* head, uint32_t* last, uint32_t* count, uint32_t* nparts)
+{
+  for(uint32_t t = 0; t < ntiles; ++t)
+  {
+    head[t] = last[t] = PART_NONE;
+    count[t] = 0;
+  }
+  *nparts = 0;
+  /* Psot = 0: the tile part runs to the end of the stream, before a final EOC */
+  const uint64_t open_end = len - ((len >= 2 && cs[len - 2] == 0xFF && cs[len - 1] == 0xD9) ? 2 : 0);
+  ByteCursor c{cs, sot, len, true};
+  uint32_t n = 0;
+  for(;;)
+  {
+    const uint64_t at = c.p;
+    const uint32_t m = c.u16();
+    if(!c.ok || m == 0xFFD9)
+      break; /* a missing EOC is tolerated */
+    if(m != 0xFF90)
+      return PR_EXPECTED_SOT;
+    const uint32_t lsot = c.u16(), isot = c.u16(), psot = c.u32(), tpsot = c.u8();
+    c.u8(); /* TNsot */
+    if(!c.ok || lsot != 10 || isot >= ntiles)
+      return PR_BAD_SOT;
+    if(tpsot != count[isot])
+      return PR_TP_ORDER;
+    ++count[isot];
+    const uint64_t tp_end = psot ? at + psot : open_end;
+    if(tp_end > len || tp_end < c.p)
+      return PR_PSOT;
+    for(;;)
+    { /* tile-part header: PLT, COM and unknown segments are skipped */
+      const uint32_t tm = c.u16();
+      if(!c.ok)
+        return PR_TP_TRUNCATED;
+      if(tm == 0xFF93)
+        break;
+      const uint32_t L = c.u16();
+      if(!c.ok || L < 2 || c.p + (L - 2) > tp_end)
+        return PR_TP_SEGMENT;
+      if(tm == 0xFF52 || tm == 0xFF53 || tm == 0xFF5C || tm == 0xFF5D || tm == 0xFF5E || tm == 0xFF5F || tm == 0xFF61)
+        return PR_TP_MARKER;
+      c.p += L - 2;
+    }
+    if(n >= cap)
+      return PR_PART_TABLE;
+    parts[n] = PartRange{at + 12, c.p, tp_end, isot, PART_NONE};
+    if(last[isot] == PART_NONE)
+      head[isot] = n;
+    else
+      parts[last[isot]].next = n;
+    last[isot] = n;
+    *nparts = ++n;
+    c.p = tp_end;
+  }
+  return PR_NONE;
+}
+
+/* packet-header bits: MSB first, the byte after 0xFF carries 7 bits (T.800 B.10.1); reading past end gives 0 bits and
+   sets overrun */
+struct BitReader
+{
+  const uint8_t* cs;
+  uint64_t p, end;
+  uint32_t cur;
+  int left;
+  bool prev_ff, overrun;
+  B2K_HD void init(const uint8_t* b, uint64_t at, uint64_t e)
+  {
+    cs = b;
+    p = at;
+    end = e;
+    cur = 0;
+    left = 0;
+    prev_ff = overrun = false;
+  }
+  B2K_HD uint32_t get()
+  {
+    if(left == 0)
+    {
+      if(p >= end)
+      {
+        overrun = true;
+        return 0;
+      }
+      cur = cs[p++];
+      left = prev_ff ? 7 : 8;
+      prev_ff = cur == 0xFF;
+    }
+    --left;
+    return (cur >> left) & 1u;
+  }
+  B2K_HD uint32_t get_bits(int n)
+  {
+    uint32_t v = 0;
+    for(int i = 0; i < n; ++i)
+      v = (v << 1) | get();
+    return v;
+  }
+  /* the header ends byte aligned; a final 0xFF is followed by one stuffed byte */
+  B2K_HD uint64_t finish()
+  {
+    left = 0;
+    if(prev_ff && p < end)
+      ++p;
+    prev_ff = false;
+    return p;
+  }
+};
+
+/* tag-tree decoder (T.800 B.10.2) over the node layout of tag_encode (leaves first, the root last), nodes initialised to
+   {TAG_INF, 0}: true when leaf (x, y) is below threshold, its value then in *value */
+B2K_HD bool tag_decode(BitReader& br, TagNode* nd, uint32_t w, uint32_t h, uint32_t nodes, int levels, uint32_t x, uint32_t y,
+                       uint32_t threshold, uint32_t* value)
+{
+  uint32_t low = 0, base = nodes;
+  TagNode* t = nullptr;
+  for(int l = levels - 1; l >= 0; --l)
+  {
+    const uint32_t lw = tag_level_w(w, l);
+    base -= lw * tag_level_w(h, l);
+    t = &nd[base + (y >> l) * lw + (x >> l)];
+    if(low > t->low)
+      t->low = low;
+    else
+      low = t->low;
+    uint32_t v = t->value;
+    while(low < threshold && low < v)
+    {
+      if(br.get())
+        v = low;
+      else
+        ++low;
+    }
+    t->value = v;
+    t->low = low;
+  }
+  *value = t->value;
+  return t->value < threshold;
+}
+
+/* One packet (one quality layer) at p of the tile part that ends at tp_end, as the host's parse_tile_packets reads it:
+ * optional SOP, the header bits, EPH when COD asks for it, the body.  pk.band[].first index blk / kmax; tags holds
+ * packet_tag_nodes(pk) nodes.  The packet's blocks in blk must be zero.  *p moves past the packet.  PR_NONE or the failure. */
+template <class Packet>
+B2K_HD uint32_t parse_packet(const uint8_t* cs, const Packet& pk, uint64_t* at, uint64_t tp_end, const uint8_t* kmax, ParsedBlock* blk,
+                             TagNode* tags, bool sop, bool eph)
+{
+  uint64_t p = *at;
+  if(sop && (int64_t)(tp_end - p) >= 6 && cs[p] == 0xFF && cs[p + 1] == 0x91)
+    p += 6; /* SOP may be there when COD allows it (A.8.1) */
+  BitReader br;
+  br.init(cs, p, tp_end);
+  if(br.get())
+  {
+    for(uint32_t b = 0; b < pk.nbands; ++b)
+    {
+      const uint32_t gw = pk.band[b].gw, gh = pk.band[b].gh, n = gw * gh;
+      if(!n)
+        continue;
+      int levels = 0;
+      const uint32_t nodes = tag_nodes(gw, gh, &levels);
+      TagNode* incl = tags;
+      TagNode* imsb = tags + nodes;
+      for(uint32_t i = 0; i < 2 * nodes; ++i)
+        tags[i] = TagNode{TAG_INF, 0};
+      for(uint32_t i = 0; i < n; ++i)
+      {
+        const uint32_t x = i % gw, y = i / gw;
+        uint32_t v = 0;
+        if(!tag_decode(br, incl, gw, gh, nodes, levels, x, y, 1, &v))
+          continue;
+        uint32_t zbp = 0;
+        for(uint32_t th = 1;; ++th)
+        {
+          if(tag_decode(br, imsb, gw, gh, nodes, levels, x, y, th, &v))
+          {
+            zbp = v;
+            break;
+          }
+          if(th > 64 || br.overrun)
+            return PR_ZBP;
+        }
+        uint32_t npass; /* number of passes, B.10.6 */
+        if(!br.get())
+          npass = 1;
+        else if(!br.get())
+          npass = 2;
+        else
+        {
+          const uint32_t v2 = br.get_bits(2);
+          if(v2 < 3)
+            npass = 3 + v2;
+          else
+          {
+            const uint32_t v5 = br.get_bits(5);
+            npass = v5 < 31 ? 6 + v5 : 37 + br.get_bits(7);
+          }
+        }
+        if(npass > 3)
+          return PR_PASSES;
+        int lblock = 3;
+        while(br.get())
+          if(++lblock > 32)
+            return PR_LBLOCK;
+        /* HT: the cleanup pass is one segment, the refinement passes another (T.814 B.10.7) */
+        const uint32_t len1 = br.get_bits(lblock);
+        const int l2 = lblock + floorlog2(npass - 1);
+        const uint32_t len2 = npass > 1 ? br.get_bits(l2 < 32 ? l2 : 32) : 0;
+        const uint32_t kb = kmax[pk.band[b].first + i];
+        if(zbp > kb)
+          return PR_ZBP_KMAX;
+        if(len1 < 2)
+          return PR_SHORT_CLEANUP;
+        ParsedBlock& B = blk[pk.band[b].first + i];
+        B.numbps = (uint8_t)(kb - zbp);
+        B.numpasses = (uint8_t)npass;
+        B.length = len1;
+        B.length2 = len2;
+      }
+    }
+  }
+  if(br.overrun)
+    return PR_HEADER_RUN;
+  p = br.finish();
+  if(eph)
+  { /* EPH shall follow every packet header when COD says so (A.8.2) */
+    if((int64_t)(tp_end - p) < 2 || cs[p] != 0xFF || cs[p + 1] != 0x92)
+      return PR_EPH;
+    p += 2;
+  }
+  /* the body: the included blocks' bytes in header order (a block is in one packet only, so numpasses marks it) */
+  for(uint32_t b = 0; b < pk.nbands; ++b)
+  {
+    const uint32_t n = pk.band[b].gw * pk.band[b].gh;
+    for(uint32_t i = 0; i < n; ++i)
+    {
+      ParsedBlock& B = blk[pk.band[b].first + i];
+      if(!B.numpasses)
+        continue;
+      const uint32_t sz = B.length + B.length2; /* 32-bit, as the host parser adds them */
+      if(tp_end - p < sz)
+        return PR_BODY_RUN;
+      B.offset = p;
+      p += sz;
+    }
+  }
+  *at = p;
+  return PR_NONE;
+}
+
+/* One tile's packets from its tile parts, as the host's parse_tile_packets reads them.  packets[0, np) are the tile's
+ * packets in code-stream order; tags: packet_tag_nodes of the largest of them.  blk must hold the tile's blocks cleared to
+ * zero.  A packet never straddles tile parts; where the data ends the remaining packets stay uncoded.  PR_NONE or the
+ * failure. */
+template <class Packet>
+B2K_HD uint32_t parse_tile(const uint8_t* cs, const PartRange* parts, uint32_t first_part, const Packet* packets, uint64_t np,
+                           const uint8_t* kmax, ParsedBlock* blk, TagNode* tags, bool sop, bool eph)
+{
+  if(first_part == PART_NONE)
+    return PR_NONE; /* a tile without a tile part decodes as all zero */
+  uint32_t part = first_part;
+  uint64_t p = parts[part].begin, tp_end = parts[part].end;
+  for(uint64_t k = 0; k < np; ++k)
+  {
+    while(p == tp_end && parts[part].next != PART_NONE)
+    {
+      part = parts[part].next;
+      p = parts[part].begin;
+      tp_end = parts[part].end;
+    }
+    if(p == tp_end)
+      break;
+    if(const uint32_t r = parse_packet(cs, packets[k], &p, tp_end, kmax, blk, tags, sop, eph))
+      return r;
+  }
+  return PR_NONE;
+}
+
+/* Packet starts from PLT (A.7.3).  A tile is indexed when every one of its tile parts carries PLT segments (Zplt 0, 1, ...
+ * in its header), every Iplt entry is complete, at least 1 and at most 32 bits, the entries of each part add up to exactly
+ * its packet data, and the parts hold exactly np entries together.  Then packet k of the tile starts at start[k], ends at
+ * end[k] and lies in the tile part that ends at part_end[k] -- where the host's walk would meet it, provided each packet
+ * before it ends where PLT says.  A PLT that is not understood only means "not indexed": the tile is walked. */
+B2K_HD bool plt_index(const uint8_t* cs, const PartRange* parts, uint32_t first_part, uint64_t np, uint64_t* start, uint64_t* end,
+                      uint64_t* part_end)
+{
+  if(first_part == PART_NONE)
+    return false;
+  uint64_t k = 0;
+  for(uint32_t part = first_part; part != PART_NONE; part = parts[part].next)
+  {
+    const PartRange& R = parts[part];
+    if(R.begin < R.hdr + 2 || R.begin > R.end)
+      return false;
+    uint64_t q = R.hdr, at = R.begin;
+    const uint64_t sod = R.begin - 2;
+    uint32_t z = 0;
+    while(q + 4 <= sod)
+    { /* the tile-part header's segments; their lengths were checked by locate_tile_parts */
+      const uint32_t m = ((uint32_t)cs[q] << 8) | cs[q + 1], L = ((uint32_t)cs[q + 2] << 8) | cs[q + 3];
+      const uint64_t seg_end = q + 2 + L;
+      if(m == 0xFF58)
+      {
+        if(L < 3 || seg_end > sod || cs[q + 4] != z)
+          return false;
+        ++z;
+        uint64_t v = 0;
+        int nb = 0;
+        for(uint64_t i = q + 5; i < seg_end; ++i)
+        {
+          v = (v << 7) | (cs[i] & 0x7F);
+          if(++nb > 5 || v > 0xFFFFFFFFull)
+            return false;
+          if(cs[i] & 0x80)
+            continue;
+          if(v == 0 || k >= np || R.end - at < v)
+            return false;
+          start[k] = at;
+          at += v;
+          end[k] = at;
+          part_end[k] = R.end;
+          ++k;
+          v = 0;
+          nb = 0;
+        }
+        if(nb)
+          return false; /* an entry that runs past its segment */
+      }
+      q = seg_end;
+    }
+    if(!z || at != R.end)
+      return false;
+  }
+  return k == np;
+}
+
+/* prepare_decode's rule (engine.cu) for one coded block: missing MSBs, passes and refinement length; false when it has
+   refinement passes to decode */
+B2K_HD void block_decode_fields(const ParsedBlock& b, uint8_t kmax, uint8_t* mmsbs, uint8_t* passes, uint32_t* length2)
+{
+  const int nb = b.length ? b.numbps : 0;
+  const int m = (int)kmax - nb;
+  *mmsbs = (uint8_t)(m > 0 ? m : 0);
+  /* no refinement bytes, or a cleanup pass already at bit-plane 1, leave nothing to refine */
+  *passes = (b.length && b.numpasses > 1 && b.length2 > 0 && *mmsbs < 29) ? b.numpasses : 1;
+  *length2 = *passes > 1 ? b.length2 : 0;
+}
+
+} // namespace t2
+} // namespace b2k

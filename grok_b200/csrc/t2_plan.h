@@ -37,8 +37,19 @@ struct Plan
   std::vector<DevPart> parts;
   uint64_t hdr_bytes = 0, tag_nodes = 0;
 };
+struct MainHeader /* what a code stream's main header says (b2k_parse_main_header) */
+{
+  b2k_coding cp{};
+  int progression = 0;
+  bool sop = false, eph = false;
+  uint64_t sot = 0;        /* where the first SOT starts */
+  bool short_read = false; /* the failure came from reaching the end of the bytes given */
+};
 } // namespace t2
 } // namespace b2k
+
+/* the main header of cs[0, len), read by b2k_codestream_parse's own code: 0, or its return code with b2k_last_error set */
+int b2k_parse_main_header(const uint8_t* cs, uint64_t len, b2k::t2::MainHeader& h);
 
 /* the plan of the code stream b2k_codestream_write(cp, r, flags) writes, for the block table `blocks` (every block of the
    tiles of r, enumeration order) and r->num_tiles = num_tiles.  0, or -1 with b2k_last_error set in the cases, and with the

@@ -516,6 +516,22 @@ B2K_API int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const b2k
  * (geometry and flags) is made once per coding and flags and kept with the engine's cached job. */
 B2K_API int64_t b2k_encode_codestream_device(b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img,
                                              uint32_t flags, void* cuda_stream, const uint8_t** cs);
+/* A complete HTJ2K code stream in device memory (cs, len bytes, on the engine's GPU) -> the image in img.
+ * Equal, for every input, to copying cs to the host and calling b2k_codestream_parse + b2k_decode_device:
+ * the same return code, the same b2k_last_error text for 1 and -1, the same pixels for 0.  Only the main header (a
+ * 64 KiB prefix, longer when the header is) and a small parse status cross PCIe; the tile parts and packet headers are
+ * parsed by kernels.  cs is read after the work queued on cuda_stream, which then waits for the image writes. */
+B2K_API int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const b2k_device_planes* img,
+                                             void* cuda_stream, b2k_coding* cp_out, double* ms_total);
+/* Stage hook / size query: the block table b2k_codestream_parse would return for the same bytes (offsets into cs),
+ * parsed by the device kernels.  blocks = NULL: read the main header only and return the block count (Python's
+ * decode_codestream_device makes this call first when it needs the image's shape, so it reads the header twice). */
+B2K_API int64_t b2k_codestream_parse_device(b2k_engine* e, const uint8_t* cs, uint64_t len, void* cuda_stream,
+                                            b2k_coding* cp_out, b2k_block* blocks, uint64_t cap_blocks);
+/* How the last device parse on this engine read its tiles: tiles whose packets were parsed one thread per packet from
+ * their PLT packet starts, and tiles with data walked packet after packet (no PLT, a PLT that does not add up, or a packet
+ * that did not end where PLT said).  The results do not depend on the split; the time does. */
+B2K_API int32_t b2k_codestream_parse_device_stats(b2k_engine* e, uint32_t* tiles_indexed, uint32_t* tiles_walked);
 
 /* Geometry only (host): enumerate the blocks of the selected tiles, lengths zero.  Returns the
  * count; fills at most cap entries. */
