@@ -66,7 +66,7 @@ assert BLOCK_DTYPE.itemsize == C.sizeof(Block), (BLOCK_DTYPE.itemsize, C.sizeof(
 # plugin_decompress (C++-ABI callback struct) is declared in csrc/plugin_decode_abi.h, not in the C header
 EXPORTS = ["minpf_post_load_plugin", "plugin_init", "plugin_get_debug_state", "gpup_encode_mem", "gpup_tile_free",
            "b2k_engine_create", "b2k_engine_destroy", "b2k_last_error", "b2k_host_alloc", "b2k_host_free",
-           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_decode_codestream_device", "b2k_codestream_parse_device", "b2k_codestream_parse_device_stats", "b2k_enumerate",
+           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_decode_codestream_device", "b2k_codestream_parse_device", "b2k_codestream_parse_device_stats", "b2k_codestream_parse_window_device", "b2k_decode_codestream_window_device", "b2k_codestream_window_device_stats", "b2k_enumerate",
            "b2k_result_to_gpup_tile", "b2k_job_create", "b2k_job_destroy", "b2k_job_upload", "b2k_job_forward",
            "b2k_job_t1_encode", "b2k_job_t1_decode", "b2k_job_t1_decode_blocks", "b2k_job_inverse", "b2k_job_roundtrip", "b2k_job_roundtrip_n", "b2k_job_roundtrip_pipelined_n", "b2k_job_download",
            "b2k_job_download_coeffs", "b2k_job_upload_coeffs", "b2k_job_fetch_result", "b2k_job_num_blocks",
@@ -660,10 +660,12 @@ class Engine:
         reduce work as in decode_window (the Coding is then the virtual one).  out: a CUDA array of the (window's) shape
         in `layout`, or None for a new torch tensor of `dtype` (default torch.uint16) on the engine's GPU.
         cs may itself be on the engine's GPU (a 1-D contiguous uint8 CUDA array): it is then parsed there
-        (b2k_decode_codestream_device) and never crosses PCIe; window / reduce are not available on that path."""
+        (b2k_decode_codestream_device) and never crosses PCIe; window / reduce are not available on that path: a window
+        of a code stream in device memory is decode_window_device."""
         if hasattr(cs, "__cuda_array_interface__"):
             if window is not None or reduce:
-                raise NotHandled("decode_codestream_device: window / reduce are not available for a code stream in device memory")
+                raise NotHandled("decode_codestream_device: window / reduce of a code stream in device memory are "
+                                 "decode_window_device's")
             return self._decode_device_codestream(cs, out, dtype, layout, stream)
         cs = np.ascontiguousarray(cs, dtype=np.uint8)
         if window is not None or reduce:
@@ -713,6 +715,77 @@ class Engine:
         L.b2k_codestream_parse_device_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
         _check(L.b2k_codestream_parse_device_stats(self._h, C.byref(ix), C.byref(wk)), "b2k_codestream_parse_device_stats")
         return ix.value, wk.value
+
+    def _parse_window_device(self, ptr, n, win, reduce, handle, blocks=None):
+        L = lib()
+        L.b2k_codestream_parse_window_device.restype = C.c_int64
+        L.b2k_codestream_parse_window_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.c_void_p,
+                                                         C.POINTER(Coding), C.c_void_p, C.c_uint64]
+        cp = Coding()
+        m = L.b2k_codestream_parse_window_device(self._h, ptr, n, win, reduce, handle, C.byref(cp),
+                                                 None if blocks is None else blocks.ctypes.data, 0 if blocks is None else len(blocks))
+        if m < 0 or m == 1:
+            raise (NotHandled if m == 1 else EngineError)("b2k_codestream_parse_window_device: " + (L.b2k_last_error() or b"").decode())
+        return cp, m
+
+    @staticmethod
+    def _window_rect(cp, window, reduce):
+        """the window's pixels at 1 / 2**reduce on the virtual coding's canvas, as codestream_parse_window gives them"""
+        if window is None:
+            return (cp.x0, cp.y0, cp.x1, cp.y1)
+        sh = (1 << reduce) - 1
+        x0, y0, x1, y1 = [(v + sh) >> reduce for v in window]
+        return (max(x0, cp.x0), max(y0, cp.y0), min(x1, cp.x1), min(y1, cp.y1))
+
+    def codestream_parse_window_device(self, cs, window=None, reduce=0, stream=None):
+        """b2k_codestream_parse_window_device -> (virtual Coding, block table, rect), as codestream_parse_window of the
+        stream's bytes gives them, for a code stream on the engine's GPU (a 1-D uint8 CUDA array) parsed there.  Only the
+        wanted tiles' tile-part headers and packets are read."""
+        ptr, n = self._device_codestream_bytes(cs)
+        handle = _stream_handle(stream, cs)
+        win = (C.c_uint32 * 4)(*window) if window is not None else None
+        cp, nb = self._parse_window_device(ptr, n, win, reduce, handle)
+        blocks = np.zeros(nb, BLOCK_DTYPE)
+        cp, m = self._parse_window_device(ptr, n, win, reduce, handle, blocks)
+        if m != nb:
+            raise EngineError("b2k_codestream_parse_window_device: %d blocks, then %d" % (nb, m))
+        return cp, blocks, self._window_rect(cp, window, reduce)
+
+    def decode_window_device(self, cs, window=None, reduce=0, out=None, dtype=None, layout="CHW", stream=None):
+        """Windowed / reduced-resolution decode of a code stream on the engine's GPU (a 1-D uint8 CUDA array), into an
+        image on the GPU: decode_codestream_device(host bytes, window=, reduce=) without the stream leaving the device.
+        Only the tiles the window touches are parsed, copied and decoded.  out: a CUDA array of the window's shape at
+        1 / 2**reduce in `layout`, or None for a new torch tensor of `dtype` (default torch.uint16).  Returns
+        (virtual Coding, out)."""
+        ptr, n = self._device_codestream_bytes(cs)
+        handle = _stream_handle(stream, cs)
+        win = (C.c_uint32 * 4)(*window) if window is not None else None
+        cp, _ = self._parse_window_device(ptr, n, win, reduce, handle)   # the main header: the window's shape
+        x0, y0, x1, y1 = self._window_rect(cp, window, reduce)
+        h, w = y1 - y0, x1 - x0
+        if out is None:
+            import torch
+            shape = (cp.numcomps, h, w) if layout == "CHW" else (h, w, cp.numcomps)
+            out = torch.empty(shape, dtype=torch.uint16 if dtype is None else dtype, device="cuda:%d" % self.device)
+        img = device_planes(out, cp.numcomps, h, w, layout, writable=True)
+        L = lib()
+        L.b2k_decode_codestream_window_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32,
+                                                          C.POINTER(DevicePlanes), C.c_void_p, C.POINTER(Coding),
+                                                          C.POINTER(C.c_uint32), C.POINTER(C.c_double)]
+        rect = (C.c_uint32 * 4)()
+        ms = C.c_double()
+        _check_handled(L.b2k_decode_codestream_window_device(self._h, ptr, n, win, reduce, C.byref(img), handle, C.byref(cp),
+                                                             rect, C.byref(ms)), "b2k_decode_codestream_window_device")
+        assert tuple(rect) == (x0, y0, x1, y1), (tuple(rect), (x0, y0, x1, y1))
+        return cp, out
+
+    def codestream_window_device_stats(self):
+        """(wanted tiles, bytes copied into the engine's arena) of the last windowed device parse on this engine"""
+        t, b = C.c_uint32(), C.c_uint64()
+        L = lib()
+        L.b2k_codestream_window_device_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
+        _check(L.b2k_codestream_window_device_stats(self._h, C.byref(t), C.byref(b)), "b2k_codestream_window_device_stats")
+        return t.value, b.value
 
     def _decode_device_codestream(self, cs, out, dtype, layout, stream):
         ptr, n = self._device_codestream_bytes(cs)

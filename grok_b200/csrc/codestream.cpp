@@ -1289,29 +1289,14 @@ int b2k_parse_main_header(const uint8_t* cs, uint64_t len, t2::MainHeader& h)
   return 0;
 }
 
-/* window: x0,y0,x1,y1 on the full-resolution canvas, or NULL for the whole image; reduce: highest resolutions to drop.
-   *cp_out is the coding to DECODE WITH: for a window / reduced decode a virtual image that holds exactly the tiles the
-   window touches, at the reduced resolution (see b2k_codestream_parse_window below). */
-static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* window, uint32_t reduce, b2k_coding* cp_out,
-                          b2k_block* blocks, uint64_t cap_blocks)
+int b2k_window_coding(const b2k_coding& cp, const uint32_t* window, uint32_t reduce, t2::WindowCoding& wc)
 {
-  if(!cs || !cp_out)
-    return -1;
   auto fail = [&](const char* m, int rc) {
     b2k_set_error(m);
-    return (int64_t)rc;
-  };
-  t2::MainHeader mh;
-  if(int rc = b2k_parse_main_header(cs, len, mh))
     return rc;
-  Cursor c{cs + mh.sot, cs + len};
-  const b2k_coding cp = mh.cp;
-  const int progression = mh.progression;
-  const bool use_sop = mh.sop, use_eph = mh.eph;
+  };
   const std::vector<BandQuant> q = band_quant(cp);
   const TileGrid g = tile_grid(cp);
-  const uint32_t ntiles = g.nx * g.ny;
-
   /* ---- the tiles to deliver and the coding to decode them with ---------------------------------------------------
    * Whole image at full resolution: the stream's own coding.  Otherwise a VIRTUAL image: its area is the bounding box
    * of the tiles the window touches (clipped to the image), its tile grid is the stream's grid re-anchored at the first
@@ -1356,6 +1341,7 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
     const bool one_tile = tb_x - ta_x == 1 && tb_y - ta_y == 1;
     if(one_tile)
       vcp.tx0 = vcp.ty0 = vcp.tw = vcp.th = 0; /* the tile is the (virtual) image: no grid to keep aligned */
+    wc.box = vcp;
     if(reduce)
     {
       const uint32_t m = (1u << reduce) - 1u;
@@ -1378,7 +1364,8 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
    * four lifting steps of 9/7 -- taken as 2 and 5.  A block of resolution r >= 1 lives in band coordinates, i.e. those
    * of resolution r - 1.  Blocks outside are handed back with length 0 ("not in any packet": decoded as zeros): their
    * coefficients cannot reach the window. */
-  std::vector<Rect> need;
+  std::vector<Rect>& need = wc.need;
+  need.clear();
   if(window && !whole)
   {
     const uint32_t m = (1u << reduce) - 1u;
@@ -1398,6 +1385,88 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
       }
     }
   }
+  wc.whole = whole;
+  wc.ta_x = ta_x;
+  wc.ta_y = ta_y;
+  wc.tb_x = tb_x;
+  wc.tb_y = tb_y;
+  wc.vcp = vcp;
+  if(whole)
+    wc.box = cp;
+  return 0;
+}
+
+int b2k_window_blocks(const t2::WindowCoding& wc, const b2k_block* vblocks, uint64_t nv, std::vector<b2k_block>& box_blocks,
+                      std::vector<uint32_t>& vmap)
+{
+  const b2k_coding& box = wc.box;
+  const TileGrid bg = tile_grid(box);
+  const uint32_t nt = bg.nx * bg.ny;
+  const std::vector<BandQuant> bq = band_quant(box);
+  box_blocks.clear();
+  vmap.assign(nv, 0);
+  uint64_t k = 0;
+  for(uint32_t t = 0; t < nt; ++t)
+  {
+    const size_t first = box_blocks.size();
+    enumerate_tile_blocks(box, t, tile_rect(box, bg, t), bq, box_blocks);
+    for(size_t i = first; i < box_blocks.size(); ++i)
+    { /* the virtual tile's own enumeration: the box tile's blocks of the kept resolutions follow in the same order */
+      const b2k_block& b = box_blocks[i];
+      if(b.resno >= wc.vcp.numres)
+        continue;
+      const b2k_block* v = k < nv ? &vblocks[k] : nullptr;
+      if(!v || v->tile != t || v->comp != b.comp || v->resno != b.resno || v->band_index != b.band_index || v->precno != b.precno ||
+         v->cblkno != b.cblkno || v->x1 - v->x0 != b.x1 - b.x0 || v->y1 - v->y0 != b.y1 - b.y0)
+      {
+        b2k_set_error("internal: virtual and original block enumerations disagree");
+        return -1;
+      }
+      vmap[k++] = (uint32_t)i;
+    }
+    if(k < nv && vblocks[k].tile == t)
+    {
+      b2k_set_error("internal: virtual tile holds a different number of blocks");
+      return -1;
+    }
+  }
+  if(k != nv || box_blocks.size() > 0xFFFFFFFFull)
+  {
+    b2k_set_error("internal: virtual tile holds a different number of blocks");
+    return -1;
+  }
+  return 0;
+}
+
+/* window: x0,y0,x1,y1 on the full-resolution canvas, or NULL for the whole image; reduce: highest resolutions to drop.
+   *cp_out is the coding to DECODE WITH: for a window / reduced decode a virtual image that holds exactly the tiles the
+   window touches, at the reduced resolution (see b2k_codestream_parse_window below). */
+static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* window, uint32_t reduce, b2k_coding* cp_out,
+                          b2k_block* blocks, uint64_t cap_blocks)
+{
+  if(!cs || !cp_out)
+    return -1;
+  auto fail = [&](const char* m, int rc) {
+    b2k_set_error(m);
+    return (int64_t)rc;
+  };
+  t2::MainHeader mh;
+  if(int rc = b2k_parse_main_header(cs, len, mh))
+    return rc;
+  Cursor c{cs + mh.sot, cs + len};
+  const b2k_coding cp = mh.cp;
+  const int progression = mh.progression;
+  const bool use_sop = mh.sop, use_eph = mh.eph;
+  const std::vector<BandQuant> q = band_quant(cp);
+  const TileGrid g = tile_grid(cp);
+  const uint32_t ntiles = g.nx * g.ny;
+  t2::WindowCoding wc;
+  if(int rc = b2k_window_coding(cp, window, reduce, wc))
+    return rc;
+  const bool whole = wc.whole;
+  const uint32_t ta_x = wc.ta_x, ta_y = wc.ta_y, tb_x = wc.tb_x, tb_y = wc.tb_y;
+  const b2k_coding& vcp = wc.vcp;
+  const std::vector<Rect>& need = wc.need;
   const TileGrid vg = tile_grid(vcp);
   const uint32_t vnt = vg.nx * vg.ny;
   if(!whole && (vg.nx != tb_x - ta_x || vg.ny != tb_y - ta_y))

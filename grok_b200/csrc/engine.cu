@@ -67,6 +67,10 @@ struct b2k_engine
   cudaEvent_t caller_ev = nullptr; /* b2k_encode_device / b2k_decode_device: orders the engine's streams after the caller's */
   uint8_t* d_cs = nullptr;         /* b2k_encode_codestream_device: the last code stream */
   uint64_t cs_cap = 0;
+  /* b2k_codestream_window_device_stats: the last windowed device parse's wanted tiles and the bytes its arena takes */
+  bool have_window_stats = false;
+  uint32_t window_tiles = 0;
+  uint64_t window_bytes = 0;
 };
 
 /* ---- device memory cache --------------------------------------------------------------------------------------
@@ -382,6 +386,8 @@ struct b2k_device_job
   bool dec_has_refinement = false; /* the block table of the current decode carries SigProp / MagRef passes */
   T2Job* t2 = nullptr;             /* b2k_encode_codestream_device: the code stream's plan for the flags of the last call */
   T2Parse* t2p = nullptr;          /* b2k_decode_codestream_device: the packet plan for the last stream's progression / SOP / EPH */
+  T2Parse* t2w = nullptr;          /* b2k_decode_codestream_window_device: the box coding's plan (this job's coding is the virtual one) */
+  bool last_parse_window = false;  /* the last device parse was a windowed one (b2k_codestream_parse_device_stats) */
 };
 
 /* -------------------------------------------------------------------------------------------- */
@@ -842,6 +848,7 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
   cudaStreamSynchronize(J->eng->stream);
   b2k_t2_destroy(J->t2);
   b2k_t2_parse_destroy(J->t2p);
+  b2k_t2_parse_destroy(J->t2w);
   cudaFree(J->img.base);
   cudaFree(J->d_stage);
   cudaFree(J->coef.base);
@@ -2711,17 +2718,21 @@ static int read_device_main_header(const uint8_t* cs, uint64_t len, cudaStream_t
 }
 
 /* the header, the job of its coding, the stream in the job's arena and its parse on st, up to the status.  With dec the
-   decoder's descriptors are built too.  0, or b2k_codestream_parse's return code with its text. */
+   decoder's descriptors are built too.  header_read: h already holds the main header, read after the caller's work.  0, or
+   b2k_codestream_parse's return code with its text. */
 static int parse_device_codestream(b2k_engine* e, const uint8_t* cs, uint64_t len, cudaStream_t caller, b2k::t2::MainHeader& h,
-                                   b2k_device_job** out, bool dec, bool* refinement, uint64_t cap_blocks = UINT64_MAX)
+                                   b2k_device_job** out, bool dec, bool* refinement, uint64_t cap_blocks = UINT64_MAX,
+                                   bool header_read = false)
 {
   cudaStream_t st = e->stream;
   CUDA_TRY(cudaSetDevice(e->device));
-  /* what the caller queued before the call (the kernel, receive or read that produced cs) comes first */
-  CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
-  CUDA_TRY(cudaStreamWaitEvent(st, e->caller_ev, 0));
-  if(int rc = read_device_main_header(cs, len, st, h))
-    return rc;
+  if(!header_read)
+  { /* what the caller queued before the call (the kernel, receive or read that produced cs) comes first */
+    CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
+    CUDA_TRY(cudaStreamWaitEvent(st, e->caller_ev, 0));
+    if(int rc = read_device_main_header(cs, len, st, h))
+      return rc;
+  }
   int rc = 0;
   b2k_device_job* J = cached_job(e, &h.cp, 1, 0, &rc);
   if(rc)
@@ -2750,6 +2761,7 @@ static int parse_device_codestream(b2k_engine* e, const uint8_t* cs, uint64_t le
     J->bytes_cap = len + 4096;
   }
   J->arena_sized = false; /* the arena now holds a caller's stream, not this job's coding of its image */
+  J->last_parse_window = false;
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   CUDA_TRY(cudaMemcpyAsync(J->d_bytes, cs, len, cudaMemcpyDeviceToDevice, st));
   if(b2k_t2_parse_enqueue(J->t2p, J->d_bytes, len, h.sot, J->d_enc_desc, J->d_dec_quant, dec ? J->d_dec_desc : nullptr, st))
@@ -2790,27 +2802,16 @@ extern "C" int64_t b2k_codestream_parse_device(b2k_engine* e, const uint8_t* cs,
   return (int64_t)n;
 }
 
-extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const b2k_device_planes* img,
-                                                void* cuda_stream, b2k_coding* cp_out, double* ms_total)
+/* after a parse into J's descriptors: block decode -> inverse -> the caller's device image, which holds `window` (x0, y0,
+   x1, y1 on cp's canvas) or, window = NULL, the whole image; the caller's stream then waits for the image writes */
+static int32_t decode_parsed(b2k_engine* e, b2k_device_job* J, const b2k_coding& cp, const b2k_device_planes* img, const Rect* window,
+                             bool refinement, cudaStream_t caller, double* ms_total)
 {
-  if(!e || !cp_out)
-    return -1;
-  if(check_device_bytes(e, cs, len))
-    return -1;
-  std::lock_guard<std::mutex> lock(e->mu);
-  const auto wall0 = std::chrono::steady_clock::now();
-  cudaStream_t caller = caller_stream(cuda_stream);
-  b2k::t2::MainHeader h;
-  b2k_device_job* J = nullptr;
-  bool refinement = false;
-  if(int rc = parse_device_codestream(e, cs, len, caller, h, &J, true, &refinement))
-    return rc;
-  *cp_out = h.cp;
-  DBG_T("device decode: parsed");
-  if(int rc = check_device_planes(e, &h.cp, img))
+  if(int rc = check_device_planes(e, &cp, img))
     return rc;
   Transport T;
-  device_samples(T, *img, h.cp.x0, h.cp.y0);
+  device_samples(T, *img, window ? window->x0 : cp.x0, window ? window->y0 : cp.y0);
+  T.window = window;
   if(resolve_transport(J, T, true))
     return -1;
   cudaStream_t st = e->stream;
@@ -2829,7 +2830,6 @@ extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs
   CUDA_TRY(cudaStreamWaitEvent(caller, e->caller_ev, 0));
   CUDA_TRY(cudaEventSynchronize(J->ev[1]));
   CUDA_TRY(cudaGetLastError());
-  DBG_T("device decode: done");
   float t = 0;
   cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
   if(ms_total) *ms_total = t;
@@ -2843,16 +2843,223 @@ extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs
   return 0;
 }
 
+extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const b2k_device_planes* img,
+                                                void* cuda_stream, b2k_coding* cp_out, double* ms_total)
+{
+  if(!e || !cp_out)
+    return -1;
+  if(check_device_bytes(e, cs, len))
+    return -1;
+  std::lock_guard<std::mutex> lock(e->mu);
+  const auto wall0 = std::chrono::steady_clock::now();
+  cudaStream_t caller = caller_stream(cuda_stream);
+  b2k::t2::MainHeader h;
+  b2k_device_job* J = nullptr;
+  bool refinement = false;
+  if(int rc = parse_device_codestream(e, cs, len, caller, h, &J, true, &refinement))
+    return rc;
+  *cp_out = h.cp;
+  DBG_T("device decode: parsed");
+  const int32_t rc = decode_parsed(e, J, h.cp, img, nullptr, refinement, caller, ms_total);
+  DBG_T("device decode: done");
+  return rc;
+}
+
+/* ---- windows of code streams in device memory (b2k_codestream_parse_window_device / b2k_decode_codestream_window_device)
+ * The host reads the main header and derives the virtual coding as b2k_codestream_parse_window does (b2k_window_coding);
+ * the device parses the wanted tiles' packets in place from cs against the box coding's plan, then one gather copies only
+ * those tiles' packet data into the virtual job's arena.  A window that covers every tile at full resolution is the
+ * stream's own coding: the whole-stream path.  Synchronisations: the header, the parse status, the end of the decode. */
+struct DeviceWindow
+{
+  b2k::t2::MainHeader h;
+  b2k::t2::WindowCoding wc;
+  Rect rect{}; /* the window's pixels at 1 / 2^reduce on the virtual canvas */
+};
+
+/* the header and the window's coding, read after the caller's queued work: 0 or the host parser's code and text */
+static int device_window_coding(b2k_engine* e, const uint8_t* cs, uint64_t len, const uint32_t* window, uint32_t reduce,
+                                cudaStream_t caller, DeviceWindow& w)
+{
+  CUDA_TRY(cudaSetDevice(e->device));
+  CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
+  CUDA_TRY(cudaStreamWaitEvent(e->stream, e->caller_ev, 0));
+  if(int rc = read_device_main_header(cs, len, e->stream, w.h))
+    return rc;
+  if(int rc = b2k_window_coding(w.h.cp, window, reduce, w.wc))
+    return rc;
+  const b2k_coding& v = w.wc.vcp;
+  w.rect = Rect{v.x0, v.y0, v.x1, v.y1};
+  if(window)
+  {
+    const uint32_t m = (1u << reduce) - 1u;
+    w.rect = Rect{std::max((uint32_t)(((uint64_t)window[0] + m) >> reduce), v.x0), std::max((uint32_t)(((uint64_t)window[1] + m) >> reduce), v.y0),
+                  std::min((uint32_t)(((uint64_t)window[2] + m) >> reduce), v.x1), std::min((uint32_t)(((uint64_t)window[3] + m) >> reduce), v.y1)};
+  }
+  return 0;
+}
+
+/* the windowed parse on st up to the status (and, with dec, the gather into the arena): 0, or the host parser's code and text */
+static int parse_device_window(b2k_engine* e, const uint8_t* cs, uint64_t len, const DeviceWindow& w, uint32_t reduce,
+                               b2k_device_job** out, bool dec, bool* refinement, uint64_t cap_blocks)
+{
+  cudaStream_t st = e->stream;
+  int rc = 0;
+  b2k_device_job* J = cached_job(e, &w.wc.vcp, 1, 0, &rc);
+  if(rc)
+    return rc;
+  *out = J;
+  if(cap_blocks < J->blocks.size())
+  {
+    g_err = "block table too small";
+    return -1;
+  }
+  const uint32_t flags = B2K_CS_PROG(w.h.progression) | (w.h.sop ? B2K_CS_SOP : 0u) | (w.h.eph ? B2K_CS_EPH : 0u);
+  if(!b2k_t2_window_matches(J->t2w, w.wc.box, flags, reduce))
+  { /* box geometry, progression and reduce: planned once for every window with the same tile box */
+    b2k_t2_parse_destroy(J->t2w);
+    J->t2w = nullptr;
+    if(b2k_t2_window_create(w.wc, flags, reduce, J->blocks.data(), J->blocks.size(), J->coded_index.data(), J->coded_index.size(), &J->t2w))
+      return -1;
+  }
+  J->last_parse_window = true;
+  J->arena_sized = false;
+  const TileGrid g = tile_grid(w.h.cp);
+  CUDA_TRY(cudaEventRecord(J->ev[0], st));
+  if(b2k_t2_window_enqueue(J->t2w, cs, len, w.h.sot, g.nx, g.nx * g.ny, w.wc, J->d_enc_desc, J->d_dec_quant, dec ? J->d_dec_desc : nullptr,
+                           st))
+    return -1;
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if(int prc = b2k_t2_parse_result(J->t2w, refinement))
+    return prc;
+  if(!dec)
+    return 0;
+  const uint64_t bytes = b2k_t2_window_bytes(J->t2w);
+  if(bytes + 64 > J->bytes_cap)
+  { /* the HT decoder reads past a block's end: the host path's slack */
+    cudaFree(J->d_bytes);
+    J->d_bytes = nullptr;
+    J->bytes_cap = 0;
+    CUDA_TRY(cudaMalloc(&J->d_bytes, bytes + 4096));
+    J->bytes_cap = bytes + 4096;
+  }
+  return b2k_t2_window_gather(J->t2w, cs, J->d_bytes, st);
+}
+
+/* a windowed parse passed its status: its wanted tiles, and the bytes of the stream its decode copies into the arena (the
+   wanted tiles' packet data; the whole stream when every tile is wanted at full resolution) */
+static void note_window_stats(b2k_engine* e, const b2k_device_job* J, uint64_t bytes)
+{
+  e->have_window_stats = true;
+  e->window_tiles = (uint32_t)J->tiles.size();
+  e->window_bytes = bytes;
+}
+
+extern "C" int64_t b2k_codestream_parse_window_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const uint32_t* window,
+                                                      uint32_t reduce, void* cuda_stream, b2k_coding* cp_out, b2k_block* blocks,
+                                                      uint64_t cap_blocks)
+{
+  if(!e || !cp_out)
+    return -1;
+  if(check_device_bytes(e, cs, len))
+    return -1;
+  std::lock_guard<std::mutex> lock(e->mu);
+  cudaStream_t caller = caller_stream(cuda_stream);
+  DeviceWindow w;
+  if(int rc = device_window_coding(e, cs, len, window, reduce, caller, w))
+    return rc;
+  if(!blocks)
+  {
+    *cp_out = w.wc.vcp;
+    return b2k_enumerate(&w.wc.vcp, 1, 0, nullptr, 0);
+  }
+  b2k_device_job* J = nullptr;
+  e->have_window_stats = false;
+  if(w.wc.whole)
+  {
+    int rc = parse_device_codestream(e, cs, len, caller, w.h, &J, false, nullptr, cap_blocks, true);
+    if(J)
+      *cp_out = w.h.cp;
+    if(rc)
+      return rc;
+    note_window_stats(e, J, len);
+    if(b2k_t2_parse_blocks(J->t2p, blocks, e->stream))
+      return -1;
+    return (int64_t)J->blocks.size();
+  }
+  int rc = parse_device_window(e, cs, len, w, reduce, &J, false, nullptr, cap_blocks);
+  if(J)
+    *cp_out = w.wc.vcp;
+  if(rc)
+    return rc;
+  note_window_stats(e, J, b2k_t2_window_bytes(J->t2w));
+  if(b2k_t2_window_blocks(J->t2w, J->blocks.data(), J->blocks.size(), w.wc.need, blocks, e->stream))
+    return -1;
+  return (int64_t)J->blocks.size();
+}
+
+extern "C" int32_t b2k_decode_codestream_window_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const uint32_t* window,
+                                                       uint32_t reduce, const b2k_device_planes* img, void* cuda_stream,
+                                                       b2k_coding* cp_out, uint32_t* rect_out, double* ms_total)
+{
+  if(!e || !cp_out)
+    return -1;
+  if(check_device_bytes(e, cs, len))
+    return -1;
+  std::lock_guard<std::mutex> lock(e->mu);
+  const auto wall0 = std::chrono::steady_clock::now();
+  cudaStream_t caller = caller_stream(cuda_stream);
+  DeviceWindow w;
+  if(int rc = device_window_coding(e, cs, len, window, reduce, caller, w))
+    return rc;
+  b2k_device_job* J = nullptr;
+  bool refinement = false;
+  e->have_window_stats = false;
+  int rc = w.wc.whole ? parse_device_codestream(e, cs, len, caller, w.h, &J, true, &refinement, UINT64_MAX, true)
+                      : parse_device_window(e, cs, len, w, reduce, &J, true, &refinement, UINT64_MAX);
+  if(rc)
+    return rc;
+  note_window_stats(e, J, w.wc.whole ? len : b2k_t2_window_bytes(J->t2w));
+  *cp_out = w.wc.vcp;
+  if(rect_out)
+  {
+    rect_out[0] = w.rect.x0;
+    rect_out[1] = w.rect.y0;
+    rect_out[2] = w.rect.x1;
+    rect_out[3] = w.rect.y1;
+  }
+  DBG_T("device window decode: parsed");
+  rc = decode_parsed(e, J, w.wc.vcp, img, &w.rect, refinement, caller, ms_total);
+  DBG_T("device window decode: done");
+  return rc;
+}
+
+extern "C" int32_t b2k_codestream_window_device_stats(b2k_engine* e, uint32_t* tiles_wanted, uint64_t* arena_bytes)
+{
+  if(!e || !tiles_wanted || !arena_bytes)
+    return -1;
+  std::lock_guard<std::mutex> lock(e->mu);
+  if(!e->have_window_stats)
+  {
+    g_err = "no windowed code stream parse has been made on the device";
+    return -1;
+  }
+  *tiles_wanted = e->window_tiles;
+  *arena_bytes = e->window_bytes;
+  return 0;
+}
+
 extern "C" int32_t b2k_codestream_parse_device_stats(b2k_engine* e, uint32_t* tiles_indexed, uint32_t* tiles_walked)
 {
   if(!e || !tiles_indexed || !tiles_walked)
     return -1;
   std::lock_guard<std::mutex> lock(e->mu);
-  if(!e->cached || !e->cached->t2p)
+  T2Parse* last = e->cached ? (e->cached->last_parse_window ? e->cached->t2w : e->cached->t2p) : nullptr;
+  if(!last)
   {
     g_err = "no code stream has been parsed on the device";
     return -1;
   }
-  b2k_t2_parse_stats(e->cached->t2p, tiles_indexed, tiles_walked);
+  b2k_t2_parse_stats(last, tiles_indexed, tiles_walked);
   return 0;
 }

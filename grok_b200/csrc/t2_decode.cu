@@ -17,8 +17,15 @@
  *                    has refinement passes.
  * Tag trees live in global scratch sized by the plan (packet_tag_nodes per packet, so every packet has its own); a walking
  * thread reuses its tile's share for every packet of the tile.
+ *
+ * A windowed parse runs the same five launches against the plan of the box coding (the wanted tiles at full resolution,
+ * whose packets are those of the stream's tiles), reading cs in place: k_t2_locate checks every SOT but reads and records
+ * only the wanted tiles' parts, under their box index, and lays their packet data end to end; k_t2_desc maps each coded
+ * block of the virtual coding to its box block, leaves the blocks outside the window's need rectangles uncoded and points
+ * the descriptors into that layout.  After the status read, k_t2_gather copies just those bytes into the job's arena.
  */
 #include <algorithm>
+#include <cstring>
 #include <string>
 #include <vector>
 
@@ -27,6 +34,7 @@
 #include "t2_plan.h"
 #include "t2_parse.h"
 #include "t2_decode.h"
+#include "geometry.h"
 
 using namespace b2k;
 using namespace b2k::t2;
@@ -44,15 +52,29 @@ struct ParseStatus
   uint32_t refinement;         /* some block has refinement passes to decode */
   uint32_t walked;             /* tiles with data parsed by the walk */
   uint32_t indexed;            /* tiles whose packets were parsed from their PLT starts */
+  unsigned long long bytes;    /* packet data of the recorded tile parts */
+};
+/* a coded block of a windowed parse's virtual coding: its box tile, the need rectangle that applies to it (resolution
+   max(resno - 1, 0)) and its rectangle in band coordinates */
+struct WinBlock
+{
+  uint32_t tile, res, x0, y0, x1, y1;
+};
+struct NeedRects /* the window's need rectangles, one per resolution of the virtual coding; n = 0: no filter */
+{
+  uint32_t n;
+  uint32_t r[B2K_MAX_RES][4];
 };
 
-__global__ void k_t2_locate(const uint8_t* __restrict__ cs, uint64_t len, uint64_t sot, uint32_t ntiles, PartRange* __restrict__ parts,
-                            uint64_t cap, uint32_t* __restrict__ head, uint32_t* __restrict__ last, uint32_t* __restrict__ count,
-                            ParseStatus* status)
+__global__ void k_t2_locate(const uint8_t* __restrict__ cs, uint64_t len, uint64_t sot, uint32_t ntiles, TileBox box,
+                            PartRange* __restrict__ parts, uint64_t cap, uint32_t* __restrict__ head, uint32_t* __restrict__ last,
+                            uint32_t* __restrict__ count, uint64_t* __restrict__ body_at, ParseStatus* status)
 {
   uint32_t n = 0;
-  status->locate = locate_tile_parts(cs, len, sot, ntiles, parts, cap, head, last, count, &n);
+  uint64_t bytes = 0;
+  status->locate = locate_tile_parts_box(cs, len, sot, ntiles, box, parts, cap, head, last, count, &n, body_at, &bytes);
   status->nparts = n;
+  status->bytes = bytes;
 }
 
 __global__ void k_t2_plt(const uint8_t* __restrict__ cs, const PartRange* __restrict__ parts, const uint32_t* __restrict__ head,
@@ -114,22 +136,50 @@ __global__ void k_t2_walk(const uint8_t* __restrict__ cs, const PartRange* __res
     atomicMin(&status->tile_err, ((unsigned long long)t << 8) | r);
 }
 
+/* win != NULL (a windowed parse): coded[k] is the box block of virtual coded block k; a block the window does not need
+   stays uncoded, and a parsed block's bytes are addressed where k_t2_gather puts them */
 __global__ void k_t2_desc(const ParsedBlock* __restrict__ blk, const uint32_t* __restrict__ coded, uint32_t ncoded,
                           const HtBlockDesc* __restrict__ enc, const float* __restrict__ quant, HtBlockDesc* __restrict__ dec,
-                          ParseStatus* status)
+                          const WinBlock* __restrict__ win, const NeedRects* __restrict__ need, const PartRange* __restrict__ parts,
+                          const uint32_t* __restrict__ head, const uint64_t* __restrict__ body_at, ParseStatus* status)
 {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if(k >= ncoded || status->locate != PR_NONE || status->tile_err != NO_ERROR)
     return;
-  const ParsedBlock b = blk[coded[k]];
+  ParsedBlock b = blk[coded[k]];
+  uint64_t at = b.offset;
+  if(win)
+  {
+    const WinBlock w = win[k];
+    if(need->n && !window_needs(need->r[w.res], w.x0, w.y0, w.x1, w.y1))
+      b = ParsedBlock{};
+    at = b.length ? gathered_offset(parts, head[w.tile], body_at, b.offset) : 0;
+  }
   HtBlockDesc d = enc[k];
   d.length = b.length;
-  d.slot_off = b.offset;
+  d.slot_off = at;
   block_decode_fields(b, d.kmax, &d.mmsbs, &d.passes, &d.length2);
   d.quant = quant[k]; /* stepsize / 2^(31-Kmax) */
   dec[k] = d;
   if(d.passes > 1)
     status->refinement = 1;
+}
+
+/* the wanted tile parts' packet data, end to end: part p (blockIdx.y strided) by a strip of CTAs along x */
+__global__ void k_t2_gather(const uint8_t* __restrict__ cs, const PartRange* __restrict__ parts, const uint64_t* __restrict__ body_at,
+                            uint32_t nparts, uint8_t* __restrict__ out)
+{
+  for(uint32_t p = blockIdx.y; p < nparts; p += gridDim.y)
+  {
+    const PartRange R = parts[p];
+    if(R.end <= R.begin)
+      continue;
+    const uint64_t n = R.end - R.begin;
+    const uint8_t* src = cs + R.begin;
+    uint8_t* dst = out + body_at[p];
+    for(uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+      dst[i] = src[i];
+  }
 }
 
 template <class T>
@@ -162,6 +212,17 @@ struct T2Parse
   ParseStatus* h_status = nullptr; /* pinned */
   PartRange* d_parts = nullptr;    /* grown with the code stream's length */
   uint64_t parts_cap = 0;
+  /* a windowed parse: the plan is the box coding's; coded block k of the virtual coding is box block d_coded[k] */
+  bool window = false;
+  b2k_coding box{};
+  uint32_t reduce = 0;
+  std::vector<uint32_t> vmap;      /* every virtual block -> its box block */
+  WinBlock* d_win = nullptr;
+  NeedRects* d_need = nullptr;
+  NeedRects* h_need = nullptr;     /* pinned */
+  uint64_t* d_body_at = nullptr;   /* per recorded part, parts_cap of them */
+  uint32_t* d_wcount = nullptr;    /* tile parts seen per stream tile */
+  uint32_t wcount_cap = 0;
 };
 
 #define T2P_TRY(expr)                                                                                                          \
@@ -249,36 +310,91 @@ int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* b
   return 0;
 }
 
+int b2k_t2_window_create(const b2k::t2::WindowCoding& wc, uint32_t flags, uint32_t reduce, const b2k_block* vblocks, uint64_t nv,
+                         const uint32_t* coded_index, uint64_t ncoded, T2Parse** out)
+{
+  *out = nullptr;
+  std::vector<b2k_block> box_blocks;
+  std::vector<uint32_t> vmap;
+  if(b2k_window_blocks(wc, vblocks, nv, box_blocks, vmap))
+    return -1;
+  const TileGrid bg = tile_grid(wc.box);
+  std::vector<uint32_t> coded_box(ncoded);
+  std::vector<WinBlock> win(ncoded);
+  for(uint64_t k = 0; k < ncoded; ++k)
+  {
+    const b2k_block& v = vblocks[coded_index[k]];
+    coded_box[k] = vmap[coded_index[k]];
+    win[k] = WinBlock{v.tile, v.resno ? v.resno - 1u : 0u, v.x0, v.y0, v.x1, v.y1};
+  }
+  T2Parse* J = nullptr;
+  if(b2k_t2_parse_create(wc.box, flags, box_blocks.data(), box_blocks.size(), bg.nx * bg.ny, coded_box.data(), ncoded, &J))
+    return -1;
+  struct Guard
+  {
+    T2Parse*& j;
+    ~Guard() { b2k_t2_parse_destroy(j); }
+  } guard{J};
+  J->window = true;
+  J->box = wc.box;
+  J->reduce = reduce;
+  J->vmap.swap(vmap);
+  T2P_TRY(cudaMalloc(&J->d_win, std::max<uint64_t>(ncoded, 1) * sizeof(WinBlock) + sizeof(NeedRects)));
+  J->d_need = reinterpret_cast<NeedRects*>(J->d_win + std::max<uint64_t>(ncoded, 1));
+  T2P_TRY(cudaMemcpy(J->d_win, win.data(), ncoded * sizeof(WinBlock), cudaMemcpyHostToDevice));
+  T2P_TRY(cudaHostAlloc(&J->h_need, sizeof(NeedRects), cudaHostAllocDefault));
+  *out = J;
+  J = nullptr;
+  return 0;
+}
+
+bool b2k_t2_window_matches(const T2Parse* J, const b2k_coding& box, uint32_t flags, uint32_t reduce)
+{
+  return J && J->window && J->flags == flags && J->reduce == reduce && memcmp(&J->box, &box, sizeof(box)) == 0;
+}
+
 void b2k_t2_parse_destroy(T2Parse* J)
 {
   if(!J)
     return;
   cudaFree(J->d_mem);
   cudaFree(J->d_parts);
+  cudaFree(J->d_body_at);
+  cudaFree(J->d_win);
+  cudaFree(J->d_wcount);
   cudaFreeHost(J->h_status);
+  cudaFreeHost(J->h_need);
   delete J;
 }
 
 uint32_t b2k_t2_parse_flags(const T2Parse* J) { return J->flags; }
 
-int b2k_t2_parse_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, const HtBlockDesc* d_enc, const float* d_quant,
-                         HtBlockDesc* d_dec, cudaStream_t st)
+/* the five launches over the plan's tiles, which are the tiles of `box` among the stream's ntiles */
+static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t ntiles, const TileBox& box, uint32_t* d_count,
+                         const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
 {
   /* every tile part takes at least the 12 bytes of its SOT, and a tile has at most 256 */
   const uint64_t need = std::min<uint64_t>(len / 12 + 1, 256ull * J->ntiles);
   if(need > J->parts_cap)
   {
     cudaFree(J->d_parts);
+    cudaFree(J->d_body_at);
     J->d_parts = nullptr;
+    J->d_body_at = nullptr;
     J->parts_cap = 0;
     const uint64_t cap = need + need / 4 + 16;
     T2P_TRY(cudaMalloc(&J->d_parts, cap * sizeof(PartRange)));
+    if(J->window)
+      T2P_TRY(cudaMalloc(&J->d_body_at, cap * sizeof(uint64_t)));
     J->parts_cap = cap;
   }
-  ParseStatus init{NO_ERROR, 0, 0, 0, 0, 0};
+  ParseStatus init{NO_ERROR, 0, 0, 0, 0, 0, 0};
   *J->h_status = init;
   T2P_TRY(cudaMemcpyAsync(J->d_status, J->h_status, sizeof(ParseStatus), cudaMemcpyHostToDevice, st));
-  k_t2_locate<<<1, 1, 0, st>>>(cs, len, sot, J->ntiles, J->d_parts, J->parts_cap, J->d_head, J->d_last, J->d_count, J->d_status);
+  if(J->window)
+    T2P_TRY(cudaMemcpyAsync(J->d_need, J->h_need, sizeof(NeedRects), cudaMemcpyHostToDevice, st));
+  k_t2_locate<<<1, 1, 0, st>>>(cs, len, sot, ntiles, box, J->d_parts, J->parts_cap, J->d_head, J->d_last, d_count, J->d_body_at,
+                               J->d_status);
   b2k_count_launch();
   const uint32_t tpb = 32; /* tiles and packets are few and each thread is a long serial chain: spread them over the SMs */
   const bool sop = (J->flags & B2K_CS_SOP) != 0, eph = (J->flags & B2K_CS_EPH) != 0;
@@ -300,11 +416,88 @@ int b2k_t2_parse_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t s
   if(d_dec && J->ncoded)
   {
     k_t2_desc<<<(unsigned)((J->ncoded + 127) / 128), 128, 0, st>>>(J->d_blk, J->d_coded, (uint32_t)J->ncoded, d_enc, d_quant, d_dec,
+                                                                   J->d_win, J->d_need, J->d_parts, J->d_head, J->d_body_at,
                                                                    J->d_status);
     b2k_count_launch();
   }
   T2P_TRY(cudaMemcpyAsync(J->h_status, J->d_status, sizeof(ParseStatus), cudaMemcpyDeviceToHost, st));
   T2P_TRY(cudaGetLastError());
+  return 0;
+}
+
+int b2k_t2_parse_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, const HtBlockDesc* d_enc, const float* d_quant,
+                         HtBlockDesc* d_dec, cudaStream_t st)
+{
+  return enqueue_parse(J, cs, len, sot, J->ntiles, TileBox{J->ntiles, 0, 0, J->ntiles, 1}, J->d_count, d_enc, d_quant, d_dec, st);
+}
+
+int b2k_t2_window_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t grid_nx, uint32_t ntiles,
+                          const b2k::t2::WindowCoding& wc, const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
+{
+  if(ntiles > J->wcount_cap)
+  {
+    cudaFree(J->d_wcount);
+    J->d_wcount = nullptr;
+    J->wcount_cap = 0;
+    T2P_TRY(cudaMalloc(&J->d_wcount, ntiles * sizeof(uint32_t)));
+    J->wcount_cap = ntiles;
+  }
+  NeedRects& n = *J->h_need;
+  n.n = (uint32_t)std::min<size_t>(wc.need.size(), B2K_MAX_RES);
+  for(uint32_t r = 0; r < n.n; ++r)
+  {
+    n.r[r][0] = wc.need[r].x0;
+    n.r[r][1] = wc.need[r].y0;
+    n.r[r][2] = wc.need[r].x1;
+    n.r[r][3] = wc.need[r].y1;
+  }
+  return enqueue_parse(J, cs, len, sot, ntiles, TileBox{grid_nx, wc.ta_x, wc.ta_y, wc.tb_x, wc.tb_y}, J->d_wcount, d_enc, d_quant, d_dec,
+                       st);
+}
+
+uint64_t b2k_t2_window_bytes(const T2Parse* J) { return J->h_status->bytes; }
+
+int b2k_t2_window_gather(const T2Parse* J, const uint8_t* cs, uint8_t* out, cudaStream_t st)
+{
+  const uint32_t nparts = J->h_status->nparts;
+  const uint64_t bytes = J->h_status->bytes;
+  if(!nparts || !bytes)
+    return 0;
+  const uint64_t per_part = bytes / nparts;
+  const unsigned gx = (unsigned)std::min<uint64_t>(256, per_part / (256 * 16) + 1);
+  k_t2_gather<<<dim3(gx, std::min<uint32_t>(nparts, 65535)), 256, 0, st>>>(cs, J->d_parts, J->d_body_at, nparts, out);
+  b2k_count_launch();
+  T2P_TRY(cudaGetLastError());
+  return 0;
+}
+
+int b2k_t2_window_blocks(const T2Parse* J, const b2k_block* vblocks, uint64_t nv, const std::vector<Rect>& need, b2k_block* out,
+                         cudaStream_t st)
+{
+  std::vector<ParsedBlock> pb(J->nblocks);
+  T2P_TRY(cudaMemcpyAsync(pb.data(), J->d_blk, J->nblocks * sizeof(ParsedBlock), cudaMemcpyDeviceToHost, st));
+  T2P_TRY(cudaStreamSynchronize(st));
+  for(uint64_t i = 0; i < nv; ++i)
+  {
+    b2k_block b = vblocks[i];
+    const ParsedBlock& p = pb[J->vmap[i]];
+    bool wanted = true;
+    if(!need.empty())
+    {
+      const Rect& n = need[b.resno ? b.resno - 1 : 0];
+      const uint32_t r[4] = {n.x0, n.y0, n.x1, n.y1};
+      wanted = window_needs(r, b.x0, b.y0, b.x1, b.y1);
+    }
+    if(wanted)
+    {
+      b.offset = p.offset;
+      b.length = p.length;
+      b.length2 = p.length2;
+      b.numbps = p.numbps;
+      b.numpasses = p.numpasses;
+    }
+    out[i] = b;
+  }
   return 0;
 }
 

@@ -116,18 +116,32 @@ struct ByteCursor
   }
 };
 
-/* The tile parts from the first SOT (at sot) to EOC or the end of the stream, in stream order, as the host parser walks
- * them (A.4.2): SOT, Psot hop, tile-part header segments up to SOD.  head[t] / last[t] / count[t] (ntiles each) are
- * scratch the walk initialises; parts holds cap entries.  Returns PR_NONE or the first failure in stream order. */
-B2K_HD uint32_t locate_tile_parts(const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t ntiles, PartRange* parts, uint64_t cap,
-                                  uint32_t* head, uint32_t* last, uint32_t* count, uint32_t* nparts)
+/* the tiles a windowed parse wants: columns [x0, x1) and rows [y0, y1) of a grid nx tiles wide.  Box tile
+   (ix - x0) + (iy - y0) * (x1 - x0) is the stream's tile ix + iy * nx. */
+struct TileBox
 {
-  for(uint32_t t = 0; t < ntiles; ++t)
-  {
+  uint32_t nx, x0, y0, x1, y1;
+  B2K_HD uint32_t tiles() const { return (x1 - x0) * (y1 - y0); }
+};
+
+/* The tile parts from the first SOT (at sot) to EOC or the end of the stream, in stream order, as the host parser walks
+ * them (A.4.2): SOT, Psot hop, tile-part header segments up to SOD.  Every SOT is checked; a tile outside `box` is hopped
+ * over through Psot without its tile-part header being read, and only the wanted tiles' parts are recorded, under their
+ * box tile index.  head[t] / last[t] (box.tiles() each) and count[t] (ntiles) are scratch the walk initialises; parts holds
+ * cap entries.  body_at (when not NULL) receives where each recorded part's packet data starts when the bodies are laid
+ * end to end, *body_bytes their total.  Returns PR_NONE or the first failure in stream order. */
+B2K_HD uint32_t locate_tile_parts_box(const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t ntiles, const TileBox& box,
+                                      PartRange* parts, uint64_t cap, uint32_t* head, uint32_t* last, uint32_t* count, uint32_t* nparts,
+                                      uint64_t* body_at, uint64_t* body_bytes)
+{
+  for(uint32_t t = 0; t < box.tiles(); ++t)
     head[t] = last[t] = PART_NONE;
+  for(uint32_t t = 0; t < ntiles; ++t)
     count[t] = 0;
-  }
   *nparts = 0;
+  uint64_t bytes = 0;
+  if(body_bytes)
+    *body_bytes = 0;
   /* Psot = 0: the tile part runs to the end of the stream, before a final EOC */
   const uint64_t open_end = len - ((len >= 2 && cs[len - 2] == 0xFF && cs[len - 1] == 0xD9) ? 2 : 0);
   ByteCursor c{cs, sot, len, true};
@@ -150,6 +164,13 @@ B2K_HD uint32_t locate_tile_parts(const uint8_t* cs, uint64_t len, uint64_t sot,
     const uint64_t tp_end = psot ? at + psot : open_end;
     if(tp_end > len || tp_end < c.p)
       return PR_PSOT;
+    const uint32_t ix = isot % box.nx, iy = isot / box.nx;
+    if(ix < box.x0 || ix >= box.x1 || iy < box.y0 || iy >= box.y1)
+    { /* not wanted: hop over it */
+      c.p = tp_end;
+      continue;
+    }
+    const uint32_t bt = (ix - box.x0) + (iy - box.y0) * (box.x1 - box.x0);
     for(;;)
     { /* tile-part header: PLT, COM and unknown segments are skipped */
       const uint32_t tm = c.u16();
@@ -166,16 +187,29 @@ B2K_HD uint32_t locate_tile_parts(const uint8_t* cs, uint64_t len, uint64_t sot,
     }
     if(n >= cap)
       return PR_PART_TABLE;
-    parts[n] = PartRange{at + 12, c.p, tp_end, isot, PART_NONE};
-    if(last[isot] == PART_NONE)
-      head[isot] = n;
+    parts[n] = PartRange{at + 12, c.p, tp_end, bt, PART_NONE};
+    if(body_at)
+      body_at[n] = bytes;
+    bytes += tp_end > c.p ? tp_end - c.p : 0;
+    if(body_bytes)
+      *body_bytes = bytes;
+    if(last[bt] == PART_NONE)
+      head[bt] = n;
     else
-      parts[last[isot]].next = n;
-    last[isot] = n;
+      parts[last[bt]].next = n;
+    last[bt] = n;
     *nparts = ++n;
     c.p = tp_end;
   }
   return PR_NONE;
+}
+
+/* every tile wanted: the tile parts of the whole stream, under their own tile index */
+B2K_HD uint32_t locate_tile_parts(const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t ntiles, PartRange* parts, uint64_t cap,
+                                  uint32_t* head, uint32_t* last, uint32_t* count, uint32_t* nparts)
+{
+  return locate_tile_parts_box(cs, len, sot, ntiles, TileBox{ntiles, 0, 0, ntiles, 1}, parts, cap, head, last, count, nparts, nullptr,
+                               nullptr);
 }
 
 /* packet-header bits: MSB first, the byte after 0xFF carries 7 bits (T.800 B.10.1); reading past end gives 0 bits and
@@ -467,6 +501,23 @@ B2K_HD void block_decode_fields(const ParsedBlock& b, uint8_t kmax, uint8_t* mms
   /* no refinement bytes, or a cleanup pass already at bit-plane 1, leave nothing to refine */
   *passes = (b.length && b.numpasses > 1 && b.length2 > 0 && *mmsbs < 29) ? b.numpasses : 1;
   *length2 = *passes > 1 ? b.length2 : 0;
+}
+
+/* a windowed decode's rule for one block of the virtual coding: its rectangle (band coordinates) meets need = x0, y0, x1,
+   y1 of resolution max(resno - 1, 0) (b2k_codestream_parse_window's need rectangles).  A block outside keeps length 0. */
+B2K_HD bool window_needs(const uint32_t* need, uint32_t x0, uint32_t y0, uint32_t x1, uint32_t y1)
+{
+  return x0 < need[2] && x1 > need[0] && y0 < need[3] && y1 > need[1];
+}
+
+/* where stream offset off of a parsed block of the tile whose first part is first lies once the tile parts' packet data
+   are laid end to end at body_at[part] (locate_tile_parts_box); a parsed block lies inside one of its tile's parts */
+B2K_HD uint64_t gathered_offset(const PartRange* parts, uint32_t first, const uint64_t* body_at, uint64_t off)
+{
+  for(uint32_t p = first; p != PART_NONE; p = parts[p].next)
+    if(off >= parts[p].begin && off < parts[p].end)
+      return body_at[p] + (off - parts[p].begin);
+  return 0;
 }
 
 } // namespace t2

@@ -8,6 +8,7 @@
 #include <stdint.h>
 #include <vector>
 #include "t2_packet.h"
+#include "geometry.h"
 #include "../../include/grok_b200.h"
 
 namespace b2k
@@ -45,11 +46,32 @@ struct MainHeader /* what a code stream's main header says (b2k_parse_main_heade
   uint64_t sot = 0;        /* where the first SOT starts */
   bool short_read = false; /* the failure came from reaching the end of the bytes given */
 };
+/* what a window and a reduce make of a stream's coding (b2k_window_coding) */
+struct WindowCoding
+{
+  bool whole = false;                 /* every tile at full resolution: the stream's own coding, nothing filtered */
+  uint32_t ta_x = 0, ta_y = 0;        /* the wanted tiles: columns [ta_x, tb_x), rows [ta_y, tb_y) of the stream's grid */
+  uint32_t tb_x = 0, tb_y = 0;
+  b2k_coding vcp{};                   /* the coding to decode with (the virtual image) */
+  b2k_coding box{};                   /* the box coding: the wanted tiles at full resolution with the stream's numres, whose
+                                         tiles, precincts and packets are those of the stream's tiles */
+  std::vector<Rect> need;             /* per resolution of vcp: the samples the window depends on; empty: no filter */
+};
 } // namespace t2
 } // namespace b2k
 
 /* the main header of cs[0, len), read by b2k_codestream_parse's own code: 0, or its return code with b2k_last_error set */
 int b2k_parse_main_header(const uint8_t* cs, uint64_t len, b2k::t2::MainHeader& h);
+
+/* the wanted tiles, the virtual coding and the window's need rectangles of b2k_codestream_parse_window(window, reduce) on a
+   stream of coding cp: 0, or its return code and text for the window errors, in its order */
+int b2k_window_coding(const b2k_coding& cp, const uint32_t* window, uint32_t reduce, b2k::t2::WindowCoding& w);
+
+/* the box coding's block enumeration, and for each of the virtual coding's blocks vblocks[0, nv) (enumeration order) the
+   box block it is: the box tile's blocks of the resolutions vcp keeps, in order.  0, or -1 with the host parser's text when
+   the two enumerations disagree. */
+int b2k_window_blocks(const b2k::t2::WindowCoding& w, const b2k_block* vblocks, uint64_t nv, std::vector<b2k_block>& box_blocks,
+                      std::vector<uint32_t>& vmap);
 
 /* the plan of the code stream b2k_codestream_write(cp, r, flags) writes, for the block table `blocks` (every block of the
    tiles of r, enumeration order) and r->num_tiles = num_tiles.  0, or -1 with b2k_last_error set in the cases, and with the

@@ -530,8 +530,32 @@ B2K_API int64_t b2k_codestream_parse_device(b2k_engine* e, const uint8_t* cs, ui
                                             b2k_coding* cp_out, b2k_block* blocks, uint64_t cap_blocks);
 /* How the last device parse on this engine read its tiles: tiles whose packets were parsed one thread per packet from
  * their PLT packet starts, and tiles with data walked packet after packet (no PLT, a PLT that does not add up, or a packet
- * that did not end where PLT said).  The results do not depend on the split; the time does. */
+ * that did not end where PLT said).  The results do not depend on the split; the time does.  After a windowed device
+ * parse, the counts are of the wanted tiles only. */
 B2K_API int32_t b2k_codestream_parse_device_stats(b2k_engine* e, uint32_t* tiles_indexed, uint32_t* tiles_walked);
+
+/* Windowed / reduced-resolution decode of a code stream in device memory: b2k_codestream_parse_window and
+ * b2k_decode_window for a stream on the engine's GPU.  Equal, for every input, to copying cs to the host and calling
+ * b2k_codestream_parse_window(cs, len, window, reduce, ...) + b2k_decode_device(virtual coding, blocks, ..., cs, ..., img,
+ * rect): the same return code and b2k_last_error text, the same virtual coding, the same block table (offsets into cs),
+ * the same pixels.  Every SOT of the stream is checked, but only the wanted tiles' tile-part headers and packets are read,
+ * in place from cs, and only their packet data is copied, into the engine's arena: the cost follows the window, not the
+ * stream.  A window that takes every tile at reduce 0 is the stream's own coding and takes b2k_decode_codestream_device's
+ * path.  Ordering against cuda_stream, the check of cs and -2 for blocks the HT decoder rejects are as there.
+ *
+ * window = x0,y0,x1,y1 on the full-resolution canvas (NULL: whole image), reduce = highest resolutions to drop.
+ * blocks == NULL: main header only, returns the block count and the virtual coding (as the host call does). */
+B2K_API int64_t b2k_codestream_parse_window_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const uint32_t* window,
+                                                   uint32_t reduce, void* cuda_stream, b2k_coding* cp_out,
+                                                   b2k_block* blocks, uint64_t cap_blocks);
+/* img holds rect_out = the window's pixels at 1/2^reduce on cp_out's canvas: x0,y0,x1,y1 of the window divided by 2^reduce
+ * (rounded up), clipped to the virtual image; the whole virtual image when window is NULL */
+B2K_API int32_t b2k_decode_codestream_window_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const uint32_t* window,
+                                                   uint32_t reduce, const b2k_device_planes* img, void* cuda_stream,
+                                                   b2k_coding* cp_out, uint32_t* rect_out, double* ms_total);
+/* last windowed device parse: wanted tiles, and bytes of their tile parts copied into the job's arena (the packet data of
+ * their tile parts; the whole stream when every tile was wanted at reduce 0) */
+B2K_API int32_t b2k_codestream_window_device_stats(b2k_engine* e, uint32_t* tiles_wanted, uint64_t* arena_bytes);
 
 /* Geometry only (host): enumerate the blocks of the selected tiles, lengths zero.  Returns the
  * count; fills at most cap entries. */
