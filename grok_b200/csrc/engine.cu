@@ -33,6 +33,7 @@
 #include "geometry.h"
 #include "t2_device.h"
 #include "t2_decode.h"
+#include "t2_parse.h"
 #include "t2_plan.h"
 
 using namespace b2k;
@@ -380,7 +381,7 @@ struct b2k_device_job
   uint64_t ring_slot_elems = 0, ring_elems = 0;
   cudaEvent_t ring_ev[16]{};
   PackTuner tune_enc, tune_dec;
-  std::vector<cudaEvent_t> q_ev;   /* per-step events of b2k_job_roundtrip_n */
+  std::vector<cudaEvent_t> q_ev;   /* per-step timing events of the round trips (roundtrip_begin) */
   std::vector<cudaEvent_t> p_ev;   /* per-chunk events of b2k_job_roundtrip_pipelined_n (scan done, chunk done) */
   std::vector<cudaStream_t> p_streams; /* its block-coder streams */
   bool dec_has_refinement = false; /* the block table of the current decode carries SigProp / MagRef passes */
@@ -1380,6 +1381,62 @@ static int download_chunk(b2k_device_job* J, const Transport& T, size_t k, cudaS
   return copy_runs(J, T.user, T.staged ? T.stage : plane_container(J->img), cs, t0, t1, T.window);
 }
 
+/* ---- bookkeeping every entry point shares ------------------------------------------------------- */
+/* The coded-byte arena holds `bytes` and the 64 the HT decoder reads past a block's end, or is replaced by one of bytes +
+   headroom + 4096.  Nothing queued still uses the old arena when it is freed.  A failed allocation leaves the job without
+   an arena (d_bytes NULL, bytes_cap 0): the next call allocates again, and b2k_job_destroy has nothing to free twice. */
+static int arena_reserve(b2k_device_job* J, uint64_t bytes, uint64_t headroom)
+{
+  if(bytes + 64 <= J->bytes_cap)
+    return 0;
+  CUDA_TRY(cudaStreamSynchronize(J->eng->stream));
+  cudaFree(J->d_bytes);
+  J->d_bytes = nullptr;
+  J->bytes_cap = 0;
+  const uint64_t cap = bytes + headroom + 4096;
+  CUDA_TRY(cudaMalloc(&J->d_bytes, cap));
+  J->bytes_cap = cap;
+  return 0;
+}
+
+/* what the HT decoder said of the blocks decoded since d_err was cleared: 0, or -2 and how many it rejected */
+static int decoder_verdict(b2k_device_job* J)
+{
+  int herr = 0;
+  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
+  if(herr)
+  {
+    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
+    return -2;
+  }
+  return 0;
+}
+
+/* what is queued on `next` from here on runs after what is queued on `first` now: the engine's stream after the caller's on
+   the way in, the caller's after the engine's on the way out */
+static int queue_after(b2k_engine* e, cudaStream_t first, cudaStream_t next)
+{
+  CUDA_TRY(cudaEventRecord(e->caller_ev, first));
+  CUDA_TRY(cudaStreamWaitEvent(next, e->caller_ev, 0));
+  return 0;
+}
+
+/* a stage hook's frame: enqueue(stream) between ev[0] and ev[1] on the engine's stream, one synchronisation, the time
+   between the two */
+template <class Enqueue>
+static int timed_stage(b2k_device_job* J, float* ms, Enqueue enqueue)
+{
+  cudaStream_t st = J->eng->stream;
+  CUDA_TRY(cudaEventRecord(J->ev[0], st));
+  if(enqueue(st)) return -1;
+  CUDA_TRY(cudaEventRecord(J->ev[1], st));
+  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
+  float t = 0;
+  CUDA_TRY(cudaEventElapsedTime(&t, J->ev[0], J->ev[1]));
+  if(ms) *ms = t;
+  return 0;
+}
+
 /* ---- stages ----------------------------------------------------------------------------------- */
 static int enqueue_forward(b2k_device_job* J, cudaStream_t st, bool time_level1, size_t t0 = 0, size_t t1 = (size_t)-1,
                            cudaEvent_t l1_begin = nullptr, cudaEvent_t l1_end = nullptr)
@@ -1453,12 +1510,7 @@ static int finish_t1_encode(b2k_device_job* J, cudaStream_t st)
   CUDA_TRY(cudaMemcpyAsync(&J->h_offsets[n], J->d_offsets + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   total = J->h_offsets[n];
-  if(total + 64 > J->bytes_cap)
-  {
-    cudaFree(J->d_bytes);
-    J->bytes_cap = total + total / 8 + 4096;
-    CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
-  }
+  if(arena_reserve(J, total, total / 8)) return -1;
   J->bytes_used = total;
   J->arena_sized = true;
   b2k_launch_ht_gather(J->d_enc_desc, J->d_out, J->d_offsets, J->d_scratch, J->d_bytes, n, J->bytes_cap, st);
@@ -1470,14 +1522,7 @@ extern "C" int32_t b2k_job_forward(b2k_device_job* J, float* ms)
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  cudaStream_t st = J->eng->stream;
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  if(enqueue_forward(J, st, true)) return -1;
-  CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
-  float t = 0;
-  CUDA_TRY(cudaEventElapsedTime(&t, J->ev[0], J->ev[1]));
-  if(ms) *ms = t;
+  if(timed_stage(J, ms, [&](cudaStream_t st) { return enqueue_forward(J, st, true); })) return -1;
   CUDA_TRY(cudaEventElapsedTime(&J->last_level1_ms, J->ev[4], J->ev[5]));
   return 0;
 }
@@ -1486,31 +1531,15 @@ extern "C" int32_t b2k_job_inverse(b2k_device_job* J, float* ms)
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  cudaStream_t st = J->eng->stream;
   J->arena_sized = false; /* the image planes now hold whatever the coefficient planes make */
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  if(enqueue_inverse(J, st)) return -1;
-  CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
-  float t = 0;
-  CUDA_TRY(cudaEventElapsedTime(&t, J->ev[0], J->ev[1]));
-  if(ms) *ms = t;
-  return 0;
+  return timed_stage(J, ms, [&](cudaStream_t st) { return enqueue_inverse(J, st); });
 }
 
 extern "C" int32_t b2k_job_t1_encode(b2k_device_job* J, float* ms, uint64_t* total_bytes)
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  cudaStream_t st = J->eng->stream;
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  if(enqueue_t1_encode(J, st)) return -1;
-  if(finish_t1_encode(J, st)) return -1;
-  CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
-  float t = 0;
-  CUDA_TRY(cudaEventElapsedTime(&t, J->ev[0], J->ev[1]));
-  if(ms) *ms = t;
+  if(timed_stage(J, ms, [&](cudaStream_t st) { return enqueue_t1_encode(J, st) || finish_t1_encode(J, st); })) return -1;
   if(total_bytes) *total_bytes = J->bytes_used;
   return 0;
 }
@@ -1537,12 +1566,8 @@ static int prepare_decode(b2k_device_job* J, const b2k_block* blocks, uint64_t n
       g_err = "an HT code block with more than 3 coding passes";
       return 1;
     }
-    const int nb = b.length ? b.numbps : 0;
-    d.mmsbs = (uint8_t)std::max(0, (int)d.kmax - nb);
-    /* ojph_block_decoder32.cpp L752-758, L790-803: no refinement bytes, or a cleanup pass already at
-       bit-plane 1, leave nothing to refine */
-    d.passes = (b.length && b.numpasses > 1 && b.length2 > 0 && d.mmsbs < 29) ? b.numpasses : 1;
-    d.length2 = d.passes > 1 ? b.length2 : 0;
+    const t2::ParsedBlock pb{b.offset, b.length, b.length2, b.numbps, b.numpasses, {}};
+    t2::block_decode_fields(pb, d.kmax, &d.mmsbs, &d.passes, &d.length2);
     if(d.passes > 1)
       J->dec_has_refinement = true;
     d.quant = J->dec_quant[k]; /* stepsize / 2^(31-Kmax), PostDecodeFiltersOJPH.h L103 */
@@ -1566,23 +1591,9 @@ extern "C" int32_t b2k_job_t1_decode(b2k_device_job* J, float* ms)
 {
   if(!J) return -1;
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  cudaStream_t st = J->eng->stream;
-  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  if(enqueue_t1_decode_own(J, st)) return -1;
-  CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
-  float t = 0;
-  CUDA_TRY(cudaEventElapsedTime(&t, J->ev[0], J->ev[1]));
-  if(ms) *ms = t;
-  int herr = 0;
-  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
-  if(herr)
-  {
-    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
-    return -2;
-  }
-  return 0;
+  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), J->eng->stream));
+  if(timed_stage(J, ms, [&](cudaStream_t st) { return enqueue_t1_decode_own(J, st); })) return -1;
+  return decoder_verdict(J);
 }
 
 /* stage hook: block-decode a caller-supplied block table (what the host's T2 parse produced, or a foreign
@@ -1594,13 +1605,7 @@ extern "C" int32_t b2k_job_t1_decode_blocks(b2k_device_job* J, const b2k_block* 
   CUDA_TRY(cudaSetDevice(J->eng->device));
   cudaStream_t st = J->eng->stream;
   J->arena_sized = false;
-  if(num_bytes + 64 > J->bytes_cap)
-  {
-    CUDA_TRY(cudaStreamSynchronize(st));
-    cudaFree(J->d_bytes);
-    J->bytes_cap = num_bytes + 4096;
-    CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
-  }
+  if(arena_reserve(J, num_bytes, 0)) return -1;
   J->dec_has_refinement = false;
   if(int prc = prepare_decode(J, blocks, num_blocks, st)) return prc;
   const uint32_t n = (uint32_t)J->h_enc_desc.size();
@@ -1613,25 +1618,16 @@ extern "C" int32_t b2k_job_t1_decode_blocks(b2k_device_job* J, const b2k_block* 
   CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
   if(num_bytes)
     CUDA_TRY(cudaMemcpyAsync(J->d_bytes, bytes, num_bytes, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  b2k_launch_ht_decode(J->d_dec_desc, J->d_bytes, J->d_recs, J->d_dec_status, n, J->max_cblk_w, J->d_err, J->cp.irreversible,
-                       J->dec_has_refinement, st);
-  if(J->dec_has_refinement)
-    b2k_launch_ht_decode_refine(J->d_dec_desc, J->d_bytes, J->d_dec_status, n, (J->cp.cblk_sty & 0x08) != 0, st);
-  CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
+  auto decode = [&](cudaStream_t) {
+    b2k_launch_ht_decode(J->d_dec_desc, J->d_bytes, J->d_recs, J->d_dec_status, n, J->max_cblk_w, J->d_err, J->cp.irreversible,
+                         J->dec_has_refinement, st);
+    if(J->dec_has_refinement)
+      b2k_launch_ht_decode_refine(J->d_dec_desc, J->d_bytes, J->d_dec_status, n, (J->cp.cblk_sty & 0x08) != 0, st);
+    return 0;
+  };
+  if(timed_stage(J, ms, decode)) return -1;
   CUDA_TRY(cudaGetLastError());
-  float t = 0;
-  CUDA_TRY(cudaEventElapsedTime(&t, J->ev[0], J->ev[1]));
-  if(ms) *ms = t;
-  int herr = 0;
-  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
-  if(herr)
-  {
-    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
-    return -2;
-  }
-  return 0;
+  return decoder_verdict(J);
 }
 
 /* One device-resident round trip, enqueued back to back with a single synchronisation at the end:
@@ -1642,61 +1638,69 @@ extern "C" int32_t b2k_job_t1_decode_blocks(b2k_device_job* J, const b2k_block* 
    reconstruction of a partial decode, so the caller uploads the image again before calling again. */
 extern "C" int32_t b2k_job_roundtrip(b2k_device_job* J, float* ms_total, float* stage_ms, uint64_t* total_bytes)
 {
-  if(!J) return -1;
+  return b2k_job_roundtrip_n(J, 1, ms_total, stage_ms, nullptr, total_bytes);
+}
+
+/* The frame the round trips share.  Each step owns `per` timing events of q_ev: e[0] its start, e[1] and e[2] around the
+   level-1 transform, e[3 + i] the end of its stage i.  Before the first step: the device, the arena sized by one
+   synchronising pass over a newly uploaded image, `events` events, the decoder's error count cleared. */
+static int roundtrip_begin(b2k_device_job* J, size_t events)
+{
   CUDA_TRY(cudaSetDevice(J->eng->device));
-  cudaStream_t st = J->eng->stream;
-  const uint32_t n = (uint32_t)J->h_enc_desc.size();
   if(!J->arena_sized)
-  { /* a new image: size the arena from a coding of it (one synchronising pass) */
-    float t;
-    uint64_t b;
-    if(int rc = b2k_job_forward(J, &t)) return rc;
-    if(int rc = b2k_job_t1_encode(J, &t, &b)) return rc;
+  {
+    if(int rc = b2k_job_forward(J, nullptr)) return rc;
+    if(int rc = b2k_job_t1_encode(J, nullptr, nullptr)) return rc;
   }
-  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  if(enqueue_forward(J, st, true)) return -1;
-  CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  if(enqueue_t1_encode(J, st)) return -1;
-  b2k_launch_ht_gather(J->d_enc_desc, J->d_out, J->d_offsets, J->d_scratch, J->d_bytes, n, J->bytes_cap, st);
-  CUDA_TRY(cudaMemcpyAsync(&J->h_offsets[n], J->d_offsets + n, sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaEventRecord(J->ev[2], st));
-  if(enqueue_t1_decode_own(J, st)) return -1;
-  CUDA_TRY(cudaEventRecord(J->ev[3], st));
-  if(enqueue_inverse(J, st)) return -1;
-  CUDA_TRY(cudaEventRecord(J->ev[6], st));
-  CUDA_TRY(cudaEventSynchronize(J->ev[6]));
+  while(J->q_ev.size() < events)
+  {
+    cudaEvent_t ev;
+    CUDA_TRY(cudaEventCreate(&ev));
+    J->q_ev.push_back(ev);
+  }
+  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), J->eng->stream));
+  return 0;
+}
+
+/* After the last step: the one synchronisation (on the end of the last step's last stage), the arena against the coded
+   size, the times (each stage's and level 1's summed over the steps), the decoder's verdict. */
+static int roundtrip_end(b2k_device_job* J, uint32_t steps, size_t per, int stages, float* ms_total, float* stage_ms, float* level1_ms,
+                         uint64_t* total_bytes)
+{
+  const uint32_t n = (uint32_t)J->h_enc_desc.size();
+  cudaEvent_t last = J->q_ev[per * (steps - 1) + 2 + stages];
+  CUDA_TRY(cudaEventSynchronize(last));
   CUDA_TRY(cudaGetLastError());
   if(J->h_offsets[n] > J->bytes_cap)
   { /* arena estimate too small (a 9/7 step drifted past its slack): grow; the caller uploads again and repeats */
-    cudaFree(J->d_bytes);
-    J->bytes_cap = J->h_offsets[n] + J->h_offsets[n] / 8 + 4096;
-    CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
+    if(arena_reserve(J, J->h_offsets[n], J->h_offsets[n] / 8)) return -1;
     g_err = "coded size grew past the arena: arena resized; the image planes hold a partial decode, upload again";
     return 2;
   }
   J->bytes_used = J->h_offsets[n];
   J->arena_sized = true;
-  float t[5] = {0, 0, 0, 0, 0};
-  cudaEventElapsedTime(&t[0], J->ev[0], J->ev[1]);
-  cudaEventElapsedTime(&t[1], J->ev[1], J->ev[2]);
-  cudaEventElapsedTime(&t[2], J->ev[2], J->ev[3]);
-  cudaEventElapsedTime(&t[3], J->ev[3], J->ev[6]);
-  cudaEventElapsedTime(&t[4], J->ev[0], J->ev[6]);
-  cudaEventElapsedTime(&J->last_level1_ms, J->ev[4], J->ev[5]);
-  if(ms_total) *ms_total = t[4];
-  if(stage_ms)
-    for(int i = 0; i < 4; ++i)
-      stage_ms[i] = t[i];
-  if(total_bytes) *total_bytes = J->bytes_used;
-  int herr = 0;
-  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
-  if(herr)
+  float sums[4] = {0, 0, 0, 0}, l1 = 0, tot = 0;
+  for(uint32_t s = 0; s < steps; ++s)
   {
-    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
-    return -2;
+    cudaEvent_t* e = J->q_ev.data() + per * s;
+    float t = 0;
+    for(int i = 0; i < stages; ++i)
+    {
+      cudaEventElapsedTime(&t, e[i ? 2 + i : 0], e[3 + i]);
+      sums[i] += t;
+    }
+    cudaEventElapsedTime(&t, e[1], e[2]);
+    l1 += t;
   }
-  return 0;
+  cudaEventElapsedTime(&tot, J->q_ev[0], last);
+  J->last_level1_ms = l1 / steps;
+  if(ms_total) *ms_total = tot;
+  if(stage_ms)
+    for(int i = 0; i < stages; ++i)
+      stage_ms[i] = sums[i];
+  if(level1_ms) *level1_ms = l1;
+  if(total_bytes) *total_bytes = J->bytes_used;
+  return decoder_verdict(J);
 }
 
 /* n device-resident round trips queued back to back on the stream, ONE synchronisation after the last: what a
@@ -1708,24 +1712,10 @@ extern "C" int32_t b2k_job_roundtrip_n(b2k_device_job* J, uint32_t steps, float*
                                        uint64_t* total_bytes)
 {
   if(!J || !steps) return -1;
-  CUDA_TRY(cudaSetDevice(J->eng->device));
   cudaStream_t st = J->eng->stream;
   const uint32_t n = (uint32_t)J->h_enc_desc.size();
-  if(!J->arena_sized)
-  { /* a new image: size the arena from a coding of it (one synchronising pass) */
-    float t;
-    uint64_t b;
-    if(int rc = b2k_job_forward(J, &t)) return rc;
-    if(int rc = b2k_job_t1_encode(J, &t, &b)) return rc;
-  }
   const size_t per = 7; /* start, l1 begin, l1 end, after forward, after encode, after decode, end */
-  while(J->q_ev.size() < per * steps)
-  {
-    cudaEvent_t ev;
-    CUDA_TRY(cudaEventCreate(&ev));
-    J->q_ev.push_back(ev);
-  }
-  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
+  if(int rc = roundtrip_begin(J, per * steps)) return rc;
   for(uint32_t s = 0; s < steps; ++s)
   {
     cudaEvent_t* e = J->q_ev.data() + per * s;
@@ -1742,45 +1732,7 @@ extern "C" int32_t b2k_job_roundtrip_n(b2k_device_job* J, uint32_t steps, float*
     if(enqueue_inverse(J, st)) return -1;
     CUDA_TRY(cudaEventRecord(e[6], st));
   }
-  CUDA_TRY(cudaEventSynchronize(J->q_ev[per * (steps - 1) + 6]));
-  CUDA_TRY(cudaGetLastError());
-  if(J->h_offsets[n] > J->bytes_cap)
-  {
-    cudaFree(J->d_bytes);
-    J->bytes_cap = J->h_offsets[n] + J->h_offsets[n] / 8 + 4096;
-    CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
-    g_err = "coded size grew past the arena: arena resized; the image planes hold a partial decode, upload again";
-    return 2;
-  }
-  J->bytes_used = J->h_offsets[n];
-  J->arena_sized = true;
-  float sums[4] = {0, 0, 0, 0}, l1 = 0, tot = 0;
-  for(uint32_t s = 0; s < steps; ++s)
-  {
-    cudaEvent_t* e = J->q_ev.data() + per * s;
-    float t = 0;
-    cudaEventElapsedTime(&t, e[0], e[3]); sums[0] += t;
-    cudaEventElapsedTime(&t, e[3], e[4]); sums[1] += t;
-    cudaEventElapsedTime(&t, e[4], e[5]); sums[2] += t;
-    cudaEventElapsedTime(&t, e[5], e[6]); sums[3] += t;
-    cudaEventElapsedTime(&t, e[1], e[2]); l1 += t;
-  }
-  cudaEventElapsedTime(&tot, J->q_ev[0], J->q_ev[per * (steps - 1) + 6]);
-  J->last_level1_ms = l1 / steps;
-  if(ms_total) *ms_total = tot;
-  if(stage_ms)
-    for(int i = 0; i < 4; ++i)
-      stage_ms[i] = sums[i];
-  if(level1_ms) *level1_ms = l1;
-  if(total_bytes) *total_bytes = J->bytes_used;
-  int herr = 0;
-  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
-  if(herr)
-  {
-    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
-    return -2;
-  }
-  return 0;
+  return roundtrip_end(J, steps, per, 4, ms_total, stage_ms, level1_ms, total_bytes);
 }
 
 /* The same n round trips with the BLOCK-CODER stage software-pipelined over tile-independent block ranges: the forward
@@ -1795,16 +1747,10 @@ extern "C" int32_t b2k_job_roundtrip_pipelined_n(b2k_device_job* J, uint32_t ste
                                                  float* stage_ms, float* level1_ms, uint64_t* total_bytes)
 {
   if(!J || !steps) return -1;
-  CUDA_TRY(cudaSetDevice(J->eng->device));
   cudaStream_t st = J->eng->stream;
   const uint32_t n = (uint32_t)J->h_enc_desc.size();
-  if(!J->arena_sized)
-  { /* a new image: size the arena from a coding of it (one synchronising pass) */
-    float t;
-    uint64_t b;
-    if(int rc = b2k_job_forward(J, &t)) return rc;
-    if(int rc = b2k_job_t1_encode(J, &t, &b)) return rc;
-  }
+  const size_t per = 5; /* start, l1 begin, l1 end, after forward, after the block coder; the next step's start ends the inverse */
+  if(int rc = roundtrip_begin(J, per * steps + 1)) return rc;
   /* measured on config 2 (tools/stage_times.py, DESIGN.md section 6): 2 ranges on 2 streams 2.62 ms against 2.82 ms back to
      back; more ranges per stream lose (phase A's serial chain is a ~0.35 ms floor per launch, the persistent encoder grid
      fills every SM's shared memory), and so does a dedicated encoder stream with a capped grid */
@@ -1825,14 +1771,6 @@ extern "C" int32_t b2k_job_roundtrip_pipelined_n(b2k_device_job* J, uint32_t ste
     CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     J->p_ev.push_back(ev);
   }
-  const size_t per = 5; /* start, l1 begin, l1 end, after forward, after the block coder; the next step's start ends the inverse */
-  while(J->q_ev.size() < per * steps + 1)
-  {
-    cudaEvent_t ev;
-    CUDA_TRY(cudaEventCreate(&ev));
-    J->q_ev.push_back(ev);
-  }
-  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
   for(uint32_t s = 0; s < steps; ++s)
   {
     cudaEvent_t* e = J->q_ev.data() + per * s;
@@ -1864,46 +1802,8 @@ extern "C" int32_t b2k_job_roundtrip_pipelined_n(b2k_device_job* J, uint32_t ste
     CUDA_TRY(cudaEventRecord(e[4], st));
     if(enqueue_inverse(J, st)) return -1;
   }
-  cudaEvent_t last = J->q_ev[per * steps];
-  CUDA_TRY(cudaEventRecord(last, st));
-  CUDA_TRY(cudaEventSynchronize(last));
-  CUDA_TRY(cudaGetLastError());
-  if(J->h_offsets[n] > J->bytes_cap)
-  {
-    cudaFree(J->d_bytes);
-    J->bytes_cap = J->h_offsets[n] + J->h_offsets[n] / 8 + 4096;
-    CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
-    g_err = "coded size grew past the arena: arena resized; the image planes hold a partial decode, upload again";
-    return 2;
-  }
-  J->bytes_used = J->h_offsets[n];
-  J->arena_sized = true;
-  float sums[3] = {0, 0, 0}, l1 = 0, tot = 0;
-  for(uint32_t s = 0; s < steps; ++s)
-  {
-    cudaEvent_t* e = J->q_ev.data() + per * s;
-    float t = 0;
-    cudaEventElapsedTime(&t, e[0], e[3]); sums[0] += t;
-    cudaEventElapsedTime(&t, e[3], e[4]); sums[1] += t;
-    cudaEventElapsedTime(&t, e[4], e[per]); sums[2] += t; /* e[per] = the next step's start, or `last` */
-    cudaEventElapsedTime(&t, e[1], e[2]); l1 += t;
-  }
-  cudaEventElapsedTime(&tot, J->q_ev[0], last);
-  J->last_level1_ms = l1 / steps;
-  if(ms_total) *ms_total = tot;
-  if(stage_ms)
-    for(int i = 0; i < 3; ++i)
-      stage_ms[i] = sums[i];
-  if(level1_ms) *level1_ms = l1;
-  if(total_bytes) *total_bytes = J->bytes_used;
-  int herr = 0;
-  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
-  if(herr)
-  {
-    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
-    return -2;
-  }
-  return 0;
+  CUDA_TRY(cudaEventRecord(J->q_ev[per * steps], st)); /* the last step's e[per]: the end of its inverse */
+  return roundtrip_end(J, steps, per, 3, ms_total, stage_ms, level1_ms, total_bytes);
 }
 
 extern "C" int32_t b2k_job_last_kernel_stats(const b2k_device_job* J, int which, float* ms, uint64_t* alg_bytes)
@@ -2239,11 +2139,8 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
   /* software pipeline over tile chunks: chunk k+1 crosses PCIe on the copy stream while chunk k
      is transformed and block-coded on the compute stream */
   cudaStream_t cs = e->copy_stream;
-  if(dev)
-  { /* what the caller queued before the call (the kernel that made the frame) comes first */
-    CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
-    CUDA_TRY(cudaStreamWaitEvent(st, e->caller_ev, 0));
-  }
+  /* what the caller queued before the call (the kernel that made the frame) comes first */
+  if(dev && queue_after(e, caller, st)) return -1;
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   CUDA_TRY(cudaStreamWaitEvent(cs, J->ev[0], 0));
   const size_t nchunks = J->chunk_tile.size() - 1;
@@ -2327,11 +2224,8 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
     }
   }
   CUDA_TRY(cudaEventRecord(J->ev[2], st));
-  if(dev)
-  { /* the caller's stream goes on once every chunk of its image has been read */
-    CUDA_TRY(cudaEventRecord(e->caller_ev, st));
-    CUDA_TRY(cudaStreamWaitEvent(caller, e->caller_ev, 0));
-  }
+  /* the caller's stream goes on once every chunk of its image has been read */
+  if(dev && queue_after(e, st, caller)) return -1;
   DBG_T("encode: chunks enqueued");
   if(dc)
     return device_t2(e, J, st, *dc);
@@ -2349,10 +2243,7 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
     { /* estimate too small: grow, compact everything again from the scratch slots, plain copy */
       pool_put(hb);
       hb = nullptr;
-      CUDA_TRY(cudaStreamSynchronize(st));
-      cudaFree(J->d_bytes);
-      J->bytes_cap = total + total / 8 + 4096;
-      CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
+      if(arena_reserve(J, total, total / 8)) return -1;
       b2k_launch_ht_gather(J->d_enc_desc, J->d_out, J->d_offsets, J->d_scratch, J->d_bytes, nb_all, J->bytes_cap, st);
       CUDA_TRY(cudaEventRecord(J->ev[3], st));
       if(int frc = fetch_result(J, st, &R, nullptr, shell)) return frc;
@@ -2569,17 +2460,9 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
     return -1;
   const bool dev = T.user.device;
   cudaStream_t st = e->stream;
-  if(num_bytes + 64 > J->bytes_cap)
-  {
-    cudaFree(J->d_bytes);
-    J->bytes_cap = num_bytes + 4096;
-    CUDA_TRY(cudaMalloc(&J->d_bytes, J->bytes_cap));
-  }
-  if(dev)
-  { /* what the caller queued before the call (e.g. the last reader of its buffer) comes first */
-    CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
-    CUDA_TRY(cudaStreamWaitEvent(st, e->caller_ev, 0));
-  }
+  if(arena_reserve(J, num_bytes, 0)) return -1;
+  /* what the caller queued before the call (e.g. the last reader of its buffer) comes first */
+  if(dev && queue_after(e, caller, st)) return -1;
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
   J->dec_has_refinement = false;
@@ -2640,11 +2523,8 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
   CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(0, nchunks)], cs));
   CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(0, nchunks)], 0));
   CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  if(dev)
-  { /* the caller's stream goes on once its image is written */
-    CUDA_TRY(cudaEventRecord(e->caller_ev, st));
-    CUDA_TRY(cudaStreamWaitEvent(caller, e->caller_ev, 0));
-  }
+  /* the caller's stream goes on once its image is written */
+  if(dev && queue_after(e, st, caller)) return -1;
   CUDA_TRY(cudaEventSynchronize(J->ev[1]));
   CUDA_TRY(cudaGetLastError());
   DBG_T("decode: done");
@@ -2653,14 +2533,7 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
   if(ms_total) *ms_total = t;
   if(T.tuner)
     T.tuner->record(T.ring, std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count());
-  int herr = 0;
-  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
-  if(herr)
-  {
-    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
-    return -2;
-  }
-  return 0;
+  return decoder_verdict(J);
 }
 
 /* ---- code streams in device memory (b2k_decode_codestream_device / b2k_codestream_parse_device) ----------------------
@@ -2728,8 +2601,7 @@ static int parse_device_codestream(b2k_engine* e, const uint8_t* cs, uint64_t le
   CUDA_TRY(cudaSetDevice(e->device));
   if(!header_read)
   { /* what the caller queued before the call (the kernel, receive or read that produced cs) comes first */
-    CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
-    CUDA_TRY(cudaStreamWaitEvent(st, e->caller_ev, 0));
+    if(queue_after(e, caller, st)) return -1;
     if(int rc = read_device_main_header(cs, len, st, h))
       return rc;
   }
@@ -2743,7 +2615,7 @@ static int parse_device_codestream(b2k_engine* e, const uint8_t* cs, uint64_t le
     g_err = "block table too small";
     return -1;
   }
-  const uint32_t flags = B2K_CS_PROG(h.progression) | (h.sop ? B2K_CS_SOP : 0u) | (h.eph ? B2K_CS_EPH : 0u);
+  const uint32_t flags = h.flags();
   if(!J->t2p || b2k_t2_parse_flags(J->t2p) != flags)
   { /* geometry and progression only: planned once for every stream of this coding */
     b2k_t2_parse_destroy(J->t2p);
@@ -2752,14 +2624,7 @@ static int parse_device_codestream(b2k_engine* e, const uint8_t* cs, uint64_t le
                            J->coded_index.size(), &J->t2p))
       return -1;
   }
-  if(len + 64 > J->bytes_cap)
-  {
-    cudaFree(J->d_bytes);
-    J->d_bytes = nullptr;
-    J->bytes_cap = 0;
-    CUDA_TRY(cudaMalloc(&J->d_bytes, len + 4096));
-    J->bytes_cap = len + 4096;
-  }
+  if(arena_reserve(J, len, 0)) return -1;
   J->arena_sized = false; /* the arena now holds a caller's stream, not this job's coding of its image */
   J->last_parse_window = false;
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
@@ -2783,8 +2648,7 @@ extern "C" int64_t b2k_codestream_parse_device(b2k_engine* e, const uint8_t* cs,
   if(!blocks)
   {
     CUDA_TRY(cudaSetDevice(e->device));
-    CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
-    CUDA_TRY(cudaStreamWaitEvent(e->stream, e->caller_ev, 0));
+    if(queue_after(e, caller, e->stream)) return -1;
     if(int rc = read_device_main_header(cs, len, e->stream, h))
       return rc;
     *cp_out = h.cp;
@@ -2826,21 +2690,13 @@ static int32_t decode_parsed(b2k_engine* e, b2k_device_job* J, const b2k_coding&
   }
   CUDA_TRY(cudaEventRecord(J->ev[1], st));
   /* the caller's stream goes on once its image is written */
-  CUDA_TRY(cudaEventRecord(e->caller_ev, st));
-  CUDA_TRY(cudaStreamWaitEvent(caller, e->caller_ev, 0));
+  if(queue_after(e, st, caller)) return -1;
   CUDA_TRY(cudaEventSynchronize(J->ev[1]));
   CUDA_TRY(cudaGetLastError());
   float t = 0;
   cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
   if(ms_total) *ms_total = t;
-  int herr = 0;
-  CUDA_TRY(cudaMemcpy(&herr, J->d_err, sizeof(int), cudaMemcpyDeviceToHost));
-  if(herr)
-  {
-    g_err = "HT decoder rejected " + std::to_string(herr) + " block(s)";
-    return -2;
-  }
-  return 0;
+  return decoder_verdict(J);
 }
 
 extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const b2k_device_planes* img,
@@ -2882,8 +2738,7 @@ static int device_window_coding(b2k_engine* e, const uint8_t* cs, uint64_t len, 
                                 cudaStream_t caller, DeviceWindow& w)
 {
   CUDA_TRY(cudaSetDevice(e->device));
-  CUDA_TRY(cudaEventRecord(e->caller_ev, caller));
-  CUDA_TRY(cudaStreamWaitEvent(e->stream, e->caller_ev, 0));
+  if(queue_after(e, caller, e->stream)) return -1;
   if(int rc = read_device_main_header(cs, len, e->stream, w.h))
     return rc;
   if(int rc = b2k_window_coding(w.h.cp, window, reduce, w.wc))
@@ -2914,7 +2769,7 @@ static int parse_device_window(b2k_engine* e, const uint8_t* cs, uint64_t len, c
     g_err = "block table too small";
     return -1;
   }
-  const uint32_t flags = B2K_CS_PROG(w.h.progression) | (w.h.sop ? B2K_CS_SOP : 0u) | (w.h.eph ? B2K_CS_EPH : 0u);
+  const uint32_t flags = w.h.flags();
   if(!b2k_t2_window_matches(J->t2w, w.wc.box, flags, reduce))
   { /* box geometry, progression and reduce: planned once for every window with the same tile box */
     b2k_t2_parse_destroy(J->t2w);
@@ -2934,15 +2789,7 @@ static int parse_device_window(b2k_engine* e, const uint8_t* cs, uint64_t len, c
     return prc;
   if(!dec)
     return 0;
-  const uint64_t bytes = b2k_t2_window_bytes(J->t2w);
-  if(bytes + 64 > J->bytes_cap)
-  { /* the HT decoder reads past a block's end: the host path's slack */
-    cudaFree(J->d_bytes);
-    J->d_bytes = nullptr;
-    J->bytes_cap = 0;
-    CUDA_TRY(cudaMalloc(&J->d_bytes, bytes + 4096));
-    J->bytes_cap = bytes + 4096;
-  }
+  if(arena_reserve(J, b2k_t2_window_bytes(J->t2w), 0)) return -1;
   return b2k_t2_window_gather(J->t2w, cs, J->d_bytes, st);
 }
 

@@ -491,14 +491,16 @@ B2K_HD bool plt_index(const uint8_t* cs, const PartRange* parts, uint32_t first_
   return k == np;
 }
 
-/* prepare_decode's rule (engine.cu) for one coded block: missing MSBs, passes and refinement length; false when it has
-   refinement passes to decode */
+/* which passes of one coded block are decoded: missing MSBs, passes and refinement length (passes > 1: it has refinement
+   passes to decode).  The one statement of the rule: the device parser (k_t2_desc) and the host path (prepare_decode,
+   engine.cu) both call it, so the decoder gets the same descriptor either way */
 B2K_HD void block_decode_fields(const ParsedBlock& b, uint8_t kmax, uint8_t* mmsbs, uint8_t* passes, uint32_t* length2)
 {
   const int nb = b.length ? b.numbps : 0;
   const int m = (int)kmax - nb;
   *mmsbs = (uint8_t)(m > 0 ? m : 0);
-  /* no refinement bytes, or a cleanup pass already at bit-plane 1, leave nothing to refine */
+  /* ojph_block_decoder32.cpp L752-758, L790-803: no refinement bytes, or a cleanup pass already at bit-plane 1, leave
+     nothing to refine */
   *passes = (b.length && b.numpasses > 1 && b.length2 > 0 && *mmsbs < 29) ? b.numpasses : 1;
   *length2 = *passes > 1 ? b.length2 : 0;
 }

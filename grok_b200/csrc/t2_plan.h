@@ -45,6 +45,8 @@ struct MainHeader /* what a code stream's main header says (b2k_parse_main_heade
   bool sop = false, eph = false;
   uint64_t sot = 0;        /* where the first SOT starts */
   bool short_read = false; /* the failure came from reaching the end of the bytes given */
+  /* the B2K_CS_* flags a plan of this stream's packets is made with */
+  uint32_t flags() const { return B2K_CS_PROG(progression) | (sop ? B2K_CS_SOP : 0u) | (eph ? B2K_CS_EPH : 0u); }
 };
 /* what a window and a reduce make of a stream's coding (b2k_window_coding) */
 struct WindowCoding

@@ -10,7 +10,9 @@ coding the engine refuses are skipped), the 9/7 degenerate-geometry shapes, a 20
 sample transports of the one-call entry points: a b2k_encode16 / b2k_decode16 round trip, b2k_encode16_interleaved,
 b2k_encode / b2k_decode with host packing forced on, 16-bit windowed decodes (b2k_decode_window), and, where torch has
 CUDA, b2k_encode_device / b2k_decode_device with uint16 tensors.  Every one-call entry point except the windowed decode
-also stores b2k_launch_count() before and after the call.  --compare exits 1 when any array differs; tolerances would
+also stores b2k_launch_count() before and after the call.  Last come the device-resident round trips (b2k_job_roundtrip,
+_roundtrip_n, _roundtrip_pipelined_n (2, 2)): on config 2 the launch count around each and its coded size, on a tiled 9/7
+image the same and the planes left after four steps.  --compare exits 1 when any array differs; tolerances would
 hide a drift of one rounding step in the 9/7 inverse, so there are none."""
 import os
 import sys
@@ -131,6 +133,26 @@ def run(outdir):
         for reduce in (0, 1):
             _, got = eng.decode_window(cs, win, reduce, dtype=np.uint16)
             arrs.update(("win%d_r%d_rec%d" % (i, reduce, c), g.copy()) for c, g in enumerate(got))
+    # the device-resident round trips: config 2 (the first call's sizing pass included) and four 9/7 steps of a tiled image
+    for tag, cp, img in (("rt_config2", G.make_coding(8192, 8192, 3, 12, numres=6, tile=(1024, 1024)),
+                          P.synthetic_image(8192, 8192, 3, 12, seed=20260924)),
+                         ("rt_97", G.make_coding(700, 500, 3, 12, numres=5, tile=(256, 192), irreversible=True),
+                          P.synthetic_image(700, 500, 3, 12, seed=23))):
+        job = eng.job(cp)
+        try:
+            job.upload(img)
+            for name, fn in (("one", job.roundtrip), ("n", lambda: job.roundtrip_n(8 if tag == "rt_config2" else 1)),
+                             ("pipelined", lambda: job.roundtrip_pipelined_n(8 if tag == "rt_config2" else 2, 2, 2))):
+                arrs["%s_%s_coded" % (tag, name)] = np.array([counted("%s_%s" % (tag, name), fn)[-1]], np.uint64)
+                print("%s %s: %d launches" % (tag, name, np.diff(arrs["%s_%s_launches" % (tag, name)])[0]))
+            rec = [np.zeros_like(p) for p in img]
+            job.download(rec)
+            if tag == "rt_97":
+                arrs.update(("rt_97_rec%d" % c, a) for c, a in enumerate(rec))
+            else:
+                arrs["rt_config2_lossless"] = np.array([all(np.array_equal(a, b) for a, b in zip(rec, img))])
+        finally:
+            job.close()
     for k, a in arrs.items():
         np.save(os.path.join(outdir, "transport.%s.npy" % k), a)
     eng.close()
