@@ -66,7 +66,7 @@ assert BLOCK_DTYPE.itemsize == C.sizeof(Block), (BLOCK_DTYPE.itemsize, C.sizeof(
 # plugin_decompress (C++-ABI callback struct) is declared in csrc/plugin_decode_abi.h, not in the C header
 EXPORTS = ["minpf_post_load_plugin", "plugin_init", "plugin_get_debug_state", "gpup_encode_mem", "gpup_tile_free",
            "b2k_engine_create", "b2k_engine_destroy", "b2k_last_error", "b2k_host_alloc", "b2k_host_free",
-           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_decode_codestream_device", "b2k_codestream_parse_device", "b2k_codestream_parse_device_stats", "b2k_codestream_parse_window_device", "b2k_decode_codestream_window_device", "b2k_codestream_window_device_stats", "b2k_enumerate",
+           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_decode_codestream_device", "b2k_decode_codestreams_device", "b2k_decode_codestreams_error", "b2k_codestream_parse_device", "b2k_codestream_parse_device_stats", "b2k_codestream_parse_window_device", "b2k_decode_codestream_window_device", "b2k_codestream_window_device_stats", "b2k_enumerate",
            "b2k_result_to_gpup_tile", "b2k_job_create", "b2k_job_destroy", "b2k_job_upload", "b2k_job_forward",
            "b2k_job_t1_encode", "b2k_job_t1_decode", "b2k_job_t1_decode_blocks", "b2k_job_inverse", "b2k_job_roundtrip", "b2k_job_roundtrip_n", "b2k_job_roundtrip_pipelined_n", "b2k_job_download",
            "b2k_job_download_coeffs", "b2k_job_upload_coeffs", "b2k_job_fetch_result", "b2k_job_num_blocks",
@@ -809,6 +809,59 @@ class Engine:
         _check_handled(L.b2k_decode_codestream_device(self._h, ptr, n, C.byref(img), handle, C.byref(cp), C.byref(ms)),
                        "b2k_decode_codestream_device")
         return cp, out
+
+    def decode_codestreams_device(self, streams, out=None, dtype=None, layout="CHW", stream=None):
+        """A batch of HTJ2K code streams on the engine's GPU (1-D contiguous uint8 CUDA arrays), all with one coding ->
+        (Coding, out, status) in one launch chain (b2k_decode_codestreams_device).  out: None for a new torch tensor
+        (n, C, H, W) or (n, H, W, C) of `dtype` (default torch.uint16), or a CUDA array of that shape.  status[i] =
+        (rc, text) is what decode_codestream_device of stream i alone returns (0, or the code it would raise with);
+        out[i] is written only where rc is 0.  Raises only when the call fails as a whole, or when no stream has a
+        coding (with stream 0's error)."""
+        n = len(streams)
+        if n == 0:
+            raise ValueError("decode_codestreams_device: no code streams")
+        ptrs = (C.c_void_p * n)()
+        lens = (C.c_uint64 * n)()
+        for i, cs in enumerate(streams):
+            if not hasattr(cs, "__cuda_array_interface__"):
+                raise ValueError("decode_codestreams_device: stream %d is not a CUDA array" % i)
+            ptrs[i], lens[i] = self._device_codestream_bytes(cs)
+        L = lib()
+        L.b2k_decode_codestreams_device.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64),
+                                                    C.POINTER(DevicePlanes), C.c_void_p, C.POINTER(Coding),
+                                                    C.POINTER(C.c_int32), C.POINTER(C.c_double)]
+        L.b2k_decode_codestreams_error.restype = C.c_char_p
+        L.b2k_decode_codestreams_error.argtypes = [C.c_void_p, C.c_uint32]
+        handle = _stream_handle(stream, out if out is not None else streams[0])
+        cp = Coding()
+        st = (C.c_int32 * n)()
+        ms = C.c_double()
+
+        def status():
+            return [(int(st[i]), (L.b2k_decode_codestreams_error(self._h, i) or b"").decode()) for i in range(n)]
+
+        # headers only: the batch's coding, which sizes the output -- and, when `out` is given, is checked against it before
+        # anything is written: a b2k_device_planes has no extent, so an `out` of the wrong shape would otherwise be written
+        # past its end
+        rc = L.b2k_decode_codestreams_device(self._h, n, ptrs, lens, None, handle, C.byref(cp), st, C.byref(ms))
+        if rc < 0:
+            raise EngineError("b2k_decode_codestreams_device: " + (L.b2k_last_error() or b"").decode())
+        if rc == n:
+            code, text = status()[0]
+            raise (NotHandled if code == 1 else EngineError)("b2k_decode_codestreams_device: stream 0: " + text)
+        h, w, nc = cp.y1 - cp.y0, cp.x1 - cp.x0, cp.numcomps
+        shape = (n, nc, h, w) if layout == "CHW" else (n, h, w, nc)
+        if out is None:
+            import torch
+            out = torch.empty(shape, dtype=torch.uint16 if dtype is None else dtype, device="cuda:%d" % self.device)
+        iface = out.__cuda_array_interface__
+        if tuple(int(v) for v in iface["shape"]) != shape:
+            raise ValueError("decode_codestreams_device: out has shape %s, the batch needs %s" % (tuple(iface["shape"]), shape))
+        imgs = (DevicePlanes * n)(*[device_planes(out[i], nc, h, w, layout, writable=True) for i in range(n)])
+        rc = L.b2k_decode_codestreams_device(self._h, n, ptrs, lens, imgs, handle, C.byref(cp), st, C.byref(ms))
+        if rc < 0:
+            raise EngineError("b2k_decode_codestreams_device: " + (L.b2k_last_error() or b"").decode())
+        return cp, out, status()
 
     def job(self, cp, tile_mod=1, tile_rem=0):
         return Job(self, cp, tile_mod, tile_rem)

@@ -100,9 +100,11 @@ void b2k_launch_ht_decode(const HtBlockDesc* d_blocks, const uint8_t* d_bytes, u
                           uint32_t nblocks, uint32_t max_w, int* d_err, int irreversible, int any_refinement, cudaStream_t st);
 void b2k_launch_ht_decode_vlc(const HtBlockDesc* d_blocks, const uint8_t* d_bytes, uint32_t* d_recs, HtBlockOut* d_status,
                               uint32_t nblocks, uint32_t max_w, cudaStream_t st);
+/* rejected blocks are counted in d_err[(first_block + b) / blocks_per_slot] for block b of the launch (blocks_per_slot 0:
+   all in d_err[0]); a batch's launch over its coded blocks from first_block on counts them per image */
 void b2k_launch_ht_decode_magsgn(const HtBlockDesc* d_blocks, const uint8_t* d_bytes, const uint32_t* d_recs,
                                  const HtBlockOut* d_status, uint32_t nblocks, uint32_t max_w, int* d_err, int irreversible,
-                                 int any_refinement, cudaStream_t st);
+                                 int any_refinement, cudaStream_t st, uint32_t first_block = 0, uint32_t blocks_per_slot = 0);
 void b2k_launch_build_dec_desc(const HtBlockDesc* d_enc, const HtBlockOut* d_out, const uint64_t* d_offsets,
                                const float* d_dec_quant, HtBlockDesc* d_dec, uint32_t n, uint64_t cap, cudaStream_t st);
 /* sample containers (sample_bytes 1, 2 or 4) <-> int32 planes.  Component c of pixel (x, y) of the container is at
@@ -111,6 +113,19 @@ void b2k_launch_container_to_planes(const void* src, uint32_t spitch, uint32_t s
                                     uint32_t dpitch, uint32_t w, uint32_t h, int sgnd, cudaStream_t st);
 void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t spitch, void* dst, uint32_t dpitch, uint32_t step,
                                     uint32_t sample_bytes, uint32_t w, uint32_t h, cudaStream_t st);
+/* a batch's images out, one launch: for each of the n entries of the device table d_dst (BatchDst), its nc components
+   (nc > 1: pixel-interleaved, step = nc) from the int32 planes src[c] to dst + y * dpitch + x * step + c samples, w x h
+   pixels.  Entries with dst NULL, or whose *err (the HT decoder's rejections in that image) is not 0, are skipped.  All
+   share sample_bytes. */
+struct BatchDst
+{
+  const int32_t* src[4];
+  void* dst;
+  const int* err;
+  uint32_t dpitch, step;
+};
+void b2k_launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint32_t spitch, uint32_t sample_bytes, uint32_t w,
+                                     uint32_t h, cudaStream_t st);
 void b2k_count_launch(void);
 
 /* host_pack.cpp: container conversion on a small host thread pool (int32 planes <-> pinned 16-bit staging) */

@@ -1065,6 +1065,20 @@ struct Cursor
    SOT starts.  0, or b2k_codestream_parse's return code and text for a main header it declines; h.short_read says the
    failure came from reaching `len`, so that a longer prefix of the same stream may parse (b2k_codestream_parse_device
    reads the header from a prefix). */
+int b2k_batch_coding_check(const t2::MainHeader& ref, uint32_t ref_index, const t2::MainHeader& h, uint32_t index)
+{
+  std::string why;
+  if(memcmp(&h.cp, &ref.cp, sizeof(b2k_coding)) != 0)
+    why = "its coding differs from that of code stream ";
+  else if(h.flags() != ref.flags())
+    why = "its progression order, SOP or EPH differ from those of code stream ";
+  if(why.empty())
+    return 0;
+  b2k_set_error(("code stream " + std::to_string(index) + ": " + why + std::to_string(ref_index) + ", which the batch takes its coding from")
+                    .c_str());
+  return 1;
+}
+
 int b2k_parse_main_header(const uint8_t* cs, uint64_t len, t2::MainHeader& h)
 {
   h = t2::MainHeader();

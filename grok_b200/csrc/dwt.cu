@@ -1863,17 +1863,15 @@ __global__ void __launch_bounds__(128) k_container_to_planes(const void* __restr
   }
 }
 
-/* NC int32 planes -> container (b2k_decode16 before the download, b2k_decode_device) */
-template <int S, int NC>
-__global__ void __launch_bounds__(128) k_planes_to_container(CPtr4 src, uint32_t spitch, void* __restrict__ dst, uint32_t dpitch,
-                                                             uint32_t step, uint32_t w, uint32_t h)
+/* NC int32 planes -> container, the rows blockIdx.y + k gridDim.y of the 8 pixels at x8 (b2k_decode16 before the download,
+   b2k_decode_device, and each image of a batch) */
+template <int S, int NC, class Src>
+__device__ __forceinline__ void planes_to_container_rows(const Src& src, uint32_t spitch, void* __restrict__ dst, uint32_t dpitch,
+                                                         uint32_t step, uint32_t w, uint32_t h, uint32_t x8)
 {
   typedef typename Sample<S>::U U;
   constexpr int BYTES = 8 * NC * S, V = BYTES % 16 == 0 ? 16 : 8;
   constexpr uint32_t MASK = S == 4 ? 0xFFFFFFFFu : (1u << (8 * S)) - 1;
-  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
-  if(x8 >= w)
-    return;
   for(uint32_t y = blockIdx.y; y < h; y += gridDim.y)
   {
     const size_t soff = (size_t)y * spitch + x8;
@@ -1881,7 +1879,7 @@ __global__ void __launch_bounds__(128) k_planes_to_container(CPtr4 src, uint32_t
     bool vec = x8 + 8 <= w && step == NC && (reinterpret_cast<uintptr_t>(d) & (V - 1)) == 0;
 #pragma unroll
     for(int c = 0; c < NC; ++c)
-      vec = vec && (reinterpret_cast<uintptr_t>(src.p[c] + soff) & 15) == 0;
+      vec = vec && (reinterpret_cast<uintptr_t>(src(c) + soff) & 15) == 0;
     if(vec)
     {
       uint32_t wd[BYTES / 4];
@@ -1891,7 +1889,7 @@ __global__ void __launch_bounds__(128) k_planes_to_container(CPtr4 src, uint32_t
 #pragma unroll
       for(int c = 0; c < NC; ++c)
       {
-        const int4 a = __ldg(reinterpret_cast<const int4*>(src.p[c] + soff)), b = __ldg(reinterpret_cast<const int4*>(src.p[c] + soff) + 1);
+        const int4 a = __ldg(reinterpret_cast<const int4*>(src(c) + soff)), b = __ldg(reinterpret_cast<const int4*>(src(c) + soff) + 1);
         const int v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 #pragma unroll
         for(int i = 0; i < 8; ++i)
@@ -1909,9 +1907,33 @@ __global__ void __launch_bounds__(128) k_planes_to_container(CPtr4 src, uint32_t
       for(uint32_t i = 0; i < n; ++i)
 #pragma unroll
         for(int c = 0; c < NC; ++c)
-          d[(size_t)i * step + c] = (U)src.p[c][soff + i];
+          d[(size_t)i * step + c] = (U)src(c)[soff + i];
     }
   }
+}
+
+template <int S, int NC>
+__global__ void __launch_bounds__(128) k_planes_to_container(CPtr4 src, uint32_t spitch, void* __restrict__ dst, uint32_t dpitch,
+                                                             uint32_t step, uint32_t w, uint32_t h)
+{
+  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  if(x8 >= w)
+    return;
+  planes_to_container_rows<S, NC>([&](int c) { return src.p[c]; }, spitch, dst, dpitch, step, w, h, x8);
+}
+
+/* the images of a batch: image blockIdx.z from its table entry; an entry without a destination, or of an image the HT
+   decoder rejected blocks of (the counter its slot's blocks were decoded into, earlier on the stream), is skipped */
+template <int S, int NC>
+__global__ void __launch_bounds__(128) k_planes_to_containers(const BatchDst* __restrict__ tab, uint32_t spitch, uint32_t w, uint32_t h)
+{
+  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  const BatchDst* E = tab + blockIdx.z;
+  void* dst = E->dst;
+  if(x8 >= w || !dst || *E->err)
+    return;
+  /* the plane pointers are read from the table where they are used */
+  planes_to_container_rows<S, NC>([E](int c) { return E->src[c]; }, spitch, dst, E->dpitch, E->step, w, h, x8);
 }
 
 dim3 convert_grid(uint32_t w, uint32_t h) { return dim3((w + 8 * 128 - 1) / (8 * 128), h < 65535u ? h : 65535u); }
@@ -1976,6 +1998,44 @@ void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t 
     default: launch_planes_to_container<4>(P, nc, spitch, dst, dpitch, step, w, h, st); break;
   }
   b2k_count_launch();
+}
+
+namespace
+{
+template <int S>
+void launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint32_t spitch, uint32_t w, uint32_t h, cudaStream_t st)
+{
+  dim3 grid = convert_grid(w, h);
+  /* the rows of every image: enough CTAs for the GPU without a grid of 65535 x 65535 */
+  grid.y = std::min<uint32_t>(grid.y, std::max<uint32_t>(1u, 16384u / std::max(1u, n)));
+  grid.y = std::min<uint32_t>(std::max<uint32_t>(grid.y, 8u), std::max(1u, h));
+  const dim3 block(128);
+  for(uint32_t i0 = 0; i0 < n; i0 += 65535u) /* one launch below 65536 images */
+  {
+    grid.z = std::min<uint32_t>(n - i0, 65535u);
+    switch(nc)
+    {
+      case 1: k_planes_to_containers<S, 1><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
+      case 2: k_planes_to_containers<S, 2><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
+      case 3: k_planes_to_containers<S, 3><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
+      default: k_planes_to_containers<S, 4><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
+    }
+    b2k_count_launch();
+  }
+}
+} // namespace
+
+void b2k_launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint32_t spitch, uint32_t sample_bytes, uint32_t w,
+                                     uint32_t h, cudaStream_t st)
+{
+  if(!n || !w || !h)
+    return;
+  switch(sample_bytes)
+  {
+    case 1: launch_planes_to_containers<1>(d_dst, n, nc, spitch, w, h, st); break;
+    case 2: launch_planes_to_containers<2>(d_dst, n, nc, spitch, w, h, st); break;
+    default: launch_planes_to_containers<4>(d_dst, n, nc, spitch, w, h, st); break;
+  }
 }
 
 /* one launch of a DWT kernel whose warps stage through WarpPipe<Stage>; the shared-memory limit it needs is raised once

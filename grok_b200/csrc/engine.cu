@@ -72,6 +72,17 @@ struct b2k_engine
   bool have_window_stats = false;
   uint32_t window_tiles = 0;
   uint64_t window_bytes = 0;
+  /* b2k_decode_codestreams_device: the batch job (beside `cached`, so that single and batch calls alternate without
+     replanning), each stream's text of the last call, and the gather tables and header staging of a call */
+  b2k_device_job* batch = nullptr;
+  bool last_parse_batch = false;   /* b2k_codestream_parse_device_stats reports the batch's totals */
+  std::vector<std::string> batch_errors;
+  CopyEntry* d_copy = nullptr;
+  CopyEntry* h_copy = nullptr;     /* pinned */
+  uint32_t copy_cap = 0;
+  uint8_t* d_hdr = nullptr;        /* the header prefixes, end to end */
+  uint8_t* h_hdr = nullptr;        /* pinned */
+  uint64_t hdr_cap = 0;
 };
 
 /* ---- device memory cache --------------------------------------------------------------------------------------
@@ -337,6 +348,13 @@ struct b2k_device_job
   TileGrid grid{};
   std::vector<uint32_t> tiles;
   std::vector<Rect> tile_rects;
+  /* a batch job (b2k_decode_codestreams_device) holds `slots` images of one coding: slot s of component c is plane
+     s * numcomps + c of img, coef and ll[], and the selected tiles are slot 0's tiles, then slot 1's, ...  slot_tiles per
+     slot; tile_slot[ti] is selected tile ti's slot.  A single image is one slot. */
+  uint32_t slots = 1, slot_tiles = 0;
+  std::vector<uint32_t> tile_slot;
+  BatchDst* d_batch_dst = nullptr; /* the conversion's table: per component (or one for interleaved images), per slot */
+  BatchDst* h_batch_dst = nullptr; /* pinned */
   std::vector<BandQuant> quant;
   std::vector<b2k_block> blocks;       /* every block, enumeration order */
   std::vector<uint32_t> coded_index;   /* blocks with area, index into `blocks` */
@@ -438,6 +456,15 @@ extern "C" void b2k_engine_destroy(b2k_engine* e)
     b2k_job_destroy(e->cached);
     e->cached = nullptr;
   }
+  if(e->batch)
+  {
+    b2k_job_destroy(e->batch);
+    e->batch = nullptr;
+  }
+  cudaFree(e->d_copy);
+  cudaFreeHost(e->h_copy);
+  cudaFree(e->d_hdr);
+  cudaFreeHost(e->h_hdr);
   if(e->stream)
     cudaStreamDestroy(e->stream);
   if(e->copy_stream)
@@ -550,6 +577,7 @@ static int build_dwt_plan(b2k_device_job* J)
         const Rect tc = J->tile_rects[ti];
         if(tc.empty())
           continue;
+        const int sc = (int)J->tile_slot[ti] * ncomp; /* the slot's first plane */
         for(int c = 0; c < ncomp;)
         {
           const bool group = cp.mct && c == 0;
@@ -561,9 +589,9 @@ static int build_dwt_plan(b2k_device_job* J)
           d.comp0 = (uint8_t)c;
           for(int k = 0; k < nc; ++k)
           {
-            d.in[k] = J->img.at(c + k, tc.x0, tc.y0);
+            d.in[k] = J->img.at(sc + c + k, tc.x0, tc.y0);
             d.in_pitch = J->img.pitch;
-            d.out_c[k] = J->coef.at(c + k, tc.x0, tc.y0);
+            d.out_c[k] = J->coef.at(sc + c + k, tc.x0, tc.y0);
             d.out_ll[k] = d.out_c[k];
             d.c_pitch = d.ll_pitch = J->coef.pitch;
             d.shift[k] = dc;
@@ -608,6 +636,7 @@ static int build_dwt_plan(b2k_device_job* J)
         const Rect r = resolution_rect(tc, cp.numres, resno);
         if(r.empty())
           continue;
+        const int sc = (int)J->tile_slot[ti] * ncomp; /* the slot's first plane */
         for(int c = 0; c < ncomp;)
         {
           const bool group = (lvl == 1 && cp.mct && c == 0);
@@ -619,7 +648,7 @@ static int build_dwt_plan(b2k_device_job* J)
           const uint32_t llx = (r.x0 + 1) >> 1, lly = (r.y0 + 1) >> 1;
           for(int k = 0; k < nc; ++k)
           {
-            const int cc = c + k;
+            const int cc = sc + c + k;
             /* finer side: image at level 1, else LL scratch written by level lvl-1 */
             const Planes& fine = (lvl == 1) ? J->img : J->ll[(lvl - 1) & 1];
             d.in[k] = fine.at(cc, r.x0, r.y0);
@@ -701,27 +730,30 @@ static int build_block_plan(b2k_device_job* J)
 {
   const b2k_coding& cp = J->cp;
   J->blocks.clear();
-  for(size_t ti = 0; ti < J->tiles.size(); ++ti)
+  /* the enumeration is one slot's: every slot has the same blocks, and coded block k of slot s is descriptor
+     s * coded_index.size() + k */
+  for(size_t ti = 0; ti < J->slot_tiles; ++ti)
     enumerate_tile_blocks(cp, J->tiles[ti], J->tile_rects[ti], J->quant, J->blocks);
   /* map tile index -> rect */
   std::vector<Rect> rect_of(J->grid.nx * J->grid.ny);
-  for(size_t ti = 0; ti < J->tiles.size(); ++ti)
+  for(size_t ti = 0; ti < J->slot_tiles; ++ti)
     rect_of[J->tiles[ti]] = J->tile_rects[ti];
   uint64_t off = 0;
   std::vector<uint32_t> sel_of(J->grid.nx * J->grid.ny, 0);
-  for(size_t ti = 0; ti < J->tiles.size(); ++ti)
+  for(size_t ti = 0; ti < J->slot_tiles; ++ti)
     sel_of[J->tiles[ti]] = (uint32_t)ti;
   J->coded_first.assign(J->tiles.size() + 1, 0);
+  for(uint32_t s = 0; s < J->slots; ++s)
   for(uint32_t i = 0; i < J->blocks.size(); ++i)
   {
     const b2k_block& b = J->blocks[i];
     if(b.x1 <= b.x0 || b.y1 <= b.y0)
       continue;
-    J->coded_first[sel_of[b.tile] + 1] = (uint32_t)J->h_enc_desc.size() + 1;
+    J->coded_first[s * J->slot_tiles + sel_of[b.tile] + 1] = (uint32_t)J->h_enc_desc.size() + 1;
     const Rect& tr = rect_of[b.tile];
     const BandQuant& bq = J->quant[band_quant_index(b.resno, b.orient)];
     HtBlockDesc d{};
-    d.coef = J->coef.at(b.comp, tr.x0 + b.buf_x, tr.y0 + b.buf_y);
+    d.coef = J->coef.at((int)(s * cp.numcomps) + b.comp, tr.x0 + b.buf_x, tr.y0 + b.buf_y);
     d.pitch = J->coef.pitch;
     d.w = (uint16_t)(b.x1 - b.x0);
     d.h = (uint16_t)(b.y1 - b.y0);
@@ -748,9 +780,18 @@ static int build_block_plan(b2k_device_job* J)
     J->enc_limits.max_kmax = std::max<uint32_t>(J->enc_limits.max_kmax, d.kmax);
     J->h_enc_desc.push_back(d);
     J->dec_quant.push_back(bq.step_dec / (float)(1u << (31 - bq.kmax)));
-    J->coded_index.push_back(i);
+    if(s == 0)
+      J->coded_index.push_back(i);
   }
   J->scratch_bytes = off;
+  /* descriptor indices, coded_first and the per-quad record offsets (rec_off) are 32-bit: a batch job of too many slots
+     is refused rather than left to wrap */
+  if(J->h_enc_desc.size() >= UINT32_MAX || J->total_quads + 32 * J->group_quads + 64 > UINT32_MAX)
+  {
+    g_err = "too many code blocks for one job (" + std::to_string(J->h_enc_desc.size()) + " blocks, " +
+            std::to_string(J->total_quads + 32 * J->group_quads) + " quad records; at most 2^32 - 1 of each)";
+    return -1;
+  }
   for(size_t ti = 1; ti <= J->tiles.size(); ++ti) /* tiles without coded blocks inherit the running count */
     J->coded_first[ti] = std::max(J->coded_first[ti], J->coded_first[ti - 1]);
   {
@@ -781,15 +822,23 @@ static int build_block_plan(b2k_device_job* J)
     CUDA_TRY(cudaHostAlloc(&J->h_dec_desc, n * sizeof(HtBlockDesc), cudaHostAllocDefault));
     CUDA_TRY(cudaHostAlloc(&J->h_offsets, (n + 1) * sizeof(uint64_t), cudaHostAllocDefault));
   }
-  CUDA_TRY(cudaMalloc(&J->d_err, sizeof(int)));
-  CUDA_TRY(cudaMemset(J->d_err, 0, sizeof(int)));
+  CUDA_TRY(cudaMalloc(&J->d_err, J->slots * sizeof(int)));
+  CUDA_TRY(cudaMemset(J->d_err, 0, J->slots * sizeof(int)));
   return 0;
 }
+
+static int job_create(b2k_engine* e, const b2k_coding* cp, uint32_t tile_mod, uint32_t tile_rem, uint32_t slots, b2k_device_job** out);
 
 extern "C" int32_t b2k_job_create(b2k_engine* e, const b2k_coding* cp, uint32_t tile_mod, uint32_t tile_rem,
                                   b2k_device_job** out)
 {
-  if(!e || !cp || !out || tile_mod == 0)
+  return job_create(e, cp, tile_mod, tile_rem, 1, out);
+}
+
+/* b2k_job_create with `slots` images of the coding (a batch job) */
+static int job_create(b2k_engine* e, const b2k_coding* cp, uint32_t tile_mod, uint32_t tile_rem, uint32_t slots, b2k_device_job** out)
+{
+  if(!e || !cp || !out || tile_mod == 0 || slots == 0)
     return -1;
   *out = nullptr;
   if(const char* why = unsupported_reason(*cp))
@@ -805,16 +854,20 @@ extern "C" int32_t b2k_job_create(b2k_engine* e, const b2k_coding* cp, uint32_t 
   J->tile_rem = tile_rem;
   J->grid = tile_grid(*cp);
   J->quant = band_quant(*cp);
-  for(uint32_t t = 0; t < J->grid.nx * J->grid.ny; ++t)
-    if(t % tile_mod == tile_rem)
-    {
-      const Rect r = tile_rect(*cp, J->grid, t);
-      if(r.empty())
-        continue;
-      J->tiles.push_back(t);
-      J->tile_rects.push_back(r);
-    }
-  const int nc = cp->numcomps;
+  J->slots = slots;
+  for(uint32_t s = 0; s < slots; ++s)
+    for(uint32_t t = 0; t < J->grid.nx * J->grid.ny; ++t)
+      if(t % tile_mod == tile_rem)
+      {
+        const Rect r = tile_rect(*cp, J->grid, t);
+        if(r.empty())
+          continue;
+        J->tiles.push_back(t);
+        J->tile_rects.push_back(r);
+        J->tile_slot.push_back(s);
+      }
+  J->slot_tiles = (uint32_t)(J->tiles.size() / slots);
+  const int nc = cp->numcomps * (int)slots;
   if(alloc_planes(J->img, nc, cp->x0, cp->y0, cp->x1, cp->y1) || alloc_planes(J->coef, nc, cp->x0, cp->y0, cp->x1, cp->y1))
   {
     b2k_job_destroy(J);
@@ -867,6 +920,8 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
   cudaFree(J->d_dec_status);
   cudaFree(J->d_bytes);
   cudaFree(J->d_err);
+  cudaFree(J->d_batch_dst);
+  cudaFreeHost(J->h_batch_dst);
   cudaFreeHost(J->h_out);
   cudaFreeHost(J->h_dec_desc);
   cudaFreeHost(J->h_offsets);
@@ -2415,9 +2470,12 @@ extern "C" int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const 
 /* the block decoder over chunk k's coded blocks, from the descriptors in d_dec_desc and the bytes in d_bytes: phase A
    (serial VLC/MEL parse, one thread per block) is latency-bound and leaves the SMs nearly empty, so the chunks' parses run
    concurrently on side streams once `ready` (this chunk's descriptors + bytes are on the device) has happened, ahead of st */
-static int enqueue_block_decode(b2k_engine* e, b2k_device_job* J, size_t k, cudaEvent_t ready, cudaStream_t st)
+static int enqueue_block_decode(b2k_engine* e, b2k_device_job* J, size_t k, cudaEvent_t ready, cudaStream_t st,
+                                size_t t0 = (size_t)-1, size_t t1 = (size_t)-1)
 {
-  const uint32_t b0 = J->coded_first[J->chunk_tile[k]], b1 = J->coded_first[J->chunk_tile[k + 1]];
+  /* chunk k's tiles, or selected tiles [t0, t1) (a batch's chunk k over the slots it uses) */
+  const uint32_t b0 = J->coded_first[t0 == (size_t)-1 ? J->chunk_tile[k] : t0];
+  const uint32_t b1 = J->coded_first[t1 == (size_t)-1 ? J->chunk_tile[k + 1] : t1];
   if(b1 <= b0)
     return 0;
   cudaStream_t ax = e->aux[k & 3];
@@ -2426,8 +2484,9 @@ static int enqueue_block_decode(b2k_engine* e, b2k_device_job* J, size_t k, cuda
   b2k_launch_ht_decode_vlc(J->d_dec_desc + b0, J->d_bytes, J->d_recs, J->d_dec_status + b0, b1 - b0, J->max_cblk_w, ax);
   CUDA_TRY(cudaEventRecord(J->chunk_ev[CEV(2, k)], ax));
   CUDA_TRY(cudaStreamWaitEvent(st, J->chunk_ev[CEV(2, k)], 0));
+  /* a batch counts the blocks the HT decoder rejects per slot */
   b2k_launch_ht_decode_magsgn(J->d_dec_desc + b0, J->d_bytes, J->d_recs, J->d_dec_status + b0, b1 - b0, J->max_cblk_w, J->d_err,
-                              J->cp.irreversible, J->dec_has_refinement, st);
+                              J->cp.irreversible, J->dec_has_refinement, st, b0, J->slots > 1 ? (uint32_t)J->coded_index.size() : 0);
   if(J->dec_has_refinement)
     b2k_launch_ht_decode_refine(J->d_dec_desc + b0, J->d_bytes, J->d_dec_status + b0, b1 - b0, (J->cp.cblk_sty & 0x08) != 0, st);
   return 0;
@@ -2627,6 +2686,7 @@ static int parse_device_codestream(b2k_engine* e, const uint8_t* cs, uint64_t le
   if(arena_reserve(J, len, 0)) return -1;
   J->arena_sized = false; /* the arena now holds a caller's stream, not this job's coding of its image */
   J->last_parse_window = false;
+  e->last_parse_batch = false;
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   CUDA_TRY(cudaMemcpyAsync(J->d_bytes, cs, len, cudaMemcpyDeviceToDevice, st));
   if(b2k_t2_parse_enqueue(J->t2p, J->d_bytes, len, h.sot, J->d_enc_desc, J->d_dec_quant, dec ? J->d_dec_desc : nullptr, st))
@@ -2779,6 +2839,7 @@ static int parse_device_window(b2k_engine* e, const uint8_t* cs, uint64_t len, c
   }
   J->last_parse_window = true;
   J->arena_sized = false;
+  e->last_parse_batch = false;
   const TileGrid g = tile_grid(w.h.cp);
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   if(b2k_t2_window_enqueue(J->t2w, cs, len, w.h.sot, g.nx, g.nx * g.ny, w.wc, J->d_enc_desc, J->d_dec_quant, dec ? J->d_dec_desc : nullptr,
@@ -2902,6 +2963,8 @@ extern "C" int32_t b2k_codestream_parse_device_stats(b2k_engine* e, uint32_t* ti
     return -1;
   std::lock_guard<std::mutex> lock(e->mu);
   T2Parse* last = e->cached ? (e->cached->last_parse_window ? e->cached->t2w : e->cached->t2p) : nullptr;
+  if(e->last_parse_batch)
+    last = e->batch ? e->batch->t2p : nullptr;
   if(!last)
   {
     g_err = "no code stream has been parsed on the device";
@@ -2909,4 +2972,299 @@ extern "C" int32_t b2k_codestream_parse_device_stats(b2k_engine* e, uint32_t* ti
   }
   b2k_t2_parse_stats(last, tiles_indexed, tiles_walked);
   return 0;
+}
+
+/* ---- batches of code streams in device memory (b2k_decode_codestreams_device) --------------------------------------
+ * n streams of one coding go through one launch chain: the batch job holds n images as slots of its planes and
+ * descriptors, the parse kernels run over (stream, item), one gather lays the streams out in the arena and one conversion
+ * launch per chunk and component group writes the images.  Each stream keeps the single call's checks, in its order, and
+ * its verdict; a stream that fails is parsed no further, decodes as all-zero blocks in its own slot and is not written
+ * out, so it cannot change another stream's pixels or verdict.  Synchronisations: the header prefixes (one more round for
+ * the streams whose header runs past its prefix, all together), the parse statuses, the end. */
+static int grow_copy_table(b2k_engine* e, uint32_t n)
+{
+  if(n <= e->copy_cap)
+    return 0;
+  cudaFree(e->d_copy);
+  cudaFreeHost(e->h_copy);
+  e->d_copy = nullptr;
+  e->h_copy = nullptr;
+  e->copy_cap = 0;
+  CUDA_TRY(cudaMalloc(&e->d_copy, n * sizeof(CopyEntry)));
+  CUDA_TRY(cudaHostAlloc(&e->h_copy, n * sizeof(CopyEntry), cudaHostAllocDefault));
+  e->copy_cap = n;
+  return 0;
+}
+
+/* h_copy[0, m) -> the device, then one gather launch into out, on st */
+static int gather_streams(b2k_engine* e, uint32_t m, uint64_t max_len, uint8_t* out, cudaStream_t st)
+{
+  if(!m)
+    return 0;
+  CUDA_TRY(cudaMemcpyAsync(e->d_copy, e->h_copy, m * sizeof(CopyEntry), cudaMemcpyHostToDevice, st));
+  return b2k_copy_table(e->d_copy, m, max_len, out, st);
+}
+
+/* the main headers of the streams whose status is 0, read on st by b2k_parse_main_header from prefixes of a few KiB
+   gathered into one copy; the streams whose header runs past its prefix go round again together with twice the prefix.
+   A stream whose header fails gets its status and text.  0, or -1 for a failure of the call. */
+static int read_batch_headers(b2k_engine* e, uint32_t n, const uint8_t* const* cs, const uint64_t* len, cudaStream_t st,
+                              int32_t* status, std::vector<b2k::t2::MainHeader>& h)
+{
+  std::vector<uint64_t> want(n, 0);
+  for(uint32_t i = 0; i < n; ++i)
+    want[i] = status[i] ? 0 : std::min<uint64_t>(len[i], b2k::t2::BATCH_HEADER_PREFIX);
+  for(;;)
+  {
+    uint32_t m = 0;
+    uint64_t total = 0, longest = 0;
+    if(grow_copy_table(e, n)) return -1;
+    for(uint32_t i = 0; i < n; ++i)
+      if(want[i])
+      {
+        e->h_copy[m++] = CopyEntry{cs[i], want[i], total};
+        total += want[i];
+        longest = std::max(longest, want[i]);
+      }
+    if(!m)
+      return 0;
+    if(total > e->hdr_cap)
+    {
+      cudaFree(e->d_hdr);
+      cudaFreeHost(e->h_hdr);
+      e->d_hdr = nullptr;
+      e->h_hdr = nullptr;
+      e->hdr_cap = 0;
+      CUDA_TRY(cudaMalloc(&e->d_hdr, total));
+      CUDA_TRY(cudaHostAlloc(&e->h_hdr, total, cudaHostAllocDefault));
+      e->hdr_cap = total;
+    }
+    if(gather_streams(e, m, longest, e->d_hdr, st)) return -1;
+    CUDA_TRY(cudaMemcpyAsync(e->h_hdr, e->d_hdr, total, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    uint64_t at = 0;
+    for(uint32_t i = 0; i < n; ++i)
+    {
+      if(!want[i])
+        continue;
+      const uint64_t got = want[i];
+      const int rc = b2k_parse_main_header(e->h_hdr + at, got, h[i]);
+      at += got;
+      want[i] = 0;
+      if(rc && h[i].short_read && got < len[i])
+        want[i] = std::min<uint64_t>(len[i], 2 * got);
+      else if(rc)
+      {
+        status[i] = rc;
+        e->batch_errors[i] = g_err;
+      }
+    }
+  }
+}
+
+/* the batch job of coding cp for n streams: the cached one when its coding matches and it has n slots or more, but not
+   more than 4 n (its planes take memory in proportion to its slots: a large batch's job is not kept for small ones) */
+static b2k_device_job* cached_batch_job(b2k_engine* e, const b2k_coding& cp, uint32_t n, int* rc)
+{
+  b2k_device_job*& J = e->batch;
+  if(J && (memcmp(&J->cp, &cp, sizeof(b2k_coding)) != 0 || J->slots < n || J->slots > 4ull * n))
+  {
+    b2k_job_destroy(J);
+    J = nullptr;
+  }
+  *rc = J ? 0 : job_create(e, &cp, 1, 0, n, &J);
+  return J;
+}
+
+extern "C" int32_t b2k_decode_codestreams_device(b2k_engine* e, uint32_t n, const uint8_t* const* cs, const uint64_t* len,
+                                                 const b2k_device_planes* imgs, void* cuda_stream, b2k_coding* cp_out, int32_t* status,
+                                                 double* ms_total)
+{
+  if(!e || !cs || !len || !cp_out || !status)
+  {
+    g_err = "b2k_decode_codestreams_device: NULL argument";
+    return -1;
+  }
+  if(n == 0)
+  {
+    g_err = "b2k_decode_codestreams_device: no code streams";
+    return -1;
+  }
+  if(imgs)
+    for(uint32_t i = 1; i < n; ++i)
+      if(imgs[i].sample_bytes != imgs[0].sample_bytes)
+      {
+        g_err = "b2k_decode_codestreams_device: the images' sample_bytes differ";
+        return -1;
+      }
+  std::lock_guard<std::mutex> lock(e->mu);
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t caller = caller_stream(cuda_stream), st = e->stream;
+  e->batch_errors.assign(n, std::string());
+  auto fail = [&](uint32_t i, int32_t rc) {
+    status[i] = rc;
+    e->batch_errors[i] = g_err;
+  };
+  auto failures = [&] {
+    int32_t f = 0;
+    for(uint32_t i = 0; i < n; ++i)
+      f += status[i] != 0;
+    return f;
+  };
+  /* each stream's checks in the single call's order: its memory, its main header, the batch's coding */
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    status[i] = 0;
+    if(check_device_bytes(e, cs[i], len[i]))
+      fail(i, -1);
+  }
+  /* what the caller queued before the call (the kernels, receives or reads that produced the streams) comes first */
+  if(queue_after(e, caller, st)) return -1;
+  std::vector<b2k::t2::MainHeader> h(n);
+  if(read_batch_headers(e, n, cs, len, st, status, h)) return -1;
+  uint32_t ref = n;
+  for(uint32_t i = 0; i < n && ref == n; ++i)
+    if(!status[i])
+      ref = i;
+  if(ref == n)
+    return failures();
+  const b2k_coding cp = h[ref].cp;
+  const uint32_t flags = h[ref].flags();
+  *cp_out = cp;
+  for(uint32_t i = ref + 1; i < n; ++i)
+    if(!status[i] && b2k_batch_coding_check(h[ref], ref, h[i], i))
+      fail(i, 1);
+  if(!imgs)
+    return failures();
+  /* the job of the batch's coding; a coding the engine declines is every such stream's verdict, as in the single call */
+  int jrc = 0;
+  b2k_device_job* J = cached_batch_job(e, cp, n, &jrc);
+  if(jrc < 0)
+    return -1;
+  if(jrc)
+  {
+    for(uint32_t i = 0; i < n; ++i)
+      if(!status[i])
+        fail(i, jrc);
+    return failures();
+  }
+  if(!J->t2p || b2k_t2_parse_flags(J->t2p) != flags || b2k_t2_parse_streams(J->t2p) != J->slots)
+  { /* geometry and progression only: planned once for every batch of this coding */
+    b2k_t2_parse_destroy(J->t2p);
+    J->t2p = nullptr;
+    if(b2k_t2_parse_create(cp, flags, J->blocks.data(), J->blocks.size(), J->slot_tiles, J->coded_index.data(), J->coded_index.size(),
+                           &J->t2p, J->slots))
+      return -1;
+  }
+  /* the arena: stream i at a 256-byte boundary, the decoder's read-past slack after the last one; one gather launch */
+  std::vector<uint64_t> at(n, 0), plen(n, 0), sot(n, 0);
+  uint64_t total = 0, longest = 0;
+  uint32_t m = 0;
+  if(grow_copy_table(e, n)) return -1;
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    if(status[i])
+      continue;
+    at[i] = total;
+    plen[i] = len[i];
+    sot[i] = h[i].sot;
+    e->h_copy[m++] = CopyEntry{cs[i], len[i], total};
+    longest = std::max(longest, len[i]);
+    total = b2k::t2::batch_arena_next(total, len[i]);
+  }
+  if(arena_reserve(J, total, total / 8)) return -1;
+  J->arena_sized = false;
+  e->last_parse_batch = true;
+  CUDA_TRY(cudaEventRecord(J->ev[0], st));
+  if(gather_streams(e, m, longest, J->d_bytes, st)) return -1;
+  if(b2k_t2_batch_enqueue(J->t2p, J->d_bytes, n, at.data(), plen.data(), sot.data(), J->d_enc_desc, J->d_dec_quant, J->d_dec_desc, st))
+    return -1;
+  CUDA_TRY(cudaStreamSynchronize(st));
+  bool refinement = false;
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    if(status[i])
+      continue;
+    bool r = false;
+    if(int prc = b2k_t2_batch_result(J->t2p, i, &r))
+      fail(i, prc);
+    refinement = refinement || r;
+  }
+  /* the image descriptors; a stream whose image is unusable is decoded (its slot is its own) but not written out */
+  for(uint32_t i = 0; i < n; ++i)
+    if(!status[i])
+      if(int rc = check_device_planes(e, &cp, &imgs[i]))
+        fail(i, rc);
+  /* the conversion's tables: one per component, or one for all when every image written is pixel-interleaved */
+  const int nc = cp.numcomps;
+  bool interleaved = nc > 1;
+  for(uint32_t i = 0; i < n; ++i)
+    if(!status[i])
+      interleaved = interleaved && device_group(imgs[i], nc) == nc;
+  const int group = interleaved ? nc : 1, tables = nc / group;
+  if(!J->h_batch_dst)
+  {
+    CUDA_TRY(cudaMalloc(&J->d_batch_dst, (size_t)J->slots * 4 * sizeof(BatchDst)));
+    CUDA_TRY(cudaHostAlloc(&J->h_batch_dst, (size_t)J->slots * 4 * sizeof(BatchDst), cudaHostAllocDefault));
+  }
+  for(int t = 0; t < tables; ++t)
+    for(uint32_t i = 0; i < n; ++i)
+    {
+      BatchDst& D = J->h_batch_dst[(size_t)t * n + i];
+      D = BatchDst{};
+      if(status[i])
+        continue;
+      const int c0 = t * group;
+      for(int k = 0; k < group; ++k)
+        D.src[k] = J->img.at((int)i * nc + c0 + k, cp.x0, cp.y0);
+      D.dst = imgs[i].comp[c0];
+      D.err = J->d_err + i; /* an image the HT decoder rejected blocks of is not written */
+      D.dpitch = imgs[i].row_pitch[c0];
+      D.step = imgs[i].col_step[c0];
+    }
+  CUDA_TRY(cudaMemcpyAsync(J->d_batch_dst, J->h_batch_dst, (size_t)tables * n * sizeof(BatchDst), cudaMemcpyHostToDevice, st));
+  /* block decode -> inverse -> images, chunk by chunk over the (slot, tile) ranges of the n slots used (as many chunks as
+     the job's pipeline has, whatever its slot count); the images whose last tile a chunk holds are written after it */
+  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, n * sizeof(int), st));
+  J->dec_has_refinement = refinement;
+  const size_t used = (size_t)n * J->slot_tiles, T = J->slot_tiles;
+  const size_t nchunks = std::min<size_t>(J->chunk_tile.size() - 1, used);
+  const uint32_t w = cp.x1 - cp.x0, hgt = cp.y1 - cp.y0, sb = imgs[0].sample_bytes;
+  for(size_t k = 0; k < nchunks; ++k)
+  {
+    const size_t t0 = k * used / nchunks, t1 = (k + 1) * used / nchunks;
+    if(t1 <= t0)
+      continue;
+    if(enqueue_block_decode(e, J, k, nullptr, st, t0, t1)) return -1;
+    if(enqueue_inverse(J, st, t0, t1)) return -1;
+    const uint32_t s0 = (uint32_t)(t0 / T), s1 = (uint32_t)(t1 / T);
+    for(int t = 0; t < tables && s1 > s0; ++t)
+      b2k_launch_planes_to_containers(J->d_batch_dst + (size_t)t * n + s0, s1 - s0, group, J->img.pitch, sb, w, hgt, st);
+  }
+  CUDA_TRY(cudaEventRecord(J->ev[1], st));
+  /* the caller's stream goes on once its images are written */
+  if(queue_after(e, st, caller)) return -1;
+  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
+  CUDA_TRY(cudaGetLastError());
+  float t = 0;
+  cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
+  if(ms_total) *ms_total = t;
+  /* the HT decoder's verdict, per slot */
+  std::vector<int> herr(n, 0);
+  CUDA_TRY(cudaMemcpy(herr.data(), J->d_err, n * sizeof(int), cudaMemcpyDeviceToHost));
+  for(uint32_t i = 0; i < n; ++i)
+    if(!status[i] && herr[i])
+    {
+      g_err = "HT decoder rejected " + std::to_string(herr[i]) + " block(s)";
+      fail(i, -2);
+    }
+  return failures();
+}
+
+extern "C" const char* b2k_decode_codestreams_error(b2k_engine* e, uint32_t i)
+{
+  if(!e)
+    return "";
+  std::lock_guard<std::mutex> lock(e->mu);
+  return i < e->batch_errors.size() ? e->batch_errors[i].c_str() : "";
 }

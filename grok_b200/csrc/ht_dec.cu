@@ -415,7 +415,7 @@ template <bool IRREV, bool REFINE>
 __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32)
     k_ht_decode_magsgn(const HtBlockDesc* __restrict__ blocks, const uint8_t* __restrict__ bytes,
                        const uint32_t* __restrict__ recs, const HtBlockOut* __restrict__ status, uint32_t nblocks,
-                       uint32_t line_entries, int* __restrict__ err)
+                       uint32_t line_entries, int* __restrict__ err, uint32_t first_block, uint32_t blocks_per_slot)
 {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint32_t* rings = reinterpret_cast<uint32_t*>(smem_raw);
@@ -427,6 +427,8 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32)
     return;
   const HtBlockDesc B = blocks[bidx];
   const HtBlockOut st = status[bidx];
+  /* the rejection counter of the image the block belongs to: one per slot of a batch, one in all for a single image */
+  err += blocks_per_slot ? (first_block + bidx) / blocks_per_slot : 0;
   uint32_t* ring = rings + warp * MS_RING_WORDS;
   uint16_t* const lines = lines_all + (size_t)warp * 2 * line_entries; /* two rows of bottom-sample exponents, used alternately */
 
@@ -968,7 +970,7 @@ void b2k_launch_ht_decode_vlc(const HtBlockDesc* d_blocks, const uint8_t* d_byte
 
 void b2k_launch_ht_decode_magsgn(const HtBlockDesc* d_blocks, const uint8_t* d_bytes, const uint32_t* d_recs,
                                  const HtBlockOut* d_status, uint32_t nblocks, uint32_t max_w, int* d_err, int irreversible,
-                                 int any_refinement, cudaStream_t st)
+                                 int any_refinement, cudaStream_t st, uint32_t first_block, uint32_t blocks_per_slot)
 {
   if(!nblocks)
     return;
@@ -976,11 +978,11 @@ void b2k_launch_ht_decode_magsgn(const HtBlockDesc* d_blocks, const uint8_t* d_b
   const size_t smem = (size_t)B2K_WARPS_PER_CTA * MS_RING_WORDS * sizeof(uint32_t) +
                       (size_t)B2K_WARPS_PER_CTA * 2 * line_entries * sizeof(uint16_t);
   const uint32_t grid = (nblocks + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA;
-  using Kernel = void (*)(const HtBlockDesc*, const uint8_t*, const uint32_t*, const HtBlockOut*, uint32_t, uint32_t, int*);
+  using Kernel = void (*)(const HtBlockDesc*, const uint8_t*, const uint32_t*, const HtBlockOut*, uint32_t, uint32_t, int*, uint32_t, uint32_t);
   static const Kernel variants[4] = {k_ht_decode_magsgn<false, false>, k_ht_decode_magsgn<false, true>,
                                      k_ht_decode_magsgn<true, false>, k_ht_decode_magsgn<true, true>};
   variants[(irreversible ? 2 : 0) + (any_refinement ? 1 : 0)]<<<grid, B2K_WARPS_PER_CTA * 32, smem, st>>>(
-      d_blocks, d_bytes, d_recs, d_status, nblocks, line_entries, d_err);
+      d_blocks, d_bytes, d_recs, d_status, nblocks, line_entries, d_err, first_block, blocks_per_slot);
   b2k_count_launch();
 }
 

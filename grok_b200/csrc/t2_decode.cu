@@ -43,17 +43,6 @@ void b2k_set_error(const char* msg); /* engine.cu */
 
 namespace
 {
-constexpr unsigned long long NO_ERROR = ~0ull;
-struct ParseStatus
-{
-  unsigned long long tile_err; /* (tile << 8) | reason of the lowest failing tile, NO_ERROR when none */
-  uint32_t locate;             /* the tile-part walk's reason */
-  uint32_t nparts;
-  uint32_t refinement;         /* some block has refinement passes to decode */
-  uint32_t walked;             /* tiles with data parsed by the walk */
-  uint32_t indexed;            /* tiles whose packets were parsed from their PLT starts */
-  unsigned long long bytes;    /* packet data of the recorded tile parts */
-};
 /* a coded block of a windowed parse's virtual coding: its box tile, the need rectangle that applies to it (resolution
    max(resno - 1, 0)) and its rectangle in band coordinates */
 struct WinBlock
@@ -66,103 +55,110 @@ struct NeedRects /* the window's need rectangles, one per resolution of the virt
   uint32_t r[B2K_MAX_RES][4];
 };
 
-__global__ void k_t2_locate(const uint8_t* __restrict__ cs, uint64_t len, uint64_t sot, uint32_t ntiles, TileBox box,
-                            PartRange* __restrict__ parts, uint64_t cap, uint32_t* __restrict__ head, uint32_t* __restrict__ last,
+/* Every kernel runs over the n streams of a batch (n = 1 for a single stream), one thread per item; the threads' bodies
+   are t2_parse.h's batch_* functions, which tests/t2_batch_check.cpp runs on the host */
+__global__ void k_t2_locate(const uint8_t* __restrict__ cs, const StreamDesc* __restrict__ sd, uint32_t n, uint32_t ntiles, TileBox box,
+                            PartRange* __restrict__ parts, uint32_t* __restrict__ head, uint32_t* __restrict__ last,
                             uint32_t* __restrict__ count, uint64_t* __restrict__ body_at, ParseStatus* status)
 {
-  uint32_t n = 0;
-  uint64_t bytes = 0;
-  status->locate = locate_tile_parts_box(cs, len, sot, ntiles, box, parts, cap, head, last, count, &n, body_at, &bytes);
-  status->nparts = n;
-  status->bytes = bytes;
+  const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+  if(s < n)
+    batch_locate(cs, sd, s, ntiles, box, parts, head, last, count, body_at, status);
 }
 
-__global__ void k_t2_plt(const uint8_t* __restrict__ cs, const PartRange* __restrict__ parts, const uint32_t* __restrict__ head,
-                         const DevPart* __restrict__ tiles, uint32_t ntiles, const uint64_t* __restrict__ tile_first,
-                         ParsedBlock* __restrict__ blk, uint64_t* __restrict__ start, uint64_t* __restrict__ end,
-                         uint64_t* __restrict__ part_end, uint32_t* __restrict__ indexed, uint32_t* __restrict__ marked,
-                         ParseStatus* status)
+__global__ void k_t2_plt(const uint8_t* __restrict__ cs, const StreamDesc* __restrict__ sd, uint32_t n, const PartRange* __restrict__ parts,
+                         const uint32_t* __restrict__ head, const DevPart* __restrict__ tiles, uint32_t ntiles,
+                         const uint64_t* __restrict__ tile_first, uint64_t nblocks, uint64_t np, ParsedBlock* __restrict__ blk,
+                         uint64_t* __restrict__ start, uint64_t* __restrict__ end, uint64_t* __restrict__ part_end,
+                         uint32_t* __restrict__ indexed, uint32_t* __restrict__ marked, ParseStatus* status)
 {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if(t >= ntiles || status->locate != PR_NONE)
-    return;
-  for(uint64_t i = tile_first[t]; i < tile_first[t + 1]; ++i)
-    blk[i] = ParsedBlock{};
-  const DevPart T = tiles[t];
-  const bool ix = plt_index(cs, parts, head[t], T.p1 - T.p0, start + T.p0, end + T.p0, part_end + T.p0);
-  indexed[t] = ix;
-  marked[t] = 0;
-  if(ix && T.p1 > T.p0)
-    atomicAdd(&status->indexed, 1u);
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if(g < (uint64_t)n * ntiles)
+    batch_plt(cs, sd, g, parts, head, tiles, ntiles, tile_first, nblocks, np, blk, start, end, part_end, indexed, marked, status);
 }
 
-__global__ void k_t2_packets(const uint8_t* __restrict__ cs, const DevPacket* __restrict__ packets, uint64_t np,
-                             const uint32_t* __restrict__ pkt_tile, const uint32_t* __restrict__ indexed,
+__global__ void k_t2_packets(const uint8_t* __restrict__ cs, const StreamDesc* __restrict__ sd, uint32_t n,
+                             const DevPacket* __restrict__ packets, uint64_t np, const uint32_t* __restrict__ pkt_tile, uint32_t ntiles,
+                             uint64_t nblocks, uint64_t tag_nodes, const uint32_t* __restrict__ indexed,
                              const uint64_t* __restrict__ start, const uint64_t* __restrict__ end, const uint64_t* __restrict__ part_end,
                              const uint8_t* __restrict__ kmax, ParsedBlock* __restrict__ blk, TagNode* __restrict__ tags,
                              uint32_t* __restrict__ marked, bool sop, bool eph, const ParseStatus* status)
 {
   const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if(g >= np || status->locate != PR_NONE)
-    return;
-  const uint32_t t = pkt_tile[g];
-  if(!indexed[t])
-    return;
-  uint64_t at = start[g];
-  const DevPacket& P = packets[g];
-  if(parse_packet(cs, P, &at, part_end[g], kmax, blk, tags + P.tag_at, sop, eph) != PR_NONE || at != end[g])
-    marked[t] = 1; /* the walk decides */
+  if(g < n * np)
+    batch_packet(cs, sd, g, packets, np, pkt_tile, ntiles, nblocks, tag_nodes, indexed, start, end, part_end, kmax, blk, tags, marked, sop,
+                 eph, status);
 }
 
-__global__ void k_t2_walk(const uint8_t* __restrict__ cs, const PartRange* __restrict__ parts, const uint32_t* __restrict__ head,
-                          const DevPart* __restrict__ tiles, uint32_t ntiles, const DevPacket* __restrict__ packets,
-                          const uint8_t* __restrict__ kmax, const uint64_t* __restrict__ tile_first, ParsedBlock* __restrict__ blk,
-                          TagNode* __restrict__ tags, const uint32_t* __restrict__ indexed, const uint32_t* __restrict__ marked,
-                          bool sop, bool eph, ParseStatus* status)
+__global__ void k_t2_walk(const uint8_t* __restrict__ cs, const StreamDesc* __restrict__ sd, uint32_t n, const PartRange* __restrict__ parts,
+                          const uint32_t* __restrict__ head, const DevPart* __restrict__ tiles, uint32_t ntiles,
+                          const DevPacket* __restrict__ packets, const uint8_t* __restrict__ kmax, const uint64_t* __restrict__ tile_first,
+                          uint64_t nblocks, uint64_t tag_nodes, ParsedBlock* __restrict__ blk, TagNode* __restrict__ tags,
+                          const uint32_t* __restrict__ indexed, const uint32_t* __restrict__ marked, bool sop, bool eph,
+                          ParseStatus* status)
 {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  if(t >= ntiles || status->locate != PR_NONE || (indexed[t] && !marked[t]))
-    return;
-  const DevPart T = tiles[t];
-  if(T.p1 == T.p0)
-    return;
-  if(marked[t]) /* the packets parsed from PLT may have left fields behind */
-    for(uint64_t i = tile_first[t]; i < tile_first[t + 1]; ++i)
-      blk[i] = ParsedBlock{};
-  if(head[t] != PART_NONE)
-    atomicAdd(&status->walked, 1u);
-  const uint32_t r = parse_tile(cs, parts, head[t], packets + T.p0, T.p1 - T.p0, kmax, blk, tags + packets[T.p0].tag_at, sop, eph);
-  if(r != PR_NONE)
-    atomicMin(&status->tile_err, ((unsigned long long)t << 8) | r);
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if(g < (uint64_t)n * ntiles)
+    batch_walk(cs, sd, g, parts, head, tiles, ntiles, packets, kmax, tile_first, nblocks, tag_nodes, blk, tags, indexed, marked, sop, eph,
+               status);
 }
 
-/* win != NULL (a windowed parse): coded[k] is the box block of virtual coded block k; a block the window does not need
-   stays uncoded, and a parsed block's bytes are addressed where k_t2_gather puts them */
-__global__ void k_t2_desc(const ParsedBlock* __restrict__ blk, const uint32_t* __restrict__ coded, uint32_t ncoded,
-                          const HtBlockDesc* __restrict__ enc, const float* __restrict__ quant, HtBlockDesc* __restrict__ dec,
-                          const WinBlock* __restrict__ win, const NeedRects* __restrict__ need, const PartRange* __restrict__ parts,
-                          const uint32_t* __restrict__ head, const uint64_t* __restrict__ body_at, ParseStatus* status)
+/* a thread per (stream, coded block): descriptor s * ncoded + k from template enc[s * ncoded + k], pointing into the arena.
+   A stream whose parse failed (or was skipped) gets length-0 descriptors, which decode as all-zero blocks.  win != NULL (a
+   windowed parse, one stream): coded[k] is the box block of virtual coded block k; a block the window does not need stays
+   uncoded, and a parsed block's bytes are addressed where k_t2_gather puts them */
+__global__ void k_t2_desc(const StreamDesc* __restrict__ sd, uint32_t n, const ParsedBlock* __restrict__ blk, uint64_t nblocks,
+                          const uint32_t* __restrict__ coded, uint32_t ncoded, const HtBlockDesc* __restrict__ enc,
+                          const float* __restrict__ quant, HtBlockDesc* __restrict__ dec, const WinBlock* __restrict__ win,
+                          const NeedRects* __restrict__ need, const PartRange* __restrict__ parts, const uint32_t* __restrict__ head,
+                          const uint64_t* __restrict__ body_at, ParseStatus* status)
 {
-  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
-  if(k >= ncoded || status->locate != PR_NONE || status->tile_err != NO_ERROR)
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if(g >= (uint64_t)n * ncoded)
     return;
-  ParsedBlock b = blk[coded[k]];
+  uint32_t s = 0;
+  ParsedBlock b = batch_block(blk, nblocks, coded, g, ncoded, status, &s);
   uint64_t at = b.offset;
-  if(win)
+  if(win && b.length)
   {
-    const WinBlock w = win[k];
+    const WinBlock w = win[g];
     if(need->n && !window_needs(need->r[w.res], w.x0, w.y0, w.x1, w.y1))
       b = ParsedBlock{};
     at = b.length ? gathered_offset(parts, head[w.tile], body_at, b.offset) : 0;
   }
-  HtBlockDesc d = enc[k];
+  HtBlockDesc d = enc[g];
   d.length = b.length;
-  d.slot_off = at;
+  d.slot_off = sd[s].at + at;
   block_decode_fields(b, d.kmax, &d.mmsbs, &d.passes, &d.length2);
-  d.quant = quant[k]; /* stepsize / 2^(31-Kmax) */
-  dec[k] = d;
+  d.quant = quant[g]; /* stepsize / 2^(31-Kmax) */
+  dec[g] = d;
   if(d.passes > 1)
-    status->refinement = 1;
+    status[s].refinement = 1;
+}
+
+/* one copy per entry of a (source, length, destination) table: entry e (blockIdx.y strided) by a strip of CTAs along x;
+   16 bytes per thread and step where source and destination are both 16-byte aligned (the arena's streams start on
+   256-byte boundaries, and CUDA allocations on 256-byte ones), the bytes after the last whole 16 one by one */
+__global__ void k_copy_table(const CopyEntry* __restrict__ tab, uint32_t n, uint8_t* __restrict__ out)
+{
+  const uint64_t first = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (uint64_t)gridDim.x * blockDim.x;
+  for(uint32_t e = blockIdx.y; e < n; e += gridDim.y)
+  {
+    const CopyEntry E = tab[e];
+    uint8_t* dst = out + E.dst;
+    uint64_t done = 0;
+    if(((reinterpret_cast<uintptr_t>(E.src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0)
+    {
+      const uint64_t v = E.len / 16;
+      const uint4* s4 = reinterpret_cast<const uint4*>(E.src);
+      uint4* d4 = reinterpret_cast<uint4*>(dst);
+      for(uint64_t i = first; i < v; i += stride)
+        d4[i] = s4[i];
+      done = v * 16;
+    }
+    for(uint64_t i = done + first; i < E.len; i += stride)
+      dst[i] = E.src[i];
+  }
 }
 
 /* the wanted tile parts' packet data, end to end: part p (blockIdx.y strided) by a strip of CTAs along x */
@@ -196,6 +192,8 @@ struct T2Parse
   Plan plan;
   uint32_t flags = 0, ntiles = 0;
   uint64_t nblocks = 0, ncoded = 0;
+  uint32_t streams = 1;            /* stream capacity: the per-stream slices below are allocated for this many */
+  uint32_t last_n = 1;             /* streams of the last enqueue */
   std::vector<b2k_block> blocks; /* the enumeration, into which the parsed fields are merged */
   uint8_t* d_mem = nullptr;
   DevPacket* d_packets = nullptr;
@@ -203,14 +201,17 @@ struct T2Parse
   uint8_t* d_kmax = nullptr;
   uint64_t* d_tile_first = nullptr;
   uint32_t* d_coded = nullptr;
+  /* per stream (slice s of `streams`) */
   TagNode* d_tags = nullptr;
   ParsedBlock* d_blk = nullptr;
   uint32_t *d_head = nullptr, *d_last = nullptr, *d_count = nullptr;
   uint32_t *d_pkt_tile = nullptr, *d_indexed = nullptr, *d_marked = nullptr;
   uint64_t *d_start = nullptr, *d_end = nullptr, *d_part_end = nullptr; /* per packet, from PLT */
-  ParseStatus* d_status = nullptr;
-  ParseStatus* h_status = nullptr; /* pinned */
-  PartRange* d_parts = nullptr;    /* grown with the code stream's length */
+  ParseStatus* d_status = nullptr; /* streams statuses, then streams StreamDescs: one upload */
+  StreamDesc* d_sd = nullptr;
+  ParseStatus* h_status = nullptr; /* pinned, the same layout */
+  StreamDesc* h_sd = nullptr;
+  PartRange* d_parts = nullptr;    /* grown with the code streams' lengths */
   uint64_t parts_cap = 0;
   /* a windowed parse: the plan is the box coding's; coded block k of the virtual coding is box block d_coded[k] */
   bool window = false;
@@ -237,7 +238,7 @@ struct T2Parse
   } while(0)
 
 int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks, uint64_t nblocks, uint32_t num_tiles,
-                        const uint32_t* coded_index, uint64_t ncoded, T2Parse** out)
+                        const uint32_t* coded_index, uint64_t ncoded, T2Parse** out, uint32_t streams)
 {
   *out = nullptr;
   T2Parse* J = new T2Parse();
@@ -259,6 +260,7 @@ int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* b
   J->ntiles = num_tiles;
   J->nblocks = nblocks;
   J->ncoded = ncoded;
+  J->streams = streams = std::max(streams, 1u);
   J->blocks.assign(blocks, blocks + nblocks);
   std::vector<uint8_t> kmax(nblocks);
   std::vector<uint64_t> tile_first(num_tiles + 1, nblocks);
@@ -269,12 +271,12 @@ int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* b
   }
   for(uint32_t t = num_tiles; t-- > 0;) /* a tile without blocks starts where the next one does */
     tile_first[t] = std::min(tile_first[t], tile_first[t + 1]);
-  const uint64_t np = P.packets.size();
+  const uint64_t np = P.packets.size(), S = streams;
   auto bytes = [](uint64_t n, size_t sz) { return (n * sz + 255) & ~(uint64_t)255; };
   const uint64_t total = bytes(np, sizeof(DevPacket)) + bytes(num_tiles, sizeof(DevPart)) + bytes(nblocks, 1) +
-                         bytes(num_tiles + 1, sizeof(uint64_t)) + bytes(ncoded, sizeof(uint32_t)) + bytes(P.tag_nodes, sizeof(TagNode)) +
-                         bytes(nblocks, sizeof(ParsedBlock)) + 5 * bytes(num_tiles, sizeof(uint32_t)) + bytes(np, sizeof(uint32_t)) +
-                         3 * bytes(np, sizeof(uint64_t)) + bytes(1, sizeof(ParseStatus));
+                         bytes(num_tiles + 1, sizeof(uint64_t)) + bytes(ncoded, sizeof(uint32_t)) + bytes(S * P.tag_nodes, sizeof(TagNode)) +
+                         bytes(S * nblocks, sizeof(ParsedBlock)) + 5 * bytes(S * num_tiles, sizeof(uint32_t)) + bytes(np, sizeof(uint32_t)) +
+                         3 * bytes(S * np, sizeof(uint64_t)) + bytes(S, sizeof(ParseStatus) + sizeof(StreamDesc));
   T2P_TRY(cudaMalloc(&J->d_mem, total));
   uint8_t* p = J->d_mem;
   J->d_packets = carve<DevPacket>(p, np);
@@ -282,18 +284,19 @@ int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* b
   J->d_kmax = carve<uint8_t>(p, nblocks);
   J->d_tile_first = carve<uint64_t>(p, num_tiles + 1);
   J->d_coded = carve<uint32_t>(p, ncoded);
-  J->d_tags = carve<TagNode>(p, P.tag_nodes);
-  J->d_blk = carve<ParsedBlock>(p, nblocks);
-  J->d_head = carve<uint32_t>(p, num_tiles);
-  J->d_last = carve<uint32_t>(p, num_tiles);
-  J->d_count = carve<uint32_t>(p, num_tiles);
-  J->d_indexed = carve<uint32_t>(p, num_tiles);
-  J->d_marked = carve<uint32_t>(p, num_tiles);
+  J->d_tags = carve<TagNode>(p, S * P.tag_nodes);
+  J->d_blk = carve<ParsedBlock>(p, S * nblocks);
+  J->d_head = carve<uint32_t>(p, S * num_tiles);
+  J->d_last = carve<uint32_t>(p, S * num_tiles);
+  J->d_count = carve<uint32_t>(p, S * num_tiles);
+  J->d_indexed = carve<uint32_t>(p, S * num_tiles);
+  J->d_marked = carve<uint32_t>(p, S * num_tiles);
   J->d_pkt_tile = carve<uint32_t>(p, np);
-  J->d_start = carve<uint64_t>(p, np);
-  J->d_end = carve<uint64_t>(p, np);
-  J->d_part_end = carve<uint64_t>(p, np);
-  J->d_status = carve<ParseStatus>(p, 1);
+  J->d_start = carve<uint64_t>(p, S * np);
+  J->d_end = carve<uint64_t>(p, S * np);
+  J->d_part_end = carve<uint64_t>(p, S * np);
+  J->d_status = reinterpret_cast<ParseStatus*>(p);
+  J->d_sd = reinterpret_cast<StreamDesc*>(J->d_status + S);
   T2P_TRY(cudaMemcpy(J->d_packets, P.packets.data(), np * sizeof(DevPacket), cudaMemcpyHostToDevice));
   T2P_TRY(cudaMemcpy(J->d_tiles, P.parts.data(), num_tiles * sizeof(DevPart), cudaMemcpyHostToDevice));
   T2P_TRY(cudaMemcpy(J->d_kmax, kmax.data(), nblocks, cudaMemcpyHostToDevice));
@@ -304,7 +307,8 @@ int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* b
     for(uint64_t k = P.parts[t].p0; k < P.parts[t].p1; ++k)
       pkt_tile[k] = t;
   T2P_TRY(cudaMemcpy(J->d_pkt_tile, pkt_tile.data(), np * sizeof(uint32_t), cudaMemcpyHostToDevice));
-  T2P_TRY(cudaHostAlloc(&J->h_status, sizeof(ParseStatus), cudaHostAllocDefault));
+  T2P_TRY(cudaHostAlloc(&J->h_status, S * (sizeof(ParseStatus) + sizeof(StreamDesc)), cudaHostAllocDefault));
+  J->h_sd = reinterpret_cast<StreamDesc*>(J->h_status + S);
   *out = J;
   guard.j = nullptr;
   return 0;
@@ -369,12 +373,19 @@ void b2k_t2_parse_destroy(T2Parse* J)
 
 uint32_t b2k_t2_parse_flags(const T2Parse* J) { return J->flags; }
 
-/* the five launches over the plan's tiles, which are the tiles of `box` among the stream's ntiles */
-static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t ntiles, const TileBox& box, uint32_t* d_count,
+/* the five launches over the plan's tiles, which are the tiles of `box` among each stream's ntiles, for the n streams whose
+   h_sd[s].at / len / sot the caller filled in (sot = 0: not parsed); the part table is laid out here */
+static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint32_t n, uint32_t ntiles, const TileBox& box, uint32_t* d_count,
                          const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
 {
-  /* every tile part takes at least the 12 bytes of its SOT, and a tile has at most 256 */
-  const uint64_t need = std::min<uint64_t>(len / 12 + 1, 256ull * J->ntiles);
+  uint64_t need = 0;
+  for(uint32_t s = 0; s < n; ++s)
+  {
+    StreamDesc& D = J->h_sd[s];
+    D.parts0 = need;
+    D.parts_cap = D.sot ? part_capacity(D.len, J->ntiles) : 0;
+    need += D.parts_cap;
+  }
   if(need > J->parts_cap)
   {
     cudaFree(J->d_parts);
@@ -388,39 +399,43 @@ static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t s
       T2P_TRY(cudaMalloc(&J->d_body_at, cap * sizeof(uint64_t)));
     J->parts_cap = cap;
   }
-  ParseStatus init{NO_ERROR, 0, 0, 0, 0, 0, 0};
-  *J->h_status = init;
-  T2P_TRY(cudaMemcpyAsync(J->d_status, J->h_status, sizeof(ParseStatus), cudaMemcpyHostToDevice, st));
+  for(uint32_t s = 0; s < n; ++s)
+    J->h_status[s] = ParseStatus{NO_TILE_ERROR, J->h_sd[s].sot ? (uint32_t)PR_NONE : (uint32_t)PR_SKIPPED, 0, 0, 0, 0, 0};
+  J->last_n = n;
+  const uint64_t S = J->streams;
+  /* statuses and stream table in one copy */
+  T2P_TRY(cudaMemcpyAsync(J->d_status, J->h_status, S * sizeof(ParseStatus) + n * sizeof(StreamDesc), cudaMemcpyHostToDevice, st));
   if(J->window)
     T2P_TRY(cudaMemcpyAsync(J->d_need, J->h_need, sizeof(NeedRects), cudaMemcpyHostToDevice, st));
-  k_t2_locate<<<1, 1, 0, st>>>(cs, len, sot, ntiles, box, J->d_parts, J->parts_cap, J->d_head, J->d_last, d_count, J->d_body_at,
-                               J->d_status);
+  const uint32_t tpb = 32; /* streams, tiles and packets are few and each thread is a long serial chain: spread them over the SMs */
+  auto grid = [&](uint64_t items) { return (unsigned)((items + tpb - 1) / tpb); };
+  k_t2_locate<<<grid(n), tpb, 0, st>>>(cs, J->d_sd, n, ntiles, box, J->d_parts, J->d_head, J->d_last, d_count, J->d_body_at, J->d_status);
   b2k_count_launch();
-  const uint32_t tpb = 32; /* tiles and packets are few and each thread is a long serial chain: spread them over the SMs */
   const bool sop = (J->flags & B2K_CS_SOP) != 0, eph = (J->flags & B2K_CS_EPH) != 0;
-  const uint64_t np = J->plan.packets.size();
-  const unsigned tile_grid = (J->ntiles + tpb - 1) / tpb;
-  k_t2_plt<<<tile_grid, tpb, 0, st>>>(cs, J->d_parts, J->d_head, J->d_tiles, J->ntiles, J->d_tile_first, J->d_blk, J->d_start, J->d_end,
-                                      J->d_part_end, J->d_indexed, J->d_marked, J->d_status);
+  const uint64_t np = J->plan.packets.size(), tags = J->plan.tag_nodes;
+  k_t2_plt<<<grid((uint64_t)n * J->ntiles), tpb, 0, st>>>(cs, J->d_sd, n, J->d_parts, J->d_head, J->d_tiles, J->ntiles, J->d_tile_first,
+                                                          J->nblocks, np, J->d_blk, J->d_start, J->d_end, J->d_part_end, J->d_indexed,
+                                                          J->d_marked, J->d_status);
   b2k_count_launch();
   if(np)
   {
-    k_t2_packets<<<(unsigned)((np + tpb - 1) / tpb), tpb, 0, st>>>(cs, J->d_packets, np, J->d_pkt_tile, J->d_indexed, J->d_start, J->d_end,
-                                                                   J->d_part_end, J->d_kmax, J->d_blk, J->d_tags, J->d_marked, sop, eph,
-                                                                   J->d_status);
+    k_t2_packets<<<grid(n * np), tpb, 0, st>>>(cs, J->d_sd, n, J->d_packets, np, J->d_pkt_tile, J->ntiles, J->nblocks, tags, J->d_indexed,
+                                               J->d_start, J->d_end, J->d_part_end, J->d_kmax, J->d_blk, J->d_tags, J->d_marked, sop, eph,
+                                               J->d_status);
     b2k_count_launch();
   }
-  k_t2_walk<<<tile_grid, tpb, 0, st>>>(cs, J->d_parts, J->d_head, J->d_tiles, J->ntiles, J->d_packets, J->d_kmax, J->d_tile_first,
-                                       J->d_blk, J->d_tags, J->d_indexed, J->d_marked, sop, eph, J->d_status);
+  k_t2_walk<<<grid((uint64_t)n * J->ntiles), tpb, 0, st>>>(cs, J->d_sd, n, J->d_parts, J->d_head, J->d_tiles, J->ntiles, J->d_packets,
+                                                           J->d_kmax, J->d_tile_first, J->nblocks, tags, J->d_blk, J->d_tags, J->d_indexed,
+                                                           J->d_marked, sop, eph, J->d_status);
   b2k_count_launch();
   if(d_dec && J->ncoded)
   {
-    k_t2_desc<<<(unsigned)((J->ncoded + 127) / 128), 128, 0, st>>>(J->d_blk, J->d_coded, (uint32_t)J->ncoded, d_enc, d_quant, d_dec,
-                                                                   J->d_win, J->d_need, J->d_parts, J->d_head, J->d_body_at,
-                                                                   J->d_status);
+    k_t2_desc<<<(unsigned)((n * J->ncoded + 127) / 128), 128, 0, st>>>(J->d_sd, n, J->d_blk, J->nblocks, J->d_coded, (uint32_t)J->ncoded,
+                                                                       d_enc, d_quant, d_dec, J->d_win, J->d_need, J->d_parts, J->d_head,
+                                                                       J->d_body_at, J->d_status);
     b2k_count_launch();
   }
-  T2P_TRY(cudaMemcpyAsync(J->h_status, J->d_status, sizeof(ParseStatus), cudaMemcpyDeviceToHost, st));
+  T2P_TRY(cudaMemcpyAsync(J->h_status, J->d_status, n * sizeof(ParseStatus), cudaMemcpyDeviceToHost, st));
   T2P_TRY(cudaGetLastError());
   return 0;
 }
@@ -428,8 +443,24 @@ static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t s
 int b2k_t2_parse_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, const HtBlockDesc* d_enc, const float* d_quant,
                          HtBlockDesc* d_dec, cudaStream_t st)
 {
-  return enqueue_parse(J, cs, len, sot, J->ntiles, TileBox{J->ntiles, 0, 0, J->ntiles, 1}, J->d_count, d_enc, d_quant, d_dec, st);
+  J->h_sd[0] = StreamDesc{0, len, sot, 0, 0};
+  return enqueue_parse(J, cs, 1, J->ntiles, TileBox{J->ntiles, 0, 0, J->ntiles, 1}, J->d_count, d_enc, d_quant, d_dec, st);
 }
+
+int b2k_t2_batch_enqueue(T2Parse* J, const uint8_t* arena, uint32_t n, const uint64_t* at, const uint64_t* len, const uint64_t* sot,
+                         const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
+{
+  if(n > J->streams)
+  {
+    b2k_set_error("internal: more code streams than the parse was made for");
+    return -1;
+  }
+  for(uint32_t s = 0; s < n; ++s)
+    J->h_sd[s] = StreamDesc{at[s], len[s], sot[s], 0, 0};
+  return enqueue_parse(J, arena, n, J->ntiles, TileBox{J->ntiles, 0, 0, J->ntiles, 1}, J->d_count, d_enc, d_quant, d_dec, st);
+}
+
+uint32_t b2k_t2_parse_streams(const T2Parse* J) { return J->streams; }
 
 int b2k_t2_window_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t grid_nx, uint32_t ntiles,
                           const b2k::t2::WindowCoding& wc, const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
@@ -451,8 +482,8 @@ int b2k_t2_window_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t 
     n.r[r][2] = wc.need[r].x1;
     n.r[r][3] = wc.need[r].y1;
   }
-  return enqueue_parse(J, cs, len, sot, ntiles, TileBox{grid_nx, wc.ta_x, wc.ta_y, wc.tb_x, wc.tb_y}, J->d_wcount, d_enc, d_quant, d_dec,
-                       st);
+  J->h_sd[0] = StreamDesc{0, len, sot, 0, 0};
+  return enqueue_parse(J, cs, 1, ntiles, TileBox{grid_nx, wc.ta_x, wc.ta_y, wc.tb_x, wc.tb_y}, J->d_wcount, d_enc, d_quant, d_dec, st);
 }
 
 uint64_t b2k_t2_window_bytes(const T2Parse* J) { return J->h_status->bytes; }
@@ -501,24 +532,39 @@ int b2k_t2_window_blocks(const T2Parse* J, const b2k_block* vblocks, uint64_t nv
   return 0;
 }
 
-int b2k_t2_parse_result(const T2Parse* J, bool* refinement)
+int b2k_t2_batch_result(const T2Parse* J, uint32_t s, bool* refinement)
 {
-  const ParseStatus& s = *J->h_status;
-  uint32_t r = s.locate;
-  if(r == PR_NONE && s.tile_err != NO_ERROR)
-    r = (uint32_t)(s.tile_err & 0xFF);
+  const ParseStatus& st = J->h_status[s];
+  const uint32_t r = status_reason(st);
   if(refinement)
-    *refinement = s.refinement != 0;
+    *refinement = st.refinement != 0;
   if(r == PR_NONE)
     return 0;
   b2k_set_error(parse_reason_text(r));
   return parse_reason_rc(r);
 }
 
+int b2k_t2_parse_result(const T2Parse* J, bool* refinement) { return b2k_t2_batch_result(J, 0, refinement); }
+
 void b2k_t2_parse_stats(const T2Parse* J, uint32_t* indexed, uint32_t* walked)
 {
-  *indexed = J->h_status->indexed;
-  *walked = J->h_status->walked;
+  *indexed = *walked = 0;
+  for(uint32_t s = 0; s < J->last_n; ++s)
+  {
+    *indexed += J->h_status[s].indexed;
+    *walked += J->h_status[s].walked;
+  }
+}
+
+int b2k_copy_table(const CopyEntry* d_tab, uint32_t n, uint64_t max_len, uint8_t* out, cudaStream_t st)
+{
+  if(!n || !max_len)
+    return 0;
+  const unsigned gx = (unsigned)std::min<uint64_t>(256, max_len / (256 * 16 * 4) + 1);
+  k_copy_table<<<dim3(gx, std::min<uint32_t>(n, 65535)), 256, 0, st>>>(d_tab, n, out);
+  b2k_count_launch();
+  T2P_TRY(cudaGetLastError());
+  return 0;
 }
 
 int b2k_t2_parse_blocks(const T2Parse* J, b2k_block* out, cudaStream_t st)

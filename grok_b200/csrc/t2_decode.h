@@ -12,7 +12,7 @@ struct T2Parse; /* a job's packet plan and device buffers for one progression or
    blocks[coded_index[k]]; flags: the stream's progression order (B2K_CS_PROG) and SOP / EPH.  0, or -1 with
    b2k_last_error set. */
 int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks, uint64_t nblocks, uint32_t num_tiles,
-                        const uint32_t* coded_index, uint64_t ncoded, T2Parse** out);
+                        const uint32_t* coded_index, uint64_t ncoded, T2Parse** out, uint32_t streams = 1);
 void b2k_t2_parse_destroy(T2Parse* j);
 uint32_t b2k_t2_parse_flags(const T2Parse* j);
 /* on st: the parse of the code stream cs[0, len) in device memory, whose first SOT is at sot, then (d_dec != NULL) the
@@ -23,7 +23,26 @@ int b2k_t2_parse_enqueue(T2Parse* j, const uint8_t* cs, uint64_t len, uint64_t s
 /* once st has reached the end of b2k_t2_parse_enqueue's work: 0, or b2k_codestream_parse's return code with its text;
    *refinement: a block has refinement passes to decode */
 int b2k_t2_parse_result(const T2Parse* j, bool* refinement);
-/* after the status has arrived: tiles parsed packet by packet from their PLT starts, and tiles walked */
+/* ---- batches (b2k_decode_codestreams_device): streams of one coding, a parse made with `streams` >= n ----------------
+ * On st: the parse of the n code streams arena[at[s], at[s] + len[s]) whose first SOT is at sot[s] (sot[s] = 0: stream s
+ * failed before its tile parts and is not parsed), in the same five launches, then (d_dec != NULL) descriptor s * ncoded + k
+ * of every stream's coded block k from d_enc / d_quant's entry of the same index, pointing into the arena.  A stream that
+ * fails, or is not parsed, gets length-0 descriptors (all-zero blocks).  The statuses to the host. */
+int b2k_t2_batch_enqueue(T2Parse* j, const uint8_t* arena, uint32_t n, const uint64_t* at, const uint64_t* len, const uint64_t* sot,
+                         const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st);
+/* once the statuses have arrived: stream s's b2k_codestream_parse return code (its text set when not 0) */
+int b2k_t2_batch_result(const T2Parse* j, uint32_t s, bool* refinement);
+uint32_t b2k_t2_parse_streams(const T2Parse* j);
+/* one entry of a gather: len bytes from device address src to out + dst */
+struct CopyEntry
+{
+  const uint8_t* src;
+  uint64_t len, dst;
+};
+/* on st, one launch: every entry of the device table d_tab[0, n) (none longer than max_len) */
+int b2k_copy_table(const CopyEntry* d_tab, uint32_t n, uint64_t max_len, uint8_t* out, cudaStream_t st);
+
+/* after the status has arrived (over the streams of the last enqueue): tiles parsed packet by packet from their PLT starts, and tiles walked */
 void b2k_t2_parse_stats(const T2Parse* j, uint32_t* indexed, uint32_t* walked);
 /* after a result of 0: the block table b2k_codestream_parse returns (offsets into cs) into out[0, nblocks) */
 int b2k_t2_parse_blocks(const T2Parse* j, b2k_block* out, cudaStream_t st);

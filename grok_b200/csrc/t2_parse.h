@@ -38,6 +38,7 @@ enum ParseReason : uint32_t
   PR_EPH,           /* -1 */
   PR_BODY_RUN,      /* -1 */
   PR_PART_TABLE,    /* -1: more tile parts than the table holds (cannot happen: each takes at least 12 bytes) */
+  PR_SKIPPED,       /* a stream of a batch that failed before its tile parts: not parsed, its blocks stay uncoded */
   PR_COUNT
 };
 B2K_HD int parse_reason_rc(uint32_t r) { return (r == PR_TP_ORDER || r == PR_TP_MARKER || r == PR_PASSES) ? 1 : -1; }
@@ -510,6 +511,173 @@ B2K_HD void block_decode_fields(const ParsedBlock& b, uint8_t kmax, uint8_t* mms
 B2K_HD bool window_needs(const uint32_t* need, uint32_t x0, uint32_t y0, uint32_t x1, uint32_t y1)
 {
   return x0 < need[2] && x1 > need[0] && y0 < need[3] && y1 > need[1];
+}
+
+/* ---- batches: n code streams of one coding parsed by the same five launches -------------------------------------------
+ * The plan (packets, tag-tree offsets, Kmax) is shared; every other piece of parse state is sliced per stream.  Stream s
+ * lies at byte at of the arena (batch_arena_next), its tile parts in entries [parts0, parts0 + parts_cap) of the part
+ * table (a prefix sum of part_capacity), and its blocks, packets, tiles and tag scratch in slice s of their arrays.
+ * sot = 0: the stream failed before its tile parts and is not parsed. */
+struct StreamDesc
+{
+  uint64_t at, len, sot, parts0, parts_cap;
+};
+/* item i of stream s in a launch over n streams of `per` items each, flattened as g = s * per + i */
+struct StreamItem
+{
+  uint32_t s;
+  uint64_t i;
+};
+B2K_HD StreamItem split_stream_item(uint64_t g, uint64_t per) { return StreamItem{(uint32_t)(g / per), g % per}; }
+/* the tile-part table a stream of len bytes over ntiles tiles may need: every tile part takes at least the 12 bytes of its
+   SOT, and a tile has at most 256 */
+B2K_HD uint64_t part_capacity(uint64_t len, uint32_t ntiles)
+{
+  const uint64_t a = len / 12 + 1, b = 256ull * ntiles;
+  return a < b ? a : b;
+}
+/* where the stream after one of len bytes at `at` starts in a batch arena: the next 256-byte boundary, the base alignment
+   the single-stream decode gives its stream */
+B2K_HD uint64_t batch_arena_next(uint64_t at, uint64_t len) { return (at + len + 255) & ~(uint64_t)255; }
+
+/* the main-header prefix a batch first reads of each stream; a header that runs past it is read again with twice as many
+   bytes, all such streams together */
+constexpr uint64_t BATCH_HEADER_PREFIX = 4096;
+
+/* one stream's parse status.  tile_err: (tile << 8) | reason of the lowest failing tile, NO_TILE_ERROR when none */
+constexpr unsigned long long NO_TILE_ERROR = ~0ull;
+struct ParseStatus
+{
+  unsigned long long tile_err;
+  uint32_t locate;             /* the tile-part walk's reason (PR_SKIPPED: the stream is not parsed) */
+  uint32_t nparts;
+  uint32_t refinement;         /* some block has refinement passes to decode */
+  uint32_t walked;             /* tiles with data parsed by the walk */
+  uint32_t indexed;            /* tiles whose packets were parsed from their PLT starts */
+  unsigned long long bytes;    /* packet data of the recorded tile parts */
+};
+/* the kernels' threads update a stream's counters together; the host runs them one after another */
+B2K_HD void status_add(uint32_t* p, uint32_t v)
+{
+#ifdef __CUDA_ARCH__
+  atomicAdd(p, v);
+#else
+  *p += v;
+#endif
+}
+B2K_HD void status_min(unsigned long long* p, unsigned long long v)
+{
+#ifdef __CUDA_ARCH__
+  atomicMin(p, v);
+#else
+  if(v < *p)
+    *p = v;
+#endif
+}
+/* 0, or the stream's failure as parse_reason_* take it */
+B2K_HD uint32_t status_reason(const ParseStatus& st)
+{
+  return st.locate != PR_NONE ? st.locate : st.tile_err != NO_TILE_ERROR ? (uint32_t)(st.tile_err & 0xFF) : (uint32_t)PR_NONE;
+}
+
+/* The five kernels' threads over a batch (t2_decode.cu runs them as kernels, tests/t2_batch_check.cpp on the host in the same
+ * order).  cs is the arena; stream s is sd[s], its status status[s].  A stream whose status is set before the first step
+ * (PR_SKIPPED) is left alone.  The per-stream arrays are sliced: head / last (bt = box.tiles() each), count (ntiles each),
+ * indexed / marked (plan tiles each), blk (nblocks each), start / end / part_end (np each), tags (tag_nodes each). */
+/* step 1, thread s: the tile-part walk of stream s */
+B2K_HD void batch_locate(const uint8_t* cs, const StreamDesc* sd, uint32_t s, uint32_t ntiles, const TileBox& box, PartRange* parts,
+                         uint32_t* head, uint32_t* last, uint32_t* count, uint64_t* body_at, ParseStatus* status)
+{
+  if(status[s].locate != PR_NONE)
+    return;
+  const StreamDesc D = sd[s];
+  const uint64_t bt = box.tiles();
+  uint32_t np = 0;
+  uint64_t bytes = 0;
+  status[s].locate = locate_tile_parts_box(cs + D.at, D.len, D.sot, ntiles, box, parts + D.parts0, D.parts_cap, head + s * bt, last + s * bt,
+                                           count + (uint64_t)s * ntiles, &np, body_at ? body_at + D.parts0 : nullptr, &bytes);
+  status[s].nparts = np;
+  status[s].bytes = bytes;
+}
+
+/* step 2, thread g = s * ntiles + t (ntiles: the plan's tiles): tile t's blocks cleared, its PLT packet starts */
+template <class Part>
+B2K_HD void batch_plt(const uint8_t* cs, const StreamDesc* sd, uint64_t g, const PartRange* parts, const uint32_t* head, const Part* tiles,
+                      uint32_t ntiles, const uint64_t* tile_first, uint64_t nblocks, uint64_t np, ParsedBlock* blk, uint64_t* start,
+                      uint64_t* end, uint64_t* part_end, uint32_t* indexed, uint32_t* marked, ParseStatus* status)
+{
+  const StreamItem it = split_stream_item(g, ntiles);
+  const uint32_t s = it.s, t = (uint32_t)it.i;
+  if(status[s].locate != PR_NONE)
+    return;
+  blk += s * nblocks;
+  for(uint64_t i = tile_first[t]; i < tile_first[t + 1]; ++i)
+    blk[i] = ParsedBlock{};
+  const Part T = tiles[t];
+  const uint64_t o = s * np;
+  const bool ix = plt_index(cs + sd[s].at, parts + sd[s].parts0, head[g], T.p1 - T.p0, start + o + T.p0, end + o + T.p0, part_end + o + T.p0);
+  indexed[g] = ix;
+  marked[g] = 0;
+  if(ix && T.p1 > T.p0)
+    status_add(&status[s].indexed, 1u);
+}
+
+/* step 3, thread g = s * np + k: packet k of stream s from its PLT start, when its tile is indexed */
+template <class Packet>
+B2K_HD void batch_packet(const uint8_t* cs, const StreamDesc* sd, uint64_t g, const Packet* packets, uint64_t np, const uint32_t* pkt_tile,
+                         uint32_t ntiles, uint64_t nblocks, uint64_t tag_nodes, const uint32_t* indexed, const uint64_t* start,
+                         const uint64_t* end, const uint64_t* part_end, const uint8_t* kmax, ParsedBlock* blk, TagNode* tags,
+                         uint32_t* marked, bool sop, bool eph, const ParseStatus* status)
+{
+  const StreamItem it = split_stream_item(g, np);
+  const uint32_t s = it.s;
+  if(status[s].locate != PR_NONE)
+    return;
+  const uint64_t t = (uint64_t)s * ntiles + pkt_tile[it.i];
+  if(!indexed[t])
+    return;
+  uint64_t at = start[g];
+  const Packet& P = packets[it.i];
+  if(parse_packet(cs + sd[s].at, P, &at, part_end[g], kmax, blk + s * nblocks, tags + s * tag_nodes + P.tag_at, sop, eph) != PR_NONE ||
+     at != end[g])
+    marked[t] = 1; /* the walk decides */
+}
+
+/* step 4, thread g = s * ntiles + t: the walk of tile t of stream s when it is not indexed or is marked; the lowest failing
+   tile's reason is kept */
+template <class Part, class Packet>
+B2K_HD void batch_walk(const uint8_t* cs, const StreamDesc* sd, uint64_t g, const PartRange* parts, const uint32_t* head, const Part* tiles,
+                       uint32_t ntiles, const Packet* packets, const uint8_t* kmax, const uint64_t* tile_first, uint64_t nblocks,
+                       uint64_t tag_nodes, ParsedBlock* blk, TagNode* tags, const uint32_t* indexed, const uint32_t* marked, bool sop,
+                       bool eph, ParseStatus* status)
+{
+  const StreamItem it = split_stream_item(g, ntiles);
+  const uint32_t s = it.s, t = (uint32_t)it.i;
+  if(status[s].locate != PR_NONE || (indexed[g] && !marked[g]))
+    return;
+  const Part T = tiles[t];
+  if(T.p1 == T.p0)
+    return;
+  blk += s * nblocks;
+  if(marked[g]) /* the packets parsed from PLT may have left fields behind */
+    for(uint64_t i = tile_first[t]; i < tile_first[t + 1]; ++i)
+      blk[i] = ParsedBlock{};
+  if(head[g] != PART_NONE)
+    status_add(&status[s].walked, 1u);
+  const uint32_t r = parse_tile(cs + sd[s].at, parts + sd[s].parts0, head[g], packets + T.p0, T.p1 - T.p0, kmax, blk,
+                                tags + s * tag_nodes + packets[T.p0].tag_at, sop, eph);
+  if(r != PR_NONE)
+    status_min(&status[s].tile_err, ((unsigned long long)t << 8) | r);
+}
+
+/* step 5, thread g = s * ncoded + k: what descriptor g of coded block k (enumeration index coded[k]) of stream s decodes:
+   the parsed block, or an empty one when the stream failed or was not parsed (all-zero coefficients) */
+B2K_HD ParsedBlock batch_block(const ParsedBlock* blk, uint64_t nblocks, const uint32_t* coded, uint64_t g, uint64_t ncoded,
+                               const ParseStatus* status, uint32_t* s_out)
+{
+  const StreamItem it = split_stream_item(g, ncoded);
+  *s_out = it.s;
+  return status_reason(status[it.s]) == PR_NONE ? blk[it.s * nblocks + coded[it.i]] : ParsedBlock{};
 }
 
 /* where stream offset off of a parsed block of the tile whose first part is first lies once the tile parts' packet data

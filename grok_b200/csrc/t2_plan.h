@@ -65,6 +65,11 @@ struct WindowCoding
 /* the main header of cs[0, len), read by b2k_codestream_parse's own code: 0, or its return code with b2k_last_error set */
 int b2k_parse_main_header(const uint8_t* cs, uint64_t len, b2k::t2::MainHeader& h);
 
+/* a batch of code streams (b2k_decode_codestreams_device) takes the coding of stream ref_index, whose main header is ref:
+   0 when stream `index` (main header h) may join it, else 1 with b2k_last_error naming both streams (another b2k_coding, or
+   another progression order, SOP or EPH) */
+int b2k_batch_coding_check(const b2k::t2::MainHeader& ref, uint32_t ref_index, const b2k::t2::MainHeader& h, uint32_t index);
+
 /* the wanted tiles, the virtual coding and the window's need rectangles of b2k_codestream_parse_window(window, reduce) on a
    stream of coding cp: 0, or its return code and text for the window errors, in its order */
 int b2k_window_coding(const b2k_coding& cp, const uint32_t* window, uint32_t reduce, b2k::t2::WindowCoding& w);

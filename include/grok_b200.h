@@ -523,6 +523,31 @@ B2K_API int64_t b2k_encode_codestream_device(b2k_engine* e, const b2k_coding* cp
  * parsed by kernels.  cs is read after the work queued on cuda_stream, which then waits for the image writes. */
 B2K_API int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const b2k_device_planes* img,
                                              void* cuda_stream, b2k_coding* cp_out, double* ms_total);
+/* A batch: n HTJ2K code streams in device memory, all with one coding -> n images in device memory, in one launch chain.
+ * status[i] and b2k_decode_codestreams_error(e, i) are what b2k_decode_codestream_device(e, cs[i], len[i], &imgs[i], ...)
+ * returns alone and its b2k_last_error text: 0, 1, -1 or -2, the checks in the same order (cs[i]'s memory, the main header,
+ * the tile parts and packets, imgs[i], the HT decoder's verdict on stream i's blocks).  Status 0: imgs[i] holds exactly
+ * the single call's pixels; any other status: imgs[i] is not written.
+ * The batch's coding is that of the lowest-index stream whose main header parses (*cp_out receives it); another stream
+ * whose header parses but whose b2k_coding, progression order, SOP or EPH differ gets status 1 with a text naming that
+ * stream.  TLM, PLT, the tile-part layout and COM may differ from stream to stream.
+ * imgs == NULL: headers only -- each stream is checked up to its main header and the coding match, and cp_out and the
+ * statuses are filled from that.  Stream order as b2k_decode_codestream_device: every stream is read after the work queued
+ * on cuda_stream, which then waits for the image writes.
+ * Synchronisations: three per call (headers, parse statuses, end), one more for the streams whose main header runs past
+ * the first few KiB, all together.  For a fixed coding the launch count does not depend on n once n x tiles reaches the
+ * pipeline's chunk count.
+ * Memory: the engine keeps the batch's job (n image-sized int32 plane sets for the transform, besides the arena) for the
+ * next batch of the coding, beside the single-image job; a later batch of more streams, of fewer than a quarter as many,
+ * or of another coding replaces it, and b2k_engine_destroy frees it.
+ * Returns < 0 for a failure of the whole call (NULL arrays, n == 0, imgs whose sample_bytes differ, a CUDA error, more
+ * code blocks than one job indexes), b2k_last_error set; else the number of streams whose status is not 0. */
+B2K_API int32_t b2k_decode_codestreams_device(b2k_engine* e, uint32_t n, const uint8_t* const* cs, const uint64_t* len,
+                                              const b2k_device_planes* imgs, void* cuda_stream, b2k_coding* cp_out,
+                                              int32_t* status, double* ms_total);
+/* the b2k_last_error text of stream i in the last b2k_decode_codestreams_device call on e ("" for status 0); valid until
+   the next such call */
+B2K_API const char* b2k_decode_codestreams_error(b2k_engine* e, uint32_t i);
 /* Stage hook / size query: the block table b2k_codestream_parse would return for the same bytes (offsets into cs),
  * parsed by the device kernels.  blocks = NULL: read the main header only and return the block count (Python's
  * decode_codestream_device makes this call first when it needs the image's shape, so it reads the header twice). */
