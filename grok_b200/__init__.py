@@ -66,7 +66,7 @@ assert BLOCK_DTYPE.itemsize == C.sizeof(Block), (BLOCK_DTYPE.itemsize, C.sizeof(
 # plugin_decompress (C++-ABI callback struct) is declared in csrc/plugin_decode_abi.h, not in the C header
 EXPORTS = ["minpf_post_load_plugin", "plugin_init", "plugin_get_debug_state", "gpup_encode_mem", "gpup_tile_free",
            "b2k_engine_create", "b2k_engine_destroy", "b2k_last_error", "b2k_host_alloc", "b2k_host_free",
-           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_decode_codestream_device", "b2k_decode_codestreams_device", "b2k_decode_codestreams_error", "b2k_codestream_parse_device", "b2k_codestream_parse_device_stats", "b2k_codestream_parse_window_device", "b2k_decode_codestream_window_device", "b2k_codestream_window_device_stats", "b2k_enumerate",
+           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_decode_codestream_device", "b2k_decode_codestreams_device", "b2k_decode_codestreams_error", "b2k_encode_codestreams_device", "b2k_encode_codestreams_error", "b2k_codestream_parse_device", "b2k_codestream_parse_device_stats", "b2k_codestream_parse_window_device", "b2k_decode_codestream_window_device", "b2k_codestream_window_device_stats", "b2k_enumerate",
            "b2k_result_to_gpup_tile", "b2k_job_create", "b2k_job_destroy", "b2k_job_upload", "b2k_job_forward",
            "b2k_job_t1_encode", "b2k_job_t1_decode", "b2k_job_t1_decode_blocks", "b2k_job_inverse", "b2k_job_roundtrip", "b2k_job_roundtrip_n", "b2k_job_roundtrip_pipelined_n", "b2k_job_download",
            "b2k_job_download_coeffs", "b2k_job_upload_coeffs", "b2k_job_fetch_result", "b2k_job_num_blocks",
@@ -654,6 +654,46 @@ class Engine:
             out = torch.empty(n, dtype=torch.uint8, device="cuda:%d" % self.device)
             out.copy_(view)
         return out
+
+    def encode_codestreams_device(self, cp, images, flags=CS_TLM | CS_PLT, layout="CHW", stream=None):
+        """A batch of images on the engine's GPU, all of coding cp -> (streams, status) in one launch chain
+        (b2k_encode_codestreams_device).  images: one CUDA array (n, C, H, W) / (n, H, W, C) in `layout`, or a sequence of
+        n CUDA arrays each as encode_device takes it (device_planes: views such as RGB of RGBA need no copy).  The streams
+        are copied once, on `stream`, into one new torch.uint8 CUDA tensor: streams[i] is a view of it holding exactly
+        the bytes encode_codestream_device(cp, images[i], flags, device_output=True) returns, or None where status[i] is
+        not 0.  status[i] = (rc, text): what that single call returns (0, or the code it would raise with).  Raises only
+        when the call fails as a whole."""
+        import torch
+        n = len(images)
+        if n == 0:
+            raise ValueError("encode_codestreams_device: no images")
+        h, w, nc = cp.y1 - cp.y0, cp.x1 - cp.x0, cp.numcomps
+        imgs = (DevicePlanes * n)(*[device_planes(images[i], nc, h, w, layout) for i in range(n)])
+        handle = _stream_handle(stream, images)
+        L = lib()
+        L.b2k_encode_codestreams_device.argtypes = [C.c_void_p, C.POINTER(Coding), C.c_uint32, C.POINTER(DevicePlanes), C.c_uint32,
+                                                    C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64),
+                                                    C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(C.c_double)]
+        L.b2k_encode_codestreams_error.restype = C.c_char_p
+        L.b2k_encode_codestreams_error.argtypes = [C.c_void_p, C.c_uint32]
+        ptr = C.c_void_p()
+        off = (C.c_uint64 * n)()
+        lens = (C.c_uint64 * n)()
+        st = (C.c_int32 * n)()
+        ms = C.c_double()
+        rc = L.b2k_encode_codestreams_device(self._h, C.byref(cp), n, imgs, flags, handle, C.byref(ptr), off, lens, st, C.byref(ms))
+        if rc < 0:
+            raise EngineError("b2k_encode_codestreams_device: " + (L.b2k_last_error() or b"").decode())
+        status = [(int(st[i]), (L.b2k_encode_codestreams_error(self._h, i) or b"").decode()) for i in range(n)]
+        span = max([int(off[i]) + int(lens[i]) for i in range(n) if st[i] == 0] or [0])
+        dev = "cuda:%d" % self.device
+        s = torch.cuda.ExternalStream(handle, device=self.device) if handle else torch.cuda.default_stream(self.device)
+        with torch.cuda.stream(s):
+            out = torch.empty(span, dtype=torch.uint8, device=dev)
+            if span:
+                out.copy_(torch.as_tensor(_DeviceBytes(ptr.value, span), device=dev))
+        streams = [out[int(off[i]):int(off[i]) + int(lens[i])] if st[i] == 0 else None for i in range(n)]
+        return streams, status
 
     def decode_codestream_device(self, cs, out=None, dtype=None, layout="CHW", window=None, reduce=0, stream=None):
         """HTJ2K codestream -> (Coding, image on the GPU).  window (x0, y0, x1, y1 on the full-resolution canvas) and

@@ -126,6 +126,18 @@ struct BatchDst
 };
 void b2k_launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint32_t spitch, uint32_t sample_bytes, uint32_t w,
                                      uint32_t h, cudaStream_t st);
+/* a batch's images in, one launch: for each of the n entries of the device table d_src (BatchSrc), its nc components
+   (nc > 1: pixel-interleaved, step = nc) from src + y * spitch + x * step + c samples to the int32 plane at
+   dst + c * dplane + y * dpitch + x, w x h pixels, with the sign handling of b2k_launch_container_to_planes.  All share
+   sample_bytes; int32 planes are sample_bytes 4. */
+struct BatchSrc
+{
+  const void* src;
+  int32_t* dst; /* the first component's plane */
+  uint32_t spitch, step;
+};
+void b2k_launch_containers_to_planes(const BatchSrc* d_src, uint32_t n, int nc, uint32_t dpitch, size_t dplane, uint32_t sample_bytes,
+                                     uint32_t w, uint32_t h, int sgnd, cudaStream_t st);
 void b2k_count_launch(void);
 
 /* host_pack.cpp: container conversion on a small host thread pool (int32 planes <-> pinned 16-bit staging) */

@@ -1814,16 +1814,14 @@ struct CPtr4
   const int32_t* p[4];
 };
 
-/* container -> NC int32 planes (b2k_encode16 / b2k_encode16_interleaved after the upload, b2k_encode_device) */
-template <int S, int NC>
-__global__ void __launch_bounds__(128) k_container_to_planes(const void* __restrict__ src, uint32_t spitch, uint32_t step, Ptr4 dst,
-                                                             uint32_t dpitch, uint32_t w, uint32_t h, int sgnd)
+/* container -> NC int32 planes, the rows blockIdx.y + k gridDim.y of the 8 pixels at x8 (b2k_encode16 /
+   b2k_encode16_interleaved after the upload, b2k_encode_device, and each image of a batch) */
+template <int S, int NC, class Dst>
+__device__ __forceinline__ void container_to_planes_rows(const void* __restrict__ src, uint32_t spitch, uint32_t step, const Dst& dst,
+                                                         uint32_t dpitch, uint32_t w, uint32_t h, int sgnd, uint32_t x8)
 {
   typedef typename Sample<S>::U U;
   constexpr int BYTES = 8 * NC * S, V = BYTES % 16 == 0 ? 16 : 8;
-  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
-  if(x8 >= w)
-    return;
   for(uint32_t y = blockIdx.y; y < h; y += gridDim.y)
   {
     const U* s = static_cast<const U*>(src) + (size_t)y * spitch + (size_t)x8 * step;
@@ -1831,7 +1829,7 @@ __global__ void __launch_bounds__(128) k_container_to_planes(const void* __restr
     bool vec = x8 + 8 <= w && step == NC && (reinterpret_cast<uintptr_t>(s) & (V - 1)) == 0;
 #pragma unroll
     for(int c = 0; c < NC; ++c)
-      vec = vec && (reinterpret_cast<uintptr_t>(dst.p[c] + doff) & 15) == 0;
+      vec = vec && (reinterpret_cast<uintptr_t>(dst(c) + doff) & 15) == 0;
     if(vec)
     {
       uint32_t wd[BYTES / 4];
@@ -1846,7 +1844,7 @@ __global__ void __launch_bounds__(128) k_container_to_planes(const void* __restr
           const int e = (i * NC + c) * S; /* byte of the sample within the group */
           v[i] = widen_sample<S>(wd[e >> 2] >> ((e & 3) * 8), sgnd);
         }
-        int4* d = reinterpret_cast<int4*>(dst.p[c] + doff);
+        int4* d = reinterpret_cast<int4*>(dst(c) + doff);
         d[0] = make_int4(v[0], v[1], v[2], v[3]);
         d[1] = make_int4(v[4], v[5], v[6], v[7]);
       }
@@ -1858,9 +1856,32 @@ __global__ void __launch_bounds__(128) k_container_to_planes(const void* __restr
       for(uint32_t i = 0; i < n; ++i)
 #pragma unroll
         for(int c = 0; c < NC; ++c)
-          dst.p[c][doff + i] = widen_sample<S>(s[(size_t)i * step + c], sgnd);
+          dst(c)[doff + i] = widen_sample<S>(s[(size_t)i * step + c], sgnd);
     }
   }
+}
+
+template <int S, int NC>
+__global__ void __launch_bounds__(128) k_container_to_planes(const void* __restrict__ src, uint32_t spitch, uint32_t step, Ptr4 dst,
+                                                             uint32_t dpitch, uint32_t w, uint32_t h, int sgnd)
+{
+  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  if(x8 >= w)
+    return;
+  container_to_planes_rows<S, NC>(src, spitch, step, [&](int c) { return dst.p[c]; }, dpitch, w, h, sgnd, x8);
+}
+
+/* the images of a batch into its planes: image blockIdx.z from its table entry */
+template <int S, int NC>
+__global__ void __launch_bounds__(128) k_containers_to_planes(const BatchSrc* __restrict__ tab, uint32_t dpitch, size_t dplane, uint32_t w,
+                                                              uint32_t h, int sgnd)
+{
+  const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+  const BatchSrc* E = tab + blockIdx.z;
+  if(x8 >= w)
+    return;
+  int32_t* const dst = E->dst;
+  container_to_planes_rows<S, NC>(E->src, E->spitch, E->step, [=](int c) { return dst + c * dplane; }, dpitch, w, h, sgnd, x8);
 }
 
 /* NC int32 planes -> container, the rows blockIdx.y + k gridDim.y of the 8 pixels at x8 (b2k_decode16 before the download,
@@ -2002,13 +2023,19 @@ void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t 
 
 namespace
 {
+/* a batch conversion's grid: the rows of every image, enough CTAs for the GPU without a grid of 65535 x 65535 */
+dim3 batch_grid(uint32_t n, uint32_t w, uint32_t h)
+{
+  dim3 grid = convert_grid(w, h);
+  grid.y = std::min<uint32_t>(grid.y, std::max<uint32_t>(1u, 16384u / std::max(1u, n)));
+  grid.y = std::min<uint32_t>(std::max<uint32_t>(grid.y, 8u), std::max(1u, h));
+  return grid;
+}
+
 template <int S>
 void launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint32_t spitch, uint32_t w, uint32_t h, cudaStream_t st)
 {
-  dim3 grid = convert_grid(w, h);
-  /* the rows of every image: enough CTAs for the GPU without a grid of 65535 x 65535 */
-  grid.y = std::min<uint32_t>(grid.y, std::max<uint32_t>(1u, 16384u / std::max(1u, n)));
-  grid.y = std::min<uint32_t>(std::max<uint32_t>(grid.y, 8u), std::max(1u, h));
+  dim3 grid = batch_grid(n, w, h);
   const dim3 block(128);
   for(uint32_t i0 = 0; i0 < n; i0 += 65535u) /* one launch below 65536 images */
   {
@@ -2019,6 +2046,26 @@ void launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint
       case 2: k_planes_to_containers<S, 2><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
       case 3: k_planes_to_containers<S, 3><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
       default: k_planes_to_containers<S, 4><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
+    }
+    b2k_count_launch();
+  }
+}
+
+template <int S>
+void launch_containers_to_planes(const BatchSrc* d_src, uint32_t n, int nc, uint32_t dpitch, size_t dplane, uint32_t w, uint32_t h,
+                                 int sgnd, cudaStream_t st)
+{
+  dim3 grid = batch_grid(n, w, h);
+  const dim3 block(128);
+  for(uint32_t i0 = 0; i0 < n; i0 += 65535u)
+  {
+    grid.z = std::min<uint32_t>(n - i0, 65535u);
+    switch(nc)
+    {
+      case 1: k_containers_to_planes<S, 1><<<grid, block, 0, st>>>(d_src + i0, dpitch, dplane, w, h, sgnd); break;
+      case 2: k_containers_to_planes<S, 2><<<grid, block, 0, st>>>(d_src + i0, dpitch, dplane, w, h, sgnd); break;
+      case 3: k_containers_to_planes<S, 3><<<grid, block, 0, st>>>(d_src + i0, dpitch, dplane, w, h, sgnd); break;
+      default: k_containers_to_planes<S, 4><<<grid, block, 0, st>>>(d_src + i0, dpitch, dplane, w, h, sgnd); break;
     }
     b2k_count_launch();
   }
@@ -2035,6 +2082,19 @@ void b2k_launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, 
     case 1: launch_planes_to_containers<1>(d_dst, n, nc, spitch, w, h, st); break;
     case 2: launch_planes_to_containers<2>(d_dst, n, nc, spitch, w, h, st); break;
     default: launch_planes_to_containers<4>(d_dst, n, nc, spitch, w, h, st); break;
+  }
+}
+
+void b2k_launch_containers_to_planes(const BatchSrc* d_src, uint32_t n, int nc, uint32_t dpitch, size_t dplane, uint32_t sample_bytes,
+                                     uint32_t w, uint32_t h, int sgnd, cudaStream_t st)
+{
+  if(!n || !w || !h)
+    return;
+  switch(sample_bytes)
+  {
+    case 1: launch_containers_to_planes<1>(d_src, n, nc, dpitch, dplane, w, h, sgnd, st); break;
+    case 2: launch_containers_to_planes<2>(d_src, n, nc, dpitch, dplane, w, h, sgnd, st); break;
+    default: launch_containers_to_planes<4>(d_src, n, nc, dpitch, dplane, w, h, sgnd, st); break;
   }
 }
 

@@ -83,6 +83,11 @@ struct b2k_engine
   uint8_t* d_hdr = nullptr;        /* the header prefixes, end to end */
   uint8_t* h_hdr = nullptr;        /* pinned */
   uint64_t hdr_cap = 0;
+  /* b2k_encode_codestreams_device: the code streams of the last call (not d_cs: a batch leaves the single call's stream
+     alone) and each image's text */
+  uint8_t* d_bcs = nullptr;
+  uint64_t bcs_cap = 0;
+  std::vector<std::string> enc_batch_errors;
 };
 
 /* ---- device memory cache --------------------------------------------------------------------------------------
@@ -355,6 +360,8 @@ struct b2k_device_job
   std::vector<uint32_t> tile_slot;
   BatchDst* d_batch_dst = nullptr; /* the conversion's table: per component (or one for interleaved images), per slot */
   BatchDst* h_batch_dst = nullptr; /* pinned */
+  BatchSrc* d_batch_src = nullptr; /* b2k_encode_codestreams_device's conversion table, laid out likewise */
+  BatchSrc* h_batch_src = nullptr; /* pinned */
   std::vector<BandQuant> quant;
   std::vector<b2k_block> blocks;       /* every block, enumeration order */
   std::vector<uint32_t> coded_index;   /* blocks with area, index into `blocks` */
@@ -477,6 +484,7 @@ extern "C" void b2k_engine_destroy(b2k_engine* e)
   if(e->caller_ev)
     cudaEventDestroy(e->caller_ev);
   cudaFree(e->d_cs);
+  cudaFree(e->d_bcs);
   delete e;
 }
 
@@ -922,6 +930,8 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
   cudaFree(J->d_err);
   cudaFree(J->d_batch_dst);
   cudaFreeHost(J->h_batch_dst);
+  cudaFree(J->d_batch_src);
+  cudaFreeHost(J->h_batch_src);
   cudaFreeHost(J->h_out);
   cudaFreeHost(J->h_dec_desc);
   cudaFreeHost(J->h_offsets);
@@ -3267,4 +3277,174 @@ extern "C" const char* b2k_decode_codestreams_error(b2k_engine* e, uint32_t i)
     return "";
   std::lock_guard<std::mutex> lock(e->mu);
   return i < e->batch_errors.size() ? e->batch_errors[i].c_str() : "";
+}
+
+/* ---- batches of images in device memory (b2k_encode_codestreams_device) ---------------------------------------------
+ * n images of one coding become n code streams in one launch chain.  The images that pass their checks take slots
+ * 0..m-1 of the batch job, in image order; chunk by chunk over the (slot, tile) ranges, one conversion launch per
+ * component group brings the images whose first tile the chunk holds into their planes, then the forward transform and
+ * the block coder run over the chunk.  The device writer (t2_device.cu) then writes the m streams behind each other.
+ * A failed image takes no slot, so none of its samples is coded.  A stream the coder or the writer gives a verdict is
+ * neither placed nor gathered, and the other streams' places depend only on their own lengths: no image can change
+ * another stream's bytes.  Synchronisations: one, and a second when the output buffer has to grow. */
+extern "C" int32_t b2k_encode_codestreams_device(b2k_engine* e, const b2k_coding* cp, uint32_t n, const b2k_device_planes* imgs,
+                                                 uint32_t flags, void* cuda_stream, const uint8_t** cs, uint64_t* offset,
+                                                 uint64_t* length, int32_t* status, double* ms_total)
+{
+  if(!e || !cp || !imgs || !cs || !offset || !length || !status)
+  {
+    g_err = "b2k_encode_codestreams_device: NULL argument";
+    return -1;
+  }
+  if(n == 0)
+  {
+    g_err = "b2k_encode_codestreams_device: no images";
+    return -1;
+  }
+  for(uint32_t i = 1; i < n; ++i)
+    if(imgs[i].sample_bytes != imgs[0].sample_bytes)
+    {
+      g_err = "b2k_encode_codestreams_device: the images' sample_bytes differ";
+      return -1;
+    }
+  std::lock_guard<std::mutex> lock(e->mu);
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t caller = caller_stream(cuda_stream), st = e->stream;
+  e->enc_batch_errors.assign(n, std::string());
+  *cs = nullptr;
+  auto fail = [&](uint32_t i, int32_t rc) {
+    status[i] = rc;
+    e->enc_batch_errors[i] = g_err;
+  };
+  auto failures = [&] {
+    int32_t f = 0;
+    for(uint32_t i = 0; i < n; ++i)
+      f += status[i] != 0;
+    return f;
+  };
+  /* each image's descriptor, as the single call checks it first; the images that pass take the slots in order */
+  std::vector<uint32_t> image_of;
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    status[i] = 0;
+    offset[i] = length[i] = 0;
+    if(int rc = check_device_planes(e, cp, &imgs[i]))
+      fail(i, rc);
+    else
+      image_of.push_back(i);
+  }
+  const uint32_t m = (uint32_t)image_of.size();
+  if(!m)
+    return failures();
+  /* a verdict of the coding or the flags alone is every remaining image's, as in the single call */
+  auto fail_all = [&](int32_t rc) {
+    for(uint32_t i : image_of)
+      fail(i, rc);
+    return failures();
+  };
+  int jrc = 0;
+  b2k_device_job* J = cached_batch_job(e, *cp, m, &jrc);
+  if(jrc < 0)
+    return -1;
+  if(jrc)
+    return fail_all(jrc);
+  if(!J->t2 || b2k_t2_flags(J->t2) != flags || b2k_t2_streams(J->t2) != J->slots)
+  { /* geometry and flags only: planned once for every batch of this coding */
+    b2k_t2_destroy(J->t2);
+    J->t2 = nullptr;
+    const int trc = b2k_t2_create(*cp, flags, J->blocks.data(), J->blocks.size(), J->slot_tiles, J->coded_index.data(),
+                                  J->coded_index.size(), &J->t2, J->slots);
+    if(trc < 0)
+      return -1;
+    if(trc)
+      return fail_all(-1);
+  }
+  /* the conversion's tables: one per component, or one for all when every image is pixel-interleaved */
+  const int nc = cp->numcomps;
+  bool interleaved = nc > 1;
+  for(uint32_t i : image_of)
+    interleaved = interleaved && device_group(imgs[i], nc) == nc;
+  const int group = interleaved ? nc : 1, tables = nc / group;
+  if(!J->h_batch_src)
+  {
+    CUDA_TRY(cudaMalloc(&J->d_batch_src, (size_t)J->slots * 4 * sizeof(BatchSrc)));
+    CUDA_TRY(cudaHostAlloc(&J->h_batch_src, (size_t)J->slots * 4 * sizeof(BatchSrc), cudaHostAllocDefault));
+  }
+  for(int t = 0; t < tables; ++t)
+    for(uint32_t s = 0; s < m; ++s)
+    {
+      const b2k_device_planes& img = imgs[image_of[s]];
+      const int c0 = t * group;
+      BatchSrc& E = J->h_batch_src[(size_t)t * m + s];
+      E = BatchSrc{};
+      E.src = img.comp[c0];
+      E.spitch = img.row_pitch[c0];
+      E.step = img.col_step[c0];
+      E.dst = J->img.at((int)s * nc + c0, cp->x0, cp->y0);
+    }
+  /* what the caller queued before the call (the kernels that made the images) comes first */
+  if(queue_after(e, caller, st)) return -1;
+  CUDA_TRY(cudaEventRecord(J->ev[0], st));
+  CUDA_TRY(cudaMemcpyAsync(J->d_batch_src, J->h_batch_src, (size_t)tables * m * sizeof(BatchSrc), cudaMemcpyHostToDevice, st));
+  /* conversion -> forward transform -> block coder, chunk by chunk over the (slot, tile) ranges of the m slots used (as
+     many chunks as the job's pipeline has, whatever its slot count); an image is converted in the chunk of its first tile */
+  const size_t T = J->slot_tiles, used = (size_t)m * T;
+  const size_t nchunks = std::min<size_t>(J->chunk_tile.size() - 1, used);
+  const uint32_t w = cp->x1 - cp->x0, hgt = cp->y1 - cp->y0, sb = imgs[image_of[0]].sample_bytes;
+  for(size_t k = 0; k < nchunks; ++k)
+  {
+    const size_t t0 = k * used / nchunks, t1 = (k + 1) * used / nchunks;
+    if(t1 <= t0)
+      continue;
+    const uint32_t s0 = (uint32_t)((t0 + T - 1) / T), s1 = (uint32_t)((t1 + T - 1) / T);
+    for(int t = 0; t < tables && s1 > s0; ++t)
+      b2k_launch_containers_to_planes(J->d_batch_src + (size_t)t * m + s0, s1 - s0, group, J->img.pitch, J->img.plane_elems(), sb, w,
+                                      hgt, cp->sgnd, st);
+    if(enqueue_forward(J, st, false, t0, t1)) return -1;
+    if(enqueue_t1_blocks(J, st, t0, t1)) return -1;
+  }
+  CUDA_TRY(cudaGetLastError());
+  /* the caller's stream goes on once every image has been read */
+  if(queue_after(e, st, caller)) return -1;
+  /* the m code streams into the batch's buffer; the call's one synchronisation reads their statuses and places */
+  for(;;)
+  {
+    if(b2k_t2_enqueue(J->t2, J->d_enc_desc, J->d_out, J->d_scratch, e->d_bcs, e->bcs_cap, st, m))
+      return -1;
+    CUDA_TRY(cudaEventRecord(J->ev[1], st));
+    CUDA_TRY(cudaEventSynchronize(J->ev[1]));
+    const uint64_t need = b2k_t2_used(J->t2);
+    if(need <= e->bcs_cap)
+      break;
+    cudaFree(e->d_bcs);
+    e->d_bcs = nullptr;
+    e->bcs_cap = 0;
+    CUDA_TRY(cudaMalloc(&e->d_bcs, need + need / 8 + 4096));
+    e->bcs_cap = need + need / 8 + 4096;
+  }
+  float t = 0;
+  cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
+  if(ms_total) *ms_total = t;
+  for(uint32_t s = 0; s < m; ++s)
+  {
+    const uint32_t i = image_of[s];
+    const int64_t r = b2k_t2_result(J->t2, s);
+    if(r < 0)
+      fail(i, (int32_t)r);
+    else
+    {
+      offset[i] = b2k_t2_offset(J->t2, s);
+      length[i] = (uint64_t)r;
+    }
+  }
+  *cs = e->d_bcs;
+  return failures();
+}
+
+extern "C" const char* b2k_encode_codestreams_error(b2k_engine* e, uint32_t i)
+{
+  if(!e)
+    return "";
+  std::lock_guard<std::mutex> lock(e->mu);
+  return i < e->enc_batch_errors.size() ? e->enc_batch_errors[i].c_str() : "";
 }

@@ -1,20 +1,24 @@
 /*
  * grok_b200/csrc/t2_device.cu -- T2 on the device: the block coder's output (per-block lengths, bytes in the encoder's
- * scratch slots) becomes a complete code stream in device memory, byte-identical to b2k_codestream_write's.
+ * scratch slots) becomes n complete code streams in device memory, each byte-identical to b2k_codestream_write's.
  *
  * With one quality layer every packet is independent: its header depends on its own blocks alone.  The plan (t2_plan.h)
- * fixes everything geometry decides; per frame six launches, however many tiles:
- *   1. k_t2_headers  a thread per packet: SOP, header bits (t2_packet.h, shared with the host writer), EPH into the
- *                    packet's slot of the header scratch; header and body lengths; each block's place in the body
- *   2. k_t2_parts    a thread per tile part: PLT size and tile-part length
- *   3. k_t2_scan     one CTA: tile-part offsets, the code-stream length; main header and EOC
- *   4. k_t2_emit     a thread per tile part: SOT, PLT, SOD, TLM entry, every packet's offset
- *   5. k_t2_packets  a warp per packet: its header to its place; its blocks' absolute offsets
- *   6. the encoder's gather (ht_enc.cu): each block's bytes straight from its scratch slot to its place in the file
+ * fixes everything geometry decides and is shared by the n streams of a batch; per call six launches, however many
+ * tiles and streams.  The threads' work is t2_write.h's:
+ *   1. k_t2_headers  a thread per (stream, packet): SOP, header bits (t2_packet.h, shared with the host writer), EPH into
+ *                    the packet's slot of the stream's header scratch; header and body lengths; each block's place in the
+ *                    body; the stream's verdict (overflowed blocks, writer limits)
+ *   2. k_t2_parts    a thread per (stream, tile part): PLT size and tile-part length
+ *   3. k_t2_scan     a CTA per stream: tile-part offsets and the stream's length (0 with a verdict); the last CTA places
+ *                    the streams behind each other at 256-byte boundaries
+ *   4. k_t2_emit     a thread per (stream, tile part): SOT, PLT, SOD, TLM entry, every packet's offset; the main header
+ *                    and EOC in pieces shared out over the stream's parts
+ *   5. k_t2_packets  a warp per (stream, packet): its header to its place; its blocks' absolute offsets
+ *   6. the encoder's gather (ht_enc.cu): each block's bytes straight from its scratch slot to its place in the output
  * A thread per packet: a header is a sequential bit string with tag-tree state, and packets outnumber the threads one
  * packet's blocks could keep busy (config 2: 1152 packets of at most 192 blocks).
- * Kernels 3-6 write only when the code stream fits the caller's buffer; otherwise the caller grows it and runs them all
- * again from the same scratch slots.
+ * Kernels 3-6 write only when the streams fit the caller's buffer; otherwise the caller grows it and runs them all
+ * again from the same scratch slots.  A single code stream is the batch of one.
  */
 #include <algorithm>
 #include <cstring>
@@ -24,6 +28,7 @@
 #include "t2_packet.h"
 #include "t2_plan.h"
 #include "t2_device.h"
+#include "t2_write.h"
 
 using namespace b2k;
 using namespace b2k::t2;
@@ -32,109 +37,45 @@ void b2k_set_error(const char* msg); /* engine.cu */
 
 namespace
 {
-enum : uint32_t
-{
-  ERR_RANGE = 1,      /* a block outside the writer's range */
-  ERR_PACKET = 2,     /* a packet of 4 GiB or more */
-  ERR_PART = 4,       /* a tile part of 4 GiB or more */
-  ERR_HDR_BOUND = 8,  /* a header longer than its bound */
-};
+/* threads over n streams of `per` items: g = s * per + i */
+__device__ __forceinline__ uint64_t thread_item() { return (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; }
 
-__global__ void k_t2_headers(const DevPacket* __restrict__ packets, uint64_t np, const int32_t* __restrict__ coded,
-                             const uint8_t* __restrict__ kmax, const HtBlockOut* __restrict__ outs, uint8_t* __restrict__ hdr,
-                             TagNode* __restrict__ tags, uint32_t* __restrict__ hdr_len, uint64_t* __restrict__ body_len,
-                             uint64_t* __restrict__ dst, T2Status* status, bool sop, bool eph)
+__global__ void k_t2_headers(const DevPacket* __restrict__ packets, uint64_t np, uint64_t items, const int32_t* __restrict__ coded,
+                             const uint8_t* __restrict__ kmax, uint64_t ncoded, const HtBlockOut* __restrict__ outs,
+                             uint8_t* __restrict__ hdr, uint64_t hdr_bytes, TagNode* __restrict__ tags, uint64_t tag_nodes,
+                             uint32_t* __restrict__ hdr_len, uint64_t* __restrict__ body_len, uint64_t* __restrict__ dst,
+                             WriteStatus* status, bool sop, bool eph)
 {
-  const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if(p >= np)
-    return;
-  const DevPacket P = packets[p];
-  /* a coded block as b2k_encode reports it: one pass, one bit plane (CoderOJPH), length = the coder's total */
-  auto code = [&](uint32_t i) {
-    const int32_t c = coded[i];
-    uint32_t len = c >= 0 ? outs[c].total : 0u;
-    len = len == 0xFFFFFFFFu ? 0u : len;
-    return BlockCode{len, 0u, (uint8_t)(c >= 0 ? 1 : 0), 1, kmax[i]};
-  };
-  BitWriter bw;
-  bw.init(hdr + P.hdr_at, P.hdr_cap);
-  uint32_t err = 0;
-  if(packet_header(bw, P.band, (int)P.nbands, code, tags + P.tag_at, P.sop, sop, eph))
-    err |= ERR_RANGE;
-  if(bw.n > bw.cap)
-    err |= ERR_HDR_BOUND;
-  uint64_t rel = 0;
-  uint32_t bad = 0;
-  for(uint32_t b = 0; b < P.nbands; ++b)
-  {
-    const uint32_t n = P.band[b].gw * P.band[b].gh;
-    for(uint32_t k = 0; k < n; ++k)
-    {
-      const int32_t c = coded[P.band[b].first + k];
-      if(c < 0)
-        continue;
-      const uint32_t t = outs[c].total;
-      if(t == 0xFFFFFFFFu)
-      {
-        ++bad;
-        continue;
-      }
-      dst[c] = rel; /* relative to the body; k_t2_packets adds the body's offset */
-      rel += t;
-    }
-  }
-  if(bw.n + rel > 0xFFFFFFFFull)
-    err |= ERR_PACKET;
-  hdr_len[p] = (uint32_t)bw.n;
-  body_len[p] = rel;
-  if(bad)
-    atomicAdd(&status->bad_blocks, bad);
-  if(err)
-    atomicOr(&status->errors, err);
+  const uint64_t g = thread_item();
+  if(g < items)
+    write_header(g, packets, np, coded, kmax, ncoded, outs, hdr, hdr_bytes, tags, tag_nodes, hdr_len, body_len, dst, status, sop, eph);
 }
 
-struct PacketLen
+__global__ void k_t2_parts(const DevPart* __restrict__ parts, uint64_t nparts, uint64_t items, uint64_t np,
+                           const uint32_t* __restrict__ hdr_len, const uint64_t* __restrict__ body_len, uint64_t* __restrict__ part_plt,
+                           uint64_t* __restrict__ part_bytes, WriteStatus* status, bool plt)
 {
-  const uint32_t* hdr_len;
-  const uint64_t* body_len;
-  __device__ uint32_t operator()(uint64_t k) const { return (uint32_t)(hdr_len[k] + body_len[k]); }
-};
-
-__global__ void k_t2_parts(const DevPart* __restrict__ parts, uint64_t nparts, const uint32_t* __restrict__ hdr_len,
-                           const uint64_t* __restrict__ body_len, uint64_t* __restrict__ part_plt, uint64_t* __restrict__ part_bytes,
-                           T2Status* status, bool plt)
-{
-  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if(t >= nparts)
-    return;
-  const DevPart D = parts[t];
-  uint64_t body = 0;
-  for(uint64_t k = D.p0; k < D.p1; ++k)
-    body += hdr_len[k] + body_len[k];
-  const uint64_t pl = plt ? plt_segments(PacketLen{hdr_len, body_len}, D.p0, D.p1, nullptr) : 0;
-  const uint64_t bytes = 12 + pl + 2 + body;
-  part_plt[t] = pl;
-  part_bytes[t] = bytes;
-  if(bytes > 0xFFFFFFFFull)
-    atomicOr(&status->errors, (uint32_t)ERR_PART);
+  const uint64_t g = thread_item();
+  if(g < items)
+    write_part(g, parts, nparts, np, hdr_len, body_len, part_plt, part_bytes, status, plt);
 }
 
-/* exclusive scan of the tile-part lengths behind the main header; then, if the code stream fits, the main header and EOC */
+/* exclusive scan over count values of one CTA, in rounds of SCAN_THREADS, starting from carry: out(i, prefix); returns the
+   sum of everything (carry included).  Every thread of the CTA calls it. */
 constexpr int SCAN_THREADS = 1024;
-__global__ void __launch_bounds__(SCAN_THREADS) k_t2_scan(const uint64_t* __restrict__ part_bytes, uint64_t nparts,
-                                                          uint64_t* __restrict__ part_at, const uint8_t* __restrict__ head,
-                                                          uint64_t head_len, uint8_t* __restrict__ cs, uint64_t cap, T2Status* status)
+template <class Val, class Out>
+__device__ uint64_t cta_scan(uint64_t count, uint64_t carry, const Val& val, const Out& out)
 {
   __shared__ uint64_t warp_sum[32];
   __shared__ uint64_t carry_s;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if(threadIdx.x == 0)
-    carry_s = head_len;
+    carry_s = carry;
   __syncthreads();
-  for(uint64_t base = 0; base < nparts; base += SCAN_THREADS)
+  for(uint64_t base = 0; base < count; base += SCAN_THREADS)
   {
     const uint64_t i = base + threadIdx.x;
-    const uint64_t v = i < nparts ? part_bytes[i] : 0;
+    const uint64_t v = i < count ? val(i) : 0;
     uint64_t incl = v;
 #pragma unroll
     for(int o = 1; o < 32; o <<= 1)
@@ -145,7 +86,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_t2_scan(const uint64_t* __rest
     }
     if(lane == 31)
       warp_sum[warp] = incl;
-    const uint64_t carry = carry_s;
+    const uint64_t c = carry_s;
     __syncthreads();
     if(warp == 0)
     {
@@ -160,78 +101,81 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_t2_scan(const uint64_t* __rest
       }
       warp_sum[lane] = wi - w;
       if(lane == 31)
-        carry_s = carry + wi;
+        carry_s = c + wi;
     }
     __syncthreads();
-    if(i < nparts)
-      part_at[i] = carry + warp_sum[warp] + incl - v;
+    if(i < count)
+      out(i, c + warp_sum[warp] + incl - v);
     __syncthreads();
   }
-  const uint64_t total = carry_s + 2;
-  if(threadIdx.x == 0)
-    status->total = total;
-  if(total > cap)
-    return;
-  for(uint64_t i = threadIdx.x; i < head_len; i += SCAN_THREADS)
-    cs[i] = head[i];
-  if(threadIdx.x == 0)
-  {
-    cs[total - 2] = 0xFF; /* EOC */
-    cs[total - 1] = 0xD9;
-  }
+  const uint64_t total = carry_s;
+  __syncthreads(); /* every thread has read carry_s before the next call sets it */
+  return total;
 }
 
-__global__ void k_t2_emit(const DevPart* __restrict__ parts, uint64_t nparts, const uint64_t* __restrict__ part_at,
+/* a CTA per stream: the stream's tile-part offsets behind the main header and its total (write_total).  The last CTA to
+   finish places the streams behind each other (WriteStatus::at, WritePlace::used).  write_scan_host is the same for the
+   host. */
+__global__ void __launch_bounds__(SCAN_THREADS) k_t2_scan(const uint64_t* __restrict__ part_bytes, uint64_t nparts, uint32_t n,
+                                                          uint64_t* __restrict__ part_at, uint64_t head_len, WriteStatus* status,
+                                                          WritePlace* place)
+{
+  __shared__ bool last;
+  __shared__ unsigned long long used_s;
+  for(uint32_t s = blockIdx.x; s < n; s += gridDim.x)
+  {
+    const uint64_t o = (uint64_t)s * nparts;
+    const uint64_t end = cta_scan(
+        nparts, head_len, [&](uint64_t i) { return part_bytes[o + i]; }, [&](uint64_t i, uint64_t x) { part_at[o + i] = x; });
+    if(threadIdx.x == 0)
+      status[s].total = write_total(status[s], end);
+  }
+  __threadfence();
+  __syncthreads();
+  if(threadIdx.x == 0)
+  {
+    last = atomicAdd(&place->done, 1u) == gridDim.x - 1;
+    used_s = 0;
+  }
+  __syncthreads();
+  if(!last)
+    return;
+  __threadfence();
+  /* the streams behind each other, each at a 256-byte boundary; another CTA's totals are read through L2.  The bytes
+     used end where the last stream with a length ends: the largest at + total, offsets growing with s */
+  const volatile WriteStatus* vs = status;
+  cta_scan(
+      n, 0, [&](uint64_t s) { const uint64_t t = vs[s].total; return t ? batch_arena_next(0, t) : 0; },
+      [&](uint64_t s, uint64_t x) {
+        status[s].at = x;
+        if(const uint64_t t = vs[s].total)
+          atomicMax(&used_s, (unsigned long long)(x + t));
+      });
+  if(threadIdx.x == 0)
+    place->used = used_s;
+}
+
+__global__ void k_t2_emit(const DevPart* __restrict__ parts, uint64_t nparts, uint64_t items, uint64_t np, const uint64_t* __restrict__ part_at,
                           const uint64_t* __restrict__ part_plt, const uint64_t* __restrict__ part_bytes,
                           const uint32_t* __restrict__ hdr_len, const uint64_t* __restrict__ body_len, uint64_t* __restrict__ pkt_at,
-                          uint8_t* __restrict__ cs, uint64_t cap, const T2Status* status, bool plt, bool tlm, uint64_t tlm_at)
+                          uint8_t* __restrict__ cs, uint64_t cap, const WriteStatus* status, const WritePlace* place,
+                          const uint8_t* __restrict__ head, uint64_t head_len, bool plt, bool tlm, uint64_t tlm_at)
 {
-  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if(t >= nparts || status->total > cap)
-    return;
-  const DevPart D = parts[t];
-  uint8_t* w = cs + part_at[t];
-  put_sot(w, D.tile, (uint32_t)part_bytes[t], D.index, D.count);
-  w += 12;
-  if(plt)
-    plt_segments(PacketLen{hdr_len, body_len}, D.p0, D.p1, w);
-  w += part_plt[t];
-  w[0] = 0xFF; /* SOD */
-  w[1] = 0x93;
-  uint64_t at = part_at[t] + 12 + part_plt[t] + 2;
-  for(uint64_t k = D.p0; k < D.p1; ++k)
-  {
-    pkt_at[k] = at;
-    at += hdr_len[k] + body_len[k];
-  }
-  if(tlm)
-    put_tlm_entry(cs + tlm_at, t, D.tile, (uint32_t)part_bytes[t]);
+  const uint64_t g = thread_item();
+  if(g < items)
+    write_emit(g, parts, nparts, np, part_at, part_plt, part_bytes, hdr_len, body_len, pkt_at, cs, cap, status, place, head, head_len, plt,
+               tlm, tlm_at);
 }
 
-__global__ void k_t2_packets(const DevPacket* __restrict__ packets, uint64_t np, const int32_t* __restrict__ coded,
-                             const HtBlockOut* __restrict__ outs, const uint8_t* __restrict__ hdr, const uint32_t* __restrict__ hdr_len,
-                             const uint64_t* __restrict__ pkt_at, uint64_t* __restrict__ dst, uint8_t* __restrict__ cs, uint64_t cap,
-                             const T2Status* status)
+/* a warp per packet */
+__global__ void k_t2_packets(const DevPacket* __restrict__ packets, uint64_t np, uint64_t items, const int32_t* __restrict__ coded,
+                             uint64_t ncoded, const HtBlockOut* __restrict__ outs, const uint8_t* __restrict__ hdr, uint64_t hdr_bytes,
+                             const uint32_t* __restrict__ hdr_len, const uint64_t* __restrict__ pkt_at, uint64_t* __restrict__ dst,
+                             uint8_t* __restrict__ cs, uint64_t cap, const WriteStatus* status, const WritePlace* place)
 {
-  const uint64_t p = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const uint32_t lane = threadIdx.x & 31;
-  if(p >= np || status->total > cap)
-    return;
-  const DevPacket P = packets[p];
-  const uint64_t at = pkt_at[p];
-  const uint32_t hn = hdr_len[p];
-  for(uint32_t i = lane; i < hn; i += 32)
-    cs[at + i] = hdr[P.hdr_at + i];
-  for(uint32_t b = 0; b < P.nbands; ++b)
-  {
-    const uint32_t n = P.band[b].gw * P.band[b].gh;
-    for(uint32_t k = lane; k < n; k += 32)
-    {
-      const int32_t c = coded[P.band[b].first + k];
-      if(c >= 0 && outs[c].total != 0xFFFFFFFFu)
-        dst[c] += at + hn;
-    }
-  }
+  const uint64_t g = thread_item() >> 5;
+  if(g < items)
+    write_packet(g, threadIdx.x & 31, 32, packets, np, coded, ncoded, outs, hdr, hdr_bytes, hdr_len, pkt_at, dst, cs, cap, status, place);
 }
 
 template <class T>
@@ -247,6 +191,7 @@ struct T2Job
 {
   Plan plan;
   uint64_t ncoded = 0;
+  uint32_t streams = 1;
   uint8_t* d_mem = nullptr;
   DevPacket* d_packets = nullptr;
   DevPart* d_parts = nullptr;
@@ -257,8 +202,11 @@ struct T2Job
   TagNode* d_tags = nullptr;
   uint32_t* d_hdr_len = nullptr;
   uint64_t *d_body_len = nullptr, *d_pkt_at = nullptr, *d_part_plt = nullptr, *d_part_bytes = nullptr, *d_part_at = nullptr, *d_dst = nullptr;
-  T2Status* d_status = nullptr;
-  T2Status* h_status = nullptr; /* pinned */
+  /* the streams' statuses and the batch's placement, side by side so that one copy brings them home */
+  WriteStatus* d_status = nullptr;
+  WritePlace* d_place = nullptr;
+  WriteStatus* h_status = nullptr; /* pinned, likewise followed by the placement */
+  WritePlace* h_place = nullptr;
 };
 
 #define T2_TRY(expr)                                                                                                           \
@@ -273,7 +221,7 @@ struct T2Job
   } while(0)
 
 int b2k_t2_create(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks, uint64_t nblocks, uint32_t num_tiles,
-                  const uint32_t* coded_index, uint64_t ncoded, T2Job** out)
+                  const uint32_t* coded_index, uint64_t ncoded, T2Job** out, uint32_t streams)
 {
   *out = nullptr;
   T2Job* J = new T2Job();
@@ -283,21 +231,23 @@ int b2k_t2_create(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks,
     ~Guard() { b2k_t2_destroy(j); }
   } guard{J};
   if(b2k_t2_plan(cp, flags, blocks, nblocks, num_tiles, J->plan))
-    return -1;
+    return 1;
   const Plan& P = J->plan;
   J->ncoded = ncoded;
+  J->streams = streams;
   std::vector<int32_t> coded(nblocks, -1);
   std::vector<uint8_t> kmax(nblocks);
   for(uint64_t k = 0; k < ncoded; ++k)
     coded[coded_index[k]] = (int32_t)k;
   for(uint64_t i = 0; i < nblocks; ++i)
     kmax[i] = blocks[i].kmax;
-  const uint64_t np = P.packets.size(), nparts = P.parts.size();
+  const uint64_t np = P.packets.size(), nparts = P.parts.size(), S = streams;
+  const uint64_t status_bytes = S * sizeof(WriteStatus) + sizeof(WritePlace);
   auto bytes = [](uint64_t n, size_t sz) { return (n * sz + 255) & ~(uint64_t)255; };
   const uint64_t total = bytes(np, sizeof(DevPacket)) + bytes(nparts, sizeof(DevPart)) + bytes(P.head.size(), 1) +
-                         bytes(nblocks, sizeof(int32_t)) + bytes(nblocks, 1) + bytes(P.hdr_bytes, 1) + bytes(P.tag_nodes, sizeof(TagNode)) +
-                         bytes(np, sizeof(uint32_t)) + 2 * bytes(np, sizeof(uint64_t)) + 3 * bytes(nparts, sizeof(uint64_t)) +
-                         bytes(ncoded, sizeof(uint64_t)) + bytes(1, sizeof(T2Status));
+                         bytes(nblocks, sizeof(int32_t)) + bytes(nblocks, 1) + bytes(S * P.hdr_bytes, 1) +
+                         bytes(S * P.tag_nodes, sizeof(TagNode)) + bytes(S * np, sizeof(uint32_t)) + 2 * bytes(S * np, sizeof(uint64_t)) +
+                         3 * bytes(S * nparts, sizeof(uint64_t)) + bytes(S * ncoded, sizeof(uint64_t)) + bytes(status_bytes, 1);
   T2_TRY(cudaMalloc(&J->d_mem, total));
   uint8_t* p = J->d_mem;
   J->d_packets = carve<DevPacket>(p, np);
@@ -305,22 +255,24 @@ int b2k_t2_create(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks,
   J->d_head = carve<uint8_t>(p, P.head.size());
   J->d_coded = carve<int32_t>(p, nblocks);
   J->d_kmax = carve<uint8_t>(p, nblocks);
-  J->d_hdr = carve<uint8_t>(p, P.hdr_bytes);
-  J->d_tags = carve<TagNode>(p, P.tag_nodes);
-  J->d_hdr_len = carve<uint32_t>(p, np);
-  J->d_body_len = carve<uint64_t>(p, np);
-  J->d_pkt_at = carve<uint64_t>(p, np);
-  J->d_part_plt = carve<uint64_t>(p, nparts);
-  J->d_part_bytes = carve<uint64_t>(p, nparts);
-  J->d_part_at = carve<uint64_t>(p, nparts);
-  J->d_dst = carve<uint64_t>(p, ncoded);
-  J->d_status = carve<T2Status>(p, 1);
+  J->d_hdr = carve<uint8_t>(p, S * P.hdr_bytes);
+  J->d_tags = carve<TagNode>(p, S * P.tag_nodes);
+  J->d_hdr_len = carve<uint32_t>(p, S * np);
+  J->d_body_len = carve<uint64_t>(p, S * np);
+  J->d_pkt_at = carve<uint64_t>(p, S * np);
+  J->d_part_plt = carve<uint64_t>(p, S * nparts);
+  J->d_part_bytes = carve<uint64_t>(p, S * nparts);
+  J->d_part_at = carve<uint64_t>(p, S * nparts);
+  J->d_dst = carve<uint64_t>(p, S * ncoded);
+  J->d_status = reinterpret_cast<WriteStatus*>(carve<uint8_t>(p, status_bytes));
+  J->d_place = reinterpret_cast<WritePlace*>(J->d_status + S);
   T2_TRY(cudaMemcpy(J->d_packets, P.packets.data(), np * sizeof(DevPacket), cudaMemcpyHostToDevice));
   T2_TRY(cudaMemcpy(J->d_parts, P.parts.data(), nparts * sizeof(DevPart), cudaMemcpyHostToDevice));
   T2_TRY(cudaMemcpy(J->d_head, P.head.data(), P.head.size(), cudaMemcpyHostToDevice));
   T2_TRY(cudaMemcpy(J->d_coded, coded.data(), nblocks * sizeof(int32_t), cudaMemcpyHostToDevice));
   T2_TRY(cudaMemcpy(J->d_kmax, kmax.data(), nblocks, cudaMemcpyHostToDevice));
-  T2_TRY(cudaHostAlloc(&J->h_status, sizeof(T2Status), cudaHostAllocDefault));
+  T2_TRY(cudaHostAlloc(&J->h_status, status_bytes, cudaHostAllocDefault));
+  J->h_place = reinterpret_cast<WritePlace*>(J->h_status + S);
   *out = J;
   guard.j = nullptr;
   return 0;
@@ -336,56 +288,50 @@ void b2k_t2_destroy(T2Job* J)
 }
 
 uint32_t b2k_t2_flags(const T2Job* J) { return J->plan.flags; }
+uint32_t b2k_t2_streams(const T2Job* J) { return J->streams; }
 
 int b2k_t2_enqueue(T2Job* J, const HtBlockDesc* d_enc, const HtBlockOut* d_out, const uint8_t* d_scratch, uint8_t* cs, uint64_t cap,
-                   cudaStream_t st)
+                   cudaStream_t st, uint32_t n)
 {
   const Plan& P = J->plan;
   const uint64_t np = P.packets.size(), nparts = P.parts.size();
   const bool plt = (P.flags & B2K_CS_PLT) != 0, tlm = (P.flags & B2K_CS_TLM) != 0;
-  T2_TRY(cudaMemsetAsync(J->d_status, 0, sizeof(T2Status), st));
+  const size_t status_bytes = J->streams * sizeof(WriteStatus) + sizeof(WritePlace);
+  T2_TRY(cudaMemsetAsync(J->d_status, 0, status_bytes, st));
   const uint32_t tpb = 64; /* packets and tile parts are few: small CTAs spread them over the SMs */
   auto grid = [](uint64_t n, uint32_t per) { return (unsigned)std::max<uint64_t>(1, (n + per - 1) / per); };
-  k_t2_headers<<<grid(np, tpb), tpb, 0, st>>>(J->d_packets, np, J->d_coded, J->d_kmax, d_out, J->d_hdr, J->d_tags,
-                                                                 J->d_hdr_len, J->d_body_len, J->d_dst, J->d_status,
-                                                                 (P.flags & B2K_CS_SOP) != 0, (P.flags & B2K_CS_EPH) != 0);
+  k_t2_headers<<<grid(n * np, tpb), tpb, 0, st>>>(J->d_packets, np, n * np, J->d_coded, J->d_kmax, J->ncoded, d_out, J->d_hdr,
+                                                  P.hdr_bytes, J->d_tags, P.tag_nodes, J->d_hdr_len, J->d_body_len, J->d_dst,
+                                                  J->d_status, (P.flags & B2K_CS_SOP) != 0, (P.flags & B2K_CS_EPH) != 0);
   b2k_count_launch();
-  k_t2_parts<<<grid(nparts, tpb), tpb, 0, st>>>(J->d_parts, nparts, J->d_hdr_len, J->d_body_len, J->d_part_plt,
-                                                                   J->d_part_bytes, J->d_status, plt);
+  k_t2_parts<<<grid(n * nparts, tpb), tpb, 0, st>>>(J->d_parts, nparts, n * nparts, np, J->d_hdr_len, J->d_body_len, J->d_part_plt,
+                                                    J->d_part_bytes, J->d_status, plt);
   b2k_count_launch();
-  k_t2_scan<<<1, SCAN_THREADS, 0, st>>>(J->d_part_bytes, nparts, J->d_part_at, J->d_head, P.head.size(), cs, cap, J->d_status);
+  k_t2_scan<<<std::min<uint32_t>(n, 65535u), SCAN_THREADS, 0, st>>>(J->d_part_bytes, nparts, n, J->d_part_at, P.head.size(),
+                                                                    J->d_status, J->d_place);
   b2k_count_launch();
-  k_t2_emit<<<grid(nparts, tpb), tpb, 0, st>>>(J->d_parts, nparts, J->d_part_at, J->d_part_plt, J->d_part_bytes,
-                                                                  J->d_hdr_len, J->d_body_len, J->d_pkt_at, cs, cap, J->d_status, plt,
-                                                                  tlm, P.tlm_at);
+  k_t2_emit<<<grid(n * nparts, tpb), tpb, 0, st>>>(J->d_parts, nparts, n * nparts, np, J->d_part_at, J->d_part_plt, J->d_part_bytes,
+                                                   J->d_hdr_len, J->d_body_len, J->d_pkt_at, cs, cap, J->d_status, J->d_place, J->d_head,
+                                                   P.head.size(), plt, tlm, P.tlm_at);
   b2k_count_launch();
   const uint32_t wpb = 8; /* warps per CTA */
-  k_t2_packets<<<grid(np, wpb), wpb * 32, 0, st>>>(J->d_packets, np, J->d_coded, d_out, J->d_hdr, J->d_hdr_len,
-                                                                      J->d_pkt_at, J->d_dst, cs, cap, J->d_status);
+  k_t2_packets<<<grid(n * np, wpb), wpb * 32, 0, st>>>(J->d_packets, np, n * np, J->d_coded, J->ncoded, d_out, J->d_hdr, P.hdr_bytes,
+                                                       J->d_hdr_len, J->d_pkt_at, J->d_dst, cs, cap, J->d_status, J->d_place);
   b2k_count_launch();
-  b2k_launch_ht_gather(d_enc, d_out, J->d_dst, d_scratch, cs, (uint32_t)J->ncoded, cap, st);
-  T2_TRY(cudaMemcpyAsync(J->h_status, J->d_status, sizeof(T2Status), cudaMemcpyDeviceToHost, st));
+  b2k_launch_ht_gather(d_enc, d_out, J->d_dst, d_scratch, cs, (uint32_t)(n * J->ncoded), cap, st);
+  T2_TRY(cudaMemcpyAsync(J->h_status, J->d_status, status_bytes, cudaMemcpyDeviceToHost, st)); /* statuses and placement */
   T2_TRY(cudaGetLastError());
   return 0;
 }
 
-int64_t b2k_t2_result(const T2Job* J)
+int64_t b2k_t2_result(const T2Job* J, uint32_t s)
 {
-  const T2Status& s = *J->h_status;
-  if(s.bad_blocks)
-  {
-    b2k_set_error((std::to_string(s.bad_blocks) + " code block(s) overflowed the coder's buffers").c_str());
-    return -2;
-  }
-  const char* why = (s.errors & ERR_RANGE)       ? "code block outside the writer's range (bit planes / passes)"
-                    : (s.errors & ERR_PACKET)    ? "packet longer than 4 GiB"
-                    : (s.errors & ERR_HDR_BOUND) ? "packet header longer than its bound"
-                    : (s.errors & ERR_PART)      ? "tile part longer than 4 GiB"
-                                                 : nullptr;
-  if(why)
-  {
-    b2k_set_error(why);
-    return -1;
-  }
-  return (int64_t)s.total;
+  std::string text;
+  const int64_t r = write_verdict(J->h_status[s], &text);
+  if(r < 0)
+    b2k_set_error(text.c_str());
+  return r;
 }
+
+uint64_t b2k_t2_offset(const T2Job* J, uint32_t s) { return J->h_status[s].at; }
+uint64_t b2k_t2_used(const T2Job* J) { return J->h_place->used; }

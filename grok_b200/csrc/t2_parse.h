@@ -565,6 +565,14 @@ B2K_HD void status_add(uint32_t* p, uint32_t v)
   *p += v;
 #endif
 }
+B2K_HD void status_or(uint32_t* p, uint32_t v)
+{
+#ifdef __CUDA_ARCH__
+  atomicOr(p, v);
+#else
+  *p |= v;
+#endif
+}
 B2K_HD void status_min(unsigned long long* p, unsigned long long v)
 {
 #ifdef __CUDA_ARCH__

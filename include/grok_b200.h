@@ -516,6 +516,28 @@ B2K_API int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const b2k
  * (geometry and flags) is made once per coding and flags and kept with the engine's cached job. */
 B2K_API int64_t b2k_encode_codestream_device(b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img,
                                              uint32_t flags, void* cuda_stream, const uint8_t** cs);
+/* A batch: n images in device memory, all of coding cp -> n HTJ2K code streams in device memory, in one launch chain.
+ * status[i] and b2k_encode_codestreams_error(e, i) are what b2k_encode_codestream_device(e, cp, &imgs[i], flags, ...)
+ * returns for image i alone and its b2k_last_error text: 0 where it returns a length, else 1, -1 or -2, the checks in the
+ * same order (imgs[i]'s descriptor, the coding, the writer's plan, blocks that overflowed the coder, the writer's limits).
+ * A verdict that depends only on the coding or the flags is every image's, with the same text.  Status 0: the
+ * length[i] bytes at *cs + offset[i] are byte-identical to that single call's code stream; any other status: length[i] = 0
+ * and the image takes no bytes of the output.
+ * The streams lie in image order in one device buffer the engine owns, each at a 256-byte boundary.  It is not the buffer
+ * of b2k_encode_codestream_device, whose pointer a batch leaves valid; it stays valid until the next
+ * b2k_encode_codestreams_device on e, or b2k_engine_destroy.
+ * Stream order as b2k_encode_codestream_device: the images are read after the work queued on cuda_stream, which then
+ * waits for the engine's last read of them; the call returns once the code streams are written.  Synchronisations: one
+ * per call (statuses, offsets and lengths come home in one read), a second when the output buffer has to grow.  For a
+ * fixed coding and flags the launch count does not depend on n once n x tiles reaches the pipeline's chunk count.
+ * Returns < 0 for a failure of the whole call (NULL arrays, n == 0, imgs whose sample_bytes differ, a CUDA error, more
+ * code blocks than one job indexes), b2k_last_error set; else the number of images whose status is not 0. */
+B2K_API int32_t b2k_encode_codestreams_device(b2k_engine* e, const b2k_coding* cp, uint32_t n, const b2k_device_planes* imgs,
+                                              uint32_t flags, void* cuda_stream, const uint8_t** cs, uint64_t* offset,
+                                              uint64_t* length, int32_t* status, double* ms_total);
+/* the b2k_last_error text of image i in the last b2k_encode_codestreams_device call on e ("" for status 0); valid until
+   the next such call */
+B2K_API const char* b2k_encode_codestreams_error(b2k_engine* e, uint32_t i);
 /* A complete HTJ2K code stream in device memory (cs, len bytes, on the engine's GPU) -> the image in img.
  * Equal, for every input, to copying cs to the host and calling b2k_codestream_parse + b2k_decode_device:
  * the same return code, the same b2k_last_error text for 1 and -1, the same pixels for 0.  Only the main header (a
