@@ -115,8 +115,8 @@ void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t 
                                     uint32_t sample_bytes, uint32_t w, uint32_t h, cudaStream_t st);
 /* a batch's images out, one launch: for each of the n entries of the device table d_dst (BatchDst), its nc components
    (nc > 1: pixel-interleaved, step = nc) from the int32 planes src[c] to dst + y * dpitch + x * step + c samples, w x h
-   pixels.  Entries with dst NULL, or whose *err (the HT decoder's rejections in that image) is not 0, are skipped.  All
-   share sample_bytes. */
+   pixels.  Entries with dst NULL, or with an err whose *err (the HT decoder's rejections in that image) is not 0, are
+   skipped; an entry with err NULL is always written.  All share sample_bytes. */
 struct BatchDst
 {
   const int32_t* src[4];

@@ -1943,15 +1943,15 @@ __global__ void __launch_bounds__(128) k_planes_to_container(CPtr4 src, uint32_t
   planes_to_container_rows<S, NC>([&](int c) { return src.p[c]; }, spitch, dst, dpitch, step, w, h, x8);
 }
 
-/* the images of a batch: image blockIdx.z from its table entry; an entry without a destination, or of an image the HT
-   decoder rejected blocks of (the counter its slot's blocks were decoded into, earlier on the stream), is skipped */
+/* the images of a batch: image blockIdx.z from its table entry; an entry without a destination, or with a counter (of the
+   blocks of its slot the HT decoder rejected, earlier on the stream) that is not 0, is skipped */
 template <int S, int NC>
 __global__ void __launch_bounds__(128) k_planes_to_containers(const BatchDst* __restrict__ tab, uint32_t spitch, uint32_t w, uint32_t h)
 {
   const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
   const BatchDst* E = tab + blockIdx.z;
   void* dst = E->dst;
-  if(x8 >= w || !dst || *E->err)
+  if(x8 >= w || !dst || (E->err && *E->err))
     return;
   /* the plane pointers are read from the table where they are used */
   planes_to_container_rows<S, NC>([E](int c) { return E->src[c]; }, spitch, dst, E->dpitch, E->step, w, h, x8);

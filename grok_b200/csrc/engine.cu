@@ -75,7 +75,6 @@ struct b2k_engine
   /* b2k_decode_codestreams_device: the batch job (beside `cached`, so that single and batch calls alternate without
      replanning), each stream's text of the last call, and the gather tables and header staging of a call */
   b2k_device_job* batch = nullptr;
-  bool last_parse_batch = false;   /* b2k_codestream_parse_device_stats reports the batch's totals */
   std::vector<std::string> batch_errors;
   CopyEntry* d_copy = nullptr;
   CopyEntry* h_copy = nullptr;     /* pinned */
@@ -88,6 +87,9 @@ struct b2k_engine
   uint8_t* d_bcs = nullptr;
   uint64_t bcs_cap = 0;
   std::vector<std::string> enc_batch_errors;
+  /* b2k_codestream_parse_device_stats: the plan of the last device parse (single, window or batch); cleared when a job
+     drops that plan */
+  T2Parse* last_parse = nullptr;
 };
 
 /* ---- device memory cache --------------------------------------------------------------------------------------
@@ -413,7 +415,6 @@ struct b2k_device_job
   T2Job* t2 = nullptr;             /* b2k_encode_codestream_device: the code stream's plan for the flags of the last call */
   T2Parse* t2p = nullptr;          /* b2k_decode_codestream_device: the packet plan for the last stream's progression / SOP / EPH */
   T2Parse* t2w = nullptr;          /* b2k_decode_codestream_window_device: the box coding's plan (this job's coding is the virtual one) */
-  bool last_parse_window = false;  /* the last device parse was a windowed one (b2k_codestream_parse_device_stats) */
 };
 
 /* -------------------------------------------------------------------------------------------- */
@@ -902,6 +903,15 @@ static int job_create(b2k_engine* e, const b2k_coding* cp, uint32_t tile_mod, ui
   return 0;
 }
 
+/* one of J's parse plans goes: b2k_codestream_parse_device_stats no longer reports it */
+static void drop_parse(b2k_device_job* J, T2Parse*& p)
+{
+  if(J->eng->last_parse == p)
+    J->eng->last_parse = nullptr;
+  b2k_t2_parse_destroy(p);
+  p = nullptr;
+}
+
 extern "C" void b2k_job_destroy(b2k_device_job* J)
 {
   if(!J)
@@ -909,8 +919,8 @@ extern "C" void b2k_job_destroy(b2k_device_job* J)
   cudaSetDevice(J->eng->device);
   cudaStreamSynchronize(J->eng->stream);
   b2k_t2_destroy(J->t2);
-  b2k_t2_parse_destroy(J->t2p);
-  b2k_t2_parse_destroy(J->t2w);
+  drop_parse(J, J->t2p);
+  drop_parse(J, J->t2w);
   cudaFree(J->img.base);
   cudaFree(J->d_stage);
   cudaFree(J->coef.base);
@@ -2143,44 +2153,11 @@ static b2k_device_job* cached_job(b2k_engine* e, const b2k_coding* cp, uint32_t 
   return J;
 }
 
-/* b2k_encode_codestream_device: the code stream is written on the device (t2_device.cu) instead of a result coming home */
-struct DeviceCodestream
-{
-  uint32_t flags;
-  int64_t length = 0;
-};
-
-/* T2 on the device after the block coder, into the engine's code-stream buffer (grown, and T2 run again, when the code
-   stream outgrows it).  The call's one synchronisation reads the length. */
-static int device_t2(b2k_engine* e, b2k_device_job* J, cudaStream_t st, DeviceCodestream& dc)
-{
-  for(;;)
-  {
-    if(b2k_t2_enqueue(J->t2, J->d_enc_desc, J->d_out, J->d_scratch, e->d_cs, e->cs_cap, st))
-      return -1;
-    CUDA_TRY(cudaStreamSynchronize(st));
-    const int64_t n = b2k_t2_result(J->t2);
-    if(n < 0)
-      return (int)n;
-    if((uint64_t)n <= e->cs_cap)
-    {
-      dc.length = n;
-      return 0;
-    }
-    cudaFree(e->d_cs);
-    e->d_cs = nullptr;
-    e->cs_cap = 0;
-    CUDA_TRY(cudaMalloc(&e->d_cs, (uint64_t)n + (uint64_t)n / 8 + 4096));
-    e->cs_cap = (uint64_t)n + (uint64_t)n / 8 + 4096;
-  }
-}
-
-/* T.user: the caller's samples.  A device image (b2k_encode_device) is read after the work queued on `caller`.  With dc the
-   code stream is written on the device and *out is not touched. */
+/* T.user: the caller's samples.  A device image (b2k_encode_device) is read after the work queued on `caller`. */
 static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, uint32_t rem, b2k_result** out, Transport& T,
-                             cudaStream_t caller = nullptr, DeviceCodestream* dc = nullptr)
+                             cudaStream_t caller = nullptr)
 {
-  if(!e || !cp || (!out && !dc))
+  if(!e || !cp || !out)
     return -1;
   std::lock_guard<std::mutex> lock(e->mu);
   int rc = 0;
@@ -2188,14 +2165,6 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
   if(rc)
     return rc;
   CUDA_TRY(cudaSetDevice(e->device));
-  if(dc && (!J->t2 || b2k_t2_flags(J->t2) != dc->flags))
-  { /* geometry and flags only: planned once for every frame of this coding */
-    b2k_t2_destroy(J->t2);
-    J->t2 = nullptr;
-    if(b2k_t2_create(*cp, dc->flags, J->blocks.data(), J->blocks.size(), (uint32_t)J->tiles.size(), J->coded_index.data(),
-                     J->coded_index.size(), &J->t2))
-      return -1;
-  }
   const auto wall0 = std::chrono::steady_clock::now();
   if(resolve_transport(J, T, false))
     return -1;
@@ -2211,7 +2180,7 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
   const size_t nchunks = J->chunk_tile.size() - 1;
   /* the arena size of the previous call is the estimate: scan + compact + return every chunk's bytes while later
      chunks are still arriving (the D2H direction of PCIe is otherwise idle) */
-  const bool streamed = !dc && J->bytes_cap > 0 && nchunks > 1;
+  const bool streamed = J->bytes_cap > 0 && nchunks > 1;
   uint8_t* hb = nullptr;
   struct ArenaGuard /* the pinned arena goes back to the pool on every early return until a result owns it */
   {
@@ -2292,8 +2261,6 @@ static int32_t encode_common(b2k_engine* e, const b2k_coding* cp, uint32_t mod, 
   /* the caller's stream goes on once every chunk of its image has been read */
   if(dev && queue_after(e, st, caller)) return -1;
   DBG_T("encode: chunks enqueued");
-  if(dc)
-    return device_t2(e, J, st, *dc);
   b2k_result* R = nullptr;
   const uint32_t nb_all = (uint32_t)J->h_enc_desc.size();
   b2k_result* shell = result_shell(J); /* host work while the device finishes the last chunks */
@@ -2441,22 +2408,6 @@ extern "C" int32_t b2k_encode_device(b2k_engine* e, const b2k_coding* cp, const 
   Transport T;
   device_samples(T, *img, cp->x0, cp->y0);
   return encode_common(e, cp, tile_mod, tile_rem, out, T, caller_stream(cuda_stream));
-}
-
-extern "C" int64_t b2k_encode_codestream_device(b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img, uint32_t flags,
-                                                void* cuda_stream, const uint8_t** cs)
-{
-  if(!e || !cp || !cs)
-    return -1;
-  if(int rc = check_device_planes(e, cp, img))
-    return rc;
-  Transport T;
-  device_samples(T, *img, cp->x0, cp->y0);
-  DeviceCodestream dc{flags};
-  if(int32_t rc = encode_common(e, cp, 1, 0, nullptr, T, caller_stream(cuda_stream), &dc))
-    return rc;
-  *cs = e->d_cs;
-  return dc.length;
 }
 
 extern "C" int32_t b2k_decode_device(b2k_engine* e, const b2k_coding* cp, const b2k_block* blocks, uint64_t num_blocks,
@@ -2608,7 +2559,9 @@ static int32_t decode_common(b2k_engine* e, const b2k_coding* cp, const b2k_bloc
 /* ---- code streams in device memory (b2k_decode_codestream_device / b2k_codestream_parse_device) ----------------------
  * The main header is read on the host from a prefix of the stream, by b2k_codestream_parse's own code; the tile parts and
  * packets are parsed on the device (t2_decode.cu) from a copy of the stream in the job's arena, which also gives the HT
- * decoder the slack it reads past a block.  Synchronisations: the header, the parse status, the end of the decode. */
+ * decoder the slack it reads past a block.  A single stream is a batch of one (b2k_decode_codestreams_device below): the
+ * same header read, arena copy, parse and image write, in slot 0 of the engine's single-image job.  Synchronisations: the
+ * header, the parse status, the end of the decode. */
 static int check_device_bytes(const b2k_engine* e, const uint8_t* cs, uint64_t len)
 {
   if(len == 0)
@@ -2628,81 +2581,266 @@ static int check_device_bytes(const b2k_engine* e, const uint8_t* cs, uint64_t l
   return 0;
 }
 
-/* the main header from a prefix of cs read on st: 64 KiB, doubled while the header runs past it (a large TLM) */
-static int read_device_main_header(const uint8_t* cs, uint64_t len, cudaStream_t st, b2k::t2::MainHeader& h)
+static int grow_copy_table(b2k_engine* e, uint32_t n)
 {
-  uint64_t n = std::min<uint64_t>(len, 64u << 10);
+  if(n <= e->copy_cap)
+    return 0;
+  cudaFree(e->d_copy);
+  cudaFreeHost(e->h_copy);
+  e->d_copy = nullptr;
+  e->h_copy = nullptr;
+  e->copy_cap = 0;
+  CUDA_TRY(cudaMalloc(&e->d_copy, n * sizeof(CopyEntry)));
+  CUDA_TRY(cudaHostAlloc(&e->h_copy, n * sizeof(CopyEntry), cudaHostAllocDefault));
+  e->copy_cap = n;
+  return 0;
+}
+
+/* h_copy[0, m) into out on st: the table to the device and one gather launch, or for one entry a plain device-to-device
+   copy */
+static int gather_streams(b2k_engine* e, uint32_t m, uint64_t max_len, uint8_t* out, cudaStream_t st)
+{
+  if(m == 1)
+  {
+    CUDA_TRY(cudaMemcpyAsync(out + e->h_copy[0].dst, e->h_copy[0].src, e->h_copy[0].len, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+  if(!m)
+    return 0;
+  CUDA_TRY(cudaMemcpyAsync(e->d_copy, e->h_copy, m * sizeof(CopyEntry), cudaMemcpyHostToDevice, st));
+  return b2k_copy_table(e->d_copy, m, max_len, out, st);
+}
+
+/* the main headers h[i] of the n streams whose status is 0, read on st by b2k_parse_main_header from prefixes of `prefix`
+   bytes gathered into one copy; the streams whose header runs past its prefix go round again together with twice the
+   prefix.  A stream whose header fails gets its status and, with `errors`, its text there.  0, or -1 for a failure of the
+   call. */
+static int read_batch_headers(b2k_engine* e, uint32_t n, const uint8_t* const* cs, const uint64_t* len, uint64_t prefix, cudaStream_t st,
+                              int32_t* status, b2k::t2::MainHeader* h, std::string* errors)
+{
+  std::vector<uint64_t> want(n, 0);
+  for(uint32_t i = 0; i < n; ++i)
+    want[i] = status[i] ? 0 : std::min<uint64_t>(len[i], prefix);
   for(;;)
   {
-    uint8_t* buf = pool_get(n);
-    if(!buf)
+    uint32_t m = 0;
+    uint64_t total = 0, longest = 0;
+    if(grow_copy_table(e, n)) return -1;
+    for(uint32_t i = 0; i < n; ++i)
+      if(want[i])
+      {
+        e->h_copy[m++] = CopyEntry{cs[i], want[i], total};
+        total += want[i];
+        longest = std::max(longest, want[i]);
+      }
+    if(!m)
+      return 0;
+    if(total > e->hdr_cap)
     {
-      g_err = "no pinned memory for the main header";
-      return -1;
+      cudaFree(e->d_hdr);
+      cudaFreeHost(e->h_hdr);
+      e->d_hdr = nullptr;
+      e->h_hdr = nullptr;
+      e->hdr_cap = 0;
+      CUDA_TRY(cudaMalloc(&e->d_hdr, total));
+      CUDA_TRY(cudaHostAlloc(&e->h_hdr, total, cudaHostAllocDefault));
+      e->hdr_cap = total;
     }
-    cudaError_t ce = cudaMemcpyAsync(buf, cs, n, cudaMemcpyDeviceToHost, st);
-    if(ce == cudaSuccess)
-      ce = cudaStreamSynchronize(st);
-    const int rc = ce == cudaSuccess ? b2k_parse_main_header(buf, n, h) : -1;
-    pool_put(buf);
-    if(ce != cudaSuccess)
+    if(m == 1) /* one prefix goes to the host as it is */
+      CUDA_TRY(cudaMemcpyAsync(e->h_hdr, e->h_copy[0].src, total, cudaMemcpyDeviceToHost, st));
+    else
     {
-      g_err = std::string("code stream prefix to the host: ") + cudaGetErrorString(ce);
-      return -1;
+      if(gather_streams(e, m, longest, e->d_hdr, st)) return -1;
+      CUDA_TRY(cudaMemcpyAsync(e->h_hdr, e->d_hdr, total, cudaMemcpyDeviceToHost, st));
     }
-    if(rc && h.short_read && n < len)
+    CUDA_TRY(cudaStreamSynchronize(st));
+    uint64_t at = 0;
+    for(uint32_t i = 0; i < n; ++i)
     {
-      n = std::min<uint64_t>(len, 2 * n);
-      continue;
+      if(!want[i])
+        continue;
+      const uint64_t got = want[i];
+      const int rc = b2k_parse_main_header(e->h_hdr + at, got, h[i]);
+      at += got;
+      want[i] = 0;
+      if(rc && h[i].short_read && got < len[i])
+        want[i] = std::min<uint64_t>(len[i], 2 * got);
+      else if(rc)
+      {
+        status[i] = rc;
+        if(errors)
+          errors[i] = g_err;
+      }
     }
-    return rc;
   }
 }
 
-/* the header, the job of its coding, the stream in the job's arena and its parse on st, up to the status.  With dec the
-   decoder's descriptors are built too.  header_read: h already holds the main header, read after the caller's work.  0, or
-   b2k_codestream_parse's return code with its text. */
-static int parse_device_codestream(b2k_engine* e, const uint8_t* cs, uint64_t len, cudaStream_t caller, b2k::t2::MainHeader& h,
-                                   b2k_device_job** out, bool dec, bool* refinement, uint64_t cap_blocks = UINT64_MAX,
-                                   bool header_read = false)
+/* one stream's main header, read after the work queued on `caller` from a 64 KiB prefix, so that a large TLM costs no
+   second round trip: 0, or b2k_codestream_parse's code with its text */
+static int read_main_header(b2k_engine* e, const uint8_t* cs, uint64_t len, cudaStream_t caller, b2k::t2::MainHeader& h)
+{
+  CUDA_TRY(cudaSetDevice(e->device));
+  if(queue_after(e, caller, e->stream)) return -1;
+  int32_t status = 0;
+  if(read_batch_headers(e, 1, &cs, &len, 64u << 10, e->stream, &status, &h, nullptr)) return -1;
+  return status;
+}
+
+/* the parse on st of the streams i < n whose status is 0 (main headers h[i], progression and SOP / EPH `flags`) in slots i
+   of J: the streams laid out in the arena at 256-byte boundaries (with headroom for a larger batch when n > 1), then
+   the five parse kernels and, with dec, the decoder's descriptors.  One synchronisation; a stream that fails gets its
+   status and, with `errors`, its text there.  *refinement: a stream has refinement passes.  0, or -1 for a failure of
+   the call. */
+static int parse_streams(b2k_engine* e, b2k_device_job* J, uint32_t n, const uint8_t* const* cs, const uint64_t* len,
+                         const b2k::t2::MainHeader* h, uint32_t flags, bool dec, int32_t* status, std::string* errors, bool* refinement)
 {
   cudaStream_t st = e->stream;
-  CUDA_TRY(cudaSetDevice(e->device));
-  if(!header_read)
-  { /* what the caller queued before the call (the kernel, receive or read that produced cs) comes first */
-    if(queue_after(e, caller, st)) return -1;
-    if(int rc = read_device_main_header(cs, len, st, h))
-      return rc;
+  if(!J->t2p || b2k_t2_parse_flags(J->t2p) != flags || b2k_t2_parse_streams(J->t2p) != J->slots)
+  { /* geometry and progression only: planned once for every stream or batch of this coding */
+    drop_parse(J, J->t2p);
+    if(b2k_t2_parse_create(J->cp, flags, J->blocks.data(), J->blocks.size(), J->slot_tiles, J->coded_index.data(), J->coded_index.size(),
+                           &J->t2p, J->slots))
+      return -1;
   }
+  /* the arena: stream i at a 256-byte boundary, the decoder's read-past slack after the last one; one gather */
+  std::vector<uint64_t> at(n, 0), plen(n, 0), sot(n, 0);
+  uint64_t total = 0, longest = 0;
+  uint32_t m = 0;
+  if(grow_copy_table(e, n)) return -1;
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    if(status[i])
+      continue;
+    at[i] = total;
+    plen[i] = len[i];
+    sot[i] = h[i].sot;
+    e->h_copy[m++] = CopyEntry{cs[i], len[i], total};
+    longest = std::max(longest, len[i]);
+    total = b2k::t2::batch_arena_next(total, len[i]);
+  }
+  if(arena_reserve(J, total, n > 1 ? total / 8 : 0)) return -1;
+  J->arena_sized = false; /* the arena now holds callers' streams, not this job's coding of its image */
+  e->last_parse = J->t2p;
+  CUDA_TRY(cudaEventRecord(J->ev[0], st));
+  if(gather_streams(e, m, longest, J->d_bytes, st)) return -1;
+  if(b2k_t2_batch_enqueue(J->t2p, J->d_bytes, n, at.data(), plen.data(), sot.data(), J->d_enc_desc, J->d_dec_quant,
+                          dec ? J->d_dec_desc : nullptr, st))
+    return -1;
+  CUDA_TRY(cudaStreamSynchronize(st));
+  bool any = false;
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    if(status[i])
+      continue;
+    bool r = false;
+    if(int prc = b2k_t2_batch_result(J->t2p, i, &r))
+    {
+      status[i] = prc;
+      if(errors)
+        errors[i] = g_err;
+    }
+    any = any || r;
+  }
+  if(refinement)
+    *refinement = any;
+  return 0;
+}
+
+/* after a parse into J's descriptors: block decode -> inverse -> images, chunk by chunk over the (slot, tile) ranges of the
+   n slots used (as many chunks as the job's pipeline has, whatever its slot count).  After the chunk that holds slot i's
+   last tile, `rect` of its planes (the whole canvas, or a window on the virtual canvas) goes to imgs[i] when status[i] is
+   0, in one launch per component group.  With write_rejected the image of a slot whose blocks the HT decoder rejected
+   is written too (as b2k_decode_device writes it), else it is left alone.  The caller's stream then waits for the
+   writes.  A slot with rejected blocks gets -2 and, with `errors`, its text there.  0, or -1 for a failure of the call. */
+static int decode_slots(b2k_engine* e, b2k_device_job* J, uint32_t n, const b2k_device_planes* imgs, const Rect& rect, bool refinement,
+                        bool write_rejected, cudaStream_t caller, double* ms_total, int32_t* status, std::string* errors)
+{
+  cudaStream_t st = e->stream;
+  /* the conversion's tables: one per component, or one for all when every image written is pixel-interleaved */
+  const int nc = J->cp.numcomps;
+  bool interleaved = nc > 1;
+  for(uint32_t i = 0; i < n; ++i)
+    if(!status[i])
+      interleaved = interleaved && device_group(imgs[i], nc) == nc;
+  const int group = interleaved ? nc : 1, tables = nc / group;
+  if(!J->h_batch_dst)
+  {
+    CUDA_TRY(cudaMalloc(&J->d_batch_dst, (size_t)J->slots * 4 * sizeof(BatchDst)));
+    CUDA_TRY(cudaHostAlloc(&J->h_batch_dst, (size_t)J->slots * 4 * sizeof(BatchDst), cudaHostAllocDefault));
+  }
+  for(int t = 0; t < tables; ++t)
+    for(uint32_t i = 0; i < n; ++i)
+    {
+      BatchDst& D = J->h_batch_dst[(size_t)t * n + i];
+      D = BatchDst{};
+      if(status[i])
+        continue;
+      const int c0 = t * group;
+      for(int k = 0; k < group; ++k)
+        D.src[k] = J->img.at((int)i * nc + c0 + k, rect.x0, rect.y0);
+      D.dst = imgs[i].comp[c0];
+      D.err = write_rejected ? nullptr : J->d_err + i;
+      D.dpitch = imgs[i].row_pitch[c0];
+      D.step = imgs[i].col_step[c0];
+    }
+  CUDA_TRY(cudaMemcpyAsync(J->d_batch_dst, J->h_batch_dst, (size_t)tables * n * sizeof(BatchDst), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, n * sizeof(int), st));
+  J->dec_has_refinement = refinement;
+  const size_t used = (size_t)n * J->slot_tiles, T = J->slot_tiles;
+  const size_t nchunks = std::min<size_t>(J->chunk_tile.size() - 1, used);
+  const uint32_t sb = imgs[0].sample_bytes;
+  for(size_t k = 0; k < nchunks; ++k)
+  {
+    const size_t t0 = k * used / nchunks, t1 = (k + 1) * used / nchunks;
+    if(t1 <= t0)
+      continue;
+    if(enqueue_block_decode(e, J, k, nullptr, st, t0, t1)) return -1;
+    if(enqueue_inverse(J, st, t0, t1)) return -1;
+    const uint32_t s0 = (uint32_t)(t0 / T), s1 = (uint32_t)(t1 / T);
+    for(int t = 0; t < tables && s1 > s0; ++t)
+      b2k_launch_planes_to_containers(J->d_batch_dst + (size_t)t * n + s0, s1 - s0, group, J->img.pitch, sb, rect.w(), rect.h(), st);
+  }
+  CUDA_TRY(cudaEventRecord(J->ev[1], st));
+  /* the caller's stream goes on once its images are written */
+  if(queue_after(e, st, caller)) return -1;
+  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
+  CUDA_TRY(cudaGetLastError());
+  float t = 0;
+  cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
+  if(ms_total) *ms_total = t;
+  /* the HT decoder's verdict, per slot */
+  std::vector<int> herr(n, 0);
+  CUDA_TRY(cudaMemcpy(herr.data(), J->d_err, n * sizeof(int), cudaMemcpyDeviceToHost));
+  for(uint32_t i = 0; i < n; ++i)
+    if(!status[i] && herr[i])
+    {
+      g_err = "HT decoder rejected " + std::to_string(herr[i]) + " block(s)";
+      status[i] = -2;
+      if(errors)
+        errors[i] = g_err;
+    }
+  return 0;
+}
+
+/* the single-stream calls' job (of h's coding) and the stream's parse in its slot 0, with dec the decoder's descriptors
+   too; the caller's block table is checked first, as the host parser checks it before it looks at a tile part.  0, or
+   b2k_codestream_parse's code with its text.  *out: the job, once there is one. */
+static int parse_single(b2k_engine* e, const uint8_t* cs, uint64_t len, const b2k::t2::MainHeader& h, b2k_device_job** out, bool dec,
+                        bool* refinement, uint64_t cap_blocks = UINT64_MAX)
+{
   int rc = 0;
   b2k_device_job* J = cached_job(e, &h.cp, 1, 0, &rc);
   if(rc)
     return rc;
   *out = J;
   if(cap_blocks < J->blocks.size())
-  { /* the host parser checks the caller's table before it looks at a tile part */
+  {
     g_err = "block table too small";
     return -1;
   }
-  const uint32_t flags = h.flags();
-  if(!J->t2p || b2k_t2_parse_flags(J->t2p) != flags)
-  { /* geometry and progression only: planned once for every stream of this coding */
-    b2k_t2_parse_destroy(J->t2p);
-    J->t2p = nullptr;
-    if(b2k_t2_parse_create(h.cp, flags, J->blocks.data(), J->blocks.size(), (uint32_t)J->tiles.size(), J->coded_index.data(),
-                           J->coded_index.size(), &J->t2p))
-      return -1;
-  }
-  if(arena_reserve(J, len, 0)) return -1;
-  J->arena_sized = false; /* the arena now holds a caller's stream, not this job's coding of its image */
-  J->last_parse_window = false;
-  e->last_parse_batch = false;
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  CUDA_TRY(cudaMemcpyAsync(J->d_bytes, cs, len, cudaMemcpyDeviceToDevice, st));
-  if(b2k_t2_parse_enqueue(J->t2p, J->d_bytes, len, h.sot, J->d_enc_desc, J->d_dec_quant, dec ? J->d_dec_desc : nullptr, st))
-    return -1;
-  CUDA_TRY(cudaStreamSynchronize(st));
-  return b2k_t2_parse_result(J->t2p, refinement);
+  int32_t status = 0;
+  if(parse_streams(e, J, 1, &cs, &len, &h, h.flags(), dec, &status, nullptr, refinement)) return -1;
+  return status;
 }
 
 extern "C" int64_t b2k_codestream_parse_device(b2k_engine* e, const uint8_t* cs, uint64_t len, void* cuda_stream, b2k_coding* cp_out,
@@ -2713,19 +2851,16 @@ extern "C" int64_t b2k_codestream_parse_device(b2k_engine* e, const uint8_t* cs,
   if(check_device_bytes(e, cs, len))
     return -1;
   std::lock_guard<std::mutex> lock(e->mu);
-  cudaStream_t caller = caller_stream(cuda_stream);
   b2k::t2::MainHeader h;
+  if(int rc = read_main_header(e, cs, len, caller_stream(cuda_stream), h))
+    return rc;
   if(!blocks)
   {
-    CUDA_TRY(cudaSetDevice(e->device));
-    if(queue_after(e, caller, e->stream)) return -1;
-    if(int rc = read_device_main_header(cs, len, e->stream, h))
-      return rc;
     *cp_out = h.cp;
     return b2k_enumerate(&h.cp, 1, 0, nullptr, 0);
   }
   b2k_device_job* J = nullptr;
-  int rc = parse_device_codestream(e, cs, len, caller, h, &J, false, nullptr, cap_blocks);
+  int rc = parse_single(e, cs, len, h, &J, false, nullptr, cap_blocks);
   if(J)
     *cp_out = h.cp;
   if(rc)
@@ -2734,39 +2869,6 @@ extern "C" int64_t b2k_codestream_parse_device(b2k_engine* e, const uint8_t* cs,
   if(b2k_t2_parse_blocks(J->t2p, blocks, e->stream))
     return -1;
   return (int64_t)n;
-}
-
-/* after a parse into J's descriptors: block decode -> inverse -> the caller's device image, which holds `window` (x0, y0,
-   x1, y1 on cp's canvas) or, window = NULL, the whole image; the caller's stream then waits for the image writes */
-static int32_t decode_parsed(b2k_engine* e, b2k_device_job* J, const b2k_coding& cp, const b2k_device_planes* img, const Rect* window,
-                             bool refinement, cudaStream_t caller, double* ms_total)
-{
-  if(int rc = check_device_planes(e, &cp, img))
-    return rc;
-  Transport T;
-  device_samples(T, *img, window ? window->x0 : cp.x0, window ? window->y0 : cp.y0);
-  T.window = window;
-  if(resolve_transport(J, T, true))
-    return -1;
-  cudaStream_t st = e->stream;
-  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, sizeof(int), st));
-  J->dec_has_refinement = refinement;
-  const size_t nchunks = J->chunk_tile.size() - 1;
-  for(size_t k = 0; k < nchunks; ++k)
-  { /* the parse has finished (its status was read): the side streams need not wait for it */
-    if(enqueue_block_decode(e, J, k, nullptr, st)) return -1;
-    if(enqueue_inverse(J, st, J->chunk_tile[k], J->chunk_tile[k + 1])) return -1;
-    if(download_chunk(J, T, k, st, e->copy_stream)) return -1;
-  }
-  CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  /* the caller's stream goes on once its image is written */
-  if(queue_after(e, st, caller)) return -1;
-  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
-  CUDA_TRY(cudaGetLastError());
-  float t = 0;
-  cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
-  if(ms_total) *ms_total = t;
-  return decoder_verdict(J);
 }
 
 extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs, uint64_t len, const b2k_device_planes* img,
@@ -2780,15 +2882,21 @@ extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs
   const auto wall0 = std::chrono::steady_clock::now();
   cudaStream_t caller = caller_stream(cuda_stream);
   b2k::t2::MainHeader h;
+  if(int rc = read_main_header(e, cs, len, caller, h))
+    return rc;
   b2k_device_job* J = nullptr;
   bool refinement = false;
-  if(int rc = parse_device_codestream(e, cs, len, caller, h, &J, true, &refinement))
+  if(int rc = parse_single(e, cs, len, h, &J, true, &refinement))
     return rc;
   *cp_out = h.cp;
   DBG_T("device decode: parsed");
-  const int32_t rc = decode_parsed(e, J, h.cp, img, nullptr, refinement, caller, ms_total);
+  if(int rc = check_device_planes(e, &h.cp, img))
+    return rc;
+  int32_t status = 0;
+  if(decode_slots(e, J, 1, img, Rect{h.cp.x0, h.cp.y0, h.cp.x1, h.cp.y1}, refinement, true, caller, ms_total, &status, nullptr))
+    return -1;
   DBG_T("device decode: done");
-  return rc;
+  return status;
 }
 
 /* ---- windows of code streams in device memory (b2k_codestream_parse_window_device / b2k_decode_codestream_window_device)
@@ -2807,9 +2915,7 @@ struct DeviceWindow
 static int device_window_coding(b2k_engine* e, const uint8_t* cs, uint64_t len, const uint32_t* window, uint32_t reduce,
                                 cudaStream_t caller, DeviceWindow& w)
 {
-  CUDA_TRY(cudaSetDevice(e->device));
-  if(queue_after(e, caller, e->stream)) return -1;
-  if(int rc = read_device_main_header(cs, len, e->stream, w.h))
+  if(int rc = read_main_header(e, cs, len, caller, w.h))
     return rc;
   if(int rc = b2k_window_coding(w.h.cp, window, reduce, w.wc))
     return rc;
@@ -2842,14 +2948,12 @@ static int parse_device_window(b2k_engine* e, const uint8_t* cs, uint64_t len, c
   const uint32_t flags = w.h.flags();
   if(!b2k_t2_window_matches(J->t2w, w.wc.box, flags, reduce))
   { /* box geometry, progression and reduce: planned once for every window with the same tile box */
-    b2k_t2_parse_destroy(J->t2w);
-    J->t2w = nullptr;
+    drop_parse(J, J->t2w);
     if(b2k_t2_window_create(w.wc, flags, reduce, J->blocks.data(), J->blocks.size(), J->coded_index.data(), J->coded_index.size(), &J->t2w))
       return -1;
   }
-  J->last_parse_window = true;
+  e->last_parse = J->t2w;
   J->arena_sized = false;
-  e->last_parse_batch = false;
   const TileGrid g = tile_grid(w.h.cp);
   CUDA_TRY(cudaEventRecord(J->ev[0], st));
   if(b2k_t2_window_enqueue(J->t2w, cs, len, w.h.sot, g.nx, g.nx * g.ny, w.wc, J->d_enc_desc, J->d_dec_quant, dec ? J->d_dec_desc : nullptr,
@@ -2895,7 +2999,7 @@ extern "C" int64_t b2k_codestream_parse_window_device(b2k_engine* e, const uint8
   e->have_window_stats = false;
   if(w.wc.whole)
   {
-    int rc = parse_device_codestream(e, cs, len, caller, w.h, &J, false, nullptr, cap_blocks, true);
+    int rc = parse_single(e, cs, len, w.h, &J, false, nullptr, cap_blocks);
     if(J)
       *cp_out = w.h.cp;
     if(rc)
@@ -2933,7 +3037,7 @@ extern "C" int32_t b2k_decode_codestream_window_device(b2k_engine* e, const uint
   b2k_device_job* J = nullptr;
   bool refinement = false;
   e->have_window_stats = false;
-  int rc = w.wc.whole ? parse_device_codestream(e, cs, len, caller, w.h, &J, true, &refinement, UINT64_MAX, true)
+  int rc = w.wc.whole ? parse_single(e, cs, len, w.h, &J, true, &refinement)
                       : parse_device_window(e, cs, len, w, reduce, &J, true, &refinement, UINT64_MAX);
   if(rc)
     return rc;
@@ -2947,9 +3051,13 @@ extern "C" int32_t b2k_decode_codestream_window_device(b2k_engine* e, const uint
     rect_out[3] = w.rect.y1;
   }
   DBG_T("device window decode: parsed");
-  rc = decode_parsed(e, J, w.wc.vcp, img, &w.rect, refinement, caller, ms_total);
+  if(int crc = check_device_planes(e, &w.wc.vcp, img))
+    return crc;
+  int32_t status = 0;
+  if(decode_slots(e, J, 1, img, w.rect, refinement, true, caller, ms_total, &status, nullptr))
+    return -1;
   DBG_T("device window decode: done");
-  return rc;
+  return status;
 }
 
 extern "C" int32_t b2k_codestream_window_device_stats(b2k_engine* e, uint32_t* tiles_wanted, uint64_t* arena_bytes)
@@ -2972,15 +3080,12 @@ extern "C" int32_t b2k_codestream_parse_device_stats(b2k_engine* e, uint32_t* ti
   if(!e || !tiles_indexed || !tiles_walked)
     return -1;
   std::lock_guard<std::mutex> lock(e->mu);
-  T2Parse* last = e->cached ? (e->cached->last_parse_window ? e->cached->t2w : e->cached->t2p) : nullptr;
-  if(e->last_parse_batch)
-    last = e->batch ? e->batch->t2p : nullptr;
-  if(!last)
+  if(!e->last_parse)
   {
     g_err = "no code stream has been parsed on the device";
     return -1;
   }
-  b2k_t2_parse_stats(last, tiles_indexed, tiles_walked);
+  b2k_t2_parse_stats(e->last_parse, tiles_indexed, tiles_walked);
   return 0;
 }
 
@@ -2991,86 +3096,6 @@ extern "C" int32_t b2k_codestream_parse_device_stats(b2k_engine* e, uint32_t* ti
  * its verdict; a stream that fails is parsed no further, decodes as all-zero blocks in its own slot and is not written
  * out, so it cannot change another stream's pixels or verdict.  Synchronisations: the header prefixes (one more round for
  * the streams whose header runs past its prefix, all together), the parse statuses, the end. */
-static int grow_copy_table(b2k_engine* e, uint32_t n)
-{
-  if(n <= e->copy_cap)
-    return 0;
-  cudaFree(e->d_copy);
-  cudaFreeHost(e->h_copy);
-  e->d_copy = nullptr;
-  e->h_copy = nullptr;
-  e->copy_cap = 0;
-  CUDA_TRY(cudaMalloc(&e->d_copy, n * sizeof(CopyEntry)));
-  CUDA_TRY(cudaHostAlloc(&e->h_copy, n * sizeof(CopyEntry), cudaHostAllocDefault));
-  e->copy_cap = n;
-  return 0;
-}
-
-/* h_copy[0, m) -> the device, then one gather launch into out, on st */
-static int gather_streams(b2k_engine* e, uint32_t m, uint64_t max_len, uint8_t* out, cudaStream_t st)
-{
-  if(!m)
-    return 0;
-  CUDA_TRY(cudaMemcpyAsync(e->d_copy, e->h_copy, m * sizeof(CopyEntry), cudaMemcpyHostToDevice, st));
-  return b2k_copy_table(e->d_copy, m, max_len, out, st);
-}
-
-/* the main headers of the streams whose status is 0, read on st by b2k_parse_main_header from prefixes of a few KiB
-   gathered into one copy; the streams whose header runs past its prefix go round again together with twice the prefix.
-   A stream whose header fails gets its status and text.  0, or -1 for a failure of the call. */
-static int read_batch_headers(b2k_engine* e, uint32_t n, const uint8_t* const* cs, const uint64_t* len, cudaStream_t st,
-                              int32_t* status, std::vector<b2k::t2::MainHeader>& h)
-{
-  std::vector<uint64_t> want(n, 0);
-  for(uint32_t i = 0; i < n; ++i)
-    want[i] = status[i] ? 0 : std::min<uint64_t>(len[i], b2k::t2::BATCH_HEADER_PREFIX);
-  for(;;)
-  {
-    uint32_t m = 0;
-    uint64_t total = 0, longest = 0;
-    if(grow_copy_table(e, n)) return -1;
-    for(uint32_t i = 0; i < n; ++i)
-      if(want[i])
-      {
-        e->h_copy[m++] = CopyEntry{cs[i], want[i], total};
-        total += want[i];
-        longest = std::max(longest, want[i]);
-      }
-    if(!m)
-      return 0;
-    if(total > e->hdr_cap)
-    {
-      cudaFree(e->d_hdr);
-      cudaFreeHost(e->h_hdr);
-      e->d_hdr = nullptr;
-      e->h_hdr = nullptr;
-      e->hdr_cap = 0;
-      CUDA_TRY(cudaMalloc(&e->d_hdr, total));
-      CUDA_TRY(cudaHostAlloc(&e->h_hdr, total, cudaHostAllocDefault));
-      e->hdr_cap = total;
-    }
-    if(gather_streams(e, m, longest, e->d_hdr, st)) return -1;
-    CUDA_TRY(cudaMemcpyAsync(e->h_hdr, e->d_hdr, total, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    uint64_t at = 0;
-    for(uint32_t i = 0; i < n; ++i)
-    {
-      if(!want[i])
-        continue;
-      const uint64_t got = want[i];
-      const int rc = b2k_parse_main_header(e->h_hdr + at, got, h[i]);
-      at += got;
-      want[i] = 0;
-      if(rc && h[i].short_read && got < len[i])
-        want[i] = std::min<uint64_t>(len[i], 2 * got);
-      else if(rc)
-      {
-        status[i] = rc;
-        e->batch_errors[i] = g_err;
-      }
-    }
-  }
-}
 
 /* the batch job of coding cp for n streams: the cached one when its coding matches and it has n slots or more, but not
    more than 4 n (its planes take memory in proportion to its slots: a large batch's job is not kept for small ones) */
@@ -3131,7 +3156,7 @@ extern "C" int32_t b2k_decode_codestreams_device(b2k_engine* e, uint32_t n, cons
   /* what the caller queued before the call (the kernels, receives or reads that produced the streams) comes first */
   if(queue_after(e, caller, st)) return -1;
   std::vector<b2k::t2::MainHeader> h(n);
-  if(read_batch_headers(e, n, cs, len, st, status, h)) return -1;
+  if(read_batch_headers(e, n, cs, len, b2k::t2::BATCH_HEADER_PREFIX, st, status, h.data(), e->batch_errors.data())) return -1;
   uint32_t ref = n;
   for(uint32_t i = 0; i < n && ref == n; ++i)
     if(!status[i])
@@ -3139,7 +3164,6 @@ extern "C" int32_t b2k_decode_codestreams_device(b2k_engine* e, uint32_t n, cons
   if(ref == n)
     return failures();
   const b2k_coding cp = h[ref].cp;
-  const uint32_t flags = h[ref].flags();
   *cp_out = cp;
   for(uint32_t i = ref + 1; i < n; ++i)
     if(!status[i] && b2k_batch_coding_check(h[ref], ref, h[i], i))
@@ -3158,116 +3182,16 @@ extern "C" int32_t b2k_decode_codestreams_device(b2k_engine* e, uint32_t n, cons
         fail(i, jrc);
     return failures();
   }
-  if(!J->t2p || b2k_t2_parse_flags(J->t2p) != flags || b2k_t2_parse_streams(J->t2p) != J->slots)
-  { /* geometry and progression only: planned once for every batch of this coding */
-    b2k_t2_parse_destroy(J->t2p);
-    J->t2p = nullptr;
-    if(b2k_t2_parse_create(cp, flags, J->blocks.data(), J->blocks.size(), J->slot_tiles, J->coded_index.data(), J->coded_index.size(),
-                           &J->t2p, J->slots))
-      return -1;
-  }
-  /* the arena: stream i at a 256-byte boundary, the decoder's read-past slack after the last one; one gather launch */
-  std::vector<uint64_t> at(n, 0), plen(n, 0), sot(n, 0);
-  uint64_t total = 0, longest = 0;
-  uint32_t m = 0;
-  if(grow_copy_table(e, n)) return -1;
-  for(uint32_t i = 0; i < n; ++i)
-  {
-    if(status[i])
-      continue;
-    at[i] = total;
-    plen[i] = len[i];
-    sot[i] = h[i].sot;
-    e->h_copy[m++] = CopyEntry{cs[i], len[i], total};
-    longest = std::max(longest, len[i]);
-    total = b2k::t2::batch_arena_next(total, len[i]);
-  }
-  if(arena_reserve(J, total, total / 8)) return -1;
-  J->arena_sized = false;
-  e->last_parse_batch = true;
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  if(gather_streams(e, m, longest, J->d_bytes, st)) return -1;
-  if(b2k_t2_batch_enqueue(J->t2p, J->d_bytes, n, at.data(), plen.data(), sot.data(), J->d_enc_desc, J->d_dec_quant, J->d_dec_desc, st))
-    return -1;
-  CUDA_TRY(cudaStreamSynchronize(st));
   bool refinement = false;
-  for(uint32_t i = 0; i < n; ++i)
-  {
-    if(status[i])
-      continue;
-    bool r = false;
-    if(int prc = b2k_t2_batch_result(J->t2p, i, &r))
-      fail(i, prc);
-    refinement = refinement || r;
-  }
+  if(parse_streams(e, J, n, cs, len, h.data(), h[ref].flags(), true, status, e->batch_errors.data(), &refinement)) return -1;
   /* the image descriptors; a stream whose image is unusable is decoded (its slot is its own) but not written out */
   for(uint32_t i = 0; i < n; ++i)
     if(!status[i])
       if(int rc = check_device_planes(e, &cp, &imgs[i]))
         fail(i, rc);
-  /* the conversion's tables: one per component, or one for all when every image written is pixel-interleaved */
-  const int nc = cp.numcomps;
-  bool interleaved = nc > 1;
-  for(uint32_t i = 0; i < n; ++i)
-    if(!status[i])
-      interleaved = interleaved && device_group(imgs[i], nc) == nc;
-  const int group = interleaved ? nc : 1, tables = nc / group;
-  if(!J->h_batch_dst)
-  {
-    CUDA_TRY(cudaMalloc(&J->d_batch_dst, (size_t)J->slots * 4 * sizeof(BatchDst)));
-    CUDA_TRY(cudaHostAlloc(&J->h_batch_dst, (size_t)J->slots * 4 * sizeof(BatchDst), cudaHostAllocDefault));
-  }
-  for(int t = 0; t < tables; ++t)
-    for(uint32_t i = 0; i < n; ++i)
-    {
-      BatchDst& D = J->h_batch_dst[(size_t)t * n + i];
-      D = BatchDst{};
-      if(status[i])
-        continue;
-      const int c0 = t * group;
-      for(int k = 0; k < group; ++k)
-        D.src[k] = J->img.at((int)i * nc + c0 + k, cp.x0, cp.y0);
-      D.dst = imgs[i].comp[c0];
-      D.err = J->d_err + i; /* an image the HT decoder rejected blocks of is not written */
-      D.dpitch = imgs[i].row_pitch[c0];
-      D.step = imgs[i].col_step[c0];
-    }
-  CUDA_TRY(cudaMemcpyAsync(J->d_batch_dst, J->h_batch_dst, (size_t)tables * n * sizeof(BatchDst), cudaMemcpyHostToDevice, st));
-  /* block decode -> inverse -> images, chunk by chunk over the (slot, tile) ranges of the n slots used (as many chunks as
-     the job's pipeline has, whatever its slot count); the images whose last tile a chunk holds are written after it */
-  CUDA_TRY(cudaMemsetAsync(J->d_err, 0, n * sizeof(int), st));
-  J->dec_has_refinement = refinement;
-  const size_t used = (size_t)n * J->slot_tiles, T = J->slot_tiles;
-  const size_t nchunks = std::min<size_t>(J->chunk_tile.size() - 1, used);
-  const uint32_t w = cp.x1 - cp.x0, hgt = cp.y1 - cp.y0, sb = imgs[0].sample_bytes;
-  for(size_t k = 0; k < nchunks; ++k)
-  {
-    const size_t t0 = k * used / nchunks, t1 = (k + 1) * used / nchunks;
-    if(t1 <= t0)
-      continue;
-    if(enqueue_block_decode(e, J, k, nullptr, st, t0, t1)) return -1;
-    if(enqueue_inverse(J, st, t0, t1)) return -1;
-    const uint32_t s0 = (uint32_t)(t0 / T), s1 = (uint32_t)(t1 / T);
-    for(int t = 0; t < tables && s1 > s0; ++t)
-      b2k_launch_planes_to_containers(J->d_batch_dst + (size_t)t * n + s0, s1 - s0, group, J->img.pitch, sb, w, hgt, st);
-  }
-  CUDA_TRY(cudaEventRecord(J->ev[1], st));
-  /* the caller's stream goes on once its images are written */
-  if(queue_after(e, st, caller)) return -1;
-  CUDA_TRY(cudaEventSynchronize(J->ev[1]));
-  CUDA_TRY(cudaGetLastError());
-  float t = 0;
-  cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
-  if(ms_total) *ms_total = t;
-  /* the HT decoder's verdict, per slot */
-  std::vector<int> herr(n, 0);
-  CUDA_TRY(cudaMemcpy(herr.data(), J->d_err, n * sizeof(int), cudaMemcpyDeviceToHost));
-  for(uint32_t i = 0; i < n; ++i)
-    if(!status[i] && herr[i])
-    {
-      g_err = "HT decoder rejected " + std::to_string(herr[i]) + " block(s)";
-      fail(i, -2);
-    }
+  /* an image the HT decoder rejected blocks of is not written */
+  if(decode_slots(e, J, n, imgs, Rect{cp.x0, cp.y0, cp.x1, cp.y1}, refinement, false, caller, ms_total, status, e->batch_errors.data()))
+    return -1;
   return failures();
 }
 
@@ -3279,14 +3203,144 @@ extern "C" const char* b2k_decode_codestreams_error(b2k_engine* e, uint32_t i)
   return i < e->batch_errors.size() ? e->batch_errors[i].c_str() : "";
 }
 
-/* ---- batches of images in device memory (b2k_encode_codestreams_device) ---------------------------------------------
+/* ---- images in device memory to code streams (b2k_encode_codestream_device / b2k_encode_codestreams_device) -----------
  * n images of one coding become n code streams in one launch chain.  The images that pass their checks take slots
  * 0..m-1 of the batch job, in image order; chunk by chunk over the (slot, tile) ranges, one conversion launch per
  * component group brings the images whose first tile the chunk holds into their planes, then the forward transform and
  * the block coder run over the chunk.  The device writer (t2_device.cu) then writes the m streams behind each other.
  * A failed image takes no slot, so none of its samples is coded.  A stream the coder or the writer gives a verdict is
  * neither placed nor gathered, and the other streams' places depend only on their own lengths: no image can change
- * another stream's bytes.  Synchronisations: one, and a second when the output buffer has to grow. */
+ * another stream's bytes.  A single image is a batch of one in the engine's single-image job, written into its own
+ * buffer.  Synchronisations: one, and a second when the output buffer has to grow. */
+
+/* the images imgs[image_of[s]], which passed check_device_planes, in slots s of J, after the work queued on `caller`:
+   coded and written as code streams with `flags` into buf[0, cap), which grows as they need.  Image i's stream is
+   buf[offset[i], offset[i] + length[i]) when its status[i] stays 0; a stream the coder or writer gives a verdict gets
+   that status and, with `errors`, its text there.  0; 1 when the writer declines the flags (b2k_last_error says why, no
+   status is set); -1 for a failure of the call. */
+static int encode_images(b2k_engine* e, b2k_device_job* J, const b2k_device_planes* imgs, const std::vector<uint32_t>& image_of,
+                         uint32_t flags, cudaStream_t caller, uint8_t*& buf, uint64_t& cap, int32_t* status, uint64_t* offset,
+                         uint64_t* length, std::string* errors, double* ms_total)
+{
+  const b2k_coding& cp = J->cp;
+  cudaStream_t st = e->stream;
+  const uint32_t m = (uint32_t)image_of.size();
+  if(!J->t2 || b2k_t2_flags(J->t2) != flags || b2k_t2_streams(J->t2) != J->slots)
+  { /* geometry and flags only: planned once for every image or batch of this coding */
+    b2k_t2_destroy(J->t2);
+    J->t2 = nullptr;
+    if(int trc = b2k_t2_create(cp, flags, J->blocks.data(), J->blocks.size(), J->slot_tiles, J->coded_index.data(),
+                               J->coded_index.size(), &J->t2, J->slots))
+      return trc < 0 ? -1 : 1;
+  }
+  /* the conversion's tables: one per component, or one for all when every image is pixel-interleaved */
+  const int nc = cp.numcomps;
+  bool interleaved = nc > 1;
+  for(uint32_t i : image_of)
+    interleaved = interleaved && device_group(imgs[i], nc) == nc;
+  const int group = interleaved ? nc : 1, tables = nc / group;
+  if(!J->h_batch_src)
+  {
+    CUDA_TRY(cudaMalloc(&J->d_batch_src, (size_t)J->slots * 4 * sizeof(BatchSrc)));
+    CUDA_TRY(cudaHostAlloc(&J->h_batch_src, (size_t)J->slots * 4 * sizeof(BatchSrc), cudaHostAllocDefault));
+  }
+  for(int t = 0; t < tables; ++t)
+    for(uint32_t s = 0; s < m; ++s)
+    {
+      const b2k_device_planes& img = imgs[image_of[s]];
+      const int c0 = t * group;
+      BatchSrc& E = J->h_batch_src[(size_t)t * m + s];
+      E = BatchSrc{};
+      E.src = img.comp[c0];
+      E.spitch = img.row_pitch[c0];
+      E.step = img.col_step[c0];
+      E.dst = J->img.at((int)s * nc + c0, cp.x0, cp.y0);
+    }
+  /* what the caller queued before the call (the kernels that made the images) comes first */
+  if(queue_after(e, caller, st)) return -1;
+  CUDA_TRY(cudaEventRecord(J->ev[0], st));
+  CUDA_TRY(cudaMemcpyAsync(J->d_batch_src, J->h_batch_src, (size_t)tables * m * sizeof(BatchSrc), cudaMemcpyHostToDevice, st));
+  /* conversion -> forward transform -> block coder, chunk by chunk over the (slot, tile) ranges of the m slots used (as
+     many chunks as the job's pipeline has, whatever its slot count); an image is converted in the chunk of its first tile */
+  const size_t T = J->slot_tiles, used = (size_t)m * T;
+  const size_t nchunks = std::min<size_t>(J->chunk_tile.size() - 1, used);
+  const uint32_t w = cp.x1 - cp.x0, hgt = cp.y1 - cp.y0, sb = imgs[image_of[0]].sample_bytes;
+  for(size_t k = 0; k < nchunks; ++k)
+  {
+    const size_t t0 = k * used / nchunks, t1 = (k + 1) * used / nchunks;
+    if(t1 <= t0)
+      continue;
+    const uint32_t s0 = (uint32_t)((t0 + T - 1) / T), s1 = (uint32_t)((t1 + T - 1) / T);
+    for(int t = 0; t < tables && s1 > s0; ++t)
+      b2k_launch_containers_to_planes(J->d_batch_src + (size_t)t * m + s0, s1 - s0, group, J->img.pitch, J->img.plane_elems(), sb, w,
+                                      hgt, cp.sgnd, st);
+    if(enqueue_forward(J, st, false, t0, t1)) return -1;
+    if(enqueue_t1_blocks(J, st, t0, t1)) return -1;
+  }
+  CUDA_TRY(cudaGetLastError());
+  /* the caller's stream goes on once every image has been read */
+  if(queue_after(e, st, caller)) return -1;
+  /* the m code streams into buf; the call's one synchronisation reads their statuses and places */
+  for(;;)
+  {
+    if(b2k_t2_enqueue(J->t2, J->d_enc_desc, J->d_out, J->d_scratch, buf, cap, st, m))
+      return -1;
+    CUDA_TRY(cudaEventRecord(J->ev[1], st));
+    CUDA_TRY(cudaEventSynchronize(J->ev[1]));
+    const uint64_t need = b2k_t2_used(J->t2);
+    if(need <= cap)
+      break;
+    cudaFree(buf);
+    buf = nullptr;
+    cap = 0;
+    CUDA_TRY(cudaMalloc(&buf, need + need / 8 + 4096));
+    cap = need + need / 8 + 4096;
+  }
+  float t = 0;
+  cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
+  if(ms_total) *ms_total = t;
+  for(uint32_t s = 0; s < m; ++s)
+  {
+    const uint32_t i = image_of[s];
+    const int64_t r = b2k_t2_result(J->t2, s);
+    if(r < 0)
+    {
+      status[i] = (int32_t)r;
+      if(errors)
+        errors[i] = g_err;
+    }
+    else
+    {
+      offset[i] = b2k_t2_offset(J->t2, s);
+      length[i] = (uint64_t)r;
+    }
+  }
+  return 0;
+}
+
+extern "C" int64_t b2k_encode_codestream_device(b2k_engine* e, const b2k_coding* cp, const b2k_device_planes* img, uint32_t flags,
+                                                void* cuda_stream, const uint8_t** cs)
+{
+  if(!e || !cp || !cs)
+    return -1;
+  if(int rc = check_device_planes(e, cp, img))
+    return rc;
+  std::lock_guard<std::mutex> lock(e->mu);
+  int rc = 0;
+  b2k_device_job* J = cached_job(e, cp, 1, 0, &rc);
+  if(rc)
+    return rc;
+  CUDA_TRY(cudaSetDevice(e->device));
+  int32_t status = 0;
+  uint64_t offset = 0, length = 0;
+  if(encode_images(e, J, img, {0}, flags, caller_stream(cuda_stream), e->d_cs, e->cs_cap, &status, &offset, &length, nullptr, nullptr))
+    return -1;
+  if(status)
+    return status;
+  *cs = e->d_cs;
+  return (int64_t)length;
+}
+
 extern "C" int32_t b2k_encode_codestreams_device(b2k_engine* e, const b2k_coding* cp, uint32_t n, const b2k_device_planes* imgs,
                                                  uint32_t flags, void* cuda_stream, const uint8_t** cs, uint64_t* offset,
                                                  uint64_t* length, int32_t* status, double* ms_total)
@@ -3309,7 +3363,6 @@ extern "C" int32_t b2k_encode_codestreams_device(b2k_engine* e, const b2k_coding
     }
   std::lock_guard<std::mutex> lock(e->mu);
   CUDA_TRY(cudaSetDevice(e->device));
-  cudaStream_t caller = caller_stream(cuda_stream), st = e->stream;
   e->enc_batch_errors.assign(n, std::string());
   *cs = nullptr;
   auto fail = [&](uint32_t i, int32_t rc) {
@@ -3348,95 +3401,12 @@ extern "C" int32_t b2k_encode_codestreams_device(b2k_engine* e, const b2k_coding
     return -1;
   if(jrc)
     return fail_all(jrc);
-  if(!J->t2 || b2k_t2_flags(J->t2) != flags || b2k_t2_streams(J->t2) != J->slots)
-  { /* geometry and flags only: planned once for every batch of this coding */
-    b2k_t2_destroy(J->t2);
-    J->t2 = nullptr;
-    const int trc = b2k_t2_create(*cp, flags, J->blocks.data(), J->blocks.size(), J->slot_tiles, J->coded_index.data(),
-                                  J->coded_index.size(), &J->t2, J->slots);
-    if(trc < 0)
-      return -1;
-    if(trc)
-      return fail_all(-1);
-  }
-  /* the conversion's tables: one per component, or one for all when every image is pixel-interleaved */
-  const int nc = cp->numcomps;
-  bool interleaved = nc > 1;
-  for(uint32_t i : image_of)
-    interleaved = interleaved && device_group(imgs[i], nc) == nc;
-  const int group = interleaved ? nc : 1, tables = nc / group;
-  if(!J->h_batch_src)
-  {
-    CUDA_TRY(cudaMalloc(&J->d_batch_src, (size_t)J->slots * 4 * sizeof(BatchSrc)));
-    CUDA_TRY(cudaHostAlloc(&J->h_batch_src, (size_t)J->slots * 4 * sizeof(BatchSrc), cudaHostAllocDefault));
-  }
-  for(int t = 0; t < tables; ++t)
-    for(uint32_t s = 0; s < m; ++s)
-    {
-      const b2k_device_planes& img = imgs[image_of[s]];
-      const int c0 = t * group;
-      BatchSrc& E = J->h_batch_src[(size_t)t * m + s];
-      E = BatchSrc{};
-      E.src = img.comp[c0];
-      E.spitch = img.row_pitch[c0];
-      E.step = img.col_step[c0];
-      E.dst = J->img.at((int)s * nc + c0, cp->x0, cp->y0);
-    }
-  /* what the caller queued before the call (the kernels that made the images) comes first */
-  if(queue_after(e, caller, st)) return -1;
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  CUDA_TRY(cudaMemcpyAsync(J->d_batch_src, J->h_batch_src, (size_t)tables * m * sizeof(BatchSrc), cudaMemcpyHostToDevice, st));
-  /* conversion -> forward transform -> block coder, chunk by chunk over the (slot, tile) ranges of the m slots used (as
-     many chunks as the job's pipeline has, whatever its slot count); an image is converted in the chunk of its first tile */
-  const size_t T = J->slot_tiles, used = (size_t)m * T;
-  const size_t nchunks = std::min<size_t>(J->chunk_tile.size() - 1, used);
-  const uint32_t w = cp->x1 - cp->x0, hgt = cp->y1 - cp->y0, sb = imgs[image_of[0]].sample_bytes;
-  for(size_t k = 0; k < nchunks; ++k)
-  {
-    const size_t t0 = k * used / nchunks, t1 = (k + 1) * used / nchunks;
-    if(t1 <= t0)
-      continue;
-    const uint32_t s0 = (uint32_t)((t0 + T - 1) / T), s1 = (uint32_t)((t1 + T - 1) / T);
-    for(int t = 0; t < tables && s1 > s0; ++t)
-      b2k_launch_containers_to_planes(J->d_batch_src + (size_t)t * m + s0, s1 - s0, group, J->img.pitch, J->img.plane_elems(), sb, w,
-                                      hgt, cp->sgnd, st);
-    if(enqueue_forward(J, st, false, t0, t1)) return -1;
-    if(enqueue_t1_blocks(J, st, t0, t1)) return -1;
-  }
-  CUDA_TRY(cudaGetLastError());
-  /* the caller's stream goes on once every image has been read */
-  if(queue_after(e, st, caller)) return -1;
-  /* the m code streams into the batch's buffer; the call's one synchronisation reads their statuses and places */
-  for(;;)
-  {
-    if(b2k_t2_enqueue(J->t2, J->d_enc_desc, J->d_out, J->d_scratch, e->d_bcs, e->bcs_cap, st, m))
-      return -1;
-    CUDA_TRY(cudaEventRecord(J->ev[1], st));
-    CUDA_TRY(cudaEventSynchronize(J->ev[1]));
-    const uint64_t need = b2k_t2_used(J->t2);
-    if(need <= e->bcs_cap)
-      break;
-    cudaFree(e->d_bcs);
-    e->d_bcs = nullptr;
-    e->bcs_cap = 0;
-    CUDA_TRY(cudaMalloc(&e->d_bcs, need + need / 8 + 4096));
-    e->bcs_cap = need + need / 8 + 4096;
-  }
-  float t = 0;
-  cudaEventElapsedTime(&t, J->ev[0], J->ev[1]);
-  if(ms_total) *ms_total = t;
-  for(uint32_t s = 0; s < m; ++s)
-  {
-    const uint32_t i = image_of[s];
-    const int64_t r = b2k_t2_result(J->t2, s);
-    if(r < 0)
-      fail(i, (int32_t)r);
-    else
-    {
-      offset[i] = b2k_t2_offset(J->t2, s);
-      length[i] = (uint64_t)r;
-    }
-  }
+  const int rc = encode_images(e, J, imgs, image_of, flags, caller_stream(cuda_stream), e->d_bcs, e->bcs_cap, status, offset, length,
+                               e->enc_batch_errors.data(), ms_total);
+  if(rc < 0)
+    return -1;
+  if(rc)
+    return fail_all(-1);
   *cs = e->d_bcs;
   return failures();
 }

@@ -440,13 +440,6 @@ static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint32_t n, uint32_t nti
   return 0;
 }
 
-int b2k_t2_parse_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, const HtBlockDesc* d_enc, const float* d_quant,
-                         HtBlockDesc* d_dec, cudaStream_t st)
-{
-  J->h_sd[0] = StreamDesc{0, len, sot, 0, 0};
-  return enqueue_parse(J, cs, 1, J->ntiles, TileBox{J->ntiles, 0, 0, J->ntiles, 1}, J->d_count, d_enc, d_quant, d_dec, st);
-}
-
 int b2k_t2_batch_enqueue(T2Parse* J, const uint8_t* arena, uint32_t n, const uint64_t* at, const uint64_t* len, const uint64_t* sot,
                          const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
 {

@@ -15,19 +15,15 @@ int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* b
                         const uint32_t* coded_index, uint64_t ncoded, T2Parse** out, uint32_t streams = 1);
 void b2k_t2_parse_destroy(T2Parse* j);
 uint32_t b2k_t2_parse_flags(const T2Parse* j);
-/* on st: the parse of the code stream cs[0, len) in device memory, whose first SOT is at sot, then (d_dec != NULL) the
-   decoder's descriptors of the coded blocks from d_enc's templates and d_quant's step sizes; the status to the host.
-   Five launches, whatever the tile count. */
-int b2k_t2_parse_enqueue(T2Parse* j, const uint8_t* cs, uint64_t len, uint64_t sot, const HtBlockDesc* d_enc, const float* d_quant,
-                         HtBlockDesc* d_dec, cudaStream_t st);
-/* once st has reached the end of b2k_t2_parse_enqueue's work: 0, or b2k_codestream_parse's return code with its text;
+/* once st has reached the end of b2k_t2_window_enqueue's work: 0, or b2k_codestream_parse's return code with its text;
    *refinement: a block has refinement passes to decode */
 int b2k_t2_parse_result(const T2Parse* j, bool* refinement);
-/* ---- batches (b2k_decode_codestreams_device): streams of one coding, a parse made with `streams` >= n ----------------
+/* ---- streams of one coding (a single stream is a batch of one), a parse made with `streams` >= n --------------------
  * On st: the parse of the n code streams arena[at[s], at[s] + len[s]) whose first SOT is at sot[s] (sot[s] = 0: stream s
- * failed before its tile parts and is not parsed), in the same five launches, then (d_dec != NULL) descriptor s * ncoded + k
- * of every stream's coded block k from d_enc / d_quant's entry of the same index, pointing into the arena.  A stream that
- * fails, or is not parsed, gets length-0 descriptors (all-zero blocks).  The statuses to the host. */
+ * failed before its tile parts and is not parsed), in five launches whatever the tile count, then (d_dec != NULL)
+ * descriptor s * ncoded + k of every stream's coded block k from d_enc's templates and d_quant's step sizes of the same
+ * index, pointing into the arena.  A stream that fails, or is not parsed, gets length-0 descriptors (all-zero blocks).
+ * The statuses to the host. */
 int b2k_t2_batch_enqueue(T2Parse* j, const uint8_t* arena, uint32_t n, const uint64_t* at, const uint64_t* len, const uint64_t* sot,
                          const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st);
 /* once the statuses have arrived: stream s's b2k_codestream_parse return code (its text set when not 0) */

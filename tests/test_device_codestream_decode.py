@@ -258,6 +258,27 @@ def test_untrusted_plt_and_damage(engine):
     assert walked["cut_at_a_packet"] == (11, 1)                  # PLT runs past the data: the walk stops where it ends
 
 
+def test_ht_decoder_rejection_writes_the_image(engine):
+    """a stream the HT decoder rejects: -2 with the host path's text, and the image written all the same, with the pixels
+    b2k_codestream_parse + b2k_decode_device of its bytes write (a batch leaves such an image alone)"""
+    torch = pytest.importorskip("torch")
+    import test_device_batch_decode as B
+    bad, text = B._ht_reject(engine, torch, _base_stream(engine))
+    cp, blocks = G.codestream_parse(bad)
+    shape = (cp.numcomps, cp.y1 - cp.y0, cp.x1 - cp.x0)
+    want = torch.full(shape, B.SENTINEL, dtype=torch.uint16, device="cuda")
+    with pytest.raises(G.EngineError) as host:
+        engine.decode_device(cp, blocks, bad, want)
+    got = torch.full(shape, B.SENTINEL, dtype=torch.uint16, device="cuda")
+    with pytest.raises(G.EngineError) as dev:
+        engine.decode_codestream_device(_dev(torch, bad), out=got)
+    torch.cuda.synchronize()
+    assert " -> -2: " in str(host.value) and " -> -2: " in str(dev.value)
+    assert _reason(dev.value) == _reason(host.value) == text
+    assert not (want == B.SENTINEL).all()
+    assert torch.equal(got, want)
+
+
 # ---- ordering, reuse, size ------------------------------------------------------------------------------------------------
 def test_stream_ordering(engine):
     torch = pytest.importorskip("torch")

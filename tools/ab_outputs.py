@@ -9,9 +9,11 @@ rebuilds from them, as .npy files under OUT.  Cases: tests/test_gpu.py's GEOMS, 
 coding the engine refuses are skipped), the 9/7 degenerate-geometry shapes, a 2048^2 single-tile 9/7 image, and the
 sample transports of the one-call entry points: a b2k_encode16 / b2k_decode16 round trip, b2k_encode16_interleaved,
 b2k_encode / b2k_decode with host packing forced on, 16-bit windowed decodes (b2k_decode_window), and, where torch has
-CUDA, b2k_encode_device / b2k_decode_device with uint16 tensors.  Every one-call entry point except the windowed decode
-also stores b2k_launch_count() before and after the call.  Last come the device-resident round trips (b2k_job_roundtrip,
-_roundtrip_n, _roundtrip_pipelined_n (2, 2)): on config 2 the launch count around each and its coded size, on a tiled 9/7
+CUDA, b2k_encode_device / b2k_decode_device with uint16 tensors and the entry points whose code streams live in device
+memory (device_codestreams: single and batch encodes and decodes, the parse, windows and failures).  Every one-call entry
+point except the host windowed decode also stores the launches it made (b2k_launch_count() after the call minus before),
+so that a change in one leg's count does not show in the legs after it.  Last come the device-resident round trips
+(b2k_job_roundtrip, _roundtrip_n, _roundtrip_pipelined_n (2, 2)): on config 2 the launches of each and its coded size, on a tiled 9/7
 image the same and the planes left after four steps.  --compare exits 1 when any array differs; tolerances would
 hide a drift of one rounding step in the 9/7 inverse, so there are none."""
 import os
@@ -59,6 +61,141 @@ def one_case(G, P, eng, args):
         job.close()
 
 
+def device_codestreams(G, P, eng, torch, counted, arrs):
+    """The code-stream entry points whose streams live in device memory, on a 9-tile 12-bit image (tensors of uint16 and
+    int32, CHW and HWC): the single and batch encodes (bytes, offsets, statuses), the single decode, the parse (coding,
+    block table, stats), windows at reduce 0 and 2 (one window takes every tile, one does not), and the batch decode
+    (pixels, statuses).  Failures record the return code, the text and the Coding left in cp_out (pre-filled with 0xA5):
+    a damaged SOT, a damaged main header, a block table too small, a bad image descriptor, a stream the HT decoder
+    rejects (with the pixels the single call writes), an 8-bit container under a 12-bit coding and flags the writer
+    declines."""
+    import ctypes as C
+    import test_device_batch_decode as BD
+    import test_device_batch_encode as BE
+    import test_device_codestream_decode as E
+    L = BE._lib()
+    L.b2k_decode_codestream_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(G.DevicePlanes), C.c_void_p,
+                                               C.POINTER(G.Coding), C.POINTER(C.c_double)]
+    L.b2k_codestream_parse_device.restype = C.c_int64
+    L.b2k_codestream_parse_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(G.Coding), C.c_void_p,
+                                              C.c_uint64]
+
+    def text(rc):
+        return np.frombuffer((L.b2k_last_error() or b"").decode().encode() if rc else b"", np.uint8)
+
+    def sentinel_coding():
+        got = G.Coding()
+        C.memset(C.addressof(got), 0xA5, C.sizeof(got))
+        return got
+
+    def dev(a):
+        return torch.from_numpy(np.array(a, np.uint8)).cuda()
+
+    cp = G.make_coding(700, 500, 3, 12, numres=5, tile=(256, 192), origin=(5, 11), tile_origin=(0, 0))
+    h, w = cp.y1 - cp.y0, cp.x1 - cp.x0
+    chw = [torch.from_numpy(np.stack(P.synthetic_image(w, h, 3, 12, seed=s, origin=(5, 11))).astype(np.uint16)).cuda()
+           for s in (31, 32, 33)]
+    flags = G.CS_TLM | G.CS_PLT
+    # encodes: one image; a batch of three with a misaligned descriptor between them
+    cs = counted("dcs_enc", lambda: eng.encode_codestream_device(cp, chw[0], flags, device_output=True))
+    arrs["dcs_enc_bytes"] = cs.cpu().numpy()
+    descs = [G.device_planes(t, 3, h, w) for t in chw]
+    bad = torch.zeros(16, dtype=torch.uint16, device="cuda")
+    descs.insert(1, G.device_planes(chw[1], 3, h, w))
+    descs[1].comp[1] = bad.data_ptr() + 1
+    rc, status, got, offsets = counted("dcs_enc_batch", lambda: BE._raw_batch(eng, torch, cp, descs, flags))
+    arrs["dcs_enc_batch_rc"] = np.array([rc])
+    arrs["dcs_enc_batch_status"] = np.array([s[0] for s in status])
+    arrs["dcs_enc_batch_text"] = np.frombuffer("\n".join(s[1] for s in status).encode(), np.uint8)
+    arrs["dcs_enc_batch_offsets"] = np.array(offsets, np.uint64)
+    arrs["dcs_enc_batch_bytes"] = np.concatenate([g for g in got if g is not None])
+    # single decodes of that stream, its parse
+    for tag, dtype, layout in (("u16", torch.uint16, "CHW"), ("u16_hwc", torch.uint16, "HWC"), ("i32", torch.int32, "CHW")):
+        _, out = counted("dcs_dec_" + tag, lambda: eng.decode_codestream_device(cs, dtype=dtype, layout=layout))
+        torch.cuda.synchronize()
+        arrs["dcs_dec_%s_rec" % tag] = out.cpu().numpy()
+    pcp, blocks = counted("dcs_parse", lambda: eng.codestream_parse_device(cs))
+    arrs["dcs_parse_coding"], arrs["dcs_parse_blocks"] = np.frombuffer(bytes(pcp), np.uint8), blocks
+    arrs["dcs_parse_stats"] = np.array(eng.codestream_parse_device_stats())
+    # windows
+    for i, win in enumerate([(5, 11, 705, 511), (37, 200, 650, 333)]):
+        for reduce in (0, 2):
+            tag = "dcs_win%d_r%d" % (i, reduce)
+            vcp, out = counted(tag, lambda: eng.decode_window_device(cs, win, reduce))
+            torch.cuda.synchronize()
+            arrs[tag + "_rec"], arrs[tag + "_coding"] = out.cpu().numpy(), np.frombuffer(bytes(vcp), np.uint8)
+            arrs[tag + "_rect"] = np.array(eng._window_rect(vcp, win, reduce))
+            arrs[tag + "_stats"] = np.array(eng.codestream_window_device_stats(), np.uint64)
+            arrs[tag + "_parse_stats"] = np.array(eng.codestream_parse_device_stats())
+    # damaged streams
+    host = cs.cpu().numpy()
+    last = E._sots(host)[-1]
+    sot = host.copy()
+    sot[last + 4:last + 6] = 0xFF                                   # a tile index out of range
+    hdr = host.copy()
+    hdr[0:2] = 0                                                    # no SOC
+    good = E._base_stream(eng)                                      # the stream the batch tests find an HT rejection in
+    ht, _ = BD._ht_reject(eng, torch, good)
+    hcp = G.codestream_parse(good)[0]
+
+    def raw_decode(tag, stream, coding, misaligned=False):
+        nc, hh, ww = coding.numcomps, coding.y1 - coding.y0, coding.x1 - coding.x0
+        out = torch.full((nc, hh, ww), 0x5A, dtype=torch.uint16, device="cuda")
+        img = G.device_planes(out, nc, hh, ww, writable=True)
+        if misaligned:
+            img.comp[1] = bad.data_ptr() + 1
+        d, got, ms = dev(stream), sentinel_coding(), C.c_double()
+        rc = counted(tag, lambda: L.b2k_decode_codestream_device(eng._h, d.data_ptr(), d.numel(), C.byref(img), None, C.byref(got),
+                                                                 C.byref(ms)))
+        torch.cuda.synchronize()
+        arrs[tag + "_rc"], arrs[tag + "_text"], arrs[tag + "_cp"] = np.array([rc]), text(rc), np.frombuffer(bytes(got), np.uint8)
+        arrs[tag + "_rec"] = out.cpu().numpy()
+
+    def raw_parse(tag, stream, cap):
+        d, got = dev(stream), sentinel_coding()
+        blocks = np.zeros(max(cap, 1), G.BLOCK_DTYPE)
+        rc = counted(tag, lambda: L.b2k_codestream_parse_device(eng._h, d.data_ptr(), d.numel(), None, C.byref(got), blocks.ctypes.data,
+                                                                cap))
+        arrs[tag + "_rc"], arrs[tag + "_cp"] = np.array([rc]), np.frombuffer(bytes(got), np.uint8)
+        arrs[tag + "_text"] = text(rc < 0 or rc == 1)
+        arrs[tag + "_blocks"] = blocks
+
+    nb = len(blocks)
+    for tag, stream in (("sot", sot), ("header", hdr)):
+        raw_decode("dcs_fail_%s_dec" % tag, stream, cp)
+        raw_parse("dcs_fail_%s_parse" % tag, stream, nb)
+    raw_parse("dcs_fail_table_parse", host, nb - 1)
+    raw_decode("dcs_fail_image_dec", host, cp, misaligned=True)
+    raw_decode("dcs_fail_ht_dec", ht, hcp)
+    # a batch of good and failing streams: statuses, and the pixels of the streams that decode
+    batch = [cs, dev(sot), eng.encode_codestream_device(cp, chw[1], flags, device_output=True), dev(hdr),
+             eng.encode_codestream_device(cp, chw[2], flags, device_output=True)]
+    _, out, status = counted("dcs_dec_batch", lambda: eng.decode_codestreams_device(batch))
+    torch.cuda.synchronize()
+    arrs["dcs_dec_batch_rec"] = out.cpu().numpy()
+    arrs["dcs_dec_batch_status"] = np.array([s[0] for s in status])
+    arrs["dcs_dec_batch_text"] = np.frombuffer("\n".join(s[1] for s in status).encode(), np.uint8)
+    arrs["dcs_dec_batch_stats"] = np.array(eng.codestream_parse_device_stats())
+    hbatch = [dev(good), dev(ht), dev(good)]
+    _, out, status = counted("dcs_dec_batch_ht", lambda: eng.decode_codestreams_device(hbatch))
+    torch.cuda.synchronize()
+    arrs["dcs_dec_batch_ht_rec"] = out.cpu().numpy()
+    arrs["dcs_dec_batch_ht_status"] = np.array([s[0] for s in status])
+    # encode verdicts: an 8-bit container under a 12-bit coding, and progression order 5, which the writer declines
+    u8_image = chw[0].to(torch.uint8)
+    u8 = G.device_planes(u8_image, 3, h, w)
+    for tag, img, f in (("u8", u8, flags), ("prog5", descs[0], G.CS_PROG(5) | G.CS_PLT)):
+        rc, txt, data = counted("dcs_fail_enc_" + tag, lambda: BE._single(eng, torch, cp, img, f))
+        arrs["dcs_fail_enc_%s_rc" % tag] = np.array([rc])
+        arrs["dcs_fail_enc_%s_text" % tag] = np.frombuffer(txt.encode(), np.uint8)
+        rc, status, _, _ = counted("dcs_fail_enc_batch_" + tag, lambda: BE._raw_batch(eng, torch, cp, [img, img], f))
+        arrs["dcs_fail_enc_batch_%s_rc" % tag] = np.array([rc])
+        arrs["dcs_fail_enc_batch_%s_status" % tag] = np.frombuffer(repr(status).encode(), np.uint8)
+    for k in sorted(arrs):
+        if k.startswith("dcs_") and k.endswith("_launches"):
+            print("%s: %d launches" % (k[:-len("_launches")], arrs[k][0]))
+
+
 def run(outdir):
     import grok_b200 as G
     import oracle_pipeline as P
@@ -77,7 +214,7 @@ def run(outdir):
     def counted(name, fn):
         before = int(G.lib().b2k_launch_count())
         r = fn()
-        arrs[name + "_launches"] = np.array([before, int(G.lib().b2k_launch_count())], np.uint64)
+        arrs[name + "_launches"] = np.array([int(G.lib().b2k_launch_count()) - before], np.uint64)
         return r
 
     def keep(name, res):
@@ -126,6 +263,7 @@ def run(outdir):
             counted("dev_%s_dec" % layout, lambda: eng.decode_device(cp, blocks, data, out, layout=layout))
             torch.cuda.synchronize()
             arrs["dev_%s_rec" % layout] = out.cpu().numpy()
+        device_codestreams(G, P, eng, torch, counted, arrs)
     # 16-bit windowed decodes of a tiled image with an odd origin, at full and half resolution
     cp = G.make_coding(700, 500, 3, 12, numres=5, tile=(256, 192), origin=(5, 11), tile_origin=(0, 0), irreversible=True)
     cs = eng.encode_codestream(cp, P.synthetic_image(700, 500, 3, 12, seed=23, origin=(5, 11)))
@@ -144,7 +282,7 @@ def run(outdir):
             for name, fn in (("one", job.roundtrip), ("n", lambda: job.roundtrip_n(8 if tag == "rt_config2" else 1)),
                              ("pipelined", lambda: job.roundtrip_pipelined_n(8 if tag == "rt_config2" else 2, 2, 2))):
                 arrs["%s_%s_coded" % (tag, name)] = np.array([counted("%s_%s" % (tag, name), fn)[-1]], np.uint64)
-                print("%s %s: %d launches" % (tag, name, np.diff(arrs["%s_%s_launches" % (tag, name)])[0]))
+                print("%s %s: %d launches" % (tag, name, arrs["%s_%s_launches" % (tag, name)][0]))
             rec = [np.zeros_like(p) for p in img]
             job.download(rec)
             if tag == "rt_97":
