@@ -795,13 +795,66 @@ static void load_quad(const uint32_t* buf, uint32_t stride, uint32_t w, uint32_t
   }
 }
 
-/* HT cleanup-pass encoder: ojph_encode_codeblock32, ojph_block_encoder.cpp L542-1017.
- * buf: sign-magnitude words (sign bit 31, magnitude << (30 - missing_msbs)).
- * Returns the coded length, or -1 on a buffer overflow the reference would have reported. */
-ORC_API int orc_ht_encode(const uint32_t* buf, uint32_t missing_msbs, uint32_t width, uint32_t height,
-                          uint32_t stride, uint8_t* out, uint32_t out_cap)
+/* The choices T.814 leaves to an encoder, as orc_ht_encode_foreign takes them (bit set).  orc_ht_encode makes none of
+ * them: it codes like the reference.  Each one below is decoded by the reference decoder (oracle/_ref) to the source's
+ * bin-centre values, pinned by tests/golden/ht_foreign.npz. */
+enum
+{
+  ORC_FOREIGN_ROWS = 1,        /* any legal CxtVLC row of a u_off = 1 quad, not the one with the most e_k bits */
+  ORC_FOREIGN_RAISE_U = 2,     /* exponent bound U_q above max(E_max, kappa), up to missing_msbs + 2 */
+  ORC_FOREIGN_NO_FUSE = 4,     /* MEL and VLC terminated in separate bytes even where one byte could end both */
+  ORC_FOREIGN_PAD_MAGSGN = 8,  /* bytes after the MagSgn data that the decoder never reads */
+  ORC_FOREIGN_PAD_SCUP = 16,   /* bytes between the MEL and the VLC data (a larger Scup, at most 4079) */
+};
+
+/* per-call counts of the choices made, for the coverage tests: [0] quads whose U_q is the decoder's limit, [1] u_off = 1
+ * quads coded with a row the max-popcount rule would not pick, [2] raises dropped for want of a row with e_1 = 0;
+ * [3] the MEL bytes of the stream (where MEL ends and padding or VLC begins, for tests that edit streams) */
+static int32_t foreign_stats[4];
+ORC_API void orc_ht_encode_foreign_stats(int32_t* out) { memcpy(out, foreign_stats, sizeof(foreign_stats)); }
+
+typedef struct { uint64_t s; } orc_lcg;
+static uint32_t lcg_next(orc_lcg* g)
+{
+  g->s = g->s * 6364136223846793005ULL + 1442695040888963407ULL;
+  return (uint32_t)(g->s >> 33);
+}
+
+/* the rows of table t (0: first quad row, 1: the others) a quad (c_q, rho) may be coded with when its u_off is 1 and
+ * the samples whose exponent equals U_q are `emb`: e_1 == emb & e_k (an e_k sample has U_q - 1 bits and e_1 as its
+ * implied top bit).  Writes up to 16 candidates as enc_vlc entries; returns their count and, in *best, the index of the
+ * one orc_ht_encode's table holds (most e_k bits, the last of equals) */
+static int legal_rows(int t, int cq, int rho, int emb, uint16_t* cand, int* best)
+{
+  const uint32_t* src = t ? T814_VLC_ROWS1 : T814_VLC_ROWS0;
+  const size_t nsrc = t ? sizeof(T814_VLC_ROWS1) / 4 : sizeof(T814_VLC_ROWS0) / 4;
+  int n = 0, best_pop = -1;
+  *best = -1;
+  for(size_t j = 0; j < nsrc && n < 16; ++j)
+  {
+    int c, r, u, ek, e1, cwd, len;
+    unpack_row(src[j], &c, &r, &u, &ek, &e1, &cwd, &len);
+    if(c != cq || r != rho || u != 1 || (emb & ek) != e1)
+      continue;
+    if(__builtin_popcount((unsigned)ek) >= best_pop)
+    {
+      best_pop = __builtin_popcount((unsigned)ek);
+      *best = n;
+    }
+    cand[n++] = (uint16_t)((cwd << 8) | (len << 4) | ek);
+  }
+  return n;
+}
+
+/* HT cleanup-pass encoder: ojph_encode_codeblock32, ojph_block_encoder.cpp L542-1017, with the encoder's choices of
+ * `choices` (ORC_FOREIGN_*) made by an LCG seeded with `seed`; choices = 0 is orc_ht_encode. */
+static int ht_encode_core(const uint32_t* buf, uint32_t missing_msbs, uint32_t width, uint32_t height, uint32_t stride,
+                          uint32_t choices, uint64_t seed, uint8_t* out, uint32_t out_cap)
 {
   build_tables();
+  orc_lcg rng = {seed ^ 0x9E3779B97F4A7C15ULL};
+  memset(foreign_stats, 0, sizeof(foreign_stats));
+  const int u_limit = (int)missing_msbs + 2; /* ojph_block_decoder32.cpp L846, L1114: U_q > missing_msbs + 2 is refused */
   enum { MS_CAP = (16384 * 16 + 14) / 15, MEL_CAP = 192, VLC_CAP = 3072 - 192 };
   uint8_t* ms_buf = (uint8_t*)malloc(MS_CAP);
   uint8_t mel_buf[MEL_CAP], vlc_buf[VLC_CAP];
@@ -841,12 +894,35 @@ ORC_API int orc_ht_encode(const uint32_t* buf, uint32_t missing_msbs, uint32_t w
           kappa = (Q[j].rho & (Q[j].rho - 1)) ? imax(1, max_e) : 1;
         }
         U[j] = imax(Q[j].emax, kappa);
+        uint16_t cand[16];
+        int ncand = 0, best = -1;
+        if((choices & ORC_FOREIGN_RAISE_U) && Q[j].rho && U[j] < u_limit)
+        { /* with U_q above every exponent no sample is in EMB: a u_off = 1 row with e_1 = 0 is needed */
+          const int raise = (lcg_next(&rng) & 3) == 0 ? u_limit - U[j] : (int)(lcg_next(&rng) % (uint32_t)(u_limit - U[j] + 1));
+          if(raise > 0)
+          {
+            ncand = legal_rows(y ? 1 : 0, cq[j], Q[j].rho, 0, cand, &best);
+            if(ncand)
+              U[j] += raise;
+            else
+              foreign_stats[2]++;
+          }
+        }
         u[j] = U[j] - kappa;
         int eps = 0;
         if(u[j] > 0)
           for(int i = 0; i < 4; ++i)
-            eps |= (Q[j].e[i] == Q[j].emax) << i;
+            eps |= (Q[j].e[i] == U[j]) << i;
         tuple[j] = enc_vlc[y ? 1 : 0][(cq[j] << 8) + (Q[j].rho << 4) + eps];
+        if(u[j] > 0 && (ncand || (choices & ORC_FOREIGN_ROWS)))
+        {
+          if(!ncand)
+            ncand = legal_rows(y ? 1 : 0, cq[j], Q[j].rho, eps, cand, &best);
+          const int pick = (choices & ORC_FOREIGN_ROWS) ? (int)(lcg_next(&rng) % (uint32_t)ncand) : best;
+          tuple[j] = cand[pick];
+          foreign_stats[1] += pick != best && (cand[pick] & 0xF) != (cand[best] & 0xF);
+        }
+        foreign_stats[0] += Q[j].rho && U[j] == u_limit;
         vlc_put(&vlc, tuple[j] >> 8, (tuple[j] >> 4) & 7);
         if(cq[j] == 0)
           mel_event(&mel, Q[j].rho != 0);
@@ -914,9 +990,18 @@ ORC_API int orc_ht_encode(const uint32_t* buf, uint32_t missing_msbs, uint32_t w
   {
     int fuse = mel.tmp | vlc.tmp;
     if((((fuse ^ mel.tmp) & mel_mask) | ((fuse ^ vlc.tmp) & vlc_mask)) == 0 && fuse != 0xFF &&
-       vlc.pos > 1)
+       vlc.pos > 1 && !(choices & ORC_FOREIGN_NO_FUSE))
     {
       if(mel.pos >= mel.cap) mel.err = 1; else mel.buf[mel.pos++] = (uint8_t)fuse;
+      if(choices & ORC_FOREIGN_PAD_SCUP)
+      { /* bytes will come between the two: the fused byte ends each of them */
+        if(vlc.pos >= vlc.cap) mel.err = 1;
+        else
+        {
+          *(vlc.last - vlc.pos) = (uint8_t)fuse;
+          vlc.pos++;
+        }
+      }
     }
     else
     {
@@ -929,35 +1014,70 @@ ORC_API int orc_ht_encode(const uint32_t* buf, uint32_t missing_msbs, uint32_t w
       }
     }
   }
-  /* ms_terminate L516-535 */
+  /* ms_terminate L516-535: a last byte of ones is left out, the decoder feeds 0xFF past the segment -- unless bytes
+     follow it in the segment, which the decoder would read in its place */
+  const int ms_pad = (choices & ORC_FOREIGN_PAD_MAGSGN) != 0;
   if(ms.used)
   {
     int t = ms.maxb - ms.used;
     ms.tmp |= (0xFFu & ((1u << t) - 1)) << ms.used;
     ms.used += t;
-    if(ms.tmp != 0xFF)
+    if(ms.tmp != 0xFF || ms_pad)
     {
       if(ms.pos >= ms.cap) ms.err = 1; else ms.buf[ms.pos++] = (uint8_t)ms.tmp;
     }
   }
-  else if(ms.maxb == 7)
+  else if(ms.maxb == 7 && !ms_pad)
     ms.pos--;
+  /* padding: bytes below 0x80, so that no pair of bytes in the segment reads as a marker */
+  const uint32_t npad_ms = ms_pad ? 1 + lcg_next(&rng) % 40 : 0;
+  uint32_t npad_scup = 0;
+  if(choices & ORC_FOREIGN_PAD_SCUP)
+  {
+    const uint32_t room = 4079 > mel.pos + vlc.pos ? 4079 - (mel.pos + vlc.pos) : 0;
+    npad_scup = (lcg_next(&rng) & 7) == 0 ? room : imin((int)room, 1 + (int)(lcg_next(&rng) % 48));
+  }
 
-  int total = (int)(mel.pos + vlc.pos + ms.pos);
+  int total = (int)(mel.pos + vlc.pos + ms.pos + npad_ms + npad_scup);
   int rc = total;
   if(mel.err || vlc.err || ms.err || (uint32_t)total > out_cap)
     rc = -1;
   else
   {
-    memcpy(out, ms.buf, ms.pos);
-    memcpy(out + ms.pos, mel.buf, mel.pos);
-    memcpy(out + ms.pos + mel.pos, vlc.last - vlc.pos + 1, vlc.pos);
-    uint32_t nb = mel.pos + vlc.pos; /* L1009-1014 */
+    uint8_t* o = out;
+    memcpy(o, ms.buf, ms.pos);
+    o += ms.pos;
+    for(uint32_t i = 0; i < npad_ms; ++i)
+      *o++ = (uint8_t)(lcg_next(&rng) & 0x7F);
+    memcpy(o, mel.buf, mel.pos);
+    o += mel.pos;
+    foreign_stats[3] = (int32_t)mel.pos;
+    for(uint32_t i = 0; i < npad_scup; ++i)
+      *o++ = (uint8_t)(lcg_next(&rng) & 0x7F);
+    memcpy(o, vlc.last - vlc.pos + 1, vlc.pos);
+    uint32_t nb = mel.pos + npad_scup + vlc.pos; /* L1009-1014 */
     out[total - 1] = (uint8_t)(nb >> 4);
     out[total - 2] = (uint8_t)((out[total - 2] & 0xF0) | (nb & 0xF));
   }
   free(ms_buf); free(eab); free(enew);
   return rc;
+}
+
+/* buf: sign-magnitude words (sign bit 31, magnitude << (30 - missing_msbs)).
+ * Returns the coded length, or -1 on a buffer overflow the reference would have reported. */
+ORC_API int orc_ht_encode(const uint32_t* buf, uint32_t missing_msbs, uint32_t width, uint32_t height,
+                          uint32_t stride, uint8_t* out, uint32_t out_cap)
+{
+  return ht_encode_core(buf, missing_msbs, width, height, stride, 0, 0, out, out_cap);
+}
+
+/* TEST INFRASTRUCTURE: the same cleanup pass as another HTJ2K encoder may write it, with the choices of `choices`
+ * (ORC_FOREIGN_*) made by an LCG seeded with `seed` -- streams this project's own coders never write, for testing the
+ * decoders on them.  choices = 0 gives orc_ht_encode's bytes. */
+ORC_API int orc_ht_encode_foreign(const uint32_t* buf, uint32_t missing_msbs, uint32_t width, uint32_t height,
+                                  uint32_t stride, uint32_t choices, uint64_t seed, uint8_t* out, uint32_t out_cap)
+{
+  return ht_encode_core(buf, missing_msbs, width, height, stride, choices, seed, out, out_cap);
 }
 
 /* ------------------------------------------------------------------------------------------ */

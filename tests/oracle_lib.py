@@ -95,6 +95,31 @@ def ht_encode(sgnmag, missing_msbs, cap=24576):
     return out[:n].copy()
 
 
+# the encoder choices of orc_ht_encode_foreign (ORC_FOREIGN_* in oracle/j2k_oracle.c)
+FOREIGN_ROWS, FOREIGN_RAISE_U, FOREIGN_NO_FUSE, FOREIGN_PAD_MAGSGN, FOREIGN_PAD_SCUP = 1, 2, 4, 8, 16
+FOREIGN_ALL = 31
+
+
+def ht_encode_foreign(sgnmag, missing_msbs, choices, seed, cap=24576, stats=False):
+    """The cleanup pass as another encoder may write it: the choices set in `choices`, picked by an LCG seeded with
+    `seed` (choices = 0: ht_encode's bytes).  stats=True also returns the encoder's counts of the choices made:
+    (quads with U_q at the decoder's limit, u_off = 1 quads whose e_k the max-popcount rule would not pick, raises
+    dropped for want of a row, MEL bytes)."""
+    a = np.ascontiguousarray(sgnmag, dtype=np.uint32)
+    h, w = a.shape
+    out = np.zeros(cap, np.uint8)
+    L = lib()
+    L.orc_ht_encode_foreign.argtypes = [_u32p] + [C.c_uint32] * 5 + [C.c_uint64, _u8p, C.c_uint32]
+    n = L.orc_ht_encode_foreign(a, missing_msbs, w, h, w, choices, seed, out, cap)
+    assert n >= 0, "oracle encoder overflow"
+    if not stats:
+        return out[:n].copy()
+    s = np.zeros(4, np.int32)
+    L.orc_ht_encode_foreign_stats.argtypes = [_i32p]
+    L.orc_ht_encode_foreign_stats(s)
+    return out[:n].copy(), tuple(int(v) for v in s)
+
+
 def ht_decode(data, missing_msbs, w, h):
     d = np.concatenate([np.asarray(data, np.uint8), np.zeros(8, np.uint8)])
     out = np.zeros((h, w), np.uint32)
