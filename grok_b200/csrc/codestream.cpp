@@ -21,9 +21,11 @@
 #include "b2k_internal.h"
 #include "t2_packet.h"
 #include "t2_plan.h"
+#include "t2_write.h"
 
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -357,115 +359,6 @@ void write_main_header(const b2k_coding& cp, const TileGrid& g, const std::vecto
   }
 }
 
-/* ---- one tile's packets ----------------------------------------------------------------------------------- */
-/* A tile part is planned first (packet headers, which byte ranges of the arena follow each of them, lengths) and
-   written straight into the caller's buffer afterwards: the ~150 MB of block bytes of a config-2 image are copied
-   exactly once. */
-struct TilePlan
-{
-  std::vector<uint8_t> hdrs;          /* all packet headers, back to back */
-  std::vector<uint32_t> hdr_len;      /* per packet */
-  std::vector<uint32_t> nseg;         /* per packet: block byte ranges that follow its header */
-  std::vector<uint64_t> seg_off;      /* arena offsets */
-  std::vector<uint32_t> seg_len;
-  std::vector<uint32_t> packet_len;   /* header + body */
-  std::vector<uint8_t> res_of;        /* per packet: its resolution (tile parts may be split there) */
-  /* tile parts: [first packet, end packet), their PLT marker segments and sizes (SOT + PLT + SOD + packets) */
-  struct Part
-  {
-    size_t p0, p1, h0, s0; /* packets, offset into hdrs, first segment */
-    std::vector<uint8_t> plt;
-    uint64_t bytes;
-  };
-  std::vector<Part> parts;
-  uint64_t size() const
-  {
-    uint64_t n = 0;
-    for(const Part& pt : parts)
-      n += pt.bytes;
-    return n;
-  }
-};
-
-int plan_tile_packets(const b2k_coding& cp, const Rect& tile, const b2k_block* blk, uint32_t nblk, uint64_t arena_len,
-                      TilePlan& plan, std::string& err, int prog, bool sop, bool eph)
-{
-  uint32_t nsop = 0;
-  std::vector<Packet> pkts;
-  uint32_t expect = 0;
-  tile_packets(cp, tile, pkts, expect, prog);
-  if(expect != nblk)
-  {
-    err = "block table does not match the tile's enumeration";
-    return -1;
-  }
-  std::vector<t2::TagNode> tags;
-  auto code = [blk](uint32_t i) {
-    const b2k_block& B = blk[i];
-    return t2::BlockCode{B.length, B.length2, B.numpasses, B.numbps, B.kmax};
-  };
-  uint8_t kmax = 0;
-  for(uint32_t i = 0; i < nblk; ++i)
-    kmax = std::max(kmax, blk[i].kmax);
-  for(const Packet& pk : pkts)
-  { /* the header goes straight into plan.hdrs, grown to the bound first */
-    const size_t at = plan.hdrs.size();
-    plan.hdrs.resize(at + t2::packet_header_bound(pk.band, pk.nbands, kmax));
-    tags.resize(std::max<size_t>(tags.size(), t2::packet_tag_nodes(pk.band, pk.nbands)));
-    t2::BitWriter bw;
-    bw.init(plan.hdrs.data() + at, plan.hdrs.size() - at);
-    if(t2::packet_header(bw, pk.band, pk.nbands, code, tags.data(), nsop, sop, eph))
-    {
-      err = "code block outside the writer's range (bit planes / passes)";
-      return -1;
-    }
-    if(bw.n > bw.cap)
-    {
-      err = "packet header longer than its bound";
-      return -1;
-    }
-    nsop = (nsop + 1) & 0xFFFF;
-    plan.hdrs.resize(at + bw.n);
-    plan.hdr_len.push_back((uint32_t)bw.n);
-    plan.res_of.push_back(pk.resno);
-    uint64_t plen = bw.n;
-    uint32_t ns = 0;
-    for(int b = 0; b < pk.nbands; ++b)
-    {
-      const PacketBand& pb = pk.band[b];
-      for(uint32_t k = 0; k < pb.gw * pb.gh; ++k)
-      {
-        const b2k_block& B = blk[pb.first + k];
-        if(!(B.numpasses && B.length))
-          continue;
-        const uint64_t n = (uint64_t)B.length + (B.numpasses > 1 ? B.length2 : 0);
-        if(B.offset + n > arena_len)
-        {
-          err = "block offsets exceed the byte arena";
-          return -1;
-        }
-        if(ns && plan.seg_off.back() + plan.seg_len.back() == B.offset && (uint64_t)plan.seg_len.back() + n < 0xFFFFFFFFull)
-          plan.seg_len.back() += (uint32_t)n; /* neighbours in the arena: one copy */
-        else
-        {
-          plan.seg_off.push_back(B.offset);
-          plan.seg_len.push_back((uint32_t)n);
-          ++ns;
-        }
-        plen += n;
-      }
-    }
-    plan.nseg.push_back(ns);
-    if(plen > 0xFFFFFFFFull)
-    {
-      err = "packet longer than 4 GiB";
-      return -1;
-    }
-    plan.packet_len.push_back((uint32_t)plen);
-  }
-  return 0;
-}
-
 /* where a tile's tile parts end (packet indices): one part for the whole tile, or one per run of packets of the same
    resolution; a tile without packets still has one (empty) tile part */
 std::vector<size_t> tile_part_ends(const std::vector<uint8_t>& res_of, bool split_res)
@@ -483,86 +376,18 @@ std::vector<size_t> tile_part_ends(const std::vector<uint8_t>& res_of, bool spli
   return ends;
 }
 
-/* cut the planned packets into tile parts and build each part's PLT */
-void plan_tile_parts(TilePlan& P, bool split_res, bool want_plt)
+/* the main header for `flags`, with the TLM segments of nparts tile parts (entries zero) behind it: where TLM starts */
+uint64_t main_header(const b2k_coding& cp, uint32_t flags, uint64_t nparts, std::vector<uint8_t>& head)
 {
-  size_t p = 0, h = 0, sg = 0;
-  for(const size_t end : tile_part_ends(P.res_of, split_res))
+  write_main_header(cp, tile_grid(cp), band_quant(cp), head, (int)((flags >> 8) & 7), (flags & B2K_CS_SOP) != 0, (flags & B2K_CS_EPH) != 0);
+  const uint64_t at = head.size();
+  if(flags & B2K_CS_TLM)
   {
-    TilePlan::Part part;
-    part.p0 = p;
-    part.h0 = h;
-    part.s0 = sg;
-    uint64_t body = 0;
-    for(; p < end; ++p)
-    {
-      body += P.packet_len[p];
-      h += P.hdr_len[p];
-      sg += P.nseg[p];
-    }
-    part.p1 = p;
-    if(want_plt)
-    {
-      auto len = [&P](uint64_t k) { return P.packet_len[k]; };
-      part.plt.resize(t2::plt_segments(len, part.p0, part.p1, nullptr));
-      t2::plt_segments(len, part.p0, part.p1, part.plt.data());
-    }
-    part.bytes = 12 + part.plt.size() + 2 + body;
-    P.parts.push_back(std::move(part));
+    head.resize(at + t2::tlm_bytes(nparts), 0);
+    for(uint64_t e0 = 0; e0 < nparts; e0 += t2::TLM_PER_SEGMENT)
+      t2::put_tlm_segment(head.data() + at, e0, std::min<uint64_t>(t2::TLM_PER_SEGMENT, nparts - e0));
   }
-}
-
-} // namespace
-
-
-namespace
-{
-/* SOT, [PLT], SOD and the packets of every tile part of one planned tile, written at w (plan.size() bytes) */
-void emit_tile_parts(const TilePlan& P, uint32_t t, const uint8_t* arena, uint8_t* w)
-{
-  for(size_t pi = 0; pi < P.parts.size(); ++pi)
-  {
-    const TilePlan::Part& pt = P.parts[pi];
-    t2::put_sot(w, t, (uint32_t)pt.bytes, (uint32_t)pi, (uint32_t)P.parts.size());
-    w += 12;
-    if(!pt.plt.empty())
-    {
-      memcpy(w, pt.plt.data(), pt.plt.size());
-      w += pt.plt.size();
-    }
-    *w++ = 0xFF; /* SOD */
-    *w++ = 0x93;
-    const uint8_t* h = P.hdrs.data() + pt.h0;
-    size_t sg = pt.s0;
-    for(size_t k = pt.p0; k < pt.p1; ++k)
-    {
-      memcpy(w, h, P.hdr_len[k]);
-      w += P.hdr_len[k];
-      h += P.hdr_len[k];
-      for(uint32_t i = 0; i < P.nseg[k]; ++i, ++sg)
-      {
-        memcpy(w, arena + P.seg_off[sg], P.seg_len[sg]);
-        w += P.seg_len[sg];
-      }
-    }
-  }
-}
-
-/* TLM segments (A.7.1) for n tile parts appended to head, their entries zero; returns where they start */
-size_t append_tlm_segments(std::vector<uint8_t>& head, uint64_t n)
-{
-  const size_t at = head.size();
-  head.resize(at + t2::tlm_bytes(n), 0);
-  for(uint64_t e0 = 0; e0 < n; e0 += t2::TLM_PER_SEGMENT)
-    t2::put_tlm_segment(head.data() + at, e0, std::min<uint64_t>(t2::TLM_PER_SEGMENT, n - e0));
   return at;
-}
-/* TLM: 16-bit tile index + 32-bit length per tile part, in codestream order */
-void append_tlm(std::vector<uint8_t>& head, const std::vector<std::pair<uint32_t, uint32_t>>& ent)
-{
-  const size_t at = append_tlm_segments(head, ent.size());
-  for(size_t e = 0; e < ent.size(); ++e)
-    t2::put_tlm_entry(head.data() + at, e, ent[e].first, ent[e].second);
 }
 
 /* what b2k_codestream_write checks before it looks at a block: 0, or -1 with the error set */
@@ -593,19 +418,233 @@ int check_whole_image(const b2k_coding& cp, uint32_t num_tiles, uint32_t flags)
   return 0;
 }
 
-/* blocks of tile t are [first[t], first[t + 1]); false if the table is not in tile order */
-bool tile_block_ranges(const b2k_block* blocks, uint64_t n, uint32_t ntiles, std::vector<uint64_t>& first)
+/* the plan of tiles t % tile_mod == tile_rem of cp, whose blocks `blocks` holds in tile order; the tiles are planned on the
+   host pool.  0; 1 when the table is not those tiles' blocks in tile order (no error set); -1 with the error of the first
+   tile the plan declines, `plan` then holding the packets and tile parts of the tiles before it. */
+int plan_tiles(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks, uint64_t nblocks, uint32_t tile_mod, uint32_t tile_rem,
+               t2::Plan& plan)
 {
-  first.assign(ntiles + 1, 0);
+  plan = t2::Plan();
+  plan.flags = flags;
+  const TileGrid g = tile_grid(cp);
+  std::vector<uint32_t> mine;
+  for(uint32_t t = tile_rem; t < g.nx * g.ny; t += tile_mod)
+    mine.push_back(t);
+  std::vector<uint64_t> first(mine.size() + 1);
   uint64_t i = 0;
-  for(uint32_t t = 0; t < ntiles; ++t)
+  for(size_t k = 0; k < mine.size(); ++k)
   {
-    first[t] = i;
-    while(i < n && blocks[i].tile == t)
+    first[k] = i;
+    while(i < nblocks && blocks[i].tile == mine[k])
       ++i;
   }
-  first[ntiles] = i;
-  return i == n;
+  first[mine.size()] = i;
+  if(i != nblocks)
+    return 1;
+  const int prog = (int)((flags >> 8) & 7);
+  const bool split_res = (flags & B2K_CS_TPARTS_R) != 0 && prog <= 2; /* a tile part per resolution needs a resolution-major order */
+  struct TileSlice /* one tile's packets and parts, numbered within the tile */
+  {
+    std::vector<t2::DevPacket> packets;
+    std::vector<t2::DevPart> parts;
+    uint64_t hdr_bytes = 0, tag_nodes = 0;
+    const char* err = nullptr;
+  };
+  std::vector<TileSlice> tiles(mine.size());
+  b2k_host_parallel(mine.size(), [&](size_t k) {
+    TileSlice& T = tiles[k];
+    std::vector<Packet> pkts;
+    uint32_t expect = 0;
+    tile_packets(cp, tile_rect(cp, g, mine[k]), pkts, expect, prog);
+    if(expect != first[k + 1] - first[k])
+    {
+      T.err = "block table does not match the tile's enumeration";
+      return;
+    }
+    uint8_t kmax = 0;
+    for(uint64_t b = first[k]; b < first[k + 1]; ++b)
+      kmax = std::max(kmax, blocks[b].kmax);
+    std::vector<uint8_t> res_of;
+    for(size_t p = 0; p < pkts.size(); ++p)
+    {
+      const Packet& pk = pkts[p];
+      t2::DevPacket d{};
+      for(int b = 0; b < pk.nbands; ++b)
+        d.band[b] = t2::BandGrid{(uint32_t)first[k] + pk.band[b].first, pk.band[b].gw, pk.band[b].gh};
+      d.nbands = pk.nbands;
+      d.sop = (uint32_t)(p & 0xFFFF);
+      const uint64_t cap = t2::packet_header_bound(pk.band, pk.nbands, kmax);
+      if(cap > 0xFFFFFFFFull)
+      {
+        T.err = "packet longer than 4 GiB";
+        return;
+      }
+      d.hdr_cap = (uint32_t)cap;
+      d.hdr_at = T.hdr_bytes;
+      d.tag_at = T.tag_nodes;
+      T.hdr_bytes += cap;
+      T.tag_nodes += t2::packet_tag_nodes(pk.band, pk.nbands);
+      T.packets.push_back(d);
+      res_of.push_back(pk.resno);
+    }
+    const std::vector<size_t> ends = tile_part_ends(res_of, split_res);
+    if(ends.size() > 255)
+    {
+      T.err = "more than 255 tile parts";
+      return;
+    }
+    for(size_t j = 0, p0 = 0; j < ends.size(); p0 = ends[j++])
+      T.parts.push_back(t2::DevPart{p0, ends[j], mine[k], (uint32_t)j, (uint32_t)ends.size()});
+  });
+  for(TileSlice& T : tiles)
+  {
+    if(T.err)
+    {
+      b2k_set_error(T.err);
+      return -1;
+    }
+    const uint64_t p_first = plan.packets.size();
+    for(t2::DevPacket& d : T.packets)
+    {
+      d.hdr_at += plan.hdr_bytes;
+      d.tag_at += plan.tag_nodes;
+      plan.packets.push_back(d);
+    }
+    for(t2::DevPart& d : T.parts)
+      plan.parts.push_back(t2::DevPart{p_first + d.p0, p_first + d.p1, d.tile, d.index, d.count});
+    plan.hdr_bytes += T.hdr_bytes;
+    plan.tag_nodes += T.tag_nodes;
+  }
+  plan.tlm_at = main_header(cp, flags, plan.parts.size(), plan.head);
+  return 0;
+}
+
+/* the caller's block table as the writer's block source (t2_write.h): a block is in its packet when it has passes and
+   bytes; its body is the cleanup segment and, with more than one pass, the refinement segment, at `offset` in the arena */
+struct TableBlocks
+{
+  const b2k_block* blk;
+  uint64_t arena; /* bytes in the arena */
+  uint64_t slots; /* dst has an entry per block */
+  TableBlocks stream(uint32_t) const { return *this; }
+  t2::BlockCode operator()(uint32_t i) const
+  {
+    const b2k_block& B = blk[i];
+    return t2::BlockCode{B.length, B.length2, B.numpasses, B.numbps, B.kmax};
+  }
+  int64_t slot(uint32_t i) const { return blk[i].numpasses && blk[i].length ? (int64_t)i : -1; }
+  uint64_t bytes(int64_t i) const { return (uint64_t)blk[i].length + (blk[i].numpasses > 1 ? blk[i].length2 : 0); }
+  bool failed(int64_t i) const { return blk[i].offset + bytes(i) > arena; }
+};
+
+/* n elements, not cleared */
+template <class T>
+std::unique_ptr<T[]> scratch(uint64_t n)
+{
+  return std::unique_ptr<T[]>(new T[n]);
+}
+
+/* the text of a packet's error word: the first of its faults in the order the packet is written */
+const char* packet_error(uint32_t e)
+{
+  return (e & t2::WERR_RANGE)       ? "code block outside the writer's range (bit planes / passes)"
+         : (e & t2::WERR_HDR_BOUND) ? "packet header longer than its bound"
+         : (e & t2::WERR_BLOCK)     ? "block offsets exceed the byte arena"
+                                    : "packet longer than 4 GiB";
+}
+
+/* The host writer: the code stream of plan P and r's blocks, as one stream of the device writer's steps (t2_write.h) on the
+   host pool; then each block's bytes copied once, from r's arena to the place write_packet gave it.  whole: main header,
+   tile parts and EOC; else a shard's tile parts alone, at out + tile_at[k] when tile_at is given (tile_bytes[k] their
+   lengths).  plan_rc: the plan's return code; a declined plan's error (already set) comes after the planned tiles' faults.
+   Faults are reported for the first tile in tile order that has one: a packet's, in code-stream order, before its tile
+   parts'.  Returns the length (also when out is NULL or, without tile_at, cap is too small), or -1 with the error set. */
+int64_t write_plan(const t2::Plan& P, int plan_rc, const b2k_result* r, bool whole, uint8_t* out, uint64_t cap, uint64_t* tile_bytes,
+                   const uint64_t* tile_at)
+{
+  using namespace t2;
+  const uint64_t np = P.packets.size(), nparts = P.parts.size();
+  const TableBlocks B{r->blocks, r->num_bytes, r->num_blocks};
+  const bool sop = (P.flags & B2K_CS_SOP) != 0, eph = (P.flags & B2K_CS_EPH) != 0, plt = (P.flags & B2K_CS_PLT) != 0;
+  const bool tlm = whole && (P.flags & B2K_CS_TLM) != 0;
+  const uint64_t head_len = whole ? P.head.size() : 0;
+  /* every entry is written before it is read, so none is cleared here: the pool's threads touch the pages first */
+  const auto hdr = scratch<uint8_t>(P.hdr_bytes);
+  const auto tags = scratch<TagNode>(P.tag_nodes);
+  const auto hdr_len = scratch<uint32_t>(np), pkt_err = scratch<uint32_t>(np);
+  const auto body_len = scratch<uint64_t>(np), pkt_at = scratch<uint64_t>(np), dst = scratch<uint64_t>(r->num_blocks);
+  std::vector<uint64_t> part_plt(nparts), part_bytes(nparts), part_at(nparts);
+  WriteStatus st{};
+  WritePlace place{};
+  b2k_host_parallel(nparts, [&](size_t t) {
+    for(uint64_t p = P.parts[t].p0; p < P.parts[t].p1; ++p)
+      write_header(p, P.packets.data(), np, B, hdr.get(), P.hdr_bytes, tags.get(), P.tag_nodes, hdr_len.get(), body_len.get(),
+                   dst.get(), &st, sop, eph, pkt_err.get());
+  });
+  for(uint64_t t = 0; t < nparts; ++t)
+    write_part(t, P.parts.data(), nparts, np, hdr_len.get(), body_len.get(), part_plt.data(), part_bytes.data(), &st, plt);
+  for(uint64_t t0 = 0, t1; t0 < nparts; t0 = t1)
+  {
+    for(t1 = t0; t1 < nparts && P.parts[t1].tile == P.parts[t0].tile; ++t1)
+    {
+    }
+    for(uint64_t p = P.parts[t0].p0; p < P.parts[t1 - 1].p1; ++p)
+      if(pkt_err[p])
+      {
+        b2k_set_error(packet_error(pkt_err[p]));
+        return -1;
+      }
+    for(uint64_t t = t0; t < t1; ++t)
+      if(part_bytes[t] > 0xFFFFFFFFull)
+      {
+        b2k_set_error("tile part longer than 4 GiB");
+        return -1;
+      }
+    if(tile_bytes)
+      tile_bytes[t0] = part_bytes[t0]; /* a shard has a tile part per tile */
+  }
+  if(plan_rc)
+    return -1;
+  write_scan_host(1, part_bytes.data(), nparts, part_at.data(), head_len, &st, &place);
+  const uint64_t total = whole ? st.total : st.total - 2; /* a shard's tile parts have no EOC */
+  if(!out || (!tile_at && cap < total))
+    return (int64_t)total;
+  for(uint64_t k = 0; tile_at && k < nparts; ++k)
+  {
+    if(tile_at[k] + part_bytes[k] > cap)
+    {
+      b2k_set_error("a tile part would land outside the buffer");
+      return -1;
+    }
+    part_at[k] = tile_at[k];
+  }
+  /* every place is inside the buffer: the steps write without a bound */
+  b2k_host_parallel(nparts, [&](size_t t) {
+    write_emit(t, P.parts.data(), nparts, np, part_at.data(), part_plt.data(), part_bytes.data(), hdr_len.get(), body_len.get(),
+               pkt_at.get(), out, ~0ull, &st, &place, P.head.data(), head_len, plt, tlm, P.tlm_at);
+    for(uint64_t p = P.parts[t].p0; p < P.parts[t].p1; ++p)
+    {
+      write_packet(p, 0, 1, P.packets.data(), np, B, hdr.get(), P.hdr_bytes, hdr_len.get(), pkt_at.get(), dst.get(), out, ~0ull, &st,
+                   &place);
+      const DevPacket& D = P.packets[p];
+      uint64_t from = 0, to = 0, n = 0; /* blocks that are neighbours in the arena and in the packet: one copy */
+      for(uint32_t b = 0; b < D.nbands; ++b)
+        for(uint32_t i = D.band[b].first, e = i + D.band[b].gw * D.band[b].gh; i < e; ++i)
+          if(B.slot(i) >= 0)
+          {
+            if(r->blocks[i].offset != from + n || dst[i] != to + n)
+            {
+              if(n)
+                memcpy(out + to, r->bytes + from, n);
+              from = r->blocks[i].offset, to = dst[i], n = 0;
+            }
+            n += B.bytes(i);
+          }
+      if(n)
+        memcpy(out + to, r->bytes + from, n);
+    }
+  });
+  return (int64_t)total;
 }
 } // namespace
 
@@ -615,150 +654,19 @@ extern "C" __attribute__((visibility("default"))) int64_t b2k_codestream_write(c
 {
   if(!cp || !r)
     return -1;
-  if(check_whole_image(*cp, r->num_tiles, flags))
-    return -1;
-  const TileGrid g = tile_grid(*cp);
-  const uint32_t ntiles = g.nx * g.ny;
-  const std::vector<BandQuant> q = band_quant(*cp);
-  std::vector<uint8_t> head;
-  const int prog = (int)((flags >> 8) & 7);
-  const bool split_res = (flags & B2K_CS_TPARTS_R) != 0 && prog <= 2; /* a tile part per resolution needs a resolution-major order */
-  const bool sop = (flags & B2K_CS_SOP) != 0, eph = (flags & B2K_CS_EPH) != 0;
-  write_main_header(*cp, g, q, head, prog, sop, eph);
-
-  /* plan every tile part (their lengths feed TLM), then lay the codestream out */
-  std::vector<TilePlan> plans(ntiles);
-  std::vector<uint64_t> tile_first;
-  if(!tile_block_ranges(r->blocks, r->num_blocks, ntiles, tile_first))
-  {
-    b2k_set_error("block table is not in tile order");
-    return -1;
-  }
-  std::vector<std::string> errs(ntiles);
-  b2k_host_parallel(ntiles, [&](size_t t) { /* tiles are independent: plan them on the host pool */
-    TilePlan& P = plans[t];
-    if(plan_tile_packets(*cp, tile_rect(*cp, g, (uint32_t)t), r->blocks + tile_first[t], (uint32_t)(tile_first[t + 1] - tile_first[t]),
-                         r->num_bytes, P, errs[t], prog, sop, eph))
-    {
-      if(errs[t].empty())
-        errs[t] = "tile planning failed";
-      return;
-    }
-    plan_tile_parts(P, split_res, (flags & B2K_CS_PLT) != 0);
-    if(P.parts.size() > 255)
-      errs[t] = "more than 255 tile parts";
-  });
-  uint64_t total = 0;
-  for(uint32_t t = 0; t < ntiles; ++t)
-  {
-    if(!errs[t].empty())
-    {
-      b2k_set_error(errs[t].c_str());
-      return -1;
-    }
-    for(const TilePlan::Part& pt : plans[t].parts)
-      if(pt.bytes > 0xFFFFFFFFull)
-      {
-        b2k_set_error("tile part longer than 4 GiB");
-        return -1;
-      }
-    total += plans[t].size();
-  }
-  if(flags & B2K_CS_TLM)
-  {
-    std::vector<std::pair<uint32_t, uint32_t>> ent;
-    for(uint32_t t = 0; t < ntiles; ++t)
-      for(const TilePlan::Part& pt : plans[t].parts)
-        ent.push_back({t, (uint32_t)pt.bytes});
-    append_tlm(head, ent);
-  }
-  total += head.size() + 2; /* + EOC */
-  if(!out || cap < total)
-    return (int64_t)total;
-
-  memcpy(out, head.data(), head.size());
-  std::vector<uint64_t> tile_at(ntiles + 1, head.size());
-  for(uint32_t t = 0; t < ntiles; ++t)
-    tile_at[t + 1] = tile_at[t] + plans[t].size();
-  /* tile parts are independent byte ranges: copy them on the host pool */
-  b2k_host_parallel(ntiles, [&](size_t t) { emit_tile_parts(plans[t], (uint32_t)t, r->bytes, out + tile_at[t]); });
-  uint8_t* w = out + tile_at[ntiles];
-  *w++ = 0xFF; /* EOC */
-  *w++ = 0xD9;
-  return (int64_t)(w - out);
+  t2::Plan P;
+  const int rc = b2k_t2_plan(*cp, flags, r->blocks, r->num_blocks, r->num_tiles, P);
+  return write_plan(P, rc, r, true, out, cap, nullptr, nullptr);
 }
 
 int b2k_t2_plan(const b2k_coding& cp, uint32_t flags, const b2k_block* blocks, uint64_t nblocks, uint32_t num_tiles, t2::Plan& plan)
 {
   if(check_whole_image(cp, num_tiles, flags))
     return -1;
-  const TileGrid g = tile_grid(cp);
-  const uint32_t ntiles = g.nx * g.ny;
-  const int prog = (int)((flags >> 8) & 7);
-  const bool split_res = (flags & B2K_CS_TPARTS_R) != 0 && prog <= 2;
-  plan = t2::Plan();
-  plan.flags = flags;
-  write_main_header(cp, g, band_quant(cp), plan.head, prog, (flags & B2K_CS_SOP) != 0, (flags & B2K_CS_EPH) != 0);
-  std::vector<uint64_t> tile_first;
-  if(!tile_block_ranges(blocks, nblocks, ntiles, tile_first))
-  {
+  const int rc = plan_tiles(cp, flags, blocks, nblocks, 1, 0, plan);
+  if(rc > 0)
     b2k_set_error("block table is not in tile order");
-    return -1;
-  }
-  std::vector<Packet> pkts;
-  std::vector<uint8_t> res_of;
-  for(uint32_t t = 0; t < ntiles; ++t)
-  {
-    uint32_t expect = 0;
-    tile_packets(cp, tile_rect(cp, g, t), pkts, expect, prog);
-    if(expect != tile_first[t + 1] - tile_first[t])
-    {
-      b2k_set_error("block table does not match the tile's enumeration");
-      return -1;
-    }
-    uint8_t kmax = 0;
-    for(uint64_t i = tile_first[t]; i < tile_first[t + 1]; ++i)
-      kmax = std::max(kmax, blocks[i].kmax);
-    const uint64_t p_first = plan.packets.size();
-    res_of.clear();
-    for(size_t k = 0; k < pkts.size(); ++k)
-    {
-      const Packet& pk = pkts[k];
-      t2::DevPacket d{};
-      for(int b = 0; b < pk.nbands; ++b)
-        d.band[b] = t2::BandGrid{(uint32_t)tile_first[t] + pk.band[b].first, pk.band[b].gw, pk.band[b].gh};
-      d.nbands = pk.nbands;
-      d.sop = (uint32_t)(k & 0xFFFF);
-      const uint64_t cap = t2::packet_header_bound(pk.band, pk.nbands, kmax);
-      if(cap > 0xFFFFFFFFull)
-      {
-        b2k_set_error("packet longer than 4 GiB");
-        return -1;
-      }
-      d.hdr_cap = (uint32_t)cap;
-      d.hdr_at = plan.hdr_bytes;
-      d.tag_at = plan.tag_nodes;
-      plan.hdr_bytes += cap;
-      plan.tag_nodes += t2::packet_tag_nodes(pk.band, pk.nbands);
-      plan.packets.push_back(d);
-      res_of.push_back(pk.resno);
-    }
-    const std::vector<size_t> ends = tile_part_ends(res_of, split_res);
-    if(ends.size() > 255)
-    {
-      b2k_set_error("more than 255 tile parts");
-      return -1;
-    }
-    size_t p0 = 0;
-    for(size_t i = 0; i < ends.size(); ++i)
-    {
-      plan.parts.push_back(t2::DevPart{p_first + p0, p_first + ends[i], t, (uint32_t)i, (uint32_t)ends.size()});
-      p0 = ends[i];
-    }
-  }
-  if(flags & B2K_CS_TLM)
-    plan.tlm_at = append_tlm_segments(plan.head, plan.parts.size());
-  return 0;
+  return rc ? -1 : 0;
 }
 
 /* ---- per-rank writers (SURVEY.md 8e: "T2 can itself be sharded per tile; the writer concatenates in index order") ------
@@ -782,77 +690,19 @@ static int64_t write_tiles_impl(const b2k_coding* cp, const b2k_result* r, uint3
     return -1;
   }
   const TileGrid g = tile_grid(*cp);
-  const uint32_t ntiles = g.nx * g.ny;
-  const int prog = (int)((flags >> 8) & 7);
-  if(prog > 4 || ntiles > 65535)
+  if(((flags >> 8) & 7) > 4 || g.nx * g.ny > 65535)
   {
     b2k_set_error("unknown progression order / too many tiles");
     return -1;
   }
-  const bool sop = (flags & B2K_CS_SOP) != 0, eph = (flags & B2K_CS_EPH) != 0;
-  std::vector<uint32_t> mine;
-  for(uint32_t t = tile_rem; t < ntiles; t += tile_mod)
-    mine.push_back(t);
-  std::vector<uint64_t> first(mine.size() + 1, 0);
+  t2::Plan P;
+  const int rc = plan_tiles(*cp, flags, r->blocks, r->num_blocks, tile_mod, tile_rem, P);
+  if(rc > 0)
   {
-    uint64_t i = 0;
-    for(size_t k = 0; k < mine.size(); ++k)
-    {
-      first[k] = i;
-      while(i < r->num_blocks && r->blocks[i].tile == mine[k])
-        ++i;
-    }
-    first[mine.size()] = i;
-    if(i != r->num_blocks)
-    {
-      b2k_set_error("the block table is not the shard's tiles in tile order");
-      return -1;
-    }
+    b2k_set_error("the block table is not the shard's tiles in tile order");
+    return -1;
   }
-  std::vector<TilePlan> plans(mine.size());
-  std::vector<std::string> errs(mine.size());
-  b2k_host_parallel(mine.size(), [&](size_t k) {
-    TilePlan& P = plans[k];
-    if(plan_tile_packets(*cp, tile_rect(*cp, g, mine[k]), r->blocks + first[k], (uint32_t)(first[k + 1] - first[k]), r->num_bytes, P,
-                         errs[k], prog, sop, eph))
-    {
-      if(errs[k].empty())
-        errs[k] = "tile planning failed";
-      return;
-    }
-    plan_tile_parts(P, false, (flags & B2K_CS_PLT) != 0);
-  });
-  uint64_t total = 0;
-  std::vector<uint64_t> at(mine.size() + 1, 0);
-  for(size_t k = 0; k < mine.size(); ++k)
-  {
-    if(!errs[k].empty())
-    {
-      b2k_set_error(errs[k].c_str());
-      return -1;
-    }
-    if(plans[k].size() > 0xFFFFFFFFull)
-    {
-      b2k_set_error("tile part longer than 4 GiB");
-      return -1;
-    }
-    at[k] = total;
-    total += plans[k].size();
-    if(tile_bytes)
-      tile_bytes[k] = plans[k].size();
-  }
-  at[mine.size()] = total;
-  if(!out || (!tile_at && cap < total))
-    return (int64_t)total;
-  if(tile_at)
-    for(size_t k = 0; k < mine.size(); ++k)
-      if(tile_at[k] + plans[k].size() > cap)
-      {
-        b2k_set_error("a tile part would land outside the buffer");
-        return -1;
-      }
-  b2k_host_parallel(mine.size(), [&](size_t k) { emit_tile_parts(plans[k], mine[k], r->bytes, out + (tile_at ? tile_at[k] : at[k])); });
-  return (int64_t)total;
+  return write_plan(P, rc, r, false, out, cap, tile_bytes, tile_at);
 }
 
 extern "C" __attribute__((visibility("default"))) int64_t b2k_codestream_write_tiles(const b2k_coding* cp, const b2k_result* r, uint32_t flags,
@@ -886,22 +736,15 @@ extern "C" __attribute__((visibility("default"))) int64_t b2k_codestream_write_h
   }
   const TileGrid g = tile_grid(*cp);
   const uint32_t ntiles = g.nx * g.ny;
-  const int prog = (int)((flags >> 8) & 7);
-  if(prog > 4 || ((flags & B2K_CS_TLM) && (!tile_bytes || ntiles_in != ntiles)))
+  if(((flags >> 8) & 7) > 4 || ((flags & B2K_CS_TLM) && (!tile_bytes || ntiles_in != ntiles)))
   {
     b2k_set_error("TLM needs the length of every tile's tile part");
     return -1;
   }
-  const std::vector<BandQuant> q = band_quant(*cp);
   std::vector<uint8_t> head;
-  write_main_header(*cp, g, q, head, prog, (flags & B2K_CS_SOP) != 0, (flags & B2K_CS_EPH) != 0);
-  if(flags & B2K_CS_TLM)
-  {
-    std::vector<std::pair<uint32_t, uint32_t>> ent;
-    for(uint32_t t = 0; t < ntiles; ++t)
-      ent.push_back({t, (uint32_t)tile_bytes[t]});
-    append_tlm(head, ent);
-  }
+  const uint64_t tlm_at = main_header(*cp, flags, ntiles, head);
+  for(uint32_t t = 0; (flags & B2K_CS_TLM) && t < ntiles; ++t)
+    t2::put_tlm_entry(head.data() + tlm_at, t, t, (uint32_t)tile_bytes[t]);
   if(out && cap >= head.size())
     memcpy(out, head.data(), head.size());
   return (int64_t)head.size();

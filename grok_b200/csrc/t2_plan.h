@@ -1,8 +1,8 @@
 /*
- * grok_b200/csrc/t2_plan.h -- what the device code-stream writer (t2_device.cu) needs to know about an image's code
- * stream before any block is coded: its packets in code-stream order, its tile parts and its main header.  Geometry
- * and flags only, so one plan serves every frame of a job.  Built on the host by b2k_t2_plan (codestream.cpp) from the
- * same tile_packets() / tile-part rule / main header the host writer uses.
+ * grok_b200/csrc/t2_plan.h -- what the code-stream writer (t2_write.h, on the device and on the host) needs to know about
+ * an image's code stream before any block is coded: its packets in code-stream order, its tile parts and its main header.
+ * Geometry and flags only, so one plan serves every frame of a job.  Built on the host (codestream.cpp) by b2k_t2_plan,
+ * or for a shard's tiles by the per-rank writers; the device parser reads its packets too.
  */
 #pragma once
 #include <stdint.h>

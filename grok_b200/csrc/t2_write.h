@@ -1,14 +1,15 @@
 /*
- * grok_b200/csrc/t2_write.h -- the device code-stream writer's per-thread work over a batch of n code streams, as
- * __host__ __device__ functions.  t2_device.cu runs them as kernels; tests/t2_write_batch_check.cpp runs them on the host
- * in the same order, under the sanitizers, and compares with b2k_codestream_write.
+ * grok_b200/csrc/t2_write.h -- the code-stream writer's steps over a batch of n code streams, as __host__ __device__
+ * functions.  t2_device.cu runs them as kernels over the block coder's output; codestream.cpp runs them on the host pool
+ * over a caller's block table (b2k_codestream_write and the per-rank writers, one stream); tests/t2_write_batch_check.cpp
+ * runs the device's batch on the host, under the sanitizers.
  *
- * The plan (t2_plan.h: packets, tile parts, main header, coded-block map, Kmax) is shared by every stream; everything else
- * is sliced per stream: header scratch (hdr_bytes each), tag-tree nodes (tag_nodes each), per-packet arrays (np each),
- * per-part arrays (nparts each), block destinations (ncoded each; coded block c of stream s is s * ncoded + c, as the
- * coder's HtBlockOut is).  A thread of a launch over n streams of `per` items is g = s * per + i.
+ * The plan (t2_plan.h: packets, tile parts, main header) is shared by every stream; everything else is sliced per stream:
+ * header scratch (hdr_bytes each), tag-tree nodes (tag_nodes each), per-packet arrays (np each), per-part arrays (nparts
+ * each), block destinations (the block source's slots each).  A thread of a launch over n streams of `per` items is
+ * g = s * per + i.  The blocks come from a block source: CoderBlocks on the device, the caller's block table on the host.
  *
- * A stream's verdict is its WriteStatus: blocks that overflowed the coder, or a writer limit.  A stream with either gets
+ * A stream's verdict is its WriteStatus: blocks the source marks failed, or a writer limit.  A stream with either gets
  * total 0: it takes no bytes of the output, and its blocks are not placed (dst = NOT_PLACED, which the gather skips).
  * Stream s starts at status[s].at: the streams lie in order, each at a 256-byte boundary (batch_arena_next, as a decode
  * batch lays out its arena).  When the streams do not fit the caller's buffer (place->used > cap) nothing is written
@@ -21,8 +22,6 @@
 #include "t2_parse.h"
 #include "t2_plan.h"
 
-struct HtBlockOut;
-
 namespace b2k
 {
 namespace t2
@@ -33,6 +32,7 @@ enum : uint32_t
   WERR_PACKET = 2,     /* a packet of 4 GiB or more */
   WERR_PART = 4,       /* a tile part of 4 GiB or more */
   WERR_HDR_BOUND = 8,  /* a header longer than its bound */
+  WERR_BLOCK = 16,     /* a block its source marks failed (per-packet error words only) */
 };
 /* a block the gather must leave alone: offset + length exceeds any buffer */
 constexpr uint64_t NOT_PLACED = ~0ull >> 1;
@@ -51,28 +51,47 @@ struct WritePlace /* the batch */
   uint32_t pad;
 };
 
-/* step 1, thread g = s * np + p: SOP, header bits and EPH of packet p of stream s into its header scratch; header and body
-   lengths; each block's place in the body */
+/* the block coder's output (Out: HtBlockOut) as a block source: block i of the image is coded block coded[i] of the
+   stream, or none (< 0); one pass, one bit plane (CoderOJPH), length = the coder's total, 0xFFFFFFFF when the block
+   overflowed the coder's buffers.  A source gives block i's BlockCode (source(i)), the entry of dst its place goes to
+   (slot(i), < 0 when the packet carries no bytes of it), and that slot's body length (bytes) or that it cannot give
+   the bytes (failed). */
 template <class Out>
-B2K_HD void write_header(uint64_t g, const DevPacket* packets, uint64_t np, const int32_t* coded, const uint8_t* kmax, uint64_t ncoded,
-                         const Out* outs, uint8_t* hdr, uint64_t hdr_bytes, TagNode* tags, uint64_t tag_nodes, uint32_t* hdr_len,
-                         uint64_t* body_len, uint64_t* dst, WriteStatus* status, bool sop, bool eph)
+struct CoderBlocks
 {
-  const uint32_t s = (uint32_t)(g / np);
-  const DevPacket P = packets[g % np];
-  outs += (uint64_t)s * ncoded;
-  dst += (uint64_t)s * ncoded;
-  /* a coded block as b2k_encode reports it: one pass, one bit plane (CoderOJPH), length = the coder's total */
-  auto code = [&](uint32_t i) {
+  const int32_t* coded;
+  const uint8_t* kmax;
+  uint64_t slots;  /* coded blocks per stream */
+  const Out* outs; /* stream 0's; stream(s) is stream s's */
+  B2K_HD CoderBlocks stream(uint32_t s) const { return CoderBlocks{coded, kmax, slots, outs + (uint64_t)s * slots}; }
+  B2K_HD BlockCode operator()(uint32_t i) const
+  {
     const int32_t c = coded[i];
     uint32_t len = c >= 0 ? outs[c].total : 0u;
     len = len == 0xFFFFFFFFu ? 0u : len;
     return BlockCode{len, 0u, (uint8_t)(c >= 0 ? 1 : 0), 1, kmax[i]};
-  };
+  }
+  B2K_HD int64_t slot(uint32_t i) const { return coded[i]; }
+  B2K_HD uint64_t bytes(int64_t c) const { return outs[c].total; }
+  B2K_HD bool failed(int64_t c) const { return outs[c].total == 0xFFFFFFFFu; }
+};
+
+/* step 1, thread g = s * np + p: SOP, header bits and EPH of packet p of stream s into its header scratch; header and body
+   lengths; each block's place in the body.  With pkt_err (the host's single stream) the packet's WERR_* word goes to
+   pkt_err[g], WERR_BLOCK for a failed block, and the status is left alone; else failed blocks count in bad_blocks. */
+template <class Blocks>
+B2K_HD void write_header(uint64_t g, const DevPacket* packets, uint64_t np, const Blocks& blocks, uint8_t* hdr, uint64_t hdr_bytes,
+                         TagNode* tags, uint64_t tag_nodes, uint32_t* hdr_len, uint64_t* body_len, uint64_t* dst, WriteStatus* status,
+                         bool sop, bool eph, uint32_t* pkt_err = nullptr)
+{
+  const uint32_t s = (uint32_t)(g / np);
+  const DevPacket P = packets[g % np];
+  const Blocks B = blocks.stream(s);
+  dst += (uint64_t)s * blocks.slots;
   BitWriter bw;
   bw.init(hdr + s * hdr_bytes + P.hdr_at, P.hdr_cap);
   uint32_t err = 0;
-  if(packet_header(bw, P.band, (int)P.nbands, code, tags + s * tag_nodes + P.tag_at, P.sop, sop, eph))
+  if(packet_header(bw, P.band, (int)P.nbands, B, tags + s * tag_nodes + P.tag_at, P.sop, sop, eph))
     err |= WERR_RANGE;
   if(bw.n > bw.cap)
     err |= WERR_HDR_BOUND;
@@ -83,15 +102,15 @@ B2K_HD void write_header(uint64_t g, const DevPacket* packets, uint64_t np, cons
     const uint32_t n = P.band[b].gw * P.band[b].gh;
     for(uint32_t k = 0; k < n; ++k)
     {
-      const int32_t c = coded[P.band[b].first + k];
+      const int64_t c = B.slot(P.band[b].first + k);
       if(c < 0)
         continue;
-      const uint32_t t = outs[c].total;
-      if(t == 0xFFFFFFFFu)
+      if(B.failed(c))
       {
         ++bad;
         continue;
       }
+      const uint64_t t = B.bytes(c);
       dst[c] = rel; /* relative to the body; write_packet adds the body's offset */
       rel += t;
     }
@@ -100,10 +119,25 @@ B2K_HD void write_header(uint64_t g, const DevPacket* packets, uint64_t np, cons
     err |= WERR_PACKET;
   hdr_len[g] = (uint32_t)bw.n;
   body_len[g] = rel;
-  if(bad)
-    status_add(&status[s].bad_blocks, bad);
-  if(err)
-    status_or(&status[s].errors, err);
+  if(pkt_err)
+    pkt_err[g] = err | (bad ? (uint32_t)WERR_BLOCK : 0u);
+  else
+  {
+    if(bad)
+      status_add(&status[s].bad_blocks, bad);
+    if(err)
+      status_or(&status[s].errors, err);
+  }
+}
+
+/* step 1 over the block coder's output (CoderBlocks): the form the kernel and the batch harness call */
+template <class Out>
+B2K_HD void write_header(uint64_t g, const DevPacket* packets, uint64_t np, const int32_t* coded, const uint8_t* kmax, uint64_t ncoded,
+                         const Out* outs, uint8_t* hdr, uint64_t hdr_bytes, TagNode* tags, uint64_t tag_nodes, uint32_t* hdr_len,
+                         uint64_t* body_len, uint64_t* dst, WriteStatus* status, bool sop, bool eph)
+{
+  write_header(g, packets, np, CoderBlocks<Out>{coded, kmax, ncoded, outs}, hdr, hdr_bytes, tags, tag_nodes, hdr_len, body_len, dst,
+               status, sop, eph);
 }
 
 /* packet k's length, header and body, for plt_segments */
@@ -139,7 +173,7 @@ B2K_HD uint64_t write_total(const WriteStatus& st, uint64_t parts_end)
   return st.bad_blocks || st.errors ? 0 : parts_end + 2;
 }
 
-/* step 3, stated once for the host: the exclusive scan of each stream's tile-part lengths behind the main header
+/* step 3 on the host: the exclusive scan of each stream's tile-part lengths behind the main header
    (part_at, relative to the stream), each stream's total, and the streams placed behind each other.  The kernel
    (t2_device.cu k_t2_scan) does the same with a CTA per stream. */
 inline void write_scan_host(uint32_t n, const uint64_t* part_bytes, uint64_t nparts, uint64_t* part_at, uint64_t head_len,
@@ -166,7 +200,7 @@ inline void write_scan_host(uint32_t n, const uint64_t* part_bytes, uint64_t npa
 /* step 4, thread g = s * nparts + t: SOT, PLT, SOD and TLM entry of tile part t of stream s; every packet's offset in
    the output.  The main header (head) is written by the stream's threads too, in pieces no two threads share: part 0
    the markers before TLM, the first part of each TLM segment that segment's marker (the plan's, entries left to their
-   parts), the last part the EOC. */
+   parts), the last part the EOC.  Without a main header (head_len 0: a shard's tile parts) there is no EOC either. */
 B2K_HD void write_emit(uint64_t g, const DevPart* parts, uint64_t nparts, uint64_t np, const uint64_t* part_at, const uint64_t* part_plt,
                        const uint64_t* part_bytes, const uint32_t* hdr_len, const uint64_t* body_len, uint64_t* pkt_at, uint8_t* cs,
                        uint64_t cap, const WriteStatus* status, const WritePlace* place, const uint8_t* head, uint64_t head_len,
@@ -203,7 +237,7 @@ B2K_HD void write_emit(uint64_t g, const DevPart* parts, uint64_t nparts, uint64
       base[i] = head[i];
   if(tlm)
     put_tlm_entry(base + tlm_at, t, D.tile, (uint32_t)part_bytes[g]);
-  if(t == nparts - 1)
+  if(t == nparts - 1 && head_len)
   {
     base[status[s].total - 2] = 0xFF; /* EOC */
     base[status[s].total - 1] = 0xD9;
@@ -212,16 +246,15 @@ B2K_HD void write_emit(uint64_t g, const DevPart* parts, uint64_t nparts, uint64
 
 /* step 5, packet g = s * np + p, worked by `lanes` threads of which this is `lane`: the packet's header to its place; its
    blocks' offsets in the output, or NOT_PLACED when the stream failed or the streams do not fit */
-template <class Out>
-B2K_HD void write_packet(uint64_t g, uint32_t lane, uint32_t lanes, const DevPacket* packets, uint64_t np, const int32_t* coded,
-                         uint64_t ncoded, const Out* outs, const uint8_t* hdr, uint64_t hdr_bytes, const uint32_t* hdr_len,
-                         const uint64_t* pkt_at, uint64_t* dst, uint8_t* cs, uint64_t cap, const WriteStatus* status,
-                         const WritePlace* place)
+template <class Blocks>
+B2K_HD void write_packet(uint64_t g, uint32_t lane, uint32_t lanes, const DevPacket* packets, uint64_t np, const Blocks& blocks,
+                         const uint8_t* hdr, uint64_t hdr_bytes, const uint32_t* hdr_len, const uint64_t* pkt_at, uint64_t* dst,
+                         uint8_t* cs, uint64_t cap, const WriteStatus* status, const WritePlace* place)
 {
   const uint32_t s = (uint32_t)(g / np);
   const DevPacket P = packets[g % np];
-  outs += (uint64_t)s * ncoded;
-  dst += (uint64_t)s * ncoded;
+  const Blocks B = blocks.stream(s);
+  dst += (uint64_t)s * blocks.slots;
   const bool placed = place->used <= cap && status[s].total;
   const uint64_t at = placed ? pkt_at[g] : 0;
   const uint32_t hn = hdr_len[g];
@@ -233,11 +266,21 @@ B2K_HD void write_packet(uint64_t g, uint32_t lane, uint32_t lanes, const DevPac
     const uint32_t n = P.band[b].gw * P.band[b].gh;
     for(uint32_t k = lane; k < n; k += lanes)
     {
-      const int32_t c = coded[P.band[b].first + k];
-      if(c >= 0 && outs[c].total != 0xFFFFFFFFu)
+      const int64_t c = B.slot(P.band[b].first + k);
+      if(c >= 0 && !B.failed(c))
         dst[c] = placed ? dst[c] + at + hn : NOT_PLACED;
     }
   }
+}
+/* step 5 over the block coder's output (CoderBlocks) */
+template <class Out>
+B2K_HD void write_packet(uint64_t g, uint32_t lane, uint32_t lanes, const DevPacket* packets, uint64_t np, const int32_t* coded,
+                         uint64_t ncoded, const Out* outs, const uint8_t* hdr, uint64_t hdr_bytes, const uint32_t* hdr_len,
+                         const uint64_t* pkt_at, uint64_t* dst, uint8_t* cs, uint64_t cap, const WriteStatus* status,
+                         const WritePlace* place)
+{
+  write_packet(g, lane, lanes, packets, np, CoderBlocks<Out>{coded, nullptr, ncoded, outs}, hdr, hdr_bytes, hdr_len, pkt_at, dst, cs, cap,
+               status, place);
 }
 /* a stream's verdict as the single call reports it: its length, or -2 (blocks overflowed the coder) / -1 (the writer's
    limits) with the text b2k_encode_device / b2k_codestream_write give */

@@ -15,7 +15,8 @@
  *     stream as overflowed (total 0xFFFFFFFF), as the coder reports a block that did not fit its scratch slot.
  *   Prints one line per stream:
  *     "<name> <rc> <offset> <length> same <text>"   rc and text as the single call gives them; for rc 0 the bytes at
- *                                                   offset are those of b2k_codestream_write of the stream's table
+ *                                                   offset are those of b2k_codestream_write of the stream's table,
+ *                                                   and are written to TABLE.cs
  *     "<name> plan <text>"                          b2k_t2_plan declined the coding and flags (every stream of the batch)
  *     "<name> ... <what differs>"                   and exit 1
  */
@@ -68,7 +69,7 @@ static std::vector<uint8_t> read_file(const char* path)
 
 struct Stream
 {
-  std::string name;
+  std::string name, table_path;
   std::vector<b2k_block> table; /* as the coder reports it: coded blocks one pass, one bit plane */
   std::vector<uint8_t> data;
   long inject = -1;
@@ -257,6 +258,11 @@ static int run_batch(uint32_t flags, const b2k_coding& cp, std::vector<Stream>& 
       if(at % 256 || at < end || at + len > need)
         why = "misplaced at " + std::to_string(at);
       end = at + len;
+      if(FILE* f = fopen((S.table_path + ".cs").c_str(), "wb"))
+      {
+        fwrite(cs.data() + at, 1, len, f);
+        fclose(f);
+      }
     }
     if(why.empty())
       printf("%s %lld %llu %llu same %s\n", S.name.c_str(), (long long)(r > 0 ? 0 : r), (unsigned long long)at, (unsigned long long)len,
@@ -295,6 +301,7 @@ int main(int argc, char** argv)
     {
       Stream S;
       S.name = argv[i];
+      S.table_path = argv[i + 1];
       const std::vector<uint8_t> t = read_file(argv[i + 1]);
       S.table.resize(t.size() / sizeof(b2k_block));
       if(!S.table.empty())

@@ -1,10 +1,10 @@
 """The batched device code-stream writer (b2k_encode_codestreams_device after the block coder), run on the host by
 tests/t2_write_batch_check.cpp in the order of its steps, with the kernels' own thread bodies (t2_write.h) and per-stream
 slicing, under the address and undefined-behaviour sanitizers.  Each batch holds several streams of one coding and one
-flag set; every stream's bytes must be those of b2k_codestream_write of its block table alone, the streams must lie in
-order at 256-byte boundaries, and a stream with an overflowed block must get the single call's -2 and text and take no
-bytes, leaving every other stream as it is.  CPU only; the GPU suite (test_device_batch_encode.py) compares the device
-batch with the single device call."""
+flag set; every stream's bytes must be those of the plain-Python T2 writer (tests/oracle_t2.py) and of
+b2k_codestream_write of its block table alone, the streams must lie in order at 256-byte boundaries, and a stream with an
+overflowed block must get the single call's -2 and text and take no bytes, leaving every other stream as it is.  CPU only;
+the GPU suite (test_device_batch_encode.py) compares the device batch with the single device call."""
 import os
 import shutil
 import subprocess
@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 import grok_b200 as G
+import oracle_t2 as T2
 import test_device_codestream as DC
 import test_t2_oracle as O
 
@@ -45,8 +46,9 @@ def coder_table(table):
 
 def run(harness, tmp_path, batches):
     """batches: [(flags, cp, [(name, table, data, inject)])]; returns [[(rc, offset, length, text)]] per batch, or
-    [[('plan', text)]] for a batch the writer's plan declines; every stream checked by the harness"""
-    args, count = [], 0
+    [[('plan', text)]] for a batch the writer's plan declines; every stream checked by the harness, and every stream
+    written compared with the oracle's stream of its table"""
+    args, count, files = [], 0, []
     for b, (flags, cp, streams) in enumerate(batches):
         cpf = tmp_path / ("b%d_cp.bin" % b)
         cpf.write_bytes(bytes(cp))
@@ -56,21 +58,28 @@ def run(harness, tmp_path, batches):
             tf.write_bytes(coder_table(table).tobytes())
             df.write_bytes(np.asarray(data, np.uint8).tobytes())
             args += [name, str(tf), str(df), str(inject)]
+            files.append(tf)
             count += 1
     env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0")
     r = subprocess.run([harness] + args, capture_output=True, text=True, env=env)
     lines = r.stdout.splitlines()
     bad = [ln for ln in lines if ln.split(" ", 5)[1] != "plan" and ln.split(" ", 5)[4:5] != ["same"]]
     assert r.returncode == 0 and not bad and len(lines) == count, (r.returncode, bad[:10], r.stderr[-3000:])
-    out, k = [], 0
-    for _, _, streams in batches:
+    out, k, oracle = [], 0, {}
+    for flags, cp, streams in batches:
         rows = []
-        for _ in streams:
+        for name, table, data, _ in streams:
             f = lines[k].split(" ", 5)
             if f[1] == "plan":
                 rows.append(("plan", lines[k].split(" ", 2)[2]))
             else:
                 rows.append((int(f[1]), int(f[2]), int(f[3]), f[5] if len(f) > 5 else ""))
+            if rows[-1][0] == 0:
+                key = (id(table), id(data), flags)
+                if key not in oracle:
+                    oracle[key] = T2.write_flags(cp, coder_table(table), data, flags)
+                got = np.fromfile(str(files[k]) + ".cs", np.uint8)
+                assert np.array_equal(got, oracle[key]), (name, flags, len(got), len(oracle[key]))
             k += 1
         out.append(rows)
     return out
