@@ -460,7 +460,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32)
   const int ms_size = (int)st.ms_len;
   int ms_pos = 0;
   uint32_t ms_head = 0, ms_tail = 0;
-  bool ms_prevff = false;
+  bool ms_prevff = false, ms_prevtop = false;
   const uint32_t* rec = recs + B.rec_off;
   uint32_t r_next = lane < nq ? __ldg(rec + (size_t)lane * 32) : 0u;
   uint32_t pw0 = 0, pw1 = 0, pw2 = 0; /* this lane's three aligned words of the next 256-byte refill */
@@ -511,6 +511,14 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32)
         const unsigned lastff = __ballot_sync(0xffffffffu, (ff1 >> 31) != 0);
         const uint32_t fin = lane == 0 ? (ms_prevff ? 1u : 0u) : ((lastff >> (lane - 1)) & 1u);
         const uint32_t d0 = (ff0 << 8) | (fin << 7), d1 = (ff1 << 8) | (ff0 >> 24);
+        /* the reference ORs whole bytes into its bit buffer (frwd_read L635-648), so the top bit of a byte after 0xFF
+           lands on the next byte's lowest bit: 0 in a valid segment, carried over here for a damaged one (across the
+           lane's two words, to the next lane by ballot and to the next refill in ms_prevtop) */
+        const uint32_t c0 = v0 & d0, c1 = v1 & d1;
+        const unsigned lasttop = __ballot_sync(0xffffffffu, (c1 >> 31) != 0);
+        const uint32_t cin = lane == 0 ? (ms_prevtop ? 1u : 0u) : ((lasttop >> (lane - 1)) & 1u);
+        v0 |= (c0 << 1) | cin;
+        v1 |= (c1 << 1) | (c0 >> 31);
         auto squeeze = [](uint32_t v, uint32_t d, int& nb) -> uint32_t {
           v &= ~d;
           uint32_t h0 = v & 0xFFFFu, h1 = v >> 16;
@@ -550,6 +558,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32)
         }
         ms_tail += tot;
         ms_prevff = (lastff >> 31) & 1u;
+        ms_prevtop = (lasttop >> 31) & 1u;
         ms_pos += 256;
         __syncwarp();
       }
@@ -716,11 +725,14 @@ __device__ __forceinline__ uint32_t rf_window6(const uint32_t* row, int x0, int 
     v |= rf_bit(row, x0 + i, w) << i;
   return v;
 }
+/* Both refinement readers put a 7-bit byte's top bit where the next byte's first bit goes, as the reference's readers
+   OR whole bytes into their bit buffers: 0 in a valid segment, ORed into the next byte's lowest bit (`carry`) in a
+   damaged one */
 struct SppR
 { /* forward reader, zeros after the end (frwd_read<0>, L609-654) */
   const uint8_t* d;
   int size, pos, bits, unstuff;
-  uint32_t tmp;
+  uint32_t tmp, carry;
 };
 __device__ __forceinline__ uint32_t spp_get(SppR& s)
 {
@@ -728,8 +740,9 @@ __device__ __forceinline__ uint32_t spp_get(SppR& s)
   {
     const uint32_t b = s.pos < s.size ? (uint32_t)__ldg(s.d + s.pos) : 0u;
     s.pos++;
-    s.tmp = b;
     s.bits = 8 - s.unstuff;
+    s.tmp = b | s.carry;
+    s.carry = s.bits == 7 ? b >> 7 : 0u;
     s.unstuff = (b == 0xFFu);
   }
   const uint32_t v = s.tmp & 1u;
@@ -741,7 +754,7 @@ struct MrpR
 { /* backward reader (rev_read_mrp / rev_init_mrp, L453-541) */
   const uint8_t* last;
   int size, pos, bits, unstuff;
-  uint32_t tmp;
+  uint32_t tmp, carry;
 };
 __device__ __forceinline__ uint32_t mrp_get(MrpR& m)
 {
@@ -749,8 +762,9 @@ __device__ __forceinline__ uint32_t mrp_get(MrpR& m)
   {
     const uint32_t b = m.pos < m.size ? (uint32_t)__ldg(m.last - m.pos) : 0u;
     m.pos++;
-    m.tmp = b;
     m.bits = 8 - ((m.unstuff && (b & 0x7Fu) == 0x7Fu) ? 1 : 0);
+    m.tmp = b | m.carry;
+    m.carry = m.bits == 7 ? b >> 7 : 0u;
     m.unstuff = b > 0x8Fu;
   }
   const uint32_t v = m.tmp & 1u;
@@ -791,7 +805,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32)
   };
 
   /* ---------------- SigProp ---------------- */
-  SppR sp{seg, (int)B.length2, 0, 0, 0, 0u};
+  SppR sp{seg, (int)B.length2, 0, 0, 0, 0u, 0u};
   for(int i = lane; i < RF_WORDS; i += 32)
     R.sig[0][i] = 0;
   for(int y0 = 0; y0 < h; y0 += 4)
@@ -858,7 +872,7 @@ __global__ void __launch_bounds__(B2K_WARPS_PER_CTA * 32)
   /* ---------------- MagRef ---------------- */
   if(B.passes > 2)
   {
-    MrpR mr{seg + B.length2 - 1, (int)B.length2, 0, 0, 1, 0u};
+    MrpR mr{seg + B.length2 - 1, (int)B.length2, 0, 0, 1, 0u, 0u};
     for(int y0 = 0; y0 < h; y0 += 4)
     {
       for(int k = 0; k < 4; ++k)

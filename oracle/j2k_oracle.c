@@ -1502,30 +1502,35 @@ ORC_API int orc_ht_encode_refine(const uint32_t* buf, uint32_t missing_msbs, uin
   return rc;
 }
 
-typedef struct { const uint8_t* data; int size, pos, unstuff; uint64_t tmp; int bits; } spp_r;
+/* Both readers place a 7-bit byte's top bit where the next byte's first bit goes, as frwd_read and rev_read_mrp
+   (L609-654, L453-541) OR whole bytes into their bit buffers: in a valid segment that bit is 0, in a damaged one it is
+   ORed into the next byte's lowest bit (`carry`). */
+typedef struct { const uint8_t* data; int size, pos, unstuff; uint64_t tmp; int bits; uint32_t carry; } spp_r;
 static int spp_get(spp_r* s)
 {
   if(!s->bits)
   {
     const uint32_t b = s->pos < s->size ? s->data[s->pos] : 0;
     s->pos++;
-    s->tmp = b;
     s->bits = 8 - s->unstuff;
+    s->tmp = b | s->carry;
+    s->carry = s->bits == 7 ? b >> 7 : 0;
     s->unstuff = (b == 0xFF);
   }
   const int v = (int)(s->tmp & 1);
   s->tmp >>= 1; s->bits--;
   return v;
 }
-typedef struct { const uint8_t* last; int size, pos, unstuff; uint64_t tmp; int bits; } mrp_r;
+typedef struct { const uint8_t* last; int size, pos, unstuff; uint64_t tmp; int bits; uint32_t carry; } mrp_r;
 static int mrp_get(mrp_r* m)
 {
   if(!m->bits)
   {
     const uint32_t b = m->pos < m->size ? *(m->last - m->pos) : 0;
     m->pos++;
-    m->tmp = b;
     m->bits = 8 - ((m->unstuff && (b & 0x7F) == 0x7F) ? 1 : 0);
+    m->tmp = b | m->carry;
+    m->carry = m->bits == 7 ? b >> 7 : 0;
     m->unstuff = b > 0x8F;
   }
   const int v = (int)(m->tmp & 1);
@@ -1551,7 +1556,7 @@ ORC_API int orc_ht_decode_passes(const uint8_t* data, uint32_t lcup, uint32_t le
   for(uint32_t y = 0; y < height; ++y)
     for(uint32_t x = 0; x < width; ++x)
       cup[(size_t)y * width + x] = sig[(size_t)y * width + x] = out[(size_t)y * stride + x] != 0;
-  spp_r sp = {data + lcup, (int)len2, 0, 0, 0, 0};
+  spp_r sp = {data + lcup, (int)len2, 0, 0, 0, 0, 0};
   for(uint32_t y0 = 0; y0 < height; y0 += 4)
   {
     const uint32_t y_limit = stripe_causal ? y0 + 4 : height;
@@ -1576,7 +1581,7 @@ ORC_API int orc_ht_decode_passes(const uint8_t* data, uint32_t lcup, uint32_t le
   }
   if(num_passes > 2)
   {
-    mrp_r mr = {data + lcup + len2 - 1, (int)len2, 0, 1, 0, 0};
+    mrp_r mr = {data + lcup + len2 - 1, (int)len2, 0, 1, 0, 0, 0};
     for(uint32_t y0 = 0; y0 < height; y0 += 4)
       for(uint32_t x = 0; x < width; ++x)
         for(uint32_t y = y0; y < y0 + 4 && y < height; ++y)
