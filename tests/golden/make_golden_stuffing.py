@@ -1,10 +1,13 @@
 #!/usr/bin/env python3
 """Regenerates tests/golden/ht_stuffing.npz from the REFERENCE's own HT block coder (oracle/_ref/libgrok_ref.so, built by
 `make -C oracle ref`): the blocks tests/test_ht_coder_paths.py constructs so that the MagSgn and VLC byte stuffing reach
-the encoder's longest fix-up chains.  Run in the build container only; the fixture is committed so that a machine without
+the encoder's longest fix-up chains, the end of a block reaches every termination cell and the segments reach their
+longest.  Run in the build container only; the fixture is committed so that a machine without
 the reference tree checks the oracle against it.
 
-Per block <label> (CONSTRUCTED: the MagSgn chain blocks and the VLC-heavy first-row blocks):
+Per block <label> (CONSTRUCTED: the MagSgn chain blocks, the VLC-heavy first-row blocks, the termination blocks term-<seed>,
+the longest MEL segment per block shape mel-longest-<w>x<h> and the largest blocks for their scratch slot
+slot-<kind>-k<Kmax>-<w>x<h>):
   <label>/coef : the block's coefficients (h, w), int32 (reversible: the quantisation indices themselves)
   <label>/data : the reference encoder's bytes; every SIMD variant built here writes the same (asserted)
   <label>/dec  : what the reference decoders (all variants agree; asserted) return for them, sign-magnitude words

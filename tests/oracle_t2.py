@@ -296,9 +296,10 @@ def tlm_segments(entries):
     return bytes(o)
 
 
-def write_codestream(cp, table, data, tlm=False, plt=False, sop=False, eph=False, prog=0, tparts=False):
+def write_codestream(cp, table, data, tlm=False, plt=False, sop=False, eph=False, prog=0, tparts=False, places=None):
     """table: the FULL block table (enumeration order, all tiles), data: its byte arena.  tparts: a tile part per
-    resolution, for the resolution-major orders (LRCP, RLCP, RPCL) only, as the writer does."""
+    resolution, for the resolution-major orders (LRCP, RLCP, RPCL) only, as the writer does.  places: a dict that
+    receives, per table row whose bytes the stream carries, where in the stream they start."""
     expn, mant = P.quant_tables(cp)
     rects = P.tile_rects(cp)
     o = bytearray(b"\xff\x4f\xff\x51")
@@ -334,6 +335,7 @@ def write_codestream(cp, table, data, tlm=False, plt=False, sop=False, eph=False
     for e, m in zip(expn, mant):
         o += _u16((int(e) << 11) | int(m)) if cp.irreversible else bytes([int(e) << 3])
     parts = []                                  # (tile, bytes of the tile part)
+    spots = []                                  # (part, packet of the part, offset in the packet, row)
     split = tparts and prog <= 2
     for t, (first, blocks) in enumerate(tile_blocks(cp)):
         rows = table[first:first + len(blocks)]
@@ -354,10 +356,14 @@ def write_codestream(cp, table, data, tlm=False, plt=False, sop=False, eph=False
                     row = rows[i]
                     if row["numpasses"] and row["length"]:
                         n = int(row["length"]) + (int(row["length2"]) if row["numpasses"] > 1 else 0)
+                        spots.append([len(pk), first + i])
                         pk += bytes(data[int(row["offset"]):int(row["offset"]) + n])
             if not runs or (split and runs[-1][0] != key[0]):
                 runs.append((key[0], []))
             runs[-1][1].append(bytes(pk))
+            for sp in spots:
+                if len(sp) == 2:
+                    sp[:0] = [len(parts) + len(runs) - 1, len(runs[-1][1]) - 1]
         if not runs:                            # a tile without packets still has one (empty) tile part
             runs.append((0, []))
         assert len(runs) <= 255
@@ -365,11 +371,16 @@ def write_codestream(cp, table, data, tlm=False, plt=False, sop=False, eph=False
             pl = plt_segments([len(p) for p in pks]) if plt else b""
             body = b"".join(pks)
             psot = 12 + len(pl) + 2 + len(body)
-            parts.append((t, b"\xff\x90" + _u16(10) + _u16(t) + _u32(psot) + bytes([i, len(runs)]) + pl + b"\xff\x93" + body))
+            parts.append((t, b"\xff\x90" + _u16(10) + _u16(t) + _u32(psot) + bytes([i, len(runs)]) + pl + b"\xff\x93" + body,
+                          14 + len(pl), np.cumsum([0] + [len(p) for p in pks])))
     if tlm:
-        o += tlm_segments([(t, len(tp)) for t, tp in parts])
-    for _, tp in parts:
+        o += tlm_segments([(t, len(tp)) for t, tp, *_ in parts])
+    part_at = len(o) + np.cumsum([0] + [len(tp) for _, tp, *_ in parts])
+    for _, tp, *_ in parts:
         o += tp
+    if places is not None:
+        for part, k, off, row in spots:
+            places[row] = int(part_at[part]) + parts[part][2] + int(parts[part][3][k]) + off
     o += b"\xff\xd9"
     return np.frombuffer(bytes(o), np.uint8)
 
