@@ -2113,18 +2113,22 @@ void b2k_launch_dwt_fwd(const DwtLevelDesc* d, int ndesc, int max_jobs, int nc, 
 {
   if(ndesc <= 0 || max_jobs <= 0)
     return;
-  dim3 grid((max_jobs + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA, ndesc), block(B2K_WARPS_PER_CTA * 32);
-  if(!irreversible)
+  dim3 grid((max_jobs + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA), block(B2K_WARPS_PER_CTA * 32);
+  for(int d0 = 0; d0 < ndesc; d0 += 65535) /* descriptor blockIdx.y: one launch per 65535 of them */
   {
-    if(nc == 3) launch_dwt<RowStage<3, true>, k_dwt53_fwd<3>>(grid, block, st, d);
-    else launch_dwt<RowStage<1, true>, k_dwt53_fwd<1>>(grid, block, st, d);
+    grid.y = (unsigned)std::min(ndesc - d0, 65535);
+    if(!irreversible)
+    {
+      if(nc == 3) launch_dwt<RowStage<3, true>, k_dwt53_fwd<3>>(grid, block, st, d + d0);
+      else launch_dwt<RowStage<1, true>, k_dwt53_fwd<1>>(grid, block, st, d + d0);
+    }
+    else
+    {
+      if(nc == 3) launch_dwt<RowStage<3>, k_dwt97_fwd<3>>(grid, block, st, d + d0);
+      else launch_dwt<RowStage<1>, k_dwt97_fwd<1>>(grid, block, st, d + d0);
+    }
+    b2k_count_launch();
   }
-  else
-  {
-    if(nc == 3) launch_dwt<RowStage<3>, k_dwt97_fwd<3>>(grid, block, st, d);
-    else launch_dwt<RowStage<1>, k_dwt97_fwd<1>>(grid, block, st, d);
-  }
-  b2k_count_launch();
 }
 
 /* ---- tiles with NO wavelet level (numres = 1): what is left of the stage is the point transform -- DC shift + RCT / ICT
@@ -2218,16 +2222,20 @@ void b2k_launch_dwt_inv(const DwtLevelDesc* d, int ndesc, int max_jobs, int nc, 
 {
   if(ndesc <= 0 || max_jobs <= 0)
     return;
-  dim3 grid((max_jobs + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA, ndesc), block(B2K_WARPS_PER_CTA * 32);
-  if(!irreversible)
+  dim3 grid((max_jobs + B2K_WARPS_PER_CTA - 1) / B2K_WARPS_PER_CTA), block(B2K_WARPS_PER_CTA * 32);
+  for(int d0 = 0; d0 < ndesc; d0 += 65535) /* descriptor blockIdx.y: one launch per 65535 of them */
   {
-    if(nc == 3) launch_dwt<BandStage<3, true>, k_dwt53_inv<3>>(grid, block, st, d);
-    else launch_dwt<BandStage<1, true>, k_dwt53_inv<1>>(grid, block, st, d);
+    grid.y = (unsigned)std::min(ndesc - d0, 65535);
+    if(!irreversible)
+    {
+      if(nc == 3) launch_dwt<BandStage<3, true>, k_dwt53_inv<3>>(grid, block, st, d + d0);
+      else launch_dwt<BandStage<1, true>, k_dwt53_inv<1>>(grid, block, st, d + d0);
+    }
+    else
+    {
+      if(nc == 3) launch_dwt<BandStage<3>, k_dwt97_inv<3>>(grid, block, st, d + d0);
+      else launch_dwt<BandStage<1>, k_dwt97_inv<1>>(grid, block, st, d + d0);
+    }
+    b2k_count_launch();
   }
-  else
-  {
-    if(nc == 3) launch_dwt<BandStage<3>, k_dwt97_inv<3>>(grid, block, st, d);
-    else launch_dwt<BandStage<1>, k_dwt97_inv<1>>(grid, block, st, d);
-  }
-  b2k_count_launch();
 }
