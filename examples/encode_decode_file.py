@@ -52,6 +52,8 @@ def main():
     ap.add_argument("dst")
     ap.add_argument("--decode", action="store_true")
     ap.add_argument("--lossy", action="store_true", help="9/7 + ICT with the HT quantiser's step sizes instead of lossless 5/3 + RCT")
+    ap.add_argument("--qfactor", type=int, default=0,
+                    help="1..100: lossy 9/7 + ICT at a JPEG-style quality factor (grk_compress --qfactor's step sizes)")
     ap.add_argument("--tile", type=int, default=0)
     ap.add_argument("--device", type=int, default=0)
     a = ap.parse_args()
@@ -64,8 +66,8 @@ def main():
         return
     planes, prec = read_pnm(a.src)
     h, w = planes[0].shape
-    cp = G.make_coding(w, h, len(planes), prec, numres=6 if min(w, h) >= 64 else 2, irreversible=a.lossy,
-                       tile=(a.tile, a.tile) if a.tile else None)
+    cp = G.make_coding(w, h, len(planes), prec, numres=6 if min(w, h) >= 64 else 2, irreversible=a.lossy or a.qfactor > 0,
+                       tile=(a.tile, a.tile) if a.tile else None, qfactor=a.qfactor or None)
     cs = eng.encode_codestream(cp, planes)
     out = G.jph_wrap(cp, cs) if a.dst.endswith(".jph") else cs
     out.tofile(a.dst)

@@ -21,6 +21,18 @@ LIB_PATH = os.environ.get("B2K_LIB") or os.path.join(_HERE, "libgrokj2k_plugin.s
 GPUP_MAX_PASSES = 3 * (16 + 7) - 2
 
 
+def _by_value(array_type, doc):
+    """a ctypes array type whose instances (and rows) compare by value, as the scalar fields of two codings do"""
+    return type(array_type.__name__, (array_type,), {"__doc__": doc, "__hash__": None,
+                                                      "__eq__": lambda a, b: type(a) is type(b) and bytes(a) == bytes(b)})
+
+
+_QccExpnRow = _by_value(C.c_uint8 * 97, "one component's b2k_coding.qcc_expn")
+_QccMantRow = _by_value(C.c_uint16 * 97, "one component's b2k_coding.qcc_mant")
+_QccExpn = _by_value(_QccExpnRow * 4, "b2k_coding.qcc_expn")
+_QccMant = _by_value(_QccMantRow * 4, "b2k_coding.qcc_mant")
+
+
 class Coding(C.Structure):
     """b2k_coding (include/grok_b200.h)."""
     _fields_ = [("x0", C.c_uint32), ("y0", C.c_uint32), ("x1", C.c_uint32), ("y1", C.c_uint32),
@@ -29,7 +41,8 @@ class Coding(C.Structure):
                 ("numres", C.c_uint8), ("cblkw_exp", C.c_uint8), ("cblkh_exp", C.c_uint8),
                 ("irreversible", C.c_uint8), ("mct", C.c_uint8), ("numgbits", C.c_uint8),
                 ("prcw_exp", C.c_uint8 * 33), ("prch_exp", C.c_uint8 * 33), ("cblk_sty", C.c_uint8),
-                ("qcd_explicit", C.c_uint8), ("qcd_expn", C.c_uint8 * 97), ("qcd_mant", C.c_uint16 * 97)]
+                ("qcd_explicit", C.c_uint8), ("qcd_expn", C.c_uint8 * 97), ("qcd_mant", C.c_uint16 * 97),
+                ("qfactor", C.c_uint8), ("qcc_mask", C.c_uint8), ("qcc_expn", _QccExpn), ("qcc_mant", _QccMant)]
 
 
 class Block(C.Structure):
@@ -158,9 +171,10 @@ def _check(rc, what):
 
 
 def make_coding(width, height, numcomps=1, prec=8, sgnd=False, numres=6, tile=None, cblk=(64, 64), irreversible=False,
-                mct=None, numgbits=1, origin=(0, 0), tile_origin=None, precincts=None):
+                mct=None, numgbits=1, origin=(0, 0), tile_origin=None, precincts=None, qfactor=None):
     """Convenience constructor; defaults follow grk_compress for an HT (.jph) output:
-    6 resolutions (CodeStream.h L43), 64x64 blocks (L40), one guard bit (GrkCompress.cpp L849)."""
+    6 resolutions (CodeStream.h L43), 64x64 blocks (L40), one guard bit (GrkCompress.cpp L849).
+    qfactor: 1..100, the band steps grk_compress --qfactor derives (needs irreversible=True)."""
     cp = Coding()
     cp.x0, cp.y0 = origin
     cp.x1, cp.y1 = origin[0] + width, origin[1] + height
@@ -179,6 +193,8 @@ def make_coding(width, height, numcomps=1, prec=8, sgnd=False, numres=6, tile=No
         for r in range(numres):
             pw, ph = precincts[min(r, len(precincts) - 1)]
             cp.prcw_exp[r], cp.prch_exp[r] = int(np.log2(pw)), int(np.log2(ph))
+    if qfactor is not None:
+        cp.qfactor = qfactor
     return cp
 
 

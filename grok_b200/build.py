@@ -8,8 +8,9 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgrokj2k_plugin.so")
 SOURCES = ["engine.cu", "dwt.cu", "ht_enc.cu", "ht_dec.cu", "geometry.cpp", "plugin.cpp", "plugin_decode.cpp", "host_pack.cpp", "codestream.cpp", "stream.cpp", "plugin_batch.cpp", "t2_device.cu", "t2_decode.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+# host code: no contraction into FMAs, so that the quality-factor step tables (geometry.cpp) are the same on every target
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
-         "-Xcompiler", "-fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function", "--use_fast_math=false"]
+         "-Xcompiler", "-fPIC,-fvisibility=hidden,-Wall,-Wno-unused-function,-ffp-contract=off", "--use_fast_math=false"]
 FLAGS = [f for f in FLAGS if not f.startswith("--use_fast_math")]
 
 

@@ -267,31 +267,38 @@ void put32(std::vector<uint8_t>& o, uint32_t v)
   put16(o, v & 0xFFFF);
 }
 
-/* Ccap15's magnitude bound from the quantiser (QuantizerOJPH::get_MAGBp L259-280, ::write L281-330) */
-uint32_t magb_code(const b2k_coding& cp, const std::vector<BandQuant>& q)
+/* Ccap15's magnitude bound from the quantiser (QuantizerOJPH::get_MAGBp L259-280, ::write L281-330); q[comp][band] */
+uint32_t magb_code(const b2k_coding& cp, const std::vector<std::vector<BandQuant>>& qc)
 {
   uint32_t B = 0;
   const int ndecomp = cp.numres - 1;
-  for(size_t i = 0; i < q.size(); ++i)
+  /* Grok's own tables and a quality factor's: the reference computes MAGB from component 0's steps only (a quality
+     factor's are pushed into its quantiser from component 0, CodeStreamCompress.cpp L617-626) */
+  const bool quirk = cp.irreversible && (cp.qfactor || (!cp.qcd_explicit && !cp.qcc_mask));
+  for(size_t c = 0; c < (quirk ? 1 : qc.size()); ++c)
   {
-    if(!cp.irreversible)
-      B = std::max<uint32_t>(B, (uint32_t)q[i].expn + cp.numgbits - 1u);
-    else if(cp.qcd_explicit)
-    { /* foreign step sizes: the bound T.814 asks for (the "scalar expounded" branch of get_MAGBp) */
-      const int nb = ndecomp - (i ? (int)((i - 1) / 3) : 0);
-      B = std::max<uint32_t>(B, (uint32_t)std::max(0, (int)q[i].expn + (int)cp.numgbits - nb));
-    }
-    else
-    { /* What the reference actually writes: its Sqcd never carries the quantisation style (Quantizer.cpp L24), so
-         get_MAGBp takes the reversible branch and scans the first 3*ndecomp+1 BYTES of the 16-bit (exponent << 11 |
-         mantissa) array through the u8/u16 union (Quantizer.h L52-57, little endian).  A looser bound than the
-         standard's, still a valid one; mirrored so that main headers stay byte-identical to grk_compress's. */
-      if(i >= (size_t)(3 * ndecomp + 1))
-        break;
-      const BandQuant& w = q[i / 2];
-      const uint32_t word = ((uint32_t)w.expn << 11) | (uint32_t)w.mant;
-      const uint32_t byte = (i & 1) ? (word >> 8) & 0xFF : word & 0xFF;
-      B = std::max<uint32_t>(B, (byte >> 3) + cp.numgbits - 1u);
+    const std::vector<BandQuant>& q = qc[c];
+    for(size_t i = 0; i < q.size(); ++i)
+    {
+      if(!cp.irreversible)
+        B = std::max<uint32_t>(B, (uint32_t)q[i].expn + cp.numgbits - 1u);
+      else if(!quirk)
+      { /* foreign step sizes: the bound T.814 asks for (the "scalar expounded" branch of get_MAGBp) */
+        const int nb = ndecomp - (i ? (int)((i - 1) / 3) : 0);
+        B = std::max<uint32_t>(B, (uint32_t)std::max(0, (int)q[i].expn + (int)cp.numgbits - nb));
+      }
+      else
+      { /* What the reference actually writes: its Sqcd never carries the quantisation style (Quantizer.cpp L24), so
+           get_MAGBp takes the reversible branch and scans the first 3*ndecomp+1 BYTES of the 16-bit (exponent << 11 |
+           mantissa) array through the u8/u16 union (Quantizer.h L52-57, little endian).  A looser bound than the
+           standard's, still a valid one; mirrored so that main headers stay byte-identical to grk_compress's. */
+        if(i >= (size_t)(3 * ndecomp + 1))
+          break;
+        const BandQuant& w = q[i / 2];
+        const uint32_t word = ((uint32_t)w.expn << 11) | (uint32_t)w.mant;
+        const uint32_t byte = (i & 1) ? (word >> 8) & 0xFF : word & 0xFF;
+        B = std::max<uint32_t>(B, (byte >> 3) + cp.numgbits - 1u);
+      }
     }
   }
   if(B <= 8)
@@ -303,8 +310,21 @@ uint32_t magb_code(const b2k_coding& cp, const std::vector<BandQuant>& q)
   return 31;
 }
 
-void write_main_header(const b2k_coding& cp, const TileGrid& g, const std::vector<BandQuant>& q, std::vector<uint8_t>& o, int prog,
-                       bool sop, bool eph)
+/* Sqcd / Sqcc and the band values of one component's table (A.6.4, A.6.5) */
+void put_quant(const b2k_coding& cp, const std::vector<BandQuant>& q, std::vector<uint8_t>& o)
+{
+  o.push_back((uint8_t)((cp.numgbits << 5) | (cp.irreversible ? 2 : 0)));
+  for(const BandQuant& b : q)
+  {
+    if(cp.irreversible)
+      put16(o, ((uint32_t)b.expn << 11) | b.mant);
+    else
+      o.push_back((uint8_t)(b.expn << 3));
+  }
+}
+
+void write_main_header(const b2k_coding& cp, const TileGrid& g, const std::vector<std::vector<BandQuant>>& q, std::vector<uint8_t>& o,
+                       int prog, bool sop, bool eph)
 {
   put16(o, 0xFF4F); /* SOC */
   put16(o, 0xFF51); /* SIZ (T.800 A.5.1) */
@@ -346,17 +366,18 @@ void write_main_header(const b2k_coding& cp, const TileGrid& g, const std::vecto
   if(user_prec)
     for(int r = 0; r < cp.numres; ++r)
       o.push_back((uint8_t)(((cp.prch_exp[r] ? cp.prch_exp[r] : 15) << 4) | (cp.prcw_exp[r] ? cp.prcw_exp[r] : 15)));
-  put16(o, 0xFF5C); /* QCD (A.6.4) */
-  const uint32_t nb = (uint32_t)q.size();
-  put16(o, 3 + (cp.irreversible ? 2 * nb : nb));
-  o.push_back((uint8_t)((cp.numgbits << 5) | (cp.irreversible ? 2 : 0)));
-  for(const BandQuant& b : q)
-  {
-    if(cp.irreversible)
-      put16(o, ((uint32_t)b.expn << 11) | b.mant);
-    else
-      o.push_back((uint8_t)(b.expn << 3));
-  }
+  const uint32_t nb = (uint32_t)q[0].size(), vals = cp.irreversible ? 2 * nb : nb;
+  put16(o, 0xFF5C); /* QCD (A.6.4): component 0's table */
+  put16(o, 3 + vals);
+  put_quant(cp, q[0], o);
+  for(int c = 1; c < cp.numcomps; ++c)
+    if(!same_quant(q[c], q[0]))
+    { /* QCC (A.6.5) for every other component whose table differs, in component order; Cqcc is 8 bits (Csiz < 257) */
+      put16(o, 0xFF5D);
+      put16(o, 4 + vals);
+      o.push_back((uint8_t)c);
+      put_quant(cp, q[c], o);
+    }
 }
 
 /* where a tile's tile parts end (packet indices): one part for the whole tile, or one per run of packets of the same
@@ -379,7 +400,7 @@ std::vector<size_t> tile_part_ends(const std::vector<uint8_t>& res_of, bool spli
 /* the main header for `flags`, with the TLM segments of nparts tile parts (entries zero) behind it: where TLM starts */
 uint64_t main_header(const b2k_coding& cp, uint32_t flags, uint64_t nparts, std::vector<uint8_t>& head)
 {
-  write_main_header(cp, tile_grid(cp), band_quant(cp), head, (int)((flags >> 8) & 7), (flags & B2K_CS_SOP) != 0, (flags & B2K_CS_EPH) != 0);
+  write_main_header(cp, tile_grid(cp), component_quant(cp), head, (int)((flags >> 8) & 7), (flags & B2K_CS_SOP) != 0, (flags & B2K_CS_EPH) != 0);
   const uint64_t at = head.size();
   if(flags & B2K_CS_TLM)
   {
@@ -939,6 +960,9 @@ int b2k_parse_main_header(const uint8_t* cs, uint64_t len, t2::MainHeader& h)
   bool use_sop = false, use_eph = false;
   std::vector<uint32_t> qcd_vals;
   uint32_t sqcd = 0;
+  std::vector<uint32_t> qcc_vals[4]; /* per component named by a QCC, its Sqcc in qcc_sq */
+  uint32_t qcc_sq[4] = {0, 0, 0, 0};
+  uint8_t qcc_mask = 0;
   /* ---- main header ---- */
   for(;;)
   {
@@ -1054,12 +1078,31 @@ int b2k_parse_main_header(const uint8_t* cs, uint64_t len, t2::MainHeader& h)
         have_qcd = s.ok;
         break;
       }
+      case 0xFF5D: { /* QCC (A.6.5): Cqcc is one byte, as Csiz < 257 here */
+        if(!have_siz)
+          return fail("QCC before SIZ", -1);
+        const uint32_t comp = s.u8(), sq = s.u8();
+        if(!s.ok)
+          return fail("truncated QCC", -1);
+        if(comp >= cp.numcomps)
+          return fail("QCC names a component the image does not have", -1);
+        if((sq & 0x1F) > 2)
+          return fail("unknown quantisation style", -1);
+        qcc_vals[comp].clear();
+        while(s.ok && s.p < s.end)
+          qcc_vals[comp].push_back((sq & 0x1F) == 0 ? s.u8() : s.u16());
+        if(!s.ok || qcc_vals[comp].empty())
+          return fail("truncated QCC", -1);
+        qcc_sq[comp] = sq;
+        qcc_mask |= (uint8_t)(1u << comp);
+        break;
+      }
       case 0xFF64: /* COM */
       case 0xFF55: /* TLM: lengths are read from SOT */
       case 0xFF63: /* CRG */
         break;
-      case 0xFF53: case 0xFF5D: case 0xFF5E: case 0xFF5F: case 0xFF60: case 0xFF57:
-        return fail("COC / QCC / RGN / POC / PPM / PLM marker segments are not handled", 1);
+      case 0xFF53: case 0xFF5E: case 0xFF5F: case 0xFF60: case 0xFF57:
+        return fail("COC / RGN / POC / PPM / PLM marker segments are not handled", 1);
       default:
         if(m < 0xFF00)
           return fail("garbage in the main header", -1);
@@ -1074,43 +1117,85 @@ int b2k_parse_main_header(const uint8_t* cs, uint64_t len, t2::MainHeader& h)
     return fail("MCT with fewer than three components", -1);
   if(const char* why = unsupported_reason(cp))
     return fail(why, 1);
-  /* band exponents / mantissas: Grok's HT quantiser tables when QCD agrees with them, else QCD's own values */
+  /* band exponents / mantissas: Grok's HT quantiser tables when QCD agrees with them, or some quality factor's when QCD
+     and every QCC agree with its tables, else QCD's and the QCCs' own values */
   {
-    const uint32_t style = sqcd & 0x1F;
-    if((style != 0) != (cp.irreversible != 0))
-      return fail("quantisation style does not match the wavelet", 1);
     const size_t nbands = 3 * (size_t)(cp.numres - 1) + 1;
-    std::vector<uint32_t> vals(nbands);
-    if(style == 1)
-    { /* scalar derived (A.6.4, E.1.1.1): (e_b, m_b) = (e_0 - N_L + n_b, m_0), n_b = decomposition level of the band */
-      if(qcd_vals.empty())
-        return fail("QCD has no entry", -1);
-      const int e0 = (int)(qcd_vals[0] >> 11), m0 = (int)(qcd_vals[0] & 0x7FF), NL = cp.numres - 1;
-      for(size_t i = 0; i < nbands; ++i)
-      {
-        const int nb = i == 0 ? NL : NL - (int)((i - 1) / 3);
-        vals[i] = (uint32_t)(std::max(0, e0 - NL + nb) << 11) | (uint32_t)m0;
+    /* one QCD / QCC: (exponent << 11 | mantissa) per band; 0, else the return code with the error set */
+    auto band_values = [&](uint32_t sq, const std::vector<uint32_t>& raw, const char* none, const char* few,
+                           std::vector<uint32_t>& vals) -> int {
+      const uint32_t style = sq & 0x1F;
+      if((style != 0) != (cp.irreversible != 0))
+        return fail("quantisation style does not match the wavelet", 1);
+      if((sq >> 5) != cp.numgbits)
+        return fail("QCC with guard bits other than QCD's is not handled", 1);
+      vals.assign(nbands, 0);
+      if(style == 1)
+      { /* scalar derived (A.6.4, E.1.1.1): (e_b, m_b) = (e_0 - N_L + n_b, m_0), n_b = decomposition level of the band */
+        if(raw.empty())
+          return fail(none, -1);
+        const int e0 = (int)(raw[0] >> 11), m0 = (int)(raw[0] & 0x7FF), NL = cp.numres - 1;
+        for(size_t i = 0; i < nbands; ++i)
+        {
+          const int nb = i == 0 ? NL : NL - (int)((i - 1) / 3);
+          vals[i] = (uint32_t)(std::max(0, e0 - NL + nb) << 11) | (uint32_t)m0;
+        }
       }
-    }
-    else
-    {
-      if(qcd_vals.size() < nbands)
-        return fail("QCD has fewer entries than bands", -1);
+      else
+      {
+        if(raw.size() < nbands)
+          return fail(few, -1);
+        for(size_t i = 0; i < nbands; ++i)
+          vals[i] = style == 0 ? (raw[i] >> 3) << 11 : raw[i];
+      }
+      return 0;
+    };
+    auto agrees = [&](const std::vector<uint32_t>& vals, const std::vector<BandQuant>& q) {
+      bool same = true;
       for(size_t i = 0; i < nbands; ++i)
-        vals[i] = style == 0 ? (qcd_vals[i] >> 3) << 11 : qcd_vals[i];
+        same &= (vals[i] >> 11) == q[i].expn && (cp.irreversible ? (vals[i] & 0x7FF) == q[i].mant : true);
+      return same;
+    };
+    std::vector<uint32_t> vals[5]; /* [0..3]: what each component uses, [4]: QCD */
+    if(int rc = band_values(sqcd, qcd_vals, "QCD has no entry", "QCD has fewer entries than bands", vals[4]))
+      return rc;
+    for(int k = 0; k < cp.numcomps; ++k)
+    {
+      if(!((qcc_mask >> k) & 1))
+        vals[k] = vals[4];
+      else if(int rc = band_values(qcc_sq[k], qcc_vals[k], "QCC has no entry", "QCC has fewer entries than bands", vals[k]))
+        return rc;
     }
-    const std::vector<BandQuant> dflt = band_quant(cp);
     bool same = true;
-    for(size_t i = 0; i < nbands; ++i)
-      same &= (vals[i] >> 11) == dflt[i].expn && (cp.irreversible ? (vals[i] & 0x7FF) == dflt[i].mant : true);
+    const std::vector<BandQuant> dflt = band_quant(cp); /* Grok's HT tables: the same for every component */
+    for(int k = 0; k < cp.numcomps; ++k)
+      same &= agrees(vals[k], dflt);
+    /* some quality factor's tables?  Compared word for word with the cached tables, component 0 first, so that a stream
+       that is none of them costs one short comparison per quality factor */
+    for(int qf = 1; !same && cp.irreversible && (cp.numcomps == 1 || cp.numcomps == 3) && qf <= 100; ++qf)
+    {
+      same = true;
+      for(int k = 0; k < cp.numcomps && same; ++k)
+        same = vals[k] == qfactor_words(qf, cp.prec, cp.numres, k);
+      if(same)
+        cp.qfactor = (uint8_t)qf;
+    }
     if(!same)
     {
       cp.qcd_explicit = 1;
       for(size_t i = 0; i < nbands && i < 97; ++i)
       {
-        cp.qcd_expn[i] = (uint8_t)(vals[i] >> 11);
-        cp.qcd_mant[i] = (uint16_t)(vals[i] & 0x7FF);
+        cp.qcd_expn[i] = (uint8_t)(vals[4][i] >> 11);
+        cp.qcd_mant[i] = (uint16_t)(vals[4][i] & 0x7FF);
       }
+      cp.qcc_mask = qcc_mask;
+      for(int k = 0; k < cp.numcomps; ++k)
+        if((qcc_mask >> k) & 1)
+          for(size_t i = 0; i < nbands && i < 97; ++i)
+          {
+            cp.qcc_expn[k][i] = (uint8_t)(vals[k][i] >> 11);
+            cp.qcc_mant[k][i] = (uint16_t)(vals[k][i] & 0x7FF);
+          }
     }
   }
   if(const char* why = unsupported_reason(cp))
@@ -1152,7 +1237,7 @@ int b2k_window_coding(const b2k_coding& cp, const uint32_t* window, uint32_t red
     b2k_set_error(m);
     return rc;
   };
-  const std::vector<BandQuant> q = band_quant(cp);
+  const std::vector<std::vector<BandQuant>> q = component_quant(cp);
   const TileGrid g = tile_grid(cp);
   /* ---- the tiles to deliver and the coding to decode them with ---------------------------------------------------
    * Whole image at full resolution: the stream's own coding.  Otherwise a VIRTUAL image: its area is the bounding box
@@ -1188,12 +1273,20 @@ int b2k_window_coding(const b2k_coding& cp, const uint32_t* window, uint32_t red
     vcp.y0 = std::max(cp.y0, vcp.ty0);
     vcp.x1 = (uint32_t)std::min<uint64_t>(cp.x1, (uint64_t)g.tx0 + (uint64_t)tb_x * g.tw);
     vcp.y1 = (uint32_t)std::min<uint64_t>(cp.y1, (uint64_t)g.ty0 + (uint64_t)tb_y * g.th);
-    /* the band exponents are the stream's: spelled out, since the default tables depend on the level count */
+    /* every component's band exponents are the stream's: spelled out, since the default and the quality factor's
+       tables depend on the level count */
+    vcp.qfactor = 0;
     vcp.qcd_explicit = 1;
-    for(size_t i = 0; i < q.size() && i < 97; ++i)
+    vcp.qcc_mask = 0;
+    for(int k = 0; k < cp.numcomps; ++k)
     {
-      vcp.qcd_expn[i] = q[i].expn;
-      vcp.qcd_mant[i] = q[i].mant;
+      if(k && !same_quant(q[k], q[0]))
+        vcp.qcc_mask |= (uint8_t)(1u << k);
+      for(size_t i = 0; i < q[k].size() && i < 97; ++i)
+      {
+        (k ? vcp.qcc_expn[k][i] : vcp.qcd_expn[i]) = q[k][i].expn;
+        (k ? vcp.qcc_mant[k][i] : vcp.qcd_mant[i]) = q[k][i].mant;
+      }
     }
     const bool one_tile = tb_x - ta_x == 1 && tb_y - ta_y == 1;
     if(one_tile)
@@ -1259,7 +1352,7 @@ int b2k_window_blocks(const t2::WindowCoding& wc, const b2k_block* vblocks, uint
   const b2k_coding& box = wc.box;
   const TileGrid bg = tile_grid(box);
   const uint32_t nt = bg.nx * bg.ny;
-  const std::vector<BandQuant> bq = band_quant(box);
+  const std::vector<std::vector<BandQuant>> bq = component_quant(box);
   box_blocks.clear();
   vmap.assign(nv, 0);
   uint64_t k = 0;
@@ -1314,7 +1407,7 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
   const b2k_coding cp = mh.cp;
   const int progression = mh.progression;
   const bool use_sop = mh.sop, use_eph = mh.eph;
-  const std::vector<BandQuant> q = band_quant(cp);
+  const std::vector<std::vector<BandQuant>> q = component_quant(cp);
   const TileGrid g = tile_grid(cp);
   const uint32_t ntiles = g.nx * g.ny;
   t2::WindowCoding wc;
@@ -1328,7 +1421,7 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
   const uint32_t vnt = vg.nx * vg.ny;
   if(!whole && (vg.nx != tb_x - ta_x || vg.ny != tb_y - ta_y))
     return fail("internal: virtual tile grid", -1);
-  const std::vector<BandQuant> vq = whole ? q : band_quant(vcp);
+  const std::vector<std::vector<BandQuant>> vq = whole ? q : component_quant(vcp);
   /* block table of the virtual coding in enumeration order: sizes first, then every tile fills its own slice */
   std::vector<uint64_t> tile_first(vnt + 1, 0);
   for(uint32_t t = 0; t < vnt; ++t)

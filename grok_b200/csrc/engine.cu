@@ -364,7 +364,7 @@ struct b2k_device_job
   BatchDst* h_batch_dst = nullptr; /* pinned */
   BatchSrc* d_batch_src = nullptr; /* b2k_encode_codestreams_device's conversion table, laid out likewise */
   BatchSrc* h_batch_src = nullptr; /* pinned */
-  std::vector<BandQuant> quant;
+  std::vector<std::vector<BandQuant>> quant; /* [comp][band] */
   std::vector<b2k_block> blocks;       /* every block, enumeration order */
   std::vector<uint32_t> coded_index;   /* blocks with area, index into `blocks` */
   std::vector<float> dec_quant;        /* per coded block: decoder step / 2^(31-Kmax) */
@@ -521,7 +521,7 @@ extern "C" int64_t b2k_enumerate(const b2k_coding* cp, uint32_t tile_mod, uint32
     return -1;
   }
   const TileGrid g = tile_grid(*cp);
-  const std::vector<BandQuant> q = band_quant(*cp);
+  const std::vector<std::vector<BandQuant>> q = component_quant(*cp);
   std::vector<b2k_block> v;
   for(uint32_t t = 0; t < g.nx * g.ny; ++t)
     if(t % tile_mod == tile_rem)
@@ -760,7 +760,7 @@ static int build_block_plan(b2k_device_job* J)
       continue;
     J->coded_first[s * J->slot_tiles + sel_of[b.tile] + 1] = (uint32_t)J->h_enc_desc.size() + 1;
     const Rect& tr = rect_of[b.tile];
-    const BandQuant& bq = J->quant[band_quant_index(b.resno, b.orient)];
+    const BandQuant& bq = J->quant[b.comp][band_quant_index(b.resno, b.orient)];
     HtBlockDesc d{};
     d.coef = J->coef.at((int)(s * cp.numcomps) + b.comp, tr.x0 + b.buf_x, tr.y0 + b.buf_y);
     d.pitch = J->coef.pitch;
@@ -862,7 +862,7 @@ static int job_create(b2k_engine* e, const b2k_coding* cp, uint32_t tile_mod, ui
   J->tile_mod = tile_mod;
   J->tile_rem = tile_rem;
   J->grid = tile_grid(*cp);
-  J->quant = band_quant(*cp);
+  J->quant = component_quant(*cp);
   J->slots = slots;
   for(uint32_t s = 0; s < slots; ++s)
     for(uint32_t t = 0; t < J->grid.nx * J->grid.ny; ++t)
@@ -2041,7 +2041,7 @@ extern "C" int32_t b2k_result_merge(const b2k_coding* cp, const b2k_result* cons
   }
   const TileGrid g = tile_grid(*cp);
   const uint32_t ntiles = g.nx * g.ny;
-  const std::vector<BandQuant> q = band_quant(*cp);
+  const std::vector<std::vector<BandQuant>> q = component_quant(*cp);
   std::vector<b2k_block> all;
   for(uint32_t t = 0; t < ntiles; ++t)
     enumerate_tile_blocks(*cp, t, tile_rect(*cp, g, t), q, all);

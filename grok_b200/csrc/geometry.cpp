@@ -2,6 +2,9 @@
 #include "geometry.h"
 #include <algorithm>
 #include <cmath>
+#include <cstdio>
+#include <map>
+#include <mutex>
 
 namespace b2k {
 
@@ -100,7 +103,142 @@ static void irrev_expn_mant(float delta_b, uint8_t& e, uint16_t& m)
   m = (uint16_t)mant;
 }
 
-std::vector<BandQuant> band_quant(const b2k_coding& cp)
+/* ---- quality factor -------------------------------------------------------------------------
+ * The JPEG-style quality model grk_compress --qfactor, Kakadu's Qfactor and OpenHTJ2K share: a reference step from the
+ * quality factor, divided per band by the norm of the band's 9/7 synthesis basis function, a visual weight and the norm
+ * of the component's inverse-ICT column.  Everything is double and evaluated in the order written (geometry.cpp is
+ * compiled with -ffp-contract=off), so the tables do not depend on the target's FMA support. */
+
+/* 9/7 synthesis low-pass (7 taps) and high-pass (9 taps) filters, T.800 Annex F (Table F.4, synthesis side) */
+static const double kSyn97Lo[7] = {-0.091271763114250, -0.057543526228500, 0.591271763114250, 1.115087052457000,
+                                   0.591271763114250,  -0.057543526228500, -0.091271763114250};
+static const double kSyn97Hi[9] = {0.053497514821622,  0.033728236885750, -0.156446533057980, -0.533728236885750, 1.205898036472720,
+                                   -0.533728236885750, -0.156446533057980, 0.033728236885750,  0.053497514821622};
+/* Zeng, Daly and Lei, "An overview of the visual optimization tools in JPEG 2000" (2002), Table 2, square-root domain,
+   4:4:4: five decomposition levels from the finest, HH, LH, HL within each.  Coarser bands and LL weigh 1. */
+static const double kVisY[15] = {0.0901, 0.2758, 0.2758, 0.7018, 0.8378, 0.8378, 1.0000, 1.0000,
+                                 1.0000, 1.0000, 1.0000, 1.0000, 1.0000, 1.0000, 1.0000};
+static const double kVisCb[15] = {0.0263, 0.0863, 0.0863, 0.1362, 0.2564, 0.2564, 0.3346, 0.4691,
+                                  0.4691, 0.5444, 0.6523, 0.6523, 0.7078, 0.7797, 0.7797};
+static const double kVisCr[15] = {0.0773, 0.1835, 0.1835, 0.2598, 0.4130, 0.4130, 0.5040, 0.6464,
+                                  0.6464, 0.7220, 0.8254, 0.8254, 0.8769, 0.9424, 0.9424};
+/* norms of the columns of the inverse ICT (T.800 G.3, equation G-7), rounded to four places */
+static const double kIctNorm[3] = {1.7321, 1.8051, 1.5734};
+
+static double sum_squares(const std::vector<double>& f)
+{
+  double s = 0.0;
+  for(double t : f)
+    s += t * t;
+  return s;
+}
+
+/* f(z) -> H0(z) f(z^2): the synthesis filter one decomposition level coarser */
+static std::vector<double> coarser(const std::vector<double>& f)
+{
+  std::vector<double> r(7 + 2 * f.size() - 1, 0.0);
+  for(size_t i = 0; i < 7; ++i)
+    for(size_t j = 0; j < f.size(); ++j)
+      r[i + 2 * j] += kSyn97Lo[i] * f[j];
+  return r;
+}
+
+/* energies (sums of squared taps) of the low- and high-pass synthesis filters of decomposition level l + 1, l = 0..14;
+   computed once, the level-15 filters having some 10^5 taps */
+struct SynthesisEnergies
+{
+  double lo[15], hi[15];
+  SynthesisEnergies()
+  {
+    std::vector<double> fl(kSyn97Lo, kSyn97Lo + 7), fh(kSyn97Hi, kSyn97Hi + 9);
+    for(int l = 0; l < 15; ++l)
+    {
+      lo[l] = sum_squares(fl);
+      hi[l] = sum_squares(fh);
+      fl = coarser(fl);
+      fh = coarser(fh);
+    }
+  }
+};
+
+/* the table of quality factor q: (exponent << 11 | mantissa) per band in QCD order */
+static std::vector<uint32_t> derive_qfactor_words(int q, int prec, int D, int comp)
+{
+  /* m: the JPEG quality curve's scale; above the knee (65) the visual weights fade out, gone from the top (97) on */
+  const double knee = 2.0 * (1.0 - 65 / 100.0), top = 2.0 * (1.0 - 97 / 100.0);
+  const double m = q < 50 ? 50.0 / q : 2.0 * (1.0 - q / 100.0);
+  double alpha = 0.04, wpow = 1.0;
+  if(q >= 97)
+  {
+    wpow = 0.0;
+    alpha = 0.10;
+  }
+  else if(q > 65)
+  {
+    wpow = (std::log(top) - std::log(m)) / (std::log(top) - std::log(knee));
+    alpha = 0.10 * std::pow(0.04 / 0.10, wpow);
+  }
+  const double ref = (alpha * m + std::sqrt(0.5) * std::ldexp(1.0, -prec)) * kIctNorm[0];
+  const double cgain = kIctNorm[comp < 3 ? comp : 0];
+  const double* vis = comp == 0 ? kVisY : comp == 1 ? kVisCb : kVisCr;
+  /* squared basis norms per band, finest level first (HH, LH, HL), then LL */
+  static const SynthesisEnergies E;
+  std::vector<double> norm2;
+  for(int l = 0; l < D; ++l)
+  {
+    norm2.push_back(E.hi[l] * E.hi[l]);
+    norm2.push_back(E.lo[l] * E.hi[l]);
+    norm2.push_back(E.hi[l] * E.lo[l]);
+  }
+  norm2.push_back(D ? E.lo[D - 1] * E.lo[D - 1] : 1.0);
+  const size_t nb = norm2.size();
+  std::vector<uint32_t> words(nb);
+  for(size_t k = 0; k < nb; ++k)
+  {
+    const double w = (k == nb - 1 || k >= 15) ? 1.0 : std::pow(vis[k], wpow);
+    double step = ref / (std::sqrt(norm2[k]) * w * cgain);
+    /* step = 2^-e (1 + mu / 2^11), T.800 E.1.1.1 */
+    int e = 0;
+    for(; step < 1.0; ++e)
+      step *= 2.0;
+    int mu = (int)std::floor((step - 1.0) * 2048.0 + 0.5);
+    if(mu > 2047)
+    {
+      mu = 0;
+      --e;
+    }
+    if(e > 31)
+    {
+      e = 31;
+      mu = 0;
+    }
+    if(e < 0)
+    {
+      e = 0;
+      mu = 2047;
+    }
+    words[nb - 1 - k] = ((uint32_t)e << 11) | (uint32_t)mu; /* QCD order: LL first, then HL, LH, HH from the coarsest */
+  }
+  return words;
+}
+
+/* derived once per (quality factor, precision, levels, component) and kept: the parser tries all 100 quality factors on
+   every irreversible stream whose QCD is not Grok's default, and every band_quant of a quality-factor coding reads one */
+const std::vector<uint32_t>& qfactor_words(int q, int prec, int numres, int comp)
+{
+  static std::mutex mu;
+  static std::map<uint32_t, std::vector<uint32_t>> cache;
+  const uint32_t key = (uint32_t)q | (uint32_t)prec << 8 | (uint32_t)(numres - 1) << 16 | (uint32_t)(comp < 3 ? comp : 0) << 24;
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = cache.find(key);
+  if(it == cache.end())
+    it = cache.emplace(key, derive_qfactor_words(q, prec, numres - 1, comp < 3 ? comp : 0)).first;
+  return it->second; /* std::map nodes do not move: the reference stays valid */
+}
+
+
+
+std::vector<BandQuant> band_quant(const b2k_coding& cp, int comp)
 {
   const int D = cp.numres - 1;
   std::vector<BandQuant> q(3 * D + 1);
@@ -141,11 +279,21 @@ std::vector<BandQuant> band_quant(const b2k_coding& cp)
       s++;
     }
   }
-  if(cp.qcd_explicit)
+  const bool own = comp >= 0 && comp < 4 && ((cp.qcc_mask >> comp) & 1);
+  if(cp.qfactor && cp.irreversible)
+  {
+    const std::vector<uint32_t>& w = qfactor_words(cp.qfactor, cp.prec, cp.numres, comp);
+    for(int i = 0; i < 3 * D + 1; ++i)
+    {
+      expn[i] = (uint8_t)(w[i] >> 11);
+      mant[i] = (uint16_t)(w[i] & 0x7FF);
+    }
+  }
+  else if(own || cp.qcd_explicit)
     for(int i = 0; i < 3 * D + 1 && i < 97; ++i)
-    { /* a foreign stream's QCD (or a caller's own choice) instead of the HT quantiser's tables */
-      expn[i] = cp.qcd_expn[i];
-      mant[i] = cp.irreversible ? (uint16_t)(cp.qcd_mant[i] & 0x7FF) : 0;
+    { /* a foreign stream's QCD / QCC (or a caller's own choice) instead of the HT quantiser's tables */
+      expn[i] = own ? cp.qcc_expn[comp][i] : cp.qcd_expn[i];
+      mant[i] = cp.irreversible ? (uint16_t)((own ? cp.qcc_mant[comp][i] : cp.qcd_mant[i]) & 0x7FF) : 0;
     }
   for(int i = 0; i < 3 * D + 1; ++i)
   {
@@ -163,6 +311,36 @@ std::vector<BandQuant> band_quant(const b2k_coding& cp)
   return q;
 }
 
+/* whether component c has a table of its own (its QCC's, or a quality factor's chroma table); the others share QCD's */
+static bool own_table(const b2k_coding& cp, int c)
+{
+  return ((cp.qcc_mask >> c) & 1) || (c > 0 && cp.qfactor && cp.irreversible);
+}
+
+std::vector<std::vector<BandQuant>> component_quant(const b2k_coding& cp)
+{
+  std::vector<std::vector<BandQuant>> q;
+  int shared = -1; /* the first component that takes QCD's table */
+  for(int c = 0; c < cp.numcomps; ++c)
+  {
+    const bool own = own_table(cp, c);
+    q.push_back(own || shared < 0 ? band_quant(cp, c) : q[shared]);
+    if(!own && shared < 0)
+      shared = c;
+  }
+  return q;
+}
+
+bool same_quant(const std::vector<BandQuant>& a, const std::vector<BandQuant>& b)
+{
+  if(a.size() != b.size())
+    return false;
+  for(size_t i = 0; i < a.size(); ++i)
+    if(a[i].expn != b[i].expn || a[i].mant != b[i].mant)
+      return false;
+  return true;
+}
+
 const char* unsupported_reason(const b2k_coding& cp)
 {
   if(cp.numcomps < 1 || cp.numcomps > 4)
@@ -177,15 +355,47 @@ const char* unsupported_reason(const b2k_coding& cp)
     return "MCT needs three components";
   if(cp.x1 <= cp.x0 || cp.y1 <= cp.y0)
     return "empty image";
-  const std::vector<BandQuant> q = band_quant(cp);
-  for(const BandQuant& b : q)
-    if(b.kmax > 29 || b.kmax < 1)
-      return "band bit planes outside the 32-bit HT coder's range";
+  if(cp.qfactor > 100)
+    return "quality factor 1..100 supported";
+  if(cp.qfactor && !cp.irreversible)
+    return "a quality factor needs the irreversible 9/7 transform";
+  if(cp.qfactor && cp.numcomps != 1 && cp.numcomps != 3)
+    return "a quality factor needs one or three components";
+  if(cp.qcc_mask >> cp.numcomps)
+    return "qcc_mask names a component the image does not have";
+  bool shared_checked = false; /* the components without a table of their own share one */
+  for(int c = 0; c < cp.numcomps; ++c)
+  {
+    if(!own_table(cp, c))
+    {
+      if(shared_checked)
+        continue;
+      shared_checked = true;
+    }
+    for(const BandQuant& b : band_quant(cp, c))
+      if(b.kmax > 29 || b.kmax < 1)
+      {
+        if(cp.qfactor && b.kmax < 1)
+        { /* the reference's T2 refuses such a band too ("exceeding band maximum"): its HT coder signals one bit plane */
+          static thread_local char why[160];
+          snprintf(why, sizeof why, "quality factor %u with %u guard bit(s) leaves a band without bit planes (Kmax 0): "
+                   "use more guard bits or a higher quality factor", (unsigned)cp.qfactor, (unsigned)cp.numgbits);
+          return why;
+        }
+        return "band bit planes outside the 32-bit HT coder's range";
+      }
+  }
   return nullptr;
 }
 
 void enumerate_tile_blocks(const b2k_coding& cp, uint32_t tile_index, const Rect& tile,
                            const std::vector<BandQuant>& quant, std::vector<b2k_block>& out)
+{
+  enumerate_tile_blocks(cp, tile_index, tile, std::vector<std::vector<BandQuant>>(cp.numcomps, quant), out);
+}
+
+void enumerate_tile_blocks(const b2k_coding& cp, uint32_t tile_index, const Rect& tile,
+                           const std::vector<std::vector<BandQuant>>& quant, std::vector<b2k_block>& out)
 {
   const int numres = cp.numres;
   for(uint16_t comp = 0; comp < cp.numcomps; ++comp)
@@ -208,7 +418,7 @@ void enumerate_tile_blocks(const b2k_coding& cp, uint32_t tile_index, const Rect
       {
         const int orient = resno == 0 ? 0 : b + 1;
         const Rect band = band_rect(tc, numres, resno, orient);
-        const BandQuant& bq = quant[band_quant_index(resno, orient)];
+        const BandQuant& bq = quant[comp][band_quant_index(resno, orient)];
         for(uint64_t p = 0; p < (uint64_t)gridw * gridh; ++p)
         {
           Rect prc;

@@ -9,6 +9,7 @@
  *   Mallat buffer position of a block           canvas/tile/TileComponentWindow.h L241-264
  *   enumeration order comp->res->band->prec->cblk  scheduling/standard/CompressScheduler.cpp L84-139
  *   HT step sizes / exponents                   t2/quantizer/part15/QuantizerOJPH.cpp L150-259
+ *   quality-factor step sizes (--qfactor)       CodeStreamCompress.cpp L591-630 (derived here from T.800 F / G)
  *   band step size and Kmax                     tile_processor/TileProcessor.cpp L398-419
  * Product code (no oracle/ dependency).
  */
@@ -48,11 +49,22 @@ struct BandQuant
   float step_enc;       /* encoder convention (sub-band gain included) */
   float step_dec;       /* decoder convention (gain 0 when irreversible) */
 };
-/* index = 0 for LL, else 1 + 3*(resno-1) + (orient-1) */
-std::vector<BandQuant> band_quant(const b2k_coding& cp);
+/* Component comp's band exponents, mantissas, Kmax and steps: the one place that chooses them -- Grok's HT tables, or
+   QCD's (qcd_explicit), or the component's QCC (qcc_mask), or the quality factor's (qfactor), in rising precedence.
+   index = 0 for LL, else 1 + 3*(resno-1) + (orient-1) */
+std::vector<BandQuant> band_quant(const b2k_coding& cp, int comp = 0);
+/* grk_compress --qfactor q's table for one component: (exponent << 11 | mantissa) per band, QCD order */
+const std::vector<uint32_t>& qfactor_words(int q, int prec, int numres, int comp);
+/* band_quant of every component, indexed [comp][band] */
+std::vector<std::vector<BandQuant>> component_quant(const b2k_coding& cp);
+/* the same exponents and mantissas (what QCC is written for when it differs from QCD) */
+bool same_quant(const std::vector<BandQuant>& a, const std::vector<BandQuant>& b);
 inline int band_quant_index(int resno, int orient) { return resno == 0 ? 0 : 1 + 3 * (resno - 1) + (orient - 1); }
 
-/* append the blocks of one tile (all components) in Grok's enumeration order */
+/* append the blocks of one tile (all components) in Grok's enumeration order; q[comp] = band_quant(cp, comp) */
+void enumerate_tile_blocks(const b2k_coding& cp, uint32_t tile_index, const Rect& tile,
+                           const std::vector<std::vector<BandQuant>>& q, std::vector<b2k_block>& out);
+/* the same with one table for every component (a coding without QCC or quality factor) */
 void enumerate_tile_blocks(const b2k_coding& cp, uint32_t tile_index, const Rect& tile,
                            const std::vector<BandQuant>& q, std::vector<b2k_block>& out);
 

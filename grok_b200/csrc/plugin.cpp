@@ -219,7 +219,7 @@ extern "C" gpup_tile* b2k_result_to_gpup_tile(const b2k_coding* cp, const b2k_re
       blks.push_back(&r->blocks[i]);
   const TileGrid g = tile_grid(*cp);
   const Rect tr = tile_rect(*cp, g, tile);
-  const std::vector<BandQuant> q = band_quant(*cp);
+  const std::vector<std::vector<BandQuant>> q = component_quant(*cp);
 
   gpup_tile* T = (gpup_tile*)calloc(1, sizeof(gpup_tile));
   T->decompress_flags = 0;
@@ -249,7 +249,7 @@ extern "C" gpup_tile* b2k_result_to_gpup_tile(const b2k_coding* cp, const b2k_re
         gpup_band* band = (gpup_band*)calloc(1, sizeof(gpup_band));
         res->band[b] = band;
         band->orientation = (uint8_t)(resno == 0 ? 0 : b + 1);
-        band->stepsize = q[band_quant_index(resno, band->orientation)].step_enc;
+        band->stepsize = q[c][band_quant_index(resno, band->orientation)].step_enc;
         band->numPrecincts = nprec;
         band->precincts = (gpup_precinct**)calloc(nprec ? nprec : 1, sizeof(void*));
         for(uint64_t p = 0; p < nprec; ++p)

@@ -196,7 +196,7 @@ int32_t decode_frame(b2k_engine* eng, gpup_decompress_params* params, PLUGIN_DEC
     }
     /* ---- gather what the host parsed; compact the used bytes for the upload ---- */
     const b2k_coding& cp = ctx.cp;
-    const std::vector<BandQuant> q = band_quant(cp);
+    const std::vector<std::vector<BandQuant>> q = component_quant(cp);
     uint64_t used = 0;
     bool ok = true;
     for(size_t i = 0; i < ctx.blocks.size() && ok; ++i)
@@ -218,7 +218,7 @@ int32_t decode_frame(b2k_engine* eng, gpup_decompress_params* params, PLUGIN_DEC
         for(int r = 0; r < cp.numres && ok; ++r)
           for(int b = 0; b < (r ? 3 : 1) && ok; ++b, ++bi)
           {
-            const float mine = q[band_quant_index(r, r ? b + 1 : 0)].step_dec;
+            const float mine = q[c][band_quant_index(r, r ? b + 1 : 0)].step_dec;
             const float theirs = ctx.bands[bi]->stepsize * 2.0f;
             if(std::fabs(mine - theirs) > 1e-6f * std::fabs(mine))
               ok = false;

@@ -373,6 +373,16 @@ typedef struct b2k_coding
                                       LL, then HL, LH, HH per resolution) */
   uint8_t qcd_expn[97];
   uint16_t qcd_mant[97];
+  uint8_t qfactor;                 /* 0: off.  1..100: every component's band steps are those grk_compress --qfactor derives
+                                      for this coding (a JPEG-style quality factor: 9/7 synthesis norms, visual weights
+                                      per band and component, ICT column gains); component 0's go to QCD, the others'
+                                      to QCC.  Needs irreversible = 1 and 1 or 3 components; overrides qcd_explicit and
+                                      qcc_mask.  b2k_codestream_parse sets it when QCD / QCC hold exactly such tables */
+  uint8_t qcc_mask;                /* bit c: component c takes its band exponents / mantissas from qcc_expn[c] /
+                                      qcc_mant[c] (same band order as QCD) instead of from QCD's; the parser sets the
+                                      bit of every component a main-header QCC names */
+  uint8_t qcc_expn[4][97];
+  uint16_t qcc_mant[4][97];
 } b2k_coding;
 
 /* One coded block as the host's T2 needs it (cf. compress_synch_with_plugin,
