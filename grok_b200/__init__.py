@@ -75,28 +75,101 @@ BLOCK_DTYPE = np.dtype([("tile", "<u4"), ("comp", "<u2"), ("resno", "u1"), ("ban
                         ("length", "<u4"), ("offset", "<u8"), ("stepsize", "<f4"), ("length2", "<u4")])
 assert BLOCK_DTYPE.itemsize == C.sizeof(Block), (BLOCK_DTYPE.itemsize, C.sizeof(Block))
 
+# the streaming callbacks (b2k_encoded_fn, b2k_decoded_fn)
+_ENCODED_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(Result), C.c_int32)
+_DECODED_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int32)
+
+
+def _signatures():
+    """name -> (restype, argtypes) of every b2k_* function include/grok_b200.h declares (tests/test_host.py checks them
+    against the header), and of gpup_tile_free.  Block tables, byte buffers and device addresses pass as c_void_p."""
+    vp, pp, i32, u32, i64, u64 = C.c_void_p, C.POINTER(C.c_void_p), C.c_int32, C.c_uint32, C.c_int64, C.c_uint64
+    cp, res, img = C.POINTER(Coding), C.POINTER(Result), C.POINTER(DevicePlanes)
+    pres, pi32, pu32, pu64 = C.POINTER(res), C.POINTER(i32), C.POINTER(u32), C.POINTER(u64)
+    pf, pd = C.POINTER(C.c_float), C.POINTER(C.c_double)
+    return {
+        "b2k_engine_create": (i32, [i32, pp]),
+        "b2k_engine_destroy": (None, [vp]),
+        "b2k_last_error": (C.c_char_p, []),
+        "b2k_coding_from_gpup": (i32, [vp, vp, i32, cp]),
+        "b2k_host_alloc": (vp, [C.c_size_t]),
+        "b2k_host_free": (None, [vp]),
+        "b2k_set_host_threads": (i32, [i32]),
+        "b2k_host_pack_last": (i32, [i32]),
+        "b2k_encode": (i32, [vp, cp, pp, pu32, u32, u32, pres]),
+        "b2k_encode16": (i32, [vp, cp, pp, pu32, u32, u32, pres]),
+        "b2k_encode16_interleaved": (i32, [vp, cp, vp, u32, u32, u32, pres]),
+        "b2k_result_free": (None, [res]),
+        "b2k_decode": (i32, [vp, cp, vp, u64, vp, u64, pp, pu32, u32, u32, pd]),
+        "b2k_decode_window": (i32, [vp, cp, vp, u64, vp, u64, pp, pu32, pu32, u32, pd]),
+        "b2k_decode16": (i32, [vp, cp, vp, u64, vp, u64, pp, pu32, u32, u32, pd]),
+        "b2k_encode_device": (i32, [vp, cp, img, u32, u32, vp, pres]),
+        "b2k_decode_device": (i32, [vp, cp, vp, u64, vp, u64, img, pu32, u32, u32, vp, pd]),
+        "b2k_encode_codestream_device": (i64, [vp, cp, img, u32, vp, pp]),
+        "b2k_encode_codestreams_device": (i32, [vp, cp, u32, img, u32, vp, pp, pu64, pu64, pi32, pd]),
+        "b2k_encode_codestreams_error": (C.c_char_p, [vp, u32]),
+        "b2k_decode_codestream_device": (i32, [vp, vp, u64, img, vp, cp, pd]),
+        "b2k_decode_codestreams_device": (i32, [vp, u32, pp, pu64, img, vp, cp, pi32, pd]),
+        "b2k_decode_codestreams_error": (C.c_char_p, [vp, u32]),
+        "b2k_codestream_parse_device": (i64, [vp, vp, u64, vp, cp, vp, u64]),
+        "b2k_codestream_parse_device_stats": (i32, [vp, pu32, pu32]),
+        "b2k_codestream_parse_window_device": (i64, [vp, vp, u64, pu32, u32, vp, cp, vp, u64]),
+        "b2k_decode_codestream_window_device": (i32, [vp, vp, u64, pu32, u32, img, vp, cp, pu32, pd]),
+        "b2k_codestream_window_device_stats": (i32, [vp, pu32, pu64]),
+        "b2k_enumerate": (i64, [cp, u32, u32, vp, u64]),
+        "b2k_result_to_gpup_tile": (vp, [cp, res, u32]),
+        "gpup_tile_free": (None, [vp]),
+        "b2k_job_create": (i32, [vp, cp, u32, u32, pp]),
+        "b2k_job_destroy": (None, [vp]),
+        "b2k_job_upload": (i32, [vp, pp, pu32]),
+        "b2k_job_forward": (i32, [vp, pf]),
+        "b2k_job_t1_encode": (i32, [vp, pf, pu64]),
+        "b2k_job_t1_decode": (i32, [vp, pf]),
+        "b2k_job_inverse": (i32, [vp, pf]),
+        "b2k_job_roundtrip": (i32, [vp, pf, pf, pu64]),
+        "b2k_job_roundtrip_n": (i32, [vp, u32, pf, pf, pf, pu64]),
+        "b2k_job_roundtrip_pipelined_n": (i32, [vp, u32, u32, u32, pf, pf, pf, pu64]),
+        "b2k_job_download": (i32, [vp, pp, pu32]),
+        "b2k_job_download_coeffs": (i32, [vp, pp, pu32]),
+        "b2k_job_upload_coeffs": (i32, [vp, pp, pu32]),
+        "b2k_job_t1_decode_blocks": (i32, [vp, vp, u64, vp, u64, pf]),
+        "b2k_job_fetch_result": (i32, [vp, pres]),
+        "b2k_job_num_blocks": (u64, [vp]),
+        "b2k_result_merge": (i32, [cp, pres, u32, pres]),
+        "b2k_codestream_write": (i64, [cp, res, u32, vp, u64]),
+        "b2k_codestream_parse": (i64, [vp, u64, cp, vp, u64]),
+        "b2k_codestream_write_tiles": (i64, [cp, res, u32, u32, u32, vp, u64, vp]),
+        "b2k_codestream_write_header": (i64, [cp, u32, vp, u32, vp, u64]),
+        "b2k_codestream_write_tiles_at": (i64, [cp, res, u32, u32, u32, vp, u64, vp]),
+        "b2k_codestream_parse_window": (i64, [vp, u64, pu32, u32, cp, vp, u64]),
+        "b2k_jph_wrap": (i64, [cp, vp, u64, vp, u64]),
+        "b2k_jph_codestream": (i32, [vp, u64, pu64, pu64]),
+        "b2k_stream_encode_begin": (i32, [i32, cp, u32, u32, _ENCODED_FN, vp, pp]),
+        "b2k_stream_encode_submit": (i32, [vp, pp, pu32, vp]),
+        "b2k_stream_decode_begin": (i32, [i32, u32, u32, _DECODED_FN, vp, pp]),
+        "b2k_stream_decode_submit": (i32, [vp, cp, vp, u64, vp, u64, pp, pu32, vp]),
+        "b2k_stream_decode_submit_codestream": (i32, [vp, vp, u64, u32, pp, pu32, vp]),
+        "b2k_stream_end": (i32, [vp]),
+        "b2k_launch_count": (u64, []),
+        "b2k_job_last_kernel_stats": (i32, [vp, C.c_int, pf, pu64]),
+    }
+
+
+_SIGNATURES = _signatures()
+
 # every symbol include/grok_b200.h declares
 # plugin_decompress (C++-ABI callback struct) is declared in csrc/plugin_decode_abi.h, not in the C header
-EXPORTS = ["minpf_post_load_plugin", "plugin_init", "plugin_get_debug_state", "gpup_encode_mem", "gpup_tile_free",
-           "b2k_engine_create", "b2k_engine_destroy", "b2k_last_error", "b2k_host_alloc", "b2k_host_free",
-           "b2k_encode", "b2k_encode16", "b2k_encode16_interleaved", "b2k_result_free", "b2k_decode", "b2k_decode16", "b2k_decode_window", "b2k_encode_device", "b2k_decode_device", "b2k_encode_codestream_device", "b2k_decode_codestream_device", "b2k_decode_codestreams_device", "b2k_decode_codestreams_error", "b2k_encode_codestreams_device", "b2k_encode_codestreams_error", "b2k_codestream_parse_device", "b2k_codestream_parse_device_stats", "b2k_codestream_parse_window_device", "b2k_decode_codestream_window_device", "b2k_codestream_window_device_stats", "b2k_enumerate",
-           "b2k_result_to_gpup_tile", "b2k_job_create", "b2k_job_destroy", "b2k_job_upload", "b2k_job_forward",
-           "b2k_job_t1_encode", "b2k_job_t1_decode", "b2k_job_t1_decode_blocks", "b2k_job_inverse", "b2k_job_roundtrip", "b2k_job_roundtrip_n", "b2k_job_roundtrip_pipelined_n", "b2k_job_download",
-           "b2k_job_download_coeffs", "b2k_job_upload_coeffs", "b2k_job_fetch_result", "b2k_job_num_blocks",
-           "b2k_launch_count", "b2k_job_last_kernel_stats", "b2k_set_host_threads", "b2k_host_pack_last",
-           "b2k_codestream_write", "b2k_codestream_parse", "b2k_codestream_parse_window",
-           "b2k_codestream_write_tiles", "b2k_codestream_write_tiles_at", "b2k_codestream_write_header", "b2k_jph_wrap", "b2k_jph_codestream", "b2k_result_merge",
-           "gpup_encode_mem_tiles", "gpup_tiles_free", "plugin_decompress_codestream", "b2k_coding_from_gpup",
-           "b2k_stream_encode_begin", "b2k_stream_encode_submit", "b2k_stream_decode_begin", "b2k_stream_decode_submit",
-           "b2k_stream_decode_submit_codestream", "b2k_stream_end",
-           "gpup_batch_memory_begin", "gpup_batch_memory_submit", "gpup_batch_memory_submit_planes", "gpup_batch_memory_end",
-           "plugin_decompress", "plugin_batch_decompress_memory_begin", "plugin_batch_decompress_memory_end"]
+EXPORTS = [n for n in _SIGNATURES if n.startswith("b2k_")] + [
+    "minpf_post_load_plugin", "plugin_init", "plugin_get_debug_state", "gpup_encode_mem", "gpup_tile_free",
+    "gpup_encode_mem_tiles", "gpup_tiles_free", "plugin_decompress_codestream",
+    "gpup_batch_memory_begin", "gpup_batch_memory_submit", "gpup_batch_memory_submit_planes", "gpup_batch_memory_end",
+    "plugin_decompress", "plugin_batch_decompress_memory_begin", "plugin_batch_decompress_memory_end"]
 
 _lib = None
 
 
 def lib():
-    """Load libgrokj2k_plugin.so (built in-tree by __graft_entry__.build / grok_b200/build.py)."""
+    """Load libgrokj2k_plugin.so (built in-tree by __graft_entry__.build / grok_b200/build.py), its functions declared."""
     global _lib
     if _lib is not None:
         return _lib
@@ -104,59 +177,9 @@ def lib():
         raise RuntimeError("%s is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
                            "(there is no CPU fallback for the engine)" % LIB_PATH)
     L = C.CDLL(LIB_PATH)
-    vp, u32, i32, u64 = C.c_void_p, C.c_uint32, C.c_int32, C.c_uint64
-    pp = C.POINTER(C.c_void_p)
-    L.b2k_last_error.restype = C.c_char_p
-    L.b2k_engine_create.argtypes = [i32, pp]
-    L.b2k_engine_destroy.argtypes = [vp]
-    L.b2k_host_alloc.argtypes = [C.c_size_t]
-    L.b2k_host_alloc.restype = vp
-    L.b2k_host_free.argtypes = [vp]
-    L.b2k_encode.argtypes = [vp, C.POINTER(Coding), pp, C.POINTER(u32), u32, u32, C.POINTER(C.POINTER(Result))]
-    L.b2k_encode16.argtypes = L.b2k_encode.argtypes
-    L.b2k_encode16_interleaved.argtypes = [vp, C.POINTER(Coding), vp, u32, u32, u32, C.POINTER(C.POINTER(Result))]
-    L.b2k_result_free.argtypes = [C.POINTER(Result)]
-    L.b2k_decode.argtypes = [vp, C.POINTER(Coding), vp, u64, vp, u64, pp, C.POINTER(u32), u32, u32,
-                             C.POINTER(C.c_double)]
-    L.b2k_decode16.argtypes = L.b2k_decode.argtypes
-    L.b2k_encode_device.argtypes = [vp, C.POINTER(Coding), C.POINTER(DevicePlanes), u32, u32, vp, C.POINTER(C.POINTER(Result))]
-    L.b2k_decode_device.argtypes = [vp, C.POINTER(Coding), vp, u64, vp, u64, C.POINTER(DevicePlanes), C.POINTER(u32), u32, u32, vp,
-                                    C.POINTER(C.c_double)]
-    L.b2k_enumerate.argtypes = [C.POINTER(Coding), u32, u32, vp, u64]
-    L.b2k_enumerate.restype = C.c_int64
-    L.b2k_result_to_gpup_tile.argtypes = [C.POINTER(Coding), C.POINTER(Result), u32]
-    L.b2k_result_to_gpup_tile.restype = vp
-    L.gpup_tile_free.argtypes = [vp]
-    L.b2k_job_create.argtypes = [vp, C.POINTER(Coding), u32, u32, pp]
-    L.b2k_job_destroy.argtypes = [vp]
-    for n in ("b2k_job_upload", "b2k_job_download", "b2k_job_download_coeffs", "b2k_job_upload_coeffs"):
-        getattr(L, n).argtypes = [vp, pp, C.POINTER(u32)]
-    L.b2k_job_forward.argtypes = [vp, C.POINTER(C.c_float)]
-    L.b2k_job_inverse.argtypes = [vp, C.POINTER(C.c_float)]
-    L.b2k_job_t1_encode.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(u64)]
-    L.b2k_job_t1_decode.argtypes = [vp, C.POINTER(C.c_float)]
-    L.b2k_job_t1_decode_blocks.argtypes = [vp, vp, u64, vp, u64, C.POINTER(C.c_float)]
-    L.b2k_job_roundtrip.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(u64)]
-    L.b2k_job_roundtrip_n.argtypes = [vp, u32, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(u64)]
-    L.b2k_job_roundtrip_pipelined_n.argtypes = [vp, u32, u32, u32, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_float),
-                                                C.POINTER(u64)]
-    L.b2k_job_fetch_result.argtypes = [vp, C.POINTER(C.POINTER(Result))]
-    L.b2k_job_num_blocks.argtypes = [vp]
-    L.b2k_job_num_blocks.restype = u64
-    L.b2k_launch_count.restype = u64
-    L.b2k_set_host_threads.argtypes = [C.c_int32]
-    L.b2k_set_host_threads.restype = C.c_int32
-    L.b2k_codestream_write.argtypes = [C.POINTER(Coding), C.POINTER(Result), C.c_uint32, vp, u64]
-    L.b2k_codestream_write.restype = C.c_int64
-    L.b2k_codestream_parse.argtypes = [vp, u64, C.POINTER(Coding), vp, u64]
-    L.b2k_codestream_parse.restype = C.c_int64
-    L.b2k_result_merge.argtypes = [C.POINTER(Coding), C.POINTER(C.POINTER(Result)), u32, C.POINTER(C.POINTER(Result))]
-    L.b2k_jph_wrap.argtypes = [C.POINTER(Coding), vp, u64, vp, u64]
-    L.b2k_jph_wrap.restype = C.c_int64
-    L.b2k_jph_codestream.argtypes = [vp, u64, C.POINTER(u64), C.POINTER(u64)]
-    L.b2k_host_pack_last.argtypes = [C.c_int32]
-    L.b2k_host_pack_last.restype = C.c_int32
-    L.b2k_job_last_kernel_stats.argtypes = [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(u64)]
+    for name, (restype, argtypes) in _SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = L
     return L
 
@@ -165,9 +188,41 @@ class EngineError(RuntimeError):
     pass
 
 
-def _check(rc, what):
+class NotHandled(EngineError):
+    pass
+
+
+# message layouts: _RC for the calls that return 0 on success; _TEXT for those that return a size or a count, and for
+# b2k_jph_codestream
+_RC, _TEXT = "{what} -> {rc}: {text}", "{what}: {text}"
+
+
+def _raise_for(rc, what, not_handled=False, msg=_RC, text=None):
+    """Raise unless rc, what the b2k_* call `what` returned, is 0: NotHandled if rc is 1 and the call returns 1 for input
+    it declines (not_handled), else EngineError.  The message is msg filled in with what, rc and text (by default
+    b2k_last_error()'s)."""
     if rc != 0:
-        raise EngineError("%s -> %d: %s" % (what, rc, (lib().b2k_last_error() or b"").decode()))
+        text = (lib().b2k_last_error() or b"").decode() if text is None else text
+        raise (NotHandled if not_handled and rc == 1 else EngineError)(msg.format(what=what, rc=rc, text=text))
+
+
+def _size(call, what, not_handled=False):
+    """call(None, 0): the size a b2k_* call(buffer, capacity) needs, in items (< 0 on failure; 1 for input it declines
+    when not_handled)"""
+    n = call(None, 0)
+    if n < 0 or (not_handled and n == 1):
+        _raise_for(n, what, not_handled, _TEXT)
+    return n
+
+
+def _size_then_fill(call, what, dtype=np.uint8, not_handled=False):
+    """A new array of the size call(None, 0) asks for, filled by call(array, size)"""
+    n = _size(call, what, not_handled)
+    out = np.zeros(n, dtype)
+    m = call(out.ctypes.data, n)
+    if m != n:      # a failure, or 0 when the input changed between the calls
+        _raise_for(m or -1, what, not_handled, _TEXT)
+    return out
 
 
 def make_coding(width, height, numcomps=1, prec=8, sgnd=False, numres=6, tile=None, cblk=(64, 64), irreversible=False,
@@ -299,12 +354,6 @@ def _stream_handle(stream, image):
     return int(stream.cuda_stream) or None
 
 
-def _check_handled(rc, what):
-    if rc == 1:
-        raise NotHandled("%s -> 1: %s" % (what, (lib().b2k_last_error() or b"").decode()))
-    _check(rc, what)
-
-
 def set_host_threads(n):
     """Host threads that narrow/widen int32 planes to 16-bit PCIe containers (0 = off, <0 = default)."""
     return int(lib().b2k_set_host_threads(int(n)))
@@ -329,62 +378,49 @@ def codestream_write(cp, blocks, data, flags=CS_TLM | CS_PLT, num_tiles=None, ou
     out: optional uint8 buffer to write into (e.g. pinned); a view of the written part is returned."""
     blocks = np.ascontiguousarray(blocks, dtype=BLOCK_DTYPE)
     data = np.ascontiguousarray(data, dtype=np.uint8)
-    r = Result()
-    r.num_blocks = len(blocks)
-    r.blocks = C.cast(blocks.ctypes.data, C.POINTER(Block))
-    r.bytes = C.cast(data.ctypes.data, C.POINTER(C.c_uint8))
-    r.num_bytes = len(data)
-    r.num_tiles = int(blocks["tile"].max()) + 1 if num_tiles is None else num_tiles
+    r = result_from_tables(blocks, data, int(blocks["tile"].max()) + 1 if num_tiles is None else num_tiles)
+
+    def write(buf, cap):
+        return lib().b2k_codestream_write(C.byref(cp), C.byref(r), flags, buf, cap)
     if out is not None:
-        n = lib().b2k_codestream_write(C.byref(cp), C.byref(r), flags, out.ctypes.data, out.size)
+        n = write(out.ctypes.data, out.size)
         if 0 <= n <= out.size:
             return out[:n]
-    else:
-        n = lib().b2k_codestream_write(C.byref(cp), C.byref(r), flags, None, 0)
-    if n < 0:
-        raise EngineError("b2k_codestream_write: " + (lib().b2k_last_error() or b"").decode())
-    out = np.zeros(n, np.uint8)
-    n2 = lib().b2k_codestream_write(C.byref(cp), C.byref(r), flags, out.ctypes.data, n)
-    assert n2 == n
-    return out
+    return _size_then_fill(write, "b2k_codestream_write")
+
+
+def window_rect(cp, window, reduce):
+    """(x0, y0, x1, y1): the pixels of `window` (x0, y0, x1, y1 on the full-resolution canvas; None for the whole image)
+    at 1 / 2**reduce resolution on the canvas of cp, the virtual coding codestream_parse_window gives for them"""
+    if window is None:
+        return (cp.x0, cp.y0, cp.x1, cp.y1)
+    sh = (1 << reduce) - 1
+    x0, y0, x1, y1 = [(v + sh) >> reduce for v in window]
+    return (max(x0, cp.x0), max(y0, cp.y0), min(x1, cp.x1), min(y1, cp.y1))
 
 
 def codestream_parse_window(cs, window=None, reduce=0):
     """b2k_codestream_parse_window -> (virtual Coding, block table, rect): rect = (x0, y0, x1, y1) of the window's pixels
     at 1 / 2**reduce resolution on the virtual coding's canvas (the whole virtual image when window is None)."""
     cs = np.ascontiguousarray(cs, dtype=np.uint8)
-    L = lib()
-    L.b2k_codestream_parse_window.restype = C.c_int64
-    L.b2k_codestream_parse_window.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(Coding), C.c_void_p, C.c_uint64]
     win = (C.c_uint32 * 4)(*window) if window is not None else None
     cp = Coding()
-    n = L.b2k_codestream_parse_window(cs.ctypes.data, len(cs), win, reduce, C.byref(cp), None, 0)
-    if n <= 1:
-        raise EngineError("b2k_codestream_parse_window: %d %s" % (n, (L.b2k_last_error() or b"").decode()))
-    blocks = np.zeros(n, BLOCK_DTYPE)
-    m = L.b2k_codestream_parse_window(cs.ctypes.data, len(cs), win, reduce, C.byref(cp), blocks.ctypes.data, n)
-    if m != n:
-        raise EngineError("b2k_codestream_parse_window: %d %s" % (m, (L.b2k_last_error() or b"").decode()))
-    if window is None:
-        rect = (cp.x0, cp.y0, cp.x1, cp.y1)
-    else:
-        sh = (1 << reduce) - 1
-        x0, y0, x1, y1 = [(v + sh) >> reduce for v in window]
-        rect = (max(x0, cp.x0), max(y0, cp.y0), min(x1, cp.x1), min(y1, cp.y1))
-    return cp, blocks, rect
+
+    def parse(blocks, cap):
+        n = lib().b2k_codestream_parse_window(cs.ctypes.data, len(cs), win, reduce, C.byref(cp), blocks, cap)
+        if n <= 1:
+            _raise_for(n, "b2k_codestream_parse_window", msg="{what}: {rc} {text}")
+        return n
+    blocks = _size_then_fill(parse, "b2k_codestream_parse_window", BLOCK_DTYPE)
+    return cp, blocks, window_rect(cp, window, reduce)
 
 
 def codestream_parse(cs):
     """-> (Coding, block table with offsets into cs).  Raises NotHandled for codestreams outside the path's scope."""
     cs = np.ascontiguousarray(cs, dtype=np.uint8)
     cp = Coding()
-    n = lib().b2k_codestream_parse(cs.ctypes.data, len(cs), C.byref(cp), None, 0)
-    if n < 0 or n == 1:
-        raise (NotHandled if n == 1 else EngineError)("b2k_codestream_parse: " + (lib().b2k_last_error() or b"").decode())
-    blocks = np.zeros(n, BLOCK_DTYPE)
-    m = lib().b2k_codestream_parse(cs.ctypes.data, len(cs), C.byref(cp), blocks.ctypes.data, n)
-    if m != n:
-        raise (NotHandled if m == 1 else EngineError)("b2k_codestream_parse: " + (lib().b2k_last_error() or b"").decode())
+    blocks = _size_then_fill(lambda blocks, cap: lib().b2k_codestream_parse(cs.ctypes.data, len(cs), C.byref(cp), blocks, cap),
+                             "b2k_codestream_parse", BLOCK_DTYPE, not_handled=True)
     return cp, blocks
 
 
@@ -405,49 +441,35 @@ def codestream_write_tiles(cp, blocks, data, flags=CS_TLM | CS_PLT, tile_mod=1, 
     (b2k_codestream_write_tiles_at) and return (out, None)."""
     blocks = np.ascontiguousarray(blocks, dtype=BLOCK_DTYPE)
     data = np.ascontiguousarray(data, dtype=np.uint8)
-    r = Result()
-    r.num_blocks = len(blocks)
-    r.blocks = C.cast(blocks.ctypes.data, C.POINTER(Block))
-    r.bytes = C.cast(data.ctypes.data, C.POINTER(C.c_uint8))
-    r.num_bytes = len(data)
+    r = result_from_tables(blocks, data, 0)
     L = lib()
-    L.b2k_codestream_write_tiles.restype = C.c_int64
-    L.b2k_codestream_write_tiles.argtypes = [C.POINTER(Coding), C.POINTER(Result), C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
     g_nx = -(-(cp.x1 - cp.tx0) // cp.tw) if cp.tw else 1
     g_ny = -(-(cp.y1 - cp.ty0) // cp.th) if cp.th else 1
     nmine = len(range(tile_rem, g_nx * g_ny, tile_mod))
     lens = np.zeros(nmine, np.uint64)
     if tile_at is not None:
-        L.b2k_codestream_write_tiles_at.restype = C.c_int64
-        L.b2k_codestream_write_tiles_at.argtypes = [C.POINTER(Coding), C.POINTER(Result), C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
         ta = np.ascontiguousarray(tile_at, dtype=np.uint64)
         n = L.b2k_codestream_write_tiles_at(C.byref(cp), C.byref(r), flags, tile_mod, tile_rem, out.ctypes.data, out.size, ta.ctypes.data)
         if n < 0:
-            raise EngineError("b2k_codestream_write_tiles_at: " + (L.b2k_last_error() or b"").decode())
+            _raise_for(n, "b2k_codestream_write_tiles_at", msg=_TEXT)
         return out, None
-    n = L.b2k_codestream_write_tiles(C.byref(cp), C.byref(r), flags, tile_mod, tile_rem, None, 0, lens.ctypes.data)
-    if n < 0:
-        raise EngineError("b2k_codestream_write_tiles: " + (L.b2k_last_error() or b"").decode())
+
+    def write(buf, cap):
+        return L.b2k_codestream_write_tiles(C.byref(cp), C.byref(r), flags, tile_mod, tile_rem, buf, cap, lens.ctypes.data)
+    n = _size(write, "b2k_codestream_write_tiles")
     if sizes_only:
         return None, lens
     if out is None or out.size < n:
         out = np.zeros(max(n, 1), np.uint8)
-    assert L.b2k_codestream_write_tiles(C.byref(cp), C.byref(r), flags, tile_mod, tile_rem, out.ctypes.data, out.size, lens.ctypes.data) == n
+    assert write(out.ctypes.data, out.size) == n
     return out[:n], lens
 
 
 def codestream_write_header(cp, flags, tile_bytes_all):
     """Main header (+ TLM) from the tile-part length of every tile (b2k_codestream_write_header)."""
     tb = np.ascontiguousarray(tile_bytes_all, dtype=np.uint64)
-    L = lib()
-    L.b2k_codestream_write_header.restype = C.c_int64
-    L.b2k_codestream_write_header.argtypes = [C.POINTER(Coding), C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64]
-    n = L.b2k_codestream_write_header(C.byref(cp), flags, tb.ctypes.data, len(tb), None, 0)
-    if n < 0:
-        raise EngineError("b2k_codestream_write_header: " + (L.b2k_last_error() or b"").decode())
-    out = np.zeros(n, np.uint8)
-    assert L.b2k_codestream_write_header(C.byref(cp), flags, tb.ctypes.data, len(tb), out.ctypes.data, n) == n
-    return out
+    return _size_then_fill(lambda buf, cap: lib().b2k_codestream_write_header(C.byref(cp), flags, tb.ctypes.data, len(tb), buf, cap),
+                           "b2k_codestream_write_header")
 
 
 def merge_shards(cp, shards):
@@ -457,32 +479,22 @@ def merge_shards(cp, shards):
     rs = [result_from_tables(b, d, 0) for b, d in keep]
     arr = (C.POINTER(Result) * len(rs))(*[C.pointer(r) for r in rs])
     out = C.POINTER(Result)()
-    _check(lib().b2k_result_merge(C.byref(cp), arr, len(rs), C.byref(out)), "b2k_result_merge")
+    _raise_for(lib().b2k_result_merge(C.byref(cp), arr, len(rs), C.byref(out)), "b2k_result_merge")
     return EncodeResult(out)
 
 
 def jph_wrap(cp, cs):
     """codestream -> .jph file bytes (JP2 boxes, brand 'jph ')."""
     cs = np.ascontiguousarray(cs, dtype=np.uint8)
-    n = lib().b2k_jph_wrap(C.byref(cp), cs.ctypes.data, len(cs), None, 0)
-    if n < 0:
-        raise EngineError("b2k_jph_wrap: " + (lib().b2k_last_error() or b"").decode())
-    out = np.zeros(n, np.uint8)
-    assert lib().b2k_jph_wrap(C.byref(cp), cs.ctypes.data, len(cs), out.ctypes.data, n) == n
-    return out
+    return _size_then_fill(lambda buf, cap: lib().b2k_jph_wrap(C.byref(cp), cs.ctypes.data, len(cs), buf, cap), "b2k_jph_wrap")
 
 
 def jph_codestream(data):
     """.jph / .jp2 file bytes (or a raw codestream) -> view of the contiguous codestream."""
     data = np.ascontiguousarray(data, dtype=np.uint8)
     off, n = C.c_uint64(), C.c_uint64()
-    if lib().b2k_jph_codestream(data.ctypes.data, len(data), C.byref(off), C.byref(n)) != 0:
-        raise EngineError("b2k_jph_codestream: " + (lib().b2k_last_error() or b"").decode())
+    _raise_for(lib().b2k_jph_codestream(data.ctypes.data, len(data), C.byref(off), C.byref(n)), "b2k_jph_codestream", msg=_TEXT)
     return data[off.value:off.value + n.value]
-
-
-class NotHandled(EngineError):
-    pass
 
 
 def pinned_empty(shape, dtype):
@@ -532,7 +544,7 @@ class Engine:
     def __init__(self, device=0):
         self._h = C.c_void_p()
         self.device = device
-        _check(lib().b2k_engine_create(device, C.byref(self._h)), "b2k_engine_create")
+        _raise_for(lib().b2k_engine_create(device, C.byref(self._h)), "b2k_engine_create")
 
     def close(self):
         if self._h:
@@ -545,7 +557,7 @@ class Engine:
         ptrs, strides = _plane_ptrs(planes)
         out = C.POINTER(Result)()
         fn = "b2k_encode16" if planes[0].itemsize == 2 else "b2k_encode"
-        _check(getattr(lib(), fn)(self._h, C.byref(cp), ptrs, strides, tile_mod, tile_rem, C.byref(out)), fn)
+        _raise_for(getattr(lib(), fn)(self._h, C.byref(cp), ptrs, strides, tile_mod, tile_rem, C.byref(out)), fn)
         return EncodeResult(out)
 
     def encode_interleaved(self, cp, pixels, tile_mod=1, tile_rem=0):
@@ -553,8 +565,8 @@ class Engine:
         samples): b2k_encode16_interleaved -- the rows cross PCIe as they are, planes are made on the device."""
         assert pixels.ndim == 3 and pixels.itemsize == 2 and pixels.strides[2] == 2 and pixels.strides[1] == 2 * pixels.shape[2]
         out = C.POINTER(Result)()
-        _check(lib().b2k_encode16_interleaved(self._h, C.byref(cp), pixels.ctypes.data, pixels.strides[0] // 2, tile_mod, tile_rem,
-                                              C.byref(out)), "b2k_encode16_interleaved")
+        _raise_for(lib().b2k_encode16_interleaved(self._h, C.byref(cp), pixels.ctypes.data, pixels.strides[0] // 2, tile_mod,
+                                                  tile_rem, C.byref(out)), "b2k_encode16_interleaved")
         return EncodeResult(out)
 
     def encode_codestream(self, cp, planes, flags=CS_TLM | CS_PLT, out=None):
@@ -580,9 +592,7 @@ class Engine:
         planes of the window at 1 / 2**reduce resolution).  The planes are views of pinned buffers the engine keeps and
         reuses for later windows of the same tile-box shape: copy them to keep them."""
         cs = np.ascontiguousarray(cs, dtype=np.uint8)
-        L = lib()
         cp, blocks, rect = codestream_parse_window(cs, window, reduce)
-        n = len(blocks)
         # pinned landing planes of the WINDOW's size, kept per shape: only the window's pixels come back over PCIe
         cache = self.__dict__.setdefault("_win_planes", {})
         key = (rect[3] - rect[1], rect[2] - rect[0], cp.numcomps, np.dtype(dtype).str)
@@ -593,11 +603,8 @@ class Engine:
             out = cache[key] = [pinned_empty((key[0], key[1]), dtype) for _ in range(cp.numcomps)]
         ptrs, strides = _plane_ptrs(out)
         ms = C.c_double()
-        L.b2k_decode_window.argtypes = [C.c_void_p, C.POINTER(Coding), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
-                                        C.POINTER(C.c_void_p), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.c_uint32,
-                                        C.POINTER(C.c_double)]
-        _check(L.b2k_decode_window(self._h, C.byref(cp), blocks.ctypes.data, n, cs.ctypes.data, len(cs), ptrs, strides,
-                                   (C.c_uint32 * 4)(*rect), np.dtype(dtype).itemsize, C.byref(ms)), "b2k_decode_window")
+        _raise_for(lib().b2k_decode_window(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), cs.ctypes.data, len(cs), ptrs,
+                                           strides, (C.c_uint32 * 4)(*rect), np.dtype(dtype).itemsize, C.byref(ms)), "b2k_decode_window")
         return cp, out
 
     def decode(self, cp, blocks, data, out_planes, tile_mod=1, tile_rem=0):
@@ -606,8 +613,8 @@ class Engine:
         data = np.ascontiguousarray(data, dtype=np.uint8)
         ms = C.c_double()
         fn = "b2k_decode16" if out_planes[0].itemsize == 2 else "b2k_decode"
-        _check(getattr(lib(), fn)(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), data.ctypes.data, len(data),
-                                  ptrs, strides, tile_mod, tile_rem, C.byref(ms)), fn)
+        _raise_for(getattr(lib(), fn)(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), data.ctypes.data, len(data),
+                                      ptrs, strides, tile_mod, tile_rem, C.byref(ms)), fn)
         return ms.value
 
     # ---- images in device memory (b2k_encode_device / b2k_decode_device) ----
@@ -618,8 +625,8 @@ class Engine:
         the result equals encode() of the same samples."""
         img = device_planes(image, cp.numcomps, cp.y1 - cp.y0, cp.x1 - cp.x0, layout)
         out = C.POINTER(Result)()
-        _check_handled(lib().b2k_encode_device(self._h, C.byref(cp), C.byref(img), tile_mod, tile_rem, _stream_handle(stream, image),
-                                               C.byref(out)), "b2k_encode_device")
+        _raise_for(lib().b2k_encode_device(self._h, C.byref(cp), C.byref(img), tile_mod, tile_rem, _stream_handle(stream, image),
+                                           C.byref(out)), "b2k_encode_device", not_handled=True)
         return EncodeResult(out)
 
     def decode_device(self, cp, blocks, data, out, layout="CHW", window=None, stream=None, tile_mod=1, tile_rem=0):
@@ -635,9 +642,9 @@ class Engine:
         data = np.ascontiguousarray(data, dtype=np.uint8)
         win = (C.c_uint32 * 4)(*window) if window is not None else None
         ms = C.c_double()
-        _check_handled(lib().b2k_decode_device(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), data.ctypes.data, len(data),
-                                               C.byref(img), win, tile_mod, tile_rem, _stream_handle(stream, out), C.byref(ms)),
-                       "b2k_decode_device")
+        _raise_for(lib().b2k_decode_device(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), data.ctypes.data, len(data),
+                                           C.byref(img), win, tile_mod, tile_rem, _stream_handle(stream, out), C.byref(ms)),
+                   "b2k_decode_device", not_handled=True)
         return ms.value
 
     def encode_codestream_device(self, cp, image, flags=CS_TLM | CS_PLT, layout="CHW", stream=None, device_output=False):
@@ -656,14 +663,10 @@ class Engine:
         import torch
         img = device_planes(image, cp.numcomps, cp.y1 - cp.y0, cp.x1 - cp.x0, layout)
         handle = _stream_handle(stream, image)
-        L = lib()
-        L.b2k_encode_codestream_device.restype = C.c_int64
-        L.b2k_encode_codestream_device.argtypes = [C.c_void_p, C.POINTER(Coding), C.POINTER(DevicePlanes), C.c_uint32, C.c_void_p,
-                                                   C.POINTER(C.c_void_p)]
         ptr = C.c_void_p()
-        n = L.b2k_encode_codestream_device(self._h, C.byref(cp), C.byref(img), flags, handle, C.byref(ptr))
+        n = lib().b2k_encode_codestream_device(self._h, C.byref(cp), C.byref(img), flags, handle, C.byref(ptr))
         if n <= 1:
-            _check_handled(n, "b2k_encode_codestream_device")
+            _raise_for(n, "b2k_encode_codestream_device", not_handled=True)
         view = torch.as_tensor(_DeviceBytes(ptr.value, n), device="cuda:%d" % self.device)
         s = torch.cuda.ExternalStream(handle, device=self.device) if handle else torch.cuda.default_stream(self.device)
         with torch.cuda.stream(s):
@@ -687,11 +690,6 @@ class Engine:
         imgs = (DevicePlanes * n)(*[device_planes(images[i], nc, h, w, layout) for i in range(n)])
         handle = _stream_handle(stream, images)
         L = lib()
-        L.b2k_encode_codestreams_device.argtypes = [C.c_void_p, C.POINTER(Coding), C.c_uint32, C.POINTER(DevicePlanes), C.c_uint32,
-                                                    C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64),
-                                                    C.POINTER(C.c_uint64), C.POINTER(C.c_int32), C.POINTER(C.c_double)]
-        L.b2k_encode_codestreams_error.restype = C.c_char_p
-        L.b2k_encode_codestreams_error.argtypes = [C.c_void_p, C.c_uint32]
         ptr = C.c_void_p()
         off = (C.c_uint64 * n)()
         lens = (C.c_uint64 * n)()
@@ -699,7 +697,7 @@ class Engine:
         ms = C.c_double()
         rc = L.b2k_encode_codestreams_device(self._h, C.byref(cp), n, imgs, flags, handle, C.byref(ptr), off, lens, st, C.byref(ms))
         if rc < 0:
-            raise EngineError("b2k_encode_codestreams_device: " + (L.b2k_last_error() or b"").decode())
+            _raise_for(rc, "b2k_encode_codestreams_device", msg=_TEXT)
         status = [(int(st[i]), (L.b2k_encode_codestreams_error(self._h, i) or b"").decode()) for i in range(n)]
         span = max([int(off[i]) + int(lens[i]) for i in range(n) if st[i] == 0] or [0])
         dev = "cuda:%d" % self.device
@@ -746,66 +744,40 @@ class Engine:
             raise ValueError("a device code stream must be contiguous (strides %s)" % (tuple(strides),))
         return int(iface["data"][0] or 0), shape[0]
 
+    def _parse_call(self, ptr, n, handle, cp):
+        """b2k_codestream_parse_device of the n bytes at device address ptr into cp, as a call(blocks, capacity)"""
+        return lambda blocks, cap: lib().b2k_codestream_parse_device(self._h, ptr, n, handle, C.byref(cp), blocks, cap)
+
     def codestream_parse_device(self, cs, stream=None):
         """b2k_codestream_parse_device: (Coding, block table) of a code stream on the engine's GPU, parsed there; the
         same as codestream_parse of its bytes."""
         ptr, n = self._device_codestream_bytes(cs)
-        L = lib()
-        L.b2k_codestream_parse_device.restype = C.c_int64
-        L.b2k_codestream_parse_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(Coding), C.c_void_p, C.c_uint64]
-        handle = _stream_handle(stream, cs)
         cp = Coding()
-        nb = L.b2k_codestream_parse_device(self._h, ptr, n, handle, C.byref(cp), None, 0)
-        if nb < 0 or nb == 1:
-            raise (NotHandled if nb == 1 else EngineError)("b2k_codestream_parse_device: " + (L.b2k_last_error() or b"").decode())
-        blocks = np.zeros(nb, BLOCK_DTYPE)
-        m = L.b2k_codestream_parse_device(self._h, ptr, n, handle, C.byref(cp), blocks.ctypes.data, nb)
-        if m != nb:
-            raise (NotHandled if m == 1 else EngineError)("b2k_codestream_parse_device: " + (L.b2k_last_error() or b"").decode())
+        blocks = _size_then_fill(self._parse_call(ptr, n, _stream_handle(stream, cs), cp), "b2k_codestream_parse_device",
+                                 BLOCK_DTYPE, not_handled=True)
         return cp, blocks
 
     def codestream_parse_device_stats(self):
         """(tiles parsed packet by packet from PLT, tiles walked) of the last device parse on this engine"""
         ix, wk = C.c_uint32(), C.c_uint32()
-        L = lib()
-        L.b2k_codestream_parse_device_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
-        _check(L.b2k_codestream_parse_device_stats(self._h, C.byref(ix), C.byref(wk)), "b2k_codestream_parse_device_stats")
+        _raise_for(lib().b2k_codestream_parse_device_stats(self._h, C.byref(ix), C.byref(wk)), "b2k_codestream_parse_device_stats")
         return ix.value, wk.value
 
-    def _parse_window_device(self, ptr, n, win, reduce, handle, blocks=None):
-        L = lib()
-        L.b2k_codestream_parse_window_device.restype = C.c_int64
-        L.b2k_codestream_parse_window_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.c_void_p,
-                                                         C.POINTER(Coding), C.c_void_p, C.c_uint64]
-        cp = Coding()
-        m = L.b2k_codestream_parse_window_device(self._h, ptr, n, win, reduce, handle, C.byref(cp),
-                                                 None if blocks is None else blocks.ctypes.data, 0 if blocks is None else len(blocks))
-        if m < 0 or m == 1:
-            raise (NotHandled if m == 1 else EngineError)("b2k_codestream_parse_window_device: " + (L.b2k_last_error() or b"").decode())
-        return cp, m
-
-    @staticmethod
-    def _window_rect(cp, window, reduce):
-        """the window's pixels at 1 / 2**reduce on the virtual coding's canvas, as codestream_parse_window gives them"""
-        if window is None:
-            return (cp.x0, cp.y0, cp.x1, cp.y1)
-        sh = (1 << reduce) - 1
-        x0, y0, x1, y1 = [(v + sh) >> reduce for v in window]
-        return (max(x0, cp.x0), max(y0, cp.y0), min(x1, cp.x1), min(y1, cp.y1))
+    def _window_parse_call(self, ptr, n, win, reduce, handle, cp):
+        """b2k_codestream_parse_window_device of the n bytes at device address ptr into cp, as a call(blocks, capacity)"""
+        return lambda blocks, cap: lib().b2k_codestream_parse_window_device(self._h, ptr, n, win, reduce, handle, C.byref(cp),
+                                                                            blocks, cap)
 
     def codestream_parse_window_device(self, cs, window=None, reduce=0, stream=None):
         """b2k_codestream_parse_window_device -> (virtual Coding, block table, rect), as codestream_parse_window of the
         stream's bytes gives them, for a code stream on the engine's GPU (a 1-D uint8 CUDA array) parsed there.  Only the
         wanted tiles' tile-part headers and packets are read."""
         ptr, n = self._device_codestream_bytes(cs)
-        handle = _stream_handle(stream, cs)
         win = (C.c_uint32 * 4)(*window) if window is not None else None
-        cp, nb = self._parse_window_device(ptr, n, win, reduce, handle)
-        blocks = np.zeros(nb, BLOCK_DTYPE)
-        cp, m = self._parse_window_device(ptr, n, win, reduce, handle, blocks)
-        if m != nb:
-            raise EngineError("b2k_codestream_parse_window_device: %d blocks, then %d" % (nb, m))
-        return cp, blocks, self._window_rect(cp, window, reduce)
+        cp = Coding()
+        blocks = _size_then_fill(self._window_parse_call(ptr, n, win, reduce, _stream_handle(stream, cs), cp),
+                                 "b2k_codestream_parse_window_device", BLOCK_DTYPE, not_handled=True)
+        return cp, blocks, window_rect(cp, window, reduce)
 
     def decode_window_device(self, cs, window=None, reduce=0, out=None, dtype=None, layout="CHW", stream=None):
         """Windowed / reduced-resolution decode of a code stream on the engine's GPU (a 1-D uint8 CUDA array), into an
@@ -816,45 +788,35 @@ class Engine:
         ptr, n = self._device_codestream_bytes(cs)
         handle = _stream_handle(stream, cs)
         win = (C.c_uint32 * 4)(*window) if window is not None else None
-        cp, _ = self._parse_window_device(ptr, n, win, reduce, handle)   # the main header: the window's shape
-        x0, y0, x1, y1 = self._window_rect(cp, window, reduce)
+        cp = Coding()
+        _size(self._window_parse_call(ptr, n, win, reduce, handle, cp), "b2k_codestream_parse_window_device",
+              not_handled=True)   # the main header: the window's shape
+        x0, y0, x1, y1 = window_rect(cp, window, reduce)
         h, w = y1 - y0, x1 - x0
         if out is None:
             import torch
             shape = (cp.numcomps, h, w) if layout == "CHW" else (h, w, cp.numcomps)
             out = torch.empty(shape, dtype=torch.uint16 if dtype is None else dtype, device="cuda:%d" % self.device)
         img = device_planes(out, cp.numcomps, h, w, layout, writable=True)
-        L = lib()
-        L.b2k_decode_codestream_window_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32,
-                                                          C.POINTER(DevicePlanes), C.c_void_p, C.POINTER(Coding),
-                                                          C.POINTER(C.c_uint32), C.POINTER(C.c_double)]
         rect = (C.c_uint32 * 4)()
         ms = C.c_double()
-        _check_handled(L.b2k_decode_codestream_window_device(self._h, ptr, n, win, reduce, C.byref(img), handle, C.byref(cp),
-                                                             rect, C.byref(ms)), "b2k_decode_codestream_window_device")
+        _raise_for(lib().b2k_decode_codestream_window_device(self._h, ptr, n, win, reduce, C.byref(img), handle, C.byref(cp),
+                                                             rect, C.byref(ms)), "b2k_decode_codestream_window_device",
+                   not_handled=True)
         assert tuple(rect) == (x0, y0, x1, y1), (tuple(rect), (x0, y0, x1, y1))
         return cp, out
 
     def codestream_window_device_stats(self):
         """(wanted tiles, bytes copied into the engine's arena) of the last windowed device parse on this engine"""
         t, b = C.c_uint32(), C.c_uint64()
-        L = lib()
-        L.b2k_codestream_window_device_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
-        _check(L.b2k_codestream_window_device_stats(self._h, C.byref(t), C.byref(b)), "b2k_codestream_window_device_stats")
+        _raise_for(lib().b2k_codestream_window_device_stats(self._h, C.byref(t), C.byref(b)), "b2k_codestream_window_device_stats")
         return t.value, b.value
 
     def _decode_device_codestream(self, cs, out, dtype, layout, stream):
         ptr, n = self._device_codestream_bytes(cs)
-        L = lib()
-        L.b2k_codestream_parse_device.restype = C.c_int64
-        L.b2k_codestream_parse_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(Coding), C.c_void_p, C.c_uint64]
-        L.b2k_decode_codestream_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(DevicePlanes), C.c_void_p,
-                                                   C.POINTER(Coding), C.POINTER(C.c_double)]
         handle = _stream_handle(stream, cs)
         cp = Coding()
-        nb = L.b2k_codestream_parse_device(self._h, ptr, n, handle, C.byref(cp), None, 0)  # the main header: the image's shape
-        if nb < 0 or nb == 1:
-            raise (NotHandled if nb == 1 else EngineError)("b2k_codestream_parse_device: " + (L.b2k_last_error() or b"").decode())
+        _size(self._parse_call(ptr, n, handle, cp), "b2k_codestream_parse_device", not_handled=True)   # the main header: the image's shape
         h, w = cp.y1 - cp.y0, cp.x1 - cp.x0
         if out is None:
             import torch
@@ -862,8 +824,8 @@ class Engine:
             out = torch.empty(shape, dtype=torch.uint16 if dtype is None else dtype, device="cuda:%d" % self.device)
         img = device_planes(out, cp.numcomps, h, w, layout, writable=True)
         ms = C.c_double()
-        _check_handled(L.b2k_decode_codestream_device(self._h, ptr, n, C.byref(img), handle, C.byref(cp), C.byref(ms)),
-                       "b2k_decode_codestream_device")
+        _raise_for(lib().b2k_decode_codestream_device(self._h, ptr, n, C.byref(img), handle, C.byref(cp), C.byref(ms)),
+                   "b2k_decode_codestream_device", not_handled=True)
         return cp, out
 
     def decode_codestreams_device(self, streams, out=None, dtype=None, layout="CHW", stream=None):
@@ -883,11 +845,6 @@ class Engine:
                 raise ValueError("decode_codestreams_device: stream %d is not a CUDA array" % i)
             ptrs[i], lens[i] = self._device_codestream_bytes(cs)
         L = lib()
-        L.b2k_decode_codestreams_device.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64),
-                                                    C.POINTER(DevicePlanes), C.c_void_p, C.POINTER(Coding),
-                                                    C.POINTER(C.c_int32), C.POINTER(C.c_double)]
-        L.b2k_decode_codestreams_error.restype = C.c_char_p
-        L.b2k_decode_codestreams_error.argtypes = [C.c_void_p, C.c_uint32]
         handle = _stream_handle(stream, out if out is not None else streams[0])
         cp = Coding()
         st = (C.c_int32 * n)()
@@ -901,10 +858,10 @@ class Engine:
         # past its end
         rc = L.b2k_decode_codestreams_device(self._h, n, ptrs, lens, None, handle, C.byref(cp), st, C.byref(ms))
         if rc < 0:
-            raise EngineError("b2k_decode_codestreams_device: " + (L.b2k_last_error() or b"").decode())
+            _raise_for(rc, "b2k_decode_codestreams_device", msg=_TEXT)
         if rc == n:
             code, text = status()[0]
-            raise (NotHandled if code == 1 else EngineError)("b2k_decode_codestreams_device: stream 0: " + text)
+            _raise_for(code, "b2k_decode_codestreams_device: stream 0", not_handled=True, msg=_TEXT, text=text)
         h, w, nc = cp.y1 - cp.y0, cp.x1 - cp.x0, cp.numcomps
         shape = (n, nc, h, w) if layout == "CHW" else (n, h, w, nc)
         if out is None:
@@ -916,7 +873,7 @@ class Engine:
         imgs = (DevicePlanes * n)(*[device_planes(out[i], nc, h, w, layout, writable=True) for i in range(n)])
         rc = L.b2k_decode_codestreams_device(self._h, n, ptrs, lens, imgs, handle, C.byref(cp), st, C.byref(ms))
         if rc < 0:
-            raise EngineError("b2k_decode_codestreams_device: " + (L.b2k_last_error() or b"").decode())
+            _raise_for(rc, "b2k_decode_codestreams_device", msg=_TEXT)
         return cp, out, status()
 
     def job(self, cp, tile_mod=1, tile_rem=0):
@@ -929,7 +886,7 @@ class Job:
     def __init__(self, eng, cp, tile_mod=1, tile_rem=0):
         self._h = C.c_void_p()
         self.cp = cp
-        _check(lib().b2k_job_create(eng._h, C.byref(cp), tile_mod, tile_rem, C.byref(self._h)), "b2k_job_create")
+        _raise_for(lib().b2k_job_create(eng._h, C.byref(cp), tile_mod, tile_rem, C.byref(self._h)), "b2k_job_create")
 
     def close(self):
         if self._h:
@@ -938,7 +895,7 @@ class Job:
 
     def _planes(self, fn, planes):
         ptrs, strides = _plane_ptrs(planes)
-        _check(getattr(lib(), fn)(self._h, ptrs, strides), fn)
+        _raise_for(getattr(lib(), fn)(self._h, ptrs, strides), fn)
 
     def upload(self, planes):
         self._planes("b2k_job_upload", planes)
@@ -954,22 +911,22 @@ class Job:
 
     def forward(self):
         ms = C.c_float()
-        _check(lib().b2k_job_forward(self._h, C.byref(ms)), "b2k_job_forward")
+        _raise_for(lib().b2k_job_forward(self._h, C.byref(ms)), "b2k_job_forward")
         return ms.value
 
     def inverse(self):
         ms = C.c_float()
-        _check(lib().b2k_job_inverse(self._h, C.byref(ms)), "b2k_job_inverse")
+        _raise_for(lib().b2k_job_inverse(self._h, C.byref(ms)), "b2k_job_inverse")
         return ms.value
 
     def t1_encode(self):
         ms, total = C.c_float(), C.c_uint64()
-        _check(lib().b2k_job_t1_encode(self._h, C.byref(ms), C.byref(total)), "b2k_job_t1_encode")
+        _raise_for(lib().b2k_job_t1_encode(self._h, C.byref(ms), C.byref(total)), "b2k_job_t1_encode")
         return ms.value, total.value
 
     def t1_decode(self):
         ms = C.c_float()
-        _check(lib().b2k_job_t1_decode(self._h, C.byref(ms)), "b2k_job_t1_decode")
+        _raise_for(lib().b2k_job_t1_decode(self._h, C.byref(ms)), "b2k_job_t1_decode")
         return ms.value
 
     def t1_decode_blocks(self, blocks, data):
@@ -977,8 +934,8 @@ class Job:
         blocks = np.ascontiguousarray(blocks, dtype=BLOCK_DTYPE)
         data = np.ascontiguousarray(data, dtype=np.uint8)
         ms = C.c_float()
-        _check(lib().b2k_job_t1_decode_blocks(self._h, blocks.ctypes.data, len(blocks), data.ctypes.data, len(data), C.byref(ms)),
-               "b2k_job_t1_decode_blocks")
+        _raise_for(lib().b2k_job_t1_decode_blocks(self._h, blocks.ctypes.data, len(blocks), data.ctypes.data, len(data), C.byref(ms)),
+                   "b2k_job_t1_decode_blocks")
         return ms.value
 
     # The round trips raise EngineError on return code 2 (the coded size of a 9/7 step outgrew the byte arena): the arena
@@ -987,27 +944,27 @@ class Job:
         """`steps` round trips queued back to back, one synchronisation.  Returns (total ms, [fwd, enc, dec, inv] ms
         summed over the steps, level-1 DWT kernel ms summed, coded bytes)."""
         ms, st, l1, nb = C.c_float(), (C.c_float * 4)(), C.c_float(), C.c_uint64()
-        _check(lib().b2k_job_roundtrip_n(self._h, steps, C.byref(ms), st, C.byref(l1), C.byref(nb)), "b2k_job_roundtrip_n")
+        _raise_for(lib().b2k_job_roundtrip_n(self._h, steps, C.byref(ms), st, C.byref(l1), C.byref(nb)), "b2k_job_roundtrip_n")
         return ms.value, [float(v) for v in st], l1.value, int(nb.value)
 
     def roundtrip_pipelined_n(self, steps, chunks=0, streams=0):
         """`steps` round trips with the block-coder stage pipelined over block ranges on side streams
         (b2k_job_roundtrip_pipelined_n).  Returns (total ms, [fwd, block coder, inv] ms summed, level-1 kernel ms summed, bytes)."""
         ms, st, l1, nb = C.c_float(), (C.c_float * 3)(), C.c_float(), C.c_uint64()
-        _check(lib().b2k_job_roundtrip_pipelined_n(self._h, steps, chunks, streams, C.byref(ms), st, C.byref(l1), C.byref(nb)),
-               "b2k_job_roundtrip_pipelined_n")
+        _raise_for(lib().b2k_job_roundtrip_pipelined_n(self._h, steps, chunks, streams, C.byref(ms), st, C.byref(l1), C.byref(nb)),
+                   "b2k_job_roundtrip_pipelined_n")
         return ms.value, [float(v) for v in st], l1.value, int(nb.value)
 
     def roundtrip(self):
         """forward -> block encode -> block decode -> inverse, device-resident, one synchronisation.
         Returns (total ms, [fwd, enc, dec, inv] ms, coded bytes)."""
         ms, st, nb = C.c_float(), (C.c_float * 4)(), C.c_uint64()
-        _check(lib().b2k_job_roundtrip(self._h, C.byref(ms), st, C.byref(nb)), "b2k_job_roundtrip")
+        _raise_for(lib().b2k_job_roundtrip(self._h, C.byref(ms), st, C.byref(nb)), "b2k_job_roundtrip")
         return ms.value, list(st), nb.value
 
     def fetch_result(self):
         out = C.POINTER(Result)()
-        _check(lib().b2k_job_fetch_result(self._h, C.byref(out)), "b2k_job_fetch_result")
+        _raise_for(lib().b2k_job_fetch_result(self._h, C.byref(out)), "b2k_job_fetch_result")
         return EncodeResult(out)
 
     def num_blocks(self):
@@ -1020,51 +977,51 @@ class Job:
 
 
 def enumerate_blocks(cp, tile_mod=1, tile_rem=0):
-    n = lib().b2k_enumerate(C.byref(cp), tile_mod, tile_rem, None, 0)
-    if n < 0:
-        raise EngineError("b2k_enumerate: " + (lib().b2k_last_error() or b"").decode())
-    out = np.zeros(n, BLOCK_DTYPE)
-    lib().b2k_enumerate(C.byref(cp), tile_mod, tile_rem, out.ctypes.data, n)
-    return out
+    return _size_then_fill(lambda out, cap: lib().b2k_enumerate(C.byref(cp), tile_mod, tile_rem, out, cap), "b2k_enumerate",
+                           BLOCK_DTYPE)
 
 
 # ------------------------------------------------------------------------------------------------
 # streaming (include/grok_b200.h "streaming", csrc/stream.cpp): `depth` frames in flight on one GPU
 # ------------------------------------------------------------------------------------------------
-_ENCODED_FN = C.CFUNCTYPE(C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(Result), C.c_int32)
-_DECODED_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int32)
+class _Stream:
+    """What EncodeStream and DecodeStream share: the frames in flight, each under a key (its frame_user) with its tag and
+    what has to stay alive until its callback has run, and end()."""
+
+    def __init__(self, on_done):
+        self._tags = {}
+        self._next = 1
+        self._user_cb = on_done
+        self._h = C.c_void_p()
+
+    def _key(self, tag, *keep):
+        key = self._next
+        self._next += 1
+        self._tags[key] = (tag,) + keep
+        return C.c_void_p(key)
+
+    def _tag(self, frame_user):
+        return self._tags.pop(int(frame_user or 0), (None,))[0]
+
+    def end(self):
+        if self._h:
+            rc = lib().b2k_stream_end(self._h)
+            self._h = C.c_void_p()
+            return rc
+        return 0
 
 
-def _bind_stream():
-    L = lib()
-    if getattr(L, "_b2k_stream_bound", False):
-        return L
-    vp, u32, i32, u64 = C.c_void_p, C.c_uint32, C.c_int32, C.c_uint64
-    pp = C.POINTER(C.c_void_p)
-    L.b2k_stream_encode_begin.argtypes = [i32, C.POINTER(Coding), u32, u32, _ENCODED_FN, vp, pp]
-    L.b2k_stream_encode_submit.argtypes = [vp, pp, C.POINTER(u32), vp]
-    L.b2k_stream_decode_begin.argtypes = [i32, u32, u32, _DECODED_FN, vp, pp]
-    L.b2k_stream_decode_submit.argtypes = [vp, C.POINTER(Coding), vp, u64, vp, u64, pp, C.POINTER(u32), vp]
-    L.b2k_stream_decode_submit_codestream.argtypes = [vp, vp, u64, u32, pp, C.POINTER(u32), vp]
-    L.b2k_stream_end.argtypes = [vp]
-    L._b2k_stream_bound = True
-    return L
-
-
-class EncodeStream:
+class EncodeStream(_Stream):
     """b2k_stream_encode_*: submit(planes, tag) hands a frame to an idle worker (blocks while `depth` frames are in
     flight); on_encoded(tag, EncodeResult or None, status) runs on a worker thread -- the EncodeResult is the caller's
     (free it).  The planes must stay alive and unchanged until the callback for their frame has run."""
 
     def __init__(self, cp, depth=3, sample_bytes=4, on_encoded=None, device=0):
-        L = _bind_stream()
+        super().__init__(on_encoded)
         self._cp = cp
-        self._tags = {}
-        self._next = 1
-        self._user_cb = on_encoded
 
         def cb(_user, frame_user, result, status):
-            tag, keep = self._tags.pop(int(frame_user or 0), (None, None))
+            tag = self._tag(frame_user)
             res = EncodeResult(result) if (status == 0 and result) else None
             if self._user_cb:
                 self._user_cb(tag, res, status)
@@ -1073,66 +1030,42 @@ class EncodeStream:
             return 1 if res is not None else 0      # the EncodeResult owns the b2k_result now
 
         self._cb = _ENCODED_FN(cb)
-        self._h = C.c_void_p()
-        _check(L.b2k_stream_encode_begin(device, C.byref(cp), depth, sample_bytes, self._cb, None, C.byref(self._h)),
-               "b2k_stream_encode_begin")
+        _raise_for(lib().b2k_stream_encode_begin(device, C.byref(cp), depth, sample_bytes, self._cb, None, C.byref(self._h)),
+                   "b2k_stream_encode_begin")
 
     def submit(self, planes, tag=None):
         ptrs, strides = _plane_ptrs(planes)
-        key = self._next
-        self._next += 1
-        self._tags[key] = (tag, planes)              # keeps the planes alive until the callback
-        _check(lib().b2k_stream_encode_submit(self._h, ptrs, strides, C.c_void_p(key)), "b2k_stream_encode_submit")
-
-    def end(self):
-        if self._h:
-            rc = lib().b2k_stream_end(self._h)
-            self._h = C.c_void_p()
-            return rc
-        return 0
+        key = self._key(tag, planes)                 # keeps the planes alive until the callback
+        _raise_for(lib().b2k_stream_encode_submit(self._h, ptrs, strides, key), "b2k_stream_encode_submit")
 
 
-class DecodeStream:
+class DecodeStream(_Stream):
     """b2k_stream_decode_*: submit(cp, blocks, data, out_planes, tag) / submit_codestream(cs, out_planes, tag);
     on_decoded(tag, status) runs on a worker thread once out_planes hold the pixels."""
 
     def __init__(self, depth=3, sample_bytes=4, on_decoded=None, device=0):
-        L = _bind_stream()
-        self._tags = {}
-        self._next = 1
-        self._user_cb = on_decoded
+        super().__init__(on_decoded)
 
         def cb(_user, frame_user, status):
-            tag = self._tags.pop(int(frame_user or 0), (None,))[0]
+            tag = self._tag(frame_user)
             if self._user_cb:
                 self._user_cb(tag, status)
 
         self._cb = _DECODED_FN(cb)
-        self._h = C.c_void_p()
-        _check(L.b2k_stream_decode_begin(device, depth, sample_bytes, self._cb, None, C.byref(self._h)), "b2k_stream_decode_begin")
+        _raise_for(lib().b2k_stream_decode_begin(device, depth, sample_bytes, self._cb, None, C.byref(self._h)),
+                   "b2k_stream_decode_begin")
 
     def submit(self, cp, blocks, data, out_planes, tag=None):
         ptrs, strides = _plane_ptrs(out_planes)
         blocks = np.ascontiguousarray(blocks, dtype=BLOCK_DTYPE)
         data = np.ascontiguousarray(data, dtype=np.uint8)
-        key = self._next
-        self._next += 1
-        self._tags[key] = (tag, blocks, data, out_planes, cp)
-        _check(lib().b2k_stream_decode_submit(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), data.ctypes.data, len(data),
-                                              ptrs, strides, C.c_void_p(key)), "b2k_stream_decode_submit")
+        key = self._key(tag, blocks, data, out_planes, cp)
+        _raise_for(lib().b2k_stream_decode_submit(self._h, C.byref(cp), blocks.ctypes.data, len(blocks), data.ctypes.data, len(data),
+                                                  ptrs, strides, key), "b2k_stream_decode_submit")
 
     def submit_codestream(self, cs, out_planes, tag=None):
         ptrs, strides = _plane_ptrs(out_planes)
         cs = np.ascontiguousarray(cs, dtype=np.uint8)
-        key = self._next
-        self._next += 1
-        self._tags[key] = (tag, cs, out_planes)
-        _check(lib().b2k_stream_decode_submit_codestream(self._h, cs.ctypes.data, len(cs), len(out_planes), ptrs, strides,
-                                                         C.c_void_p(key)), "b2k_stream_decode_submit_codestream")
-
-    def end(self):
-        if self._h:
-            rc = lib().b2k_stream_end(self._h)
-            self._h = C.c_void_p()
-            return rc
-        return 0
+        key = self._key(tag, cs, out_planes)
+        _raise_for(lib().b2k_stream_decode_submit_codestream(self._h, cs.ctypes.data, len(cs), len(out_planes), ptrs, strides, key),
+                   "b2k_stream_decode_submit_codestream")

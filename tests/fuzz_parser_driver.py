@@ -18,12 +18,9 @@ from test_interop import oracle_encode   # noqa: E402
 
 def main():
     seed, rounds = int(sys.argv[1]), int(sys.argv[2])
-    L = C.CDLL(sys.argv[3]) if len(sys.argv) > 3 else G.lib()
-    L.b2k_codestream_parse_window.restype = C.c_int64
-    L.b2k_codestream_parse_window.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(G.Coding),
-                                              C.c_void_p, C.c_uint64]
-    L.b2k_jph_codestream.restype = C.c_int32
-    L.b2k_jph_codestream.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+    if len(sys.argv) > 3:
+        G.LIB_PATH = sys.argv[3]
+    L = G.lib()
     rng = np.random.default_rng(seed)
 
     def parse(buf, win, reduce):

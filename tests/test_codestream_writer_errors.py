@@ -21,15 +21,7 @@ HUGE_ARENA = 1 << 40
 
 @pytest.fixture(scope="module")
 def L():
-    L = G.lib()
-    P, u32, u64, vp = C.POINTER, C.c_uint32, C.c_uint64, C.c_void_p
-    L.b2k_codestream_write_tiles.restype = C.c_int64
-    L.b2k_codestream_write_tiles.argtypes = [P(G.Coding), P(G.Result), u32, u32, u32, vp, u64, vp]
-    L.b2k_codestream_write_tiles_at.restype = C.c_int64
-    L.b2k_codestream_write_tiles_at.argtypes = [P(G.Coding), P(G.Result), u32, u32, u32, vp, u64, vp]
-    L.b2k_codestream_write_header.restype = C.c_int64
-    L.b2k_codestream_write_header.argtypes = [P(G.Coding), u32, vp, u32, vp, u64]
-    return L
+    return G.lib()
 
 
 def coding():

@@ -23,8 +23,6 @@ def _dev(torch, cs):
 def _single(engine, torch, dcs, layout="CHW", dtype=None):
     """(rc, text, CHW image or None) of b2k_decode_codestream_device on one stream, called directly"""
     L = G.lib()
-    L.b2k_decode_codestream_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(G.DevicePlanes), C.c_void_p,
-                                               C.POINTER(G.Coding), C.POINTER(C.c_double)]
     hdr = G.Coding()
     try:
         hdr, _ = engine.codestream_parse_device(dcs)
@@ -144,10 +142,6 @@ def test_mixed_batch(engine):
     bad = torch.zeros(1, dtype=torch.uint16, device="cuda")
     imgs[2].comp[1] = bad.data_ptr() + 1                           # an invalid image descriptor: not a multiple of sample_bytes
     st, ms, bcp = (C.c_int32 * n)(), C.c_double(), G.Coding()
-    L.b2k_decode_codestreams_device.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64),
-                                                C.POINTER(G.DevicePlanes), C.c_void_p, C.POINTER(G.Coding),
-                                                C.POINTER(C.c_int32), C.POINTER(C.c_double)]
-    L.b2k_decode_codestreams_error.restype = C.c_char_p
     assert L.b2k_decode_codestreams_device(engine._h, n, ptrs, lens, imgs, None, C.byref(bcp), st, C.byref(ms)) == 2
     torch.cuda.synchronize()
     want0 = _single(engine, torch, _dev(torch, good))
@@ -243,7 +237,6 @@ def test_launches_do_not_grow_with_the_batch(engine):
         out = torch.empty_like(imgs)
         engine.decode_codestreams_device(streams, out=out)           # plan / grow once
         L = G.lib()
-        L.b2k_launch_count.restype = C.c_uint64
         before = L.b2k_launch_count()
         engine.decode_codestreams_device(streams, out=out)
         counts.append(L.b2k_launch_count() - before)

@@ -16,27 +16,13 @@ import test_device_io as D
 pytestmark = pytest.mark.gpu
 
 
-def _lib():
-    L = G.lib()
-    L.b2k_encode_codestream_device.restype = C.c_int64
-    L.b2k_encode_codestream_device.argtypes = [C.c_void_p, C.POINTER(G.Coding), C.POINTER(G.DevicePlanes), C.c_uint32, C.c_void_p,
-                                               C.POINTER(C.c_void_p)]
-    L.b2k_encode_codestreams_device.argtypes = [C.c_void_p, C.POINTER(G.Coding), C.c_uint32, C.POINTER(G.DevicePlanes), C.c_uint32,
-                                                C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
-                                                C.POINTER(C.c_int32), C.POINTER(C.c_double)]
-    L.b2k_encode_codestreams_error.restype = C.c_char_p
-    L.b2k_encode_codestreams_error.argtypes = [C.c_void_p, C.c_uint32]
-    L.b2k_launch_count.restype = C.c_uint64
-    return L
-
-
 def _bytes(torch, ptr, n):
     return torch.as_tensor(G._DeviceBytes(ptr, n), device="cuda").cpu().numpy().copy()
 
 
 def _single(engine, torch, cp, img, flags):
     """(rc, text, bytes or None) of b2k_encode_codestream_device on one image descriptor, called directly"""
-    L = _lib()
+    L = G.lib()
     ptr = C.c_void_p()
     n = L.b2k_encode_codestream_device(engine._h, C.byref(cp), C.byref(img), flags, None, C.byref(ptr))
     torch.cuda.synchronize()
@@ -47,7 +33,7 @@ def _single(engine, torch, cp, img, flags):
 
 def _raw_batch(engine, torch, cp, imgs, flags):
     """(return value, [(rc, text)], [bytes or None], offsets) of b2k_encode_codestreams_device, called directly"""
-    L = _lib()
+    L = G.lib()
     n = len(imgs)
     arr = (G.DevicePlanes * n)(*imgs)
     ptr, off, lens, st, ms = C.c_void_p(), (C.c_uint64 * n)(), (C.c_uint64 * n)(), (C.c_int32 * n)(), C.c_double()
@@ -217,7 +203,7 @@ def test_whole_call_failures(engine):
         engine.encode_codestreams_device(cp, [a, b])
     with pytest.raises(ValueError):
         engine.encode_codestreams_device(cp, [])
-    L = _lib()
+    L = G.lib()
     st = (C.c_int32 * 1)()
     assert L.b2k_encode_codestreams_device(engine._h, C.byref(cp), 0, None, 0, None, None, None, None, st, None) < 0
 
@@ -243,7 +229,7 @@ def test_hundreds_of_small_images(engine):
 
 def test_launches_do_not_grow_with_the_batch(engine):
     torch = pytest.importorskip("torch")
-    L = _lib()
+    L = G.lib()
     counts = []
     for n in (64, 160):
         cp, imgs = _small(torch, n, seed=n)
@@ -279,7 +265,7 @@ def test_one_engine_alternates():
     torch = pytest.importorskip("torch")
     eng = G.Engine(0)
     try:
-        L = _lib()
+        L = G.lib()
         cp_a, imgs_a = _small(torch, 12, seed=1)
         cp_b, imgs_b = _small(torch, 5, size=96, seed=2)
         ref_a = [eng.encode_codestream_device(cp_a, imgs_a[i], G.CS_TLM | G.CS_PLT, device_output=True) for i in range(12)]

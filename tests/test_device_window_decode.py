@@ -26,9 +26,6 @@ def _win(window):
 def _host_parse(cs, window, reduce):
     """b2k_codestream_parse_window on host bytes: (rc, text, Coding, table)"""
     L = G.lib()
-    L.b2k_codestream_parse_window.restype = C.c_int64
-    L.b2k_codestream_parse_window.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(G.Coding), C.c_void_p,
-                                              C.c_uint64]
     cs = np.ascontiguousarray(cs, np.uint8)
     cp = G.Coding()
     n = L.b2k_codestream_parse_window(cs.ctypes.data, len(cs), _win(window), reduce, C.byref(cp), None, 0)
@@ -42,9 +39,6 @@ def _host_parse(cs, window, reduce):
 def _dev_parse(engine, dcs, window, reduce, cap=None):
     """b2k_codestream_parse_window_device on a CUDA tensor: (rc, text, Coding, table)"""
     L = G.lib()
-    L.b2k_codestream_parse_window_device.restype = C.c_int64
-    L.b2k_codestream_parse_window_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.c_void_p,
-                                                     C.POINTER(G.Coding), C.c_void_p, C.c_uint64]
     cp = G.Coding()
     n = L.b2k_codestream_parse_window_device(engine._h, dcs.data_ptr(), dcs.numel(), _win(window), reduce, None, C.byref(cp), None, 0)
     if n <= 1:

@@ -29,6 +29,66 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(G.EXPORTS)
 
 
+def test_every_b2k_function_is_declared_as_the_header_declares_it():
+    """grok_b200's signature table against the prototypes of include/grok_b200.h: every b2k_* function, its argument
+    count, and per argument and return value the width and signedness of an integer or floating type, a pointer type for
+    a pointer (POINTER of the pointee, or c_void_p; a b2k_* struct by its Python mirror), the CFUNCTYPE of a callback,
+    c_char_p for a string, None for void."""
+    hdr = open(os.path.join(ROOT, "include", "grok_b200.h")).read()
+    hdr = re.sub(r"/\*.*?\*/|//[^\n]*", " ", hdr, flags=re.S)
+    protos = {name: (ret, args) for ret, name, args in
+              re.findall(r"B2K_API\s+([^;(]*?)\b(b2k_\w+)\s*\(([^)]*)\)\s*;", hdr)}
+    callbacks = {"b2k_encoded_fn": G._ENCODED_FN, "b2k_decoded_fn": G._DECODED_FN}
+    fn_protos = {name: (ret, args) for ret, name, args in
+                 re.findall(r"typedef\s+([^;(]*?)\(\s*\*\s*(\w+)\s*\)\s*\(([^)]*)\)\s*;", hdr) if name in callbacks}
+    assert len(protos) > 60 and set(fn_protos) == set(callbacks)
+    numbers = {"int8_t": (1, True), "uint8_t": (1, False), "int16_t": (2, True), "uint16_t": (2, False),
+               "int32_t": (4, True), "uint32_t": (4, False), "int64_t": (8, True), "uint64_t": (8, False),
+               "size_t": (C.sizeof(C.c_size_t), False), "int": (C.sizeof(C.c_int), True)}
+    floats = {"float": C.c_float, "double": C.c_double}
+    mirrors = {"b2k_coding": G.Coding, "b2k_block": G.Block, "b2k_result": G.Result, "b2k_device_planes": G.DevicePlanes}
+
+    def parse(decl):
+        """'const uint32_t* const* planes' -> ('uint32_t', 2)"""
+        words = [w for w in re.findall(r"\w+", decl) if w not in ("const", "struct")]
+        return words[0], decl.count("*")
+
+    def check(ctype, base, stars, what, is_return=False):
+        if stars == 0:
+            if base == "void":
+                assert ctype is None, what
+            elif base in callbacks:
+                assert ctype is callbacks[base], what
+            elif base in floats:
+                assert ctype is floats[base], what
+            else:
+                assert base in numbers, "%s: no rule for %s" % (what, base)
+                assert isinstance(ctype, type) and issubclass(ctype, C._SimpleCData) and ctype._type_ in "bBhHiIlLqQ", what
+                assert (C.sizeof(ctype), ctype(-1).value < 0) == numbers[base], what
+        elif is_return and (base, stars) == ("char", 1):
+            assert ctype is C.c_char_p, what
+        elif ctype is not C.c_void_p:
+            assert isinstance(ctype, type) and issubclass(ctype, C._Pointer), "%s: %s is not a pointer type" % (what, ctype)
+            if stars == 1 and base in mirrors:
+                assert ctype._type_ is mirrors[base], what
+            else:
+                check(ctype._type_, base, stars - 1, what)
+
+    def check_proto(name, restype, argtypes, ret, args):
+        check(restype, *parse(ret), name + " return", is_return=True)
+        params = [a for a in args.split(",") if a.strip() != "void"]
+        assert len(argtypes) == len(params), name
+        for k, (ctype, a) in enumerate(zip(argtypes, params)):
+            check(ctype, *parse(a), "%s argument %d (%s)" % (name, k, a.strip()))
+
+    for name, fn in callbacks.items():
+        check_proto(name, fn._restype_, fn._argtypes_, *fn_protos[name])
+    table = {n: sig for n, sig in G._SIGNATURES.items() if n.startswith("b2k_")}
+    assert set(table) == set(protos), set(table) ^ set(protos)
+    for name, (ret, args) in protos.items():
+        check_proto(name, *table[name], ret, args)
+
+
 _ABI_PROBE = r'''
 #include <stdio.h>
 #include <stddef.h>
@@ -361,17 +421,12 @@ def test_gpup_tile_tree_from_a_result_multi_tile_with_precincts():
         chunks.append(data)
         off += len(data)
     arena = np.concatenate(chunks)
-    r = G.Result()
-    r.num_blocks, r.blocks = len(table), C.cast(table.ctypes.data, C.POINTER(G.Block))
-    r.bytes, r.num_bytes, r.num_tiles = C.cast(arena.ctypes.data, C.POINTER(C.c_uint8)), len(arena), len(rects)
-    lib.b2k_result_to_gpup_tile.restype = C.POINTER(GpupTile)
-    lib.b2k_result_to_gpup_tile.argtypes = [C.POINTER(G.Coding), C.POINTER(G.Result), C.c_uint32]
-    lib.gpup_tile_free.argtypes = [C.POINTER(GpupTile)]
+    r = G.result_from_tables(table, arena, len(rects))
     k = 0
     for t in range(len(rects)):
         tile = lib.b2k_result_to_gpup_tile(C.byref(cp), C.byref(r), t)
         assert tile, lib.b2k_last_error()
-        T = tile.contents
+        T = C.cast(tile, C.POINTER(GpupTile)).contents
         assert T.numComponents == 3
         for c in range(3):
             tc = T.tileComponents[c].contents

@@ -275,8 +275,6 @@ def test_config4_full_size_sharded_tiles_match_grok(engine):
 def _parse_window(cs, window, reduce):
     import ctypes as C
     L = G.lib()
-    L.b2k_codestream_parse_window.restype = C.c_int64
-    L.b2k_codestream_parse_window.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint32, C.POINTER(G.Coding), C.c_void_p, C.c_uint64]
     win = (C.c_uint32 * 4)(*window) if window is not None else None
     cp = G.Coding()
     n = L.b2k_codestream_parse_window(cs.ctypes.data, len(cs), win, reduce, C.byref(cp), None, 0)

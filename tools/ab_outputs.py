@@ -73,12 +73,7 @@ def device_codestreams(G, P, eng, torch, counted, arrs):
     import test_device_batch_decode as BD
     import test_device_batch_encode as BE
     import test_device_codestream_decode as E
-    L = BE._lib()
-    L.b2k_decode_codestream_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(G.DevicePlanes), C.c_void_p,
-                                               C.POINTER(G.Coding), C.POINTER(C.c_double)]
-    L.b2k_codestream_parse_device.restype = C.c_int64
-    L.b2k_codestream_parse_device.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(G.Coding), C.c_void_p,
-                                              C.c_uint64]
+    L = G.lib()
 
     def text(rc):
         return np.frombuffer((L.b2k_last_error() or b"").decode().encode() if rc else b"", np.uint8)
@@ -124,7 +119,7 @@ def device_codestreams(G, P, eng, torch, counted, arrs):
             vcp, out = counted(tag, lambda: eng.decode_window_device(cs, win, reduce))
             torch.cuda.synchronize()
             arrs[tag + "_rec"], arrs[tag + "_coding"] = out.cpu().numpy(), np.frombuffer(bytes(vcp), np.uint8)
-            arrs[tag + "_rect"] = np.array(eng._window_rect(vcp, win, reduce))
+            arrs[tag + "_rect"] = np.array(G.window_rect(vcp, win, reduce))
             arrs[tag + "_stats"] = np.array(eng.codestream_window_device_stats(), np.uint64)
             arrs[tag + "_parse_stats"] = np.array(eng.codestream_parse_device_stats())
     # damaged streams

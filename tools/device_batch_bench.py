@@ -20,7 +20,6 @@ the batch leg's conversion, forward DWT, HT encode, T2 kernels and gather per ba
 the kernels leave to the host.  Prints one JSON line with the GPU's name and power limit; --out DIR also writes it, and
 the profiler's tables, there."""
 import argparse
-import ctypes as C
 import json
 import os
 import subprocess
@@ -122,7 +121,6 @@ def main():
     import torch
     import grok_b200 as G
     L = G.lib()
-    L.b2k_launch_count.restype = C.c_uint64
     name, power = gpu_info()
     result = dict(gpu=name, power_limit=power, steps=args.steps, warmup=args.warmup, workloads={})
     tables = []
