@@ -159,73 +159,17 @@ struct Packet
   uint32_t xpos, ypos; /* where the position-driven progressions meet this precinct on the reference grid (B.12.1.3-5) */
   PacketBand band[3] = {};
 };
-/* mirrors enumerate_tile_blocks() (geometry.cpp): same loops, counts instead of blocks */
 /* prog: 0 LRCP, 1 RLCP, 2 RPCL, 3 PCRL, 4 CPRL (one layer, so the first two coincide) */
 void tile_packets(const b2k_coding& cp, const Rect& tile, std::vector<Packet>& lrcp, uint32_t& nblocks, int prog = 0)
 {
   const int numres = cp.numres;
   std::vector<std::vector<Packet>> per_res_comp((size_t)numres * cp.numcomps);
-  uint32_t running = 0;
-  for(uint16_t comp = 0; comp < cp.numcomps; ++comp)
-    for(int resno = 0; resno < numres; ++resno)
-    {
-      const Rect res = resolution_rect(tile, numres, resno);
-      const uint32_t pw = cp.prcw_exp[resno] ? cp.prcw_exp[resno] : 15, ph = cp.prch_exp[resno] ? cp.prch_exp[resno] : 15;
-      const uint32_t px0 = (res.x0 >> pw) << pw, py0 = (res.y0 >> ph) << ph;
-      const uint64_t px1 = (uint64_t)ceil_div_pow2(res.x1, pw) << pw, py1 = (uint64_t)ceil_div_pow2(res.y1, ph) << ph;
-      uint32_t gridw = (uint32_t)((px1 >> pw) - (px0 >> pw)), gridh = (uint32_t)((py1 >> ph) - (py0 >> ph));
-      if(res.empty())
-        gridw = gridh = 0; /* an empty resolution has no precincts, hence no packets (T.800 B.6) */
-      const uint32_t bpw = resno ? pw - 1 : pw, bph = resno ? ph - 1 : ph;
-      const uint32_t bpx0 = resno ? px0 >> 1 : px0, bpy0 = resno ? py0 >> 1 : py0;
-      const uint32_t cbw = std::min<uint32_t>(cp.cblkw_exp, bpw), cbh = std::min<uint32_t>(cp.cblkh_exp, bph);
-      const int nbands = resno == 0 ? 1 : 3;
-      std::vector<Packet>& pk = per_res_comp[(size_t)resno * cp.numcomps + comp];
-      pk.resize((size_t)gridw * gridh);
-      const int nd = numres - 1 - resno;
-      for(size_t p = 0; p < pk.size(); ++p)
-      {
-        pk[p].comp = comp;
-        pk[p].resno = (uint8_t)resno;
-        pk[p].nbands = (uint8_t)nbands;
-        pk[p].precno = (uint32_t)p;
-        /* a precinct is met where its corner lies on the reference grid; the first column / row of a resolution
-           whose origin is not precinct aligned is met at the tile's edge instead */
-        const uint32_t ix = (uint32_t)(p % gridw), iy = (uint32_t)(p / gridw);
-        const uint64_t cx = ((uint64_t)(px0 >> pw) + ix) << (pw + nd), cy = ((uint64_t)(py0 >> ph) + iy) << (ph + nd);
-        pk[p].xpos = (ix == 0 && px0 != res.x0) ? tile.x0 : (uint32_t)std::min<uint64_t>(cx, 0xFFFFFFFFull);
-        pk[p].ypos = (iy == 0 && py0 != res.y0) ? tile.y0 : (uint32_t)std::min<uint64_t>(cy, 0xFFFFFFFFull);
-      }
-      for(int b = 0; b < nbands; ++b)
-      {
-        const int orient = resno == 0 ? 0 : b + 1;
-        const Rect band = band_rect(tile, numres, resno, orient);
-        /* enumerate_tile_blocks walks the precinct grid computed from the (possibly empty) resolution too */
-        const uint32_t egw = (uint32_t)((px1 >> pw) - (px0 >> pw)), egh = (uint32_t)((py1 >> ph) - (py0 >> ph));
-        for(uint64_t p = 0; p < (uint64_t)egw * egh; ++p)
-        {
-          Rect prc;
-          prc.x0 = bpx0 + (uint32_t)((p % egw) << bpw);
-          prc.y0 = bpy0 + (uint32_t)((p / egw) << bph);
-          prc.x1 = (uint32_t)std::min<uint64_t>((uint64_t)prc.x0 + (1ull << bpw), band.x1);
-          prc.y1 = (uint32_t)std::min<uint64_t>((uint64_t)prc.y0 + (1ull << bph), band.y1);
-          prc.x0 = std::max(prc.x0, band.x0);
-          prc.y0 = std::max(prc.y0, band.y0);
-          if(prc.empty())
-            continue;
-          const uint32_t gx = prc.x0 >> cbw, gy = prc.y0 >> cbh;
-          const uint32_t gw = ceil_div_pow2(prc.x1, cbw) - gx, gh = ceil_div_pow2(prc.y1, cbh) - gy;
-          if(p < pk.size())
-          {
-            pk[p].band[b].first = running;
-            pk[p].band[b].gw = gw;
-            pk[p].band[b].gh = gh;
-          }
-          running += gw * gh;
-        }
-      }
-    }
-  nblocks = running;
+  nblocks = walk_precincts(cp, tile, [&](const PrecinctBand& pb) {
+    std::vector<Packet>& pk = per_res_comp[(size_t)pb.resno * cp.numcomps + pb.comp];
+    if(pb.band_index == 0)
+      pk.push_back(Packet{pb.comp, pb.resno, pb.nbands, pb.precno, pb.xpos, pb.ypos});
+    pk[pb.precno].band[pb.band_index] = PacketBand{pb.first, pb.gw, pb.gh};
+  });
   lrcp.clear();
   for(int resno = 0; resno < numres; ++resno)
     for(uint16_t comp = 0; comp < cp.numcomps; ++comp)
@@ -1425,12 +1369,7 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
   /* block table of the virtual coding in enumeration order: sizes first, then every tile fills its own slice */
   std::vector<uint64_t> tile_first(vnt + 1, 0);
   for(uint32_t t = 0; t < vnt; ++t)
-  {
-    std::vector<Packet> pk;
-    uint32_t nb = 0;
-    tile_packets(vcp, tile_rect(vcp, vg, t), pk, nb);
-    tile_first[t + 1] = tile_first[t] + nb;
-  }
+    tile_first[t + 1] = tile_first[t] + walk_precincts(vcp, tile_rect(vcp, vg, t), [](const PrecinctBand&) {});
   const uint64_t nblocks = tile_first[vnt];
   *cp_out = vcp;
   if(!blocks)
@@ -1497,12 +1436,6 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
       rcs[vt] = parse_tile_packets(cp, tile_rect(cp, g, t), tb.data(), tile_parts[t], cs, progression, use_sop, use_eph, errs[vt]);
     if(whole)
     {
-      if(tb.size() != tile_first[vt + 1] - tile_first[vt])
-      {
-        rcs[vt] = -1;
-        errs[vt] = "internal: packet geometry and block enumeration disagree";
-        return;
-      }
       memcpy(blocks + tile_first[vt], tb.data(), tb.size() * sizeof(b2k_block));
       return;
     }
@@ -1537,7 +1470,7 @@ static int64_t parse_impl(const uint8_t* cs, uint64_t len, const uint32_t* windo
       }
       ++k;
     }
-    if(k != vb.size() || vb.size() != tile_first[vt + 1] - tile_first[vt])
+    if(k != vb.size())
     {
       rcs[vt] = -1;
       errs[vt] = "internal: virtual tile holds a different number of blocks";

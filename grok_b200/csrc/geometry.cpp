@@ -46,6 +46,19 @@ Rect resolution_rect(const Rect& tc, int numres, int resno)
   return Rect{ceil_div_pow2(tc.x0, n), ceil_div_pow2(tc.y0, n), ceil_div_pow2(tc.x1, n), ceil_div_pow2(tc.y1, n)};
 }
 
+PrecinctGrid precinct_grid(const b2k_coding& cp, const Rect& tile, int resno)
+{
+  PrecinctGrid g;
+  g.res = resolution_rect(tile, cp.numres, resno);
+  g.pw = cp.prcw_exp[resno] ? cp.prcw_exp[resno] : 15;
+  g.ph = cp.prch_exp[resno] ? cp.prch_exp[resno] : 15;
+  g.px0 = (g.res.x0 >> g.pw) << g.pw;
+  g.py0 = (g.res.y0 >> g.ph) << g.ph;
+  g.gw = g.res.empty() ? 0 : ceil_div_pow2(g.res.x1, g.pw) - (g.res.x0 >> g.pw);
+  g.gh = g.res.empty() ? 0 : ceil_div_pow2(g.res.y1, g.ph) - (g.res.y0 >> g.ph);
+  return g;
+}
+
 static uint32_t band_coord(uint32_t c, uint32_t ndecomp, uint32_t high)
 {
   if(ndecomp == 0)
@@ -397,69 +410,37 @@ void enumerate_tile_blocks(const b2k_coding& cp, uint32_t tile_index, const Rect
 void enumerate_tile_blocks(const b2k_coding& cp, uint32_t tile_index, const Rect& tile,
                            const std::vector<std::vector<BandQuant>>& quant, std::vector<b2k_block>& out)
 {
-  const int numres = cp.numres;
-  for(uint16_t comp = 0; comp < cp.numcomps; ++comp)
-  {
-    const Rect tc = tile; /* dx = dy = 1 */
-    for(int resno = 0; resno < numres; ++resno)
+  walk_precincts(cp, tile, [&](const PrecinctBand& pb) {
+    const BandQuant& bq = quant[pb.comp][band_quant_index(pb.resno, pb.orient)];
+    /* in the resolution's buffer the high-pass bands follow the lower resolution's samples */
+    const Rect lower = resolution_rect(tile, cp.numres, pb.resno ? pb.resno - 1 : 0);
+    const uint32_t bx = (pb.orient & 1) ? lower.w() : 0, by = (pb.orient & 2) ? lower.h() : 0;
+    const Rect& prc = pb.rect;
+    for(uint32_t k = 0; k < pb.gw * pb.gh; ++k)
     {
-      const Rect res = resolution_rect(tc, numres, resno);
-      const uint32_t pw = cp.prcw_exp[resno] ? cp.prcw_exp[resno] : 15, ph = cp.prch_exp[resno] ? cp.prch_exp[resno] : 15;
-      /* precinct partition of the resolution, then its grid */
-      const uint32_t px0 = (res.x0 >> pw) << pw, py0 = (res.y0 >> ph) << ph;
-      const uint64_t px1 = (uint64_t)ceil_div_pow2(res.x1, pw) << pw, py1 = (uint64_t)ceil_div_pow2(res.y1, ph) << ph;
-      const uint32_t gridw = (uint32_t)((px1 >> pw) - (px0 >> pw)), gridh = (uint32_t)((py1 >> ph) - (py0 >> ph));
-      const uint32_t bpw = resno ? pw - 1 : pw, bph = resno ? ph - 1 : ph;
-      const uint32_t bpx0 = resno ? px0 >> 1 : px0, bpy0 = resno ? py0 >> 1 : py0;
-      const uint32_t cbw = std::min<uint32_t>(cp.cblkw_exp, bpw), cbh = std::min<uint32_t>(cp.cblkh_exp, bph);
-      const Rect lower = resno ? resolution_rect(tc, numres, resno - 1) : res;
-      const int nbands = resno == 0 ? 1 : 3;
-      for(int b = 0; b < nbands; ++b)
-      {
-        const int orient = resno == 0 ? 0 : b + 1;
-        const Rect band = band_rect(tc, numres, resno, orient);
-        const BandQuant& bq = quant[comp][band_quant_index(resno, orient)];
-        for(uint64_t p = 0; p < (uint64_t)gridw * gridh; ++p)
-        {
-          Rect prc;
-          prc.x0 = bpx0 + (uint32_t)((p % gridw) << bpw);
-          prc.y0 = bpy0 + (uint32_t)((p / gridw) << bph);
-          prc.x1 = (uint32_t)std::min<uint64_t>((uint64_t)prc.x0 + (1ull << bpw), band.x1);
-          prc.y1 = (uint32_t)std::min<uint64_t>((uint64_t)prc.y0 + (1ull << bph), band.y1);
-          prc.x0 = std::max(prc.x0, band.x0);
-          prc.y0 = std::max(prc.y0, band.y0);
-          if(prc.empty())
-            continue; /* no code blocks in an empty precinct */
-          const uint32_t gx = prc.x0 >> cbw, gy = prc.y0 >> cbh;
-          const uint32_t gw = ceil_div_pow2(prc.x1, cbw) - gx, gh = ceil_div_pow2(prc.y1, cbh) - gy;
-          for(uint32_t k = 0; k < gw * gh; ++k)
-          {
-            b2k_block blk{};
-            blk.tile = tile_index;
-            blk.comp = comp;
-            blk.resno = (uint8_t)resno;
-            blk.band_index = (uint8_t)b;
-            blk.orient = (uint8_t)orient;
-            blk.kmax = bq.kmax;
-            blk.precno = (uint32_t)p;
-            blk.cblkno = k;
-            blk.x0 = std::max((gx + k % gw) << cbw, prc.x0);
-            blk.y0 = std::max((gy + k / gw) << cbh, prc.y0);
-            blk.x1 = (uint32_t)std::min<uint64_t>(((uint64_t)(gx + k % gw) + 1) << cbw, prc.x1);
-            blk.y1 = (uint32_t)std::min<uint64_t>(((uint64_t)(gy + k / gw) + 1) << cbh, prc.y1);
-            blk.buf_x = blk.x0 - band.x0 + ((resno && (orient & 1)) ? lower.w() : 0);
-            blk.buf_y = blk.y0 - band.y0 + ((resno && (orient & 2)) ? lower.h() : 0);
-            blk.length = 0;
-            blk.offset = 0;
-            blk.numbps = 0;
-            blk.numpasses = 0;
-            blk.stepsize = bq.step_enc;
-            out.push_back(blk);
-          }
-        }
-      }
+      b2k_block blk{};
+      blk.tile = tile_index;
+      blk.comp = pb.comp;
+      blk.resno = pb.resno;
+      blk.band_index = pb.band_index;
+      blk.orient = pb.orient;
+      blk.kmax = bq.kmax;
+      blk.precno = pb.precno;
+      blk.cblkno = k;
+      blk.x0 = std::max((pb.gx + k % pb.gw) << pb.cbw, prc.x0);
+      blk.y0 = std::max((pb.gy + k / pb.gw) << pb.cbh, prc.y0);
+      blk.x1 = (uint32_t)std::min<uint64_t>(((uint64_t)(pb.gx + k % pb.gw) + 1) << pb.cbw, prc.x1);
+      blk.y1 = (uint32_t)std::min<uint64_t>(((uint64_t)(pb.gy + k / pb.gw) + 1) << pb.cbh, prc.y1);
+      blk.buf_x = blk.x0 - pb.band.x0 + bx;
+      blk.buf_y = blk.y0 - pb.band.y0 + by;
+      blk.length = 0;
+      blk.offset = 0;
+      blk.numbps = 0;
+      blk.numpasses = 0;
+      blk.stepsize = bq.step_enc;
+      out.push_back(blk);
     }
-  }
+  });
 }
 
 } // namespace b2k

@@ -23,6 +23,7 @@
 
 #include "../../include/grok_b200.h"
 #include "geometry.h"
+#include "t2_packet.h"
 
 using namespace b2k;
 
@@ -121,14 +122,6 @@ extern "C" uint32_t plugin_get_debug_state(void)
   return state;
 }
 
-static int floor_log2_u32(uint32_t v)
-{
-  int l = 0;
-  while(v >>= 1)
-    ++l;
-  return l;
-}
-
 /* gpup_compress_params + gpup_image -> b2k_coding; false if the engine does not cover it */
 static bool coding_from_gpup(const gpup_compress_params* p, const gpup_image* im, b2k_coding* cp, bool allow_tiles = false)
 {
@@ -162,8 +155,8 @@ static bool coding_from_gpup(const gpup_compress_params* p, const gpup_image* im
       return false;
   }
   cp->numres = p->numresolution;
-  cp->cblkw_exp = (uint8_t)floor_log2_u32(p->cblockw_init ? p->cblockw_init : 64);
-  cp->cblkh_exp = (uint8_t)floor_log2_u32(p->cblockh_init ? p->cblockh_init : 64);
+  cp->cblkw_exp = (uint8_t)t2::floorlog2(p->cblockw_init ? p->cblockw_init : 64);
+  cp->cblkh_exp = (uint8_t)t2::floorlog2(p->cblockh_init ? p->cblockh_init : 64);
   cp->irreversible = p->irreversible;
   cp->mct = p->mct ? 1 : 0;
   if(p->mct > 1)
@@ -193,7 +186,7 @@ static bool coding_from_gpup(const gpup_compress_params* p, const gpup_image* im
         pw = sh < 32 ? p->prcw_init[spec - 1] >> sh : 0;
         ph = sh < 32 ? p->prch_init[spec - 1] >> sh : 0;
       }
-      const int ew = pw < 1 ? 1 : floor_log2_u32(pw), eh = ph < 1 ? 1 : floor_log2_u32(ph);
+      const int ew = pw < 1 ? 1 : t2::floorlog2(pw), eh = ph < 1 ? 1 : t2::floorlog2(ph);
       if(ew < 1 || eh < 1 || ew > 15 || eh > 15)
         return false; /* 1-sample precincts: b2k_coding reads exponent 0 as "default"; left to the host */
       if(rr < 33)
@@ -239,11 +232,8 @@ extern "C" gpup_tile* b2k_result_to_gpup_tile(const b2k_coding* cp, const b2k_re
       res->level = (size_t)resno;
       res->numBands = resno == 0 ? 1 : 3;
       res->band = (gpup_band**)calloc(res->numBands, sizeof(void*));
-      /* precinct grid of this resolution */
-      const Rect rr = resolution_rect(tr, numres, resno);
-      const uint32_t pw = cp->prcw_exp[resno] ? cp->prcw_exp[resno] : 15, ph = cp->prch_exp[resno] ? cp->prch_exp[resno] : 15;
-      const uint64_t gw = (uint64_t)ceil_div_pow2(rr.x1, pw) - (rr.x0 >> pw), gh = (uint64_t)ceil_div_pow2(rr.y1, ph) - (rr.y0 >> ph);
-      const uint64_t nprec = rr.empty() ? 0 : gw * gh;
+      const PrecinctGrid pg = precinct_grid(*cp, tr, resno);
+      const uint64_t nprec = (uint64_t)pg.gw * pg.gh;
       for(size_t b = 0; b < res->numBands; ++b)
       {
         gpup_band* band = (gpup_band*)calloc(1, sizeof(gpup_band));

@@ -23,6 +23,7 @@
 
 #include "plugin_decode_abi.h"
 #include "geometry.h"
+#include "t2_packet.h"
 
 using namespace b2k;
 
@@ -44,14 +45,6 @@ struct DecodeCtx
   uint64_t slab_bytes = 0;
 };
 thread_local DecodeCtx* g_ctx = nullptr;
-
-int floor_log2_u32(uint32_t v)
-{
-  int l = 0;
-  while(v >>= 1)
-    ++l;
-  return l;
-}
 
 uint32_t block_capacity(uint32_t w, uint32_t h, uint32_t kmax)
 {
@@ -83,15 +76,15 @@ int init_decompressors(gpup_header_info* h, gpup_image* image)
       return 0;
   }
   cp.numres = h->numresolutions;
-  cp.cblkw_exp = (uint8_t)floor_log2_u32(h->cblockw_init);
-  cp.cblkh_exp = (uint8_t)floor_log2_u32(h->cblockh_init);
+  cp.cblkw_exp = (uint8_t)t2::floorlog2(h->cblockw_init);
+  cp.cblkh_exp = (uint8_t)t2::floorlog2(h->cblockh_init);
   cp.irreversible = h->irreversible;
   cp.mct = h->mct;
   cp.numgbits = 1; /* Grok's HT setting (GrkCompress.cpp L849); checked per block against numBitPlanes */
   for(int r = 0; r < 33; ++r)
   {
-    cp.prcw_exp[r] = r < h->numresolutions && h->prcw_init[r] ? (uint8_t)floor_log2_u32(h->prcw_init[r]) : 15;
-    cp.prch_exp[r] = r < h->numresolutions && h->prch_init[r] ? (uint8_t)floor_log2_u32(h->prch_init[r]) : 15;
+    cp.prcw_exp[r] = r < h->numresolutions && h->prcw_init[r] ? (uint8_t)t2::floorlog2(h->prcw_init[r]) : 15;
+    cp.prch_exp[r] = r < h->numresolutions && h->prch_init[r] ? (uint8_t)t2::floorlog2(h->prch_init[r]) : 15;
     /* the host hands 1 << PPx; PPx = 0 would read as "default" in b2k_coding -> leave such streams to the host */
     if(r < h->numresolutions && (h->prcw_init[r] == 1 || h->prch_init[r] == 1))
       return 0;

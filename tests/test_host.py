@@ -405,53 +405,61 @@ def test_gpup_tile_tree_from_a_result_multi_tile_with_precincts():
     """b2k_result_to_gpup_tile (the per-tile seam of INTEGRATION.md section 2) without a GPU: a result built from
     oracle-coded blocks of a multi-tile image with user precincts is turned into the gpup_tile tree of each tile;
     walking it in Grok's order (plugin_bridge.cpp L62-111: comp -> res -> band -> precinct -> block) meets exactly the
-    enumeration's blocks, with their rectangles, bytes, pass bookkeeping (rate = length - 1) and band step sizes."""
+    enumeration's blocks, with their rectangles, bytes, pass bookkeeping (rate = length - 1) and band step sizes, and
+    every band has the oracle's precinct count.  The second image's tiles are 1 to 3 samples wide and tall, so that some
+    of their resolutions hold no samples and no precincts."""
     from gpup_ctypes import GpupTile
+    import oracle_t2 as T2
     lib = G.lib()
-    cp = G.make_coding(200, 150, 3, 8, numres=4, tile=(128, 96), precincts=[(32, 32), (64, 64)], cblk=(16, 16))
-    planes = P.synthetic_image(200, 150, 3, 8, seed=5)
-    coefs = P.forward(cp, planes)
-    table = G.enumerate_blocks(cp)
-    blks = P.enumerate_all(cp)
-    rects = P.tile_rects(cp)
-    chunks, off = [], 0
-    for i, (t, c, b) in enumerate(blks):
-        data = P.encode_block(cp, coefs, rects[t], c, b)
-        table[i]["length"], table[i]["offset"], table[i]["numbps"], table[i]["numpasses"] = len(data), off, 1, 1
-        chunks.append(data)
-        off += len(data)
-    arena = np.concatenate(chunks)
-    r = G.result_from_tables(table, arena, len(rects))
-    k = 0
-    for t in range(len(rects)):
-        tile = lib.b2k_result_to_gpup_tile(C.byref(cp), C.byref(r), t)
-        assert tile, lib.b2k_last_error()
-        T = C.cast(tile, C.POINTER(GpupTile)).contents
-        assert T.numComponents == 3
-        for c in range(3):
-            tc = T.tileComponents[c].contents
-            assert tc.numResolutions == cp.numres
-            for rr in range(cp.numres):
-                res = tc.resolutions[rr].contents
-                assert res.numBands == (1 if rr == 0 else 3)
-                for b in range(res.numBands):
-                    band = res.band[b].contents
-                    assert band.orientation == (0 if rr == 0 else b + 1)
-                    for p in range(band.numPrecincts):
-                        prc = band.precincts[p].contents
-                        for j in range(prc.numBlocks):
-                            cb = prc.blocks[j].contents
-                            row = table[k]
-                            assert (row["tile"], row["comp"], row["resno"], row["band_index"], row["precno"], row["cblkno"]) == (t, c, rr, b, p, j)
-                            assert (cb.x0, cb.y0, cb.x1, cb.y1) == (row["x0"], row["y0"], row["x1"], row["y1"])
-                            assert cb.numPasses == 1 and cb.numBitPlanes == 1 and cb.compressedDataLength == row["length"]
-                            assert cb.passes[0].rate == row["length"] - 1
-                            have = np.ctypeslib.as_array(cb.compressedData, shape=(cb.compressedDataLength,))
-                            assert np.array_equal(have, arena[int(row["offset"]):int(row["offset"]) + int(row["length"])])
-                            assert band.stepsize == row["stepsize"]
-                            k += 1
-        lib.gpup_tile_free(tile)
-    assert k == len(table)
+    for args in (dict(width=200, height=150, numres=4, tile=(128, 96), precincts=[(32, 32), (64, 64)], cblk=(16, 16)),
+                 dict(width=67, height=37, numres=6, tile=(32, 32), origin=(31, 31), tile_origin=(1, 2),
+                      precincts=[(4, 4), (8, 8), (16, 16)], cblk=(8, 8))):
+        cp = G.make_coding(numcomps=3, prec=8, **args)
+        planes = P.synthetic_image(args["width"], args["height"], 3, 8, seed=5, origin=args.get("origin", (0, 0)))
+        coefs = P.forward(cp, planes)
+        table = G.enumerate_blocks(cp)
+        blks = P.enumerate_all(cp)
+        rects = P.tile_rects(cp)
+        chunks, off = [], 0
+        for i, (t, c, b) in enumerate(blks):
+            data = P.encode_block(cp, coefs, rects[t], c, b)
+            table[i]["length"], table[i]["offset"], table[i]["numbps"], table[i]["numpasses"] = len(data), off, 1, 1
+            chunks.append(data)
+            off += len(data)
+        arena = np.concatenate(chunks)
+        r = G.result_from_tables(table, arena, len(rects))
+        k = 0
+        for t in range(len(rects)):
+            tile = lib.b2k_result_to_gpup_tile(C.byref(cp), C.byref(r), t)
+            assert tile, lib.b2k_last_error()
+            T = C.cast(tile, C.POINTER(GpupTile)).contents
+            assert T.numComponents == 3
+            for c in range(3):
+                tc = T.tileComponents[c].contents
+                assert tc.numResolutions == cp.numres
+                for rr in range(cp.numres):
+                    res = tc.resolutions[rr].contents
+                    assert res.numBands == (1 if rr == 0 else 3)
+                    _, _, _, _, _, gw, gh = T2.resolution_grid(cp, rects[t], rr)
+                    for b in range(res.numBands):
+                        band = res.band[b].contents
+                        assert band.orientation == (0 if rr == 0 else b + 1)
+                        assert band.numPrecincts == gw * gh
+                        for p in range(band.numPrecincts):
+                            prc = band.precincts[p].contents
+                            for j in range(prc.numBlocks):
+                                cb = prc.blocks[j].contents
+                                row = table[k]
+                                assert (row["tile"], row["comp"], row["resno"], row["band_index"], row["precno"], row["cblkno"]) == (t, c, rr, b, p, j)
+                                assert (cb.x0, cb.y0, cb.x1, cb.y1) == (row["x0"], row["y0"], row["x1"], row["y1"])
+                                assert cb.numPasses == 1 and cb.numBitPlanes == 1 and cb.compressedDataLength == row["length"]
+                                assert cb.passes[0].rate == row["length"] - 1
+                                have = np.ctypeslib.as_array(cb.compressedData, shape=(cb.compressedDataLength,))
+                                assert np.array_equal(have, arena[int(row["offset"]):int(row["offset"]) + int(row["length"])])
+                                assert band.stepsize == row["stepsize"]
+                                k += 1
+            lib.gpup_tile_free(tile)
+        assert k == len(table)
 
 
 def test_bench_reference_arm_runs_to_completion_and_prints_its_json_line():

@@ -31,6 +31,10 @@ GEOMS = {
     # small precincts at an odd origin: precincts cut by the tile edge, bands of one block
     "small-precincts": dict(width=133, height=117, numcomps=1, prec=8, numres=5, origin=(3, 5),
                             precincts=[(8, 8), (16, 16), (32, 32)], cblk=(8, 8)),
+    # tiles 1 to 3 samples wide and tall at an odd origin, five wavelet levels and small precincts: resolutions without
+    # samples, hence without precincts or packets, beside ones whose only precinct is cut by the tile edge
+    "sliver-tiles": dict(width=67, height=37, numcomps=3, prec=8, numres=6, tile=(32, 32), origin=(31, 31), tile_origin=(1, 2),
+                         precincts=[(4, 4), (8, 8), (16, 16)], cblk=(8, 8)),
     # 4x4 blocks: 16 x 16 blocks in the LL band's one precinct, a five-level tag tree
     "4x4-blocks": dict(width=256, height=192, numcomps=1, prec=8, numres=3, cblk=(4, 4)),
     # no wavelet level over ragged tiles
