@@ -116,6 +116,7 @@ def _signatures():
         "b2k_codestream_parse_window_device": (i64, [vp, vp, u64, pu32, u32, vp, cp, vp, u64]),
         "b2k_decode_codestream_window_device": (i32, [vp, vp, u64, pu32, u32, img, vp, cp, pu32, pd]),
         "b2k_codestream_window_device_stats": (i32, [vp, pu32, pu64]),
+        "b2k_decode_codestreams_window_device": (i32, [vp, u32, pp, pu64, pu32, u32, img, vp, cp, pu32, pi32, pd]),
         "b2k_enumerate": (i64, [cp, u32, u32, vp, u64]),
         "b2k_result_to_gpup_tile": (vp, [cp, res, u32]),
         "gpup_tile_free": (None, [vp]),
@@ -875,6 +876,97 @@ class Engine:
         if rc < 0:
             _raise_for(rc, "b2k_decode_codestreams_device", msg=_TEXT)
         return cp, out, status()
+
+    def decode_windows_device(self, streams, windows=None, reduce=0, out=None, dtype=None, layout="CHW", stream=None):
+        """A batch of windows: HTJ2K code streams on the engine's GPU (1-D contiguous uint8 CUDA arrays), each with its
+        window at 1 / 2**reduce -> (virtual Coding, out, rects, status) in one launch chain
+        (b2k_decode_codestreams_window_device).  windows: None (every whole image), one (x0, y0, x1, y1) on the
+        full-resolution canvas for every stream, or one per stream.  rects[i] is the window's pixels on the virtual
+        canvas, as decode_window_device gives them.  out: None for new torch tensors of `dtype` (default torch.uint16) --
+        one (n, C, h, w) / (n, h, w, C) tensor when the rects of the streams that pass their headers share one size, else a
+        list of n tensors each of its rect's size -- or a CUDA array or list of n CUDA arrays of those shapes, checked
+        before anything is written.  status[i] = (rc, text) is what decode_window_device of stream i alone returns (0,
+        or the code it would raise with); out[i] is written only where rc is 0.  Raises only when the call fails as a
+        whole, or when no stream has a coding (with stream 0's error)."""
+        n = len(streams)
+        if n == 0:
+            raise ValueError("decode_windows_device: no code streams")
+        ptrs = (C.c_void_p * n)()
+        lens = (C.c_uint64 * n)()
+        for i, cs in enumerate(streams):
+            if not hasattr(cs, "__cuda_array_interface__"):
+                raise ValueError("decode_windows_device: stream %d is not a CUDA array" % i)
+            ptrs[i], lens[i] = self._device_codestream_bytes(cs)
+        win = None
+        if windows is not None:
+            ws = [tuple(windows)] * n if len(windows) == 4 and all(np.isscalar(v) for v in windows) else [tuple(w) for w in windows]
+            if len(ws) != n or any(len(w) != 4 for w in ws):
+                raise ValueError("decode_windows_device: windows must be one (x0, y0, x1, y1) or one per stream")
+            win = (C.c_uint32 * (4 * n))(*[int(v) for w in ws for v in w])
+        L = lib()
+        first_out = out[0] if isinstance(out, (list, tuple)) and out else out
+        handle = _stream_handle(stream, first_out if first_out is not None else streams[0])
+        cp = Coding()
+        rects = (C.c_uint32 * (4 * n))()
+        st = (C.c_int32 * n)()
+        ms = C.c_double()
+
+        def status():
+            return [(int(st[i]), (L.b2k_decode_codestreams_error(self._h, i) or b"").decode()) for i in range(n)]
+
+        # headers only: the virtual coding and every stream's rect, which size the outputs and check a given `out`
+        rc = L.b2k_decode_codestreams_window_device(self._h, n, ptrs, lens, win, reduce, None, handle, C.byref(cp), rects, st,
+                                                    C.byref(ms))
+        if rc < 0:
+            _raise_for(rc, "b2k_decode_codestreams_window_device", msg=_TEXT)
+        if rc == n:
+            code, text = status()[0]
+            _raise_for(code, "b2k_decode_codestreams_window_device: stream 0", not_handled=True, msg=_TEXT, text=text)
+        nc = cp.numcomps
+        rect = [tuple(int(v) for v in rects[4 * i:4 * i + 4]) for i in range(n)]
+        size = [(r[3] - r[1], r[2] - r[0]) for r in rect]
+        sizes = {size[i] for i in range(n) if st[i] == 0}
+
+        def shape(hw):
+            return (nc,) + hw if layout == "CHW" else hw + (nc,)
+
+        if out is None:
+            import torch
+            dev, dt = "cuda:%d" % self.device, torch.uint16 if dtype is None else dtype
+            if len(sizes) == 1:
+                out = torch.empty((n,) + shape(sizes.pop()), dtype=dt, device=dev)
+            else:
+                out = [torch.empty(shape(size[i]), dtype=dt, device=dev) for i in range(n)]
+        if isinstance(out, (list, tuple)):
+            if len(out) != n:
+                raise ValueError("decode_windows_device: out holds %d images, the batch has %d" % (len(out), n))
+            images = list(out)
+            want = [shape(size[i]) for i in range(n)]
+        else:
+            if len(sizes) > 1:
+                raise ValueError("decode_windows_device: the rects differ in size (%s): out must be a list" % sorted(sizes))
+            full = tuple(int(v) for v in out.__cuda_array_interface__["shape"])
+            if len(full) != 4 or full[0] != n or (sizes and full[1:] != shape(next(iter(sizes)))):
+                raise ValueError("decode_windows_device: out has shape %s, the batch needs %s"
+                                 % (full, (n,) + shape(next(iter(sizes))) if sizes else n))
+            images = [out[i] for i in range(n)]
+            want = [full[1:]] * n
+        imgs = (DevicePlanes * n)()
+        for i in range(n):
+            got = tuple(int(v) for v in images[i].__cuda_array_interface__["shape"])
+            if st[i] == 0:
+                if got != want[i]:
+                    raise ValueError("decode_windows_device: out[%d] has shape %s, its rect needs %s" % (i, got, want[i]))
+                imgs[i] = device_planes(images[i], nc, size[i][0], size[i][1], layout, writable=True)
+        sb = {imgs[i].sample_bytes for i in range(n) if st[i] == 0}
+        for i in range(n):   # a stream that failed its headers is not written: its descriptor only carries the sample size
+            if st[i] != 0:
+                imgs[i].sample_bytes = min(sb) if sb else 2
+        rc = L.b2k_decode_codestreams_window_device(self._h, n, ptrs, lens, win, reduce, imgs, handle, C.byref(cp), rects, st,
+                                                    C.byref(ms))
+        if rc < 0:
+            _raise_for(rc, "b2k_decode_codestreams_window_device", msg=_TEXT)
+        return cp, out, [tuple(int(v) for v in rects[4 * i:4 * i + 4]) for i in range(n)], status()
 
     def job(self, cp, tile_mod=1, tile_rem=0):
         return Job(self, cp, tile_mod, tile_rem)

@@ -114,18 +114,20 @@ void b2k_launch_container_to_planes(const void* src, uint32_t spitch, uint32_t s
 void b2k_launch_planes_to_container(const int32_t* const* src, int nc, uint32_t spitch, void* dst, uint32_t dpitch, uint32_t step,
                                     uint32_t sample_bytes, uint32_t w, uint32_t h, cudaStream_t st);
 /* a batch's images out, one launch: for each of the n entries of the device table d_dst (BatchDst), its nc components
-   (nc > 1: pixel-interleaved, step = nc) from the int32 planes src[c] to dst + y * dpitch + x * step + c samples, w x h
-   pixels.  Entries with dst NULL, or with an err whose *err (the HT decoder's rejections in that image) is not 0, are
-   skipped; an entry with err NULL is always written.  All share sample_bytes. */
+   (nc > 1: pixel-interleaved, step = nc) from the int32 planes src[c] to dst + y * dpitch + x * step + c samples, the
+   entry's w x h pixels.  Entries with dst NULL, or with an err whose *err (the HT decoder's rejections in that image) is
+   not 0, are skipped; an entry with err NULL is always written.  All share sample_bytes; max_w x max_h (the largest
+   entry) sizes the grid. */
 struct BatchDst
 {
   const int32_t* src[4];
   void* dst;
   const int* err;
   uint32_t dpitch, step;
+  uint32_t w, h;
 };
-void b2k_launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint32_t spitch, uint32_t sample_bytes, uint32_t w,
-                                     uint32_t h, cudaStream_t st);
+void b2k_launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint32_t spitch, uint32_t sample_bytes, uint32_t max_w,
+                                     uint32_t max_h, cudaStream_t st);
 /* a batch's images in, one launch: for each of the n entries of the device table d_src (BatchSrc), its nc components
    (nc > 1: pixel-interleaved, step = nc) from src + y * spitch + x * step + c samples to the int32 plane at
    dst + c * dplane + y * dpitch + x, w x h pixels, with the sign handling of b2k_launch_container_to_planes.  All share

@@ -887,6 +887,23 @@ int b2k_batch_coding_check(const t2::MainHeader& ref, uint32_t ref_index, const 
   return 1;
 }
 
+int b2k_batch_window_check(const t2::MainHeader& ref, const t2::WindowCoding& rw, uint32_t ref_index, const t2::MainHeader& h,
+                           const t2::WindowCoding& w, uint32_t index)
+{
+  const TileGrid a = tile_grid(ref.cp), b = tile_grid(h.cp);
+  std::string why;
+  if(memcmp(&rw.vcp, &w.vcp, sizeof(b2k_coding)) != 0 || memcmp(&rw.box, &w.box, sizeof(b2k_coding)) != 0 || rw.whole != w.whole ||
+     a.nx != b.nx || a.ny != b.ny || rw.ta_x != w.ta_x || rw.ta_y != w.ta_y || rw.tb_x != w.tb_x || rw.tb_y != w.tb_y)
+    why = "its window's coding (tile grid, wanted tiles or virtual coding) differs from that of code stream ";
+  else if(h.flags() != ref.flags())
+    why = "its progression order, SOP or EPH differ from those of code stream ";
+  if(why.empty())
+    return 0;
+  b2k_set_error(("code stream " + std::to_string(index) + ": " + why + std::to_string(ref_index) + ", which the batch takes its coding from")
+                    .c_str());
+  return 1;
+}
+
 int b2k_parse_main_header(const uint8_t* cs, uint64_t len, t2::MainHeader& h)
 {
   h = t2::MainHeader();

@@ -1943,18 +1943,20 @@ __global__ void __launch_bounds__(128) k_planes_to_container(CPtr4 src, uint32_t
   planes_to_container_rows<S, NC>([&](int c) { return src.p[c]; }, spitch, dst, dpitch, step, w, h, x8);
 }
 
-/* the images of a batch: image blockIdx.z from its table entry; an entry without a destination, or with a counter (of the
-   blocks of its slot the HT decoder rejected, earlier on the stream) that is not 0, is skipped */
+/* the images of a batch: image blockIdx.z from its table entry, at its own size within the grid of the largest; an entry
+   without a destination, or with a counter (of the blocks of its slot the HT decoder rejected, earlier on the stream)
+   that is not 0, is skipped */
 template <int S, int NC>
-__global__ void __launch_bounds__(128) k_planes_to_containers(const BatchDst* __restrict__ tab, uint32_t spitch, uint32_t w, uint32_t h)
+__global__ void __launch_bounds__(128) k_planes_to_containers(const BatchDst* __restrict__ tab, uint32_t spitch)
 {
   const uint32_t x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
   const BatchDst* E = tab + blockIdx.z;
   void* dst = E->dst;
+  const uint32_t w = E->w;
   if(x8 >= w || !dst || (E->err && *E->err))
     return;
   /* the plane pointers are read from the table where they are used */
-  planes_to_container_rows<S, NC>([E](int c) { return E->src[c]; }, spitch, dst, E->dpitch, E->step, w, h, x8);
+  planes_to_container_rows<S, NC>([E](int c) { return E->src[c]; }, spitch, dst, E->dpitch, E->step, w, E->h, x8);
 }
 
 dim3 convert_grid(uint32_t w, uint32_t h) { return dim3((w + 8 * 128 - 1) / (8 * 128), h < 65535u ? h : 65535u); }
@@ -2042,10 +2044,10 @@ void launch_planes_to_containers(const BatchDst* d_dst, uint32_t n, int nc, uint
     grid.z = std::min<uint32_t>(n - i0, 65535u);
     switch(nc)
     {
-      case 1: k_planes_to_containers<S, 1><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
-      case 2: k_planes_to_containers<S, 2><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
-      case 3: k_planes_to_containers<S, 3><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
-      default: k_planes_to_containers<S, 4><<<grid, block, 0, st>>>(d_dst + i0, spitch, w, h); break;
+      case 1: k_planes_to_containers<S, 1><<<grid, block, 0, st>>>(d_dst + i0, spitch); break;
+      case 2: k_planes_to_containers<S, 2><<<grid, block, 0, st>>>(d_dst + i0, spitch); break;
+      case 3: k_planes_to_containers<S, 3><<<grid, block, 0, st>>>(d_dst + i0, spitch); break;
+      default: k_planes_to_containers<S, 4><<<grid, block, 0, st>>>(d_dst + i0, spitch); break;
     }
     b2k_count_launch();
   }

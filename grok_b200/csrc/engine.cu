@@ -2748,11 +2748,11 @@ static int parse_streams(b2k_engine* e, b2k_device_job* J, uint32_t n, const uin
 
 /* after a parse into J's descriptors: block decode -> inverse -> images, chunk by chunk over the (slot, tile) ranges of the
    n slots used (as many chunks as the job's pipeline has, whatever its slot count).  After the chunk that holds slot i's
-   last tile, `rect` of its planes (the whole canvas, or a window on the virtual canvas) goes to imgs[i] when status[i] is
-   0, in one launch per component group.  With write_rejected the image of a slot whose blocks the HT decoder rejected
+   last tile, rects[i] of its planes (the whole canvas, or a window on the virtual canvas) goes to imgs[i] when status[i]
+   is 0, in one launch per component group.  With write_rejected the image of a slot whose blocks the HT decoder rejected
    is written too (as b2k_decode_device writes it), else it is left alone.  The caller's stream then waits for the
    writes.  A slot with rejected blocks gets -2 and, with `errors`, its text there.  0, or -1 for a failure of the call. */
-static int decode_slots(b2k_engine* e, b2k_device_job* J, uint32_t n, const b2k_device_planes* imgs, const Rect& rect, bool refinement,
+static int decode_slots(b2k_engine* e, b2k_device_job* J, uint32_t n, const b2k_device_planes* imgs, const Rect* rects, bool refinement,
                         bool write_rejected, cudaStream_t caller, double* ms_total, int32_t* status, std::string* errors)
 {
   cudaStream_t st = e->stream;
@@ -2763,6 +2763,7 @@ static int decode_slots(b2k_engine* e, b2k_device_job* J, uint32_t n, const b2k_
     if(!status[i])
       interleaved = interleaved && device_group(imgs[i], nc) == nc;
   const int group = interleaved ? nc : 1, tables = nc / group;
+  uint32_t max_w = 0, max_h = 0;
   if(!J->h_batch_dst)
   {
     CUDA_TRY(cudaMalloc(&J->d_batch_dst, (size_t)J->slots * 4 * sizeof(BatchDst)));
@@ -2776,12 +2777,17 @@ static int decode_slots(b2k_engine* e, b2k_device_job* J, uint32_t n, const b2k_
       if(status[i])
         continue;
       const int c0 = t * group;
+      const Rect& r = rects[i];
       for(int k = 0; k < group; ++k)
-        D.src[k] = J->img.at((int)i * nc + c0 + k, rect.x0, rect.y0);
+        D.src[k] = J->img.at((int)i * nc + c0 + k, r.x0, r.y0);
       D.dst = imgs[i].comp[c0];
       D.err = write_rejected ? nullptr : J->d_err + i;
       D.dpitch = imgs[i].row_pitch[c0];
       D.step = imgs[i].col_step[c0];
+      D.w = r.w();
+      D.h = r.h();
+      max_w = std::max(max_w, D.w);
+      max_h = std::max(max_h, D.h);
     }
   CUDA_TRY(cudaMemcpyAsync(J->d_batch_dst, J->h_batch_dst, (size_t)tables * n * sizeof(BatchDst), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemsetAsync(J->d_err, 0, n * sizeof(int), st));
@@ -2798,7 +2804,7 @@ static int decode_slots(b2k_engine* e, b2k_device_job* J, uint32_t n, const b2k_
     if(enqueue_inverse(J, st, t0, t1)) return -1;
     const uint32_t s0 = (uint32_t)(t0 / T), s1 = (uint32_t)(t1 / T);
     for(int t = 0; t < tables && s1 > s0; ++t)
-      b2k_launch_planes_to_containers(J->d_batch_dst + (size_t)t * n + s0, s1 - s0, group, J->img.pitch, sb, rect.w(), rect.h(), st);
+      b2k_launch_planes_to_containers(J->d_batch_dst + (size_t)t * n + s0, s1 - s0, group, J->img.pitch, sb, max_w, max_h, st);
   }
   CUDA_TRY(cudaEventRecord(J->ev[1], st));
   /* the caller's stream goes on once its images are written */
@@ -2893,7 +2899,8 @@ extern "C" int32_t b2k_decode_codestream_device(b2k_engine* e, const uint8_t* cs
   if(int rc = check_device_planes(e, &h.cp, img))
     return rc;
   int32_t status = 0;
-  if(decode_slots(e, J, 1, img, Rect{h.cp.x0, h.cp.y0, h.cp.x1, h.cp.y1}, refinement, true, caller, ms_total, &status, nullptr))
+  const Rect whole{h.cp.x0, h.cp.y0, h.cp.x1, h.cp.y1};
+  if(decode_slots(e, J, 1, img, &whole, refinement, true, caller, ms_total, &status, nullptr))
     return -1;
   DBG_T("device decode: done");
   return status;
@@ -2911,12 +2918,10 @@ struct DeviceWindow
   Rect rect{}; /* the window's pixels at 1 / 2^reduce on the virtual canvas */
 };
 
-/* the header and the window's coding, read after the caller's queued work: 0 or the host parser's code and text */
-static int device_window_coding(b2k_engine* e, const uint8_t* cs, uint64_t len, const uint32_t* window, uint32_t reduce,
-                                cudaStream_t caller, DeviceWindow& w)
+/* the window's coding of a stream whose main header w.h has been read, and the window's pixels: 0, or the host parser's
+   code and text for the window errors */
+static int window_coding(const uint32_t* window, uint32_t reduce, DeviceWindow& w)
 {
-  if(int rc = read_main_header(e, cs, len, caller, w.h))
-    return rc;
   if(int rc = b2k_window_coding(w.h.cp, window, reduce, w.wc))
     return rc;
   const b2k_coding& v = w.wc.vcp;
@@ -2930,11 +2935,80 @@ static int device_window_coding(b2k_engine* e, const uint8_t* cs, uint64_t len, 
   return 0;
 }
 
-/* the windowed parse on st up to the status (and, with dec, the gather into the arena): 0, or the host parser's code and text */
+/* the header and the window's coding, read after the caller's queued work: 0 or the host parser's code and text */
+static int device_window_coding(b2k_engine* e, const uint8_t* cs, uint64_t len, const uint32_t* window, uint32_t reduce,
+                                cudaStream_t caller, DeviceWindow& w)
+{
+  if(int rc = read_main_header(e, cs, len, caller, w.h))
+    return rc;
+  return window_coding(window, reduce, w);
+}
+
+/* the windowed parse on e->stream of the streams i < n whose status is 0 (w[i]: their headers and window codings, all with
+   w[ref]'s box coding, tile box and flags), read in place, in slots i of J: the five parse kernels and, with dec, the
+   arena layout and the decoder's descriptors, then after the statuses the gather of the parsed streams' wanted packet
+   data into the arena.  One synchronisation; a stream that fails gets its status and, with `errors`, its text there.
+   *refinement: a stream has refinement passes.  0, or -1 for a failure of the call. */
+static int parse_windows(b2k_engine* e, b2k_device_job* J, uint32_t n, const uint8_t* const* cs, const uint64_t* len, const DeviceWindow* w,
+                         uint32_t ref, uint32_t reduce, bool dec, int32_t* status, std::string* errors, bool* refinement)
+{
+  cudaStream_t st = e->stream;
+  const DeviceWindow& R = w[ref];
+  const uint32_t flags = R.h.flags();
+  if(!b2k_t2_window_matches(J->t2w, R.wc.box, flags, reduce, J->slots))
+  { /* box geometry, progression and reduce: planned once for every window with the same tile box */
+    drop_parse(J, J->t2w);
+    if(b2k_t2_window_create(R.wc, flags, reduce, J->blocks.data(), J->blocks.size(), J->coded_index.data(), J->coded_index.size(), &J->t2w,
+                            J->slots))
+      return -1;
+  }
+  e->last_parse = J->t2w;
+  J->arena_sized = false;
+  std::vector<uint64_t> sot(n, 0);
+  std::vector<const std::vector<Rect>*> need(n, nullptr);
+  for(uint32_t i = 0; i < n; ++i)
+    if(!status[i])
+    {
+      sot[i] = w[i].h.sot;
+      need[i] = &w[i].wc.need;
+    }
+  const TileGrid g = tile_grid(R.h.cp);
+  const b2k::t2::TileBox box{g.nx, R.wc.ta_x, R.wc.ta_y, R.wc.tb_x, R.wc.tb_y};
+  CUDA_TRY(cudaEventRecord(J->ev[0], st));
+  if(b2k_t2_window_enqueue(J->t2w, n, cs, len, sot.data(), need.data(), box, g.nx * g.ny, J->d_enc_desc, J->d_dec_quant,
+                           dec ? J->d_dec_desc : nullptr, st))
+    return -1;
+  CUDA_TRY(cudaStreamSynchronize(st));
+  bool any = false;
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    if(status[i])
+      continue;
+    bool r = false;
+    if(int prc = b2k_t2_batch_result(J->t2w, i, &r))
+    {
+      status[i] = prc;
+      if(errors)
+        errors[i] = g_err;
+    }
+    any = any || r;
+  }
+  if(refinement)
+    *refinement = any;
+  if(!dec)
+    return 0;
+  const std::string err = g_err; /* a single stream's verdict outlives the gather */
+  if(arena_reserve(J, b2k_t2_window_arena(J->t2w), 0)) return -1;
+  if(b2k_t2_window_gather(J->t2w, J->d_bytes, st)) return -1;
+  g_err = err;
+  return 0;
+}
+
+/* the windowed parse of one stream in slot 0 of the single-image job of its virtual coding: 0, or the host parser's code
+   and text.  *out: the job, once there is one. */
 static int parse_device_window(b2k_engine* e, const uint8_t* cs, uint64_t len, const DeviceWindow& w, uint32_t reduce,
                                b2k_device_job** out, bool dec, bool* refinement, uint64_t cap_blocks)
 {
-  cudaStream_t st = e->stream;
   int rc = 0;
   b2k_device_job* J = cached_job(e, &w.wc.vcp, 1, 0, &rc);
   if(rc)
@@ -2945,27 +3019,9 @@ static int parse_device_window(b2k_engine* e, const uint8_t* cs, uint64_t len, c
     g_err = "block table too small";
     return -1;
   }
-  const uint32_t flags = w.h.flags();
-  if(!b2k_t2_window_matches(J->t2w, w.wc.box, flags, reduce))
-  { /* box geometry, progression and reduce: planned once for every window with the same tile box */
-    drop_parse(J, J->t2w);
-    if(b2k_t2_window_create(w.wc, flags, reduce, J->blocks.data(), J->blocks.size(), J->coded_index.data(), J->coded_index.size(), &J->t2w))
-      return -1;
-  }
-  e->last_parse = J->t2w;
-  J->arena_sized = false;
-  const TileGrid g = tile_grid(w.h.cp);
-  CUDA_TRY(cudaEventRecord(J->ev[0], st));
-  if(b2k_t2_window_enqueue(J->t2w, cs, len, w.h.sot, g.nx, g.nx * g.ny, w.wc, J->d_enc_desc, J->d_dec_quant, dec ? J->d_dec_desc : nullptr,
-                           st))
-    return -1;
-  CUDA_TRY(cudaStreamSynchronize(st));
-  if(int prc = b2k_t2_parse_result(J->t2w, refinement))
-    return prc;
-  if(!dec)
-    return 0;
-  if(arena_reserve(J, b2k_t2_window_bytes(J->t2w), 0)) return -1;
-  return b2k_t2_window_gather(J->t2w, cs, J->d_bytes, st);
+  int32_t status = 0;
+  if(parse_windows(e, J, 1, &cs, &len, &w, 0, reduce, dec, &status, nullptr, refinement)) return -1;
+  return status;
 }
 
 /* a windowed parse passed its status: its wanted tiles, and the bytes of the stream its decode copies into the arena (the
@@ -2973,7 +3029,7 @@ static int parse_device_window(b2k_engine* e, const uint8_t* cs, uint64_t len, c
 static void note_window_stats(b2k_engine* e, const b2k_device_job* J, uint64_t bytes)
 {
   e->have_window_stats = true;
-  e->window_tiles = (uint32_t)J->tiles.size();
+  e->window_tiles = J->slot_tiles;
   e->window_bytes = bytes;
 }
 
@@ -3054,7 +3110,7 @@ extern "C" int32_t b2k_decode_codestream_window_device(b2k_engine* e, const uint
   if(int crc = check_device_planes(e, &w.wc.vcp, img))
     return crc;
   int32_t status = 0;
-  if(decode_slots(e, J, 1, img, w.rect, refinement, true, caller, ms_total, &status, nullptr))
+  if(decode_slots(e, J, 1, img, &w.rect, refinement, true, caller, ms_total, &status, nullptr))
     return -1;
   DBG_T("device window decode: done");
   return status;
@@ -3190,7 +3246,8 @@ extern "C" int32_t b2k_decode_codestreams_device(b2k_engine* e, uint32_t n, cons
       if(int rc = check_device_planes(e, &cp, &imgs[i]))
         fail(i, rc);
   /* an image the HT decoder rejected blocks of is not written */
-  if(decode_slots(e, J, n, imgs, Rect{cp.x0, cp.y0, cp.x1, cp.y1}, refinement, false, caller, ms_total, status, e->batch_errors.data()))
+  const std::vector<Rect> whole(n, Rect{cp.x0, cp.y0, cp.x1, cp.y1});
+  if(decode_slots(e, J, n, imgs, whole.data(), refinement, false, caller, ms_total, status, e->batch_errors.data()))
     return -1;
   return failures();
 }
@@ -3201,6 +3258,119 @@ extern "C" const char* b2k_decode_codestreams_error(b2k_engine* e, uint32_t i)
     return "";
   std::lock_guard<std::mutex> lock(e->mu);
   return i < e->batch_errors.size() ? e->batch_errors[i].c_str() : "";
+}
+
+/* ---- windows of batches of code streams in device memory (b2k_decode_codestreams_window_device) ------------------------
+ * The batch of b2k_decode_codestreams_device with each stream's window and a shared reduce: the batch job is that of the
+ * virtual coding, and the windowed parse runs over (stream, item) in place from the callers' buffers, one gather copying
+ * only the wanted tiles' packet data of every stream into the arena.  When the virtual coding is the streams' own (every
+ * tile at reduce 0), the batch parse of whole streams runs instead; only the rectangles written out differ. */
+
+extern "C" int32_t b2k_decode_codestreams_window_device(b2k_engine* e, uint32_t n, const uint8_t* const* cs, const uint64_t* len,
+                                                        const uint32_t* windows, uint32_t reduce, const b2k_device_planes* imgs,
+                                                        void* cuda_stream, b2k_coding* cp_out, uint32_t* rects_out, int32_t* status,
+                                                        double* ms_total)
+{
+  if(!e || !cs || !len || !cp_out || !rects_out || !status)
+  {
+    g_err = "b2k_decode_codestreams_window_device: NULL argument";
+    return -1;
+  }
+  if(n == 0)
+  {
+    g_err = "b2k_decode_codestreams_window_device: no code streams";
+    return -1;
+  }
+  if(imgs)
+    for(uint32_t i = 1; i < n; ++i)
+      if(imgs[i].sample_bytes != imgs[0].sample_bytes)
+      {
+        g_err = "b2k_decode_codestreams_window_device: the images' sample_bytes differ";
+        return -1;
+      }
+  std::lock_guard<std::mutex> lock(e->mu);
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t caller = caller_stream(cuda_stream), st = e->stream;
+  e->batch_errors.assign(n, std::string());
+  auto fail = [&](uint32_t i, int32_t rc) {
+    status[i] = rc;
+    e->batch_errors[i] = g_err;
+  };
+  auto failures = [&] {
+    int32_t f = 0;
+    for(uint32_t i = 0; i < n; ++i)
+      f += status[i] != 0;
+    return f;
+  };
+  /* each stream's checks in the single call's order: its memory, its main header, its window, the batch's coding */
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    status[i] = 0;
+    memset(rects_out + 4 * (size_t)i, 0, 4 * sizeof(uint32_t));
+    if(check_device_bytes(e, cs[i], len[i]))
+      fail(i, -1);
+  }
+  if(queue_after(e, caller, st)) return -1;
+  std::vector<b2k::t2::MainHeader> h(n);
+  if(read_batch_headers(e, n, cs, len, b2k::t2::BATCH_HEADER_PREFIX, st, status, h.data(), e->batch_errors.data())) return -1;
+  std::vector<DeviceWindow> w(n);
+  uint32_t ref = n;
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    if(status[i])
+      continue;
+    w[i].h = h[i];
+    if(int rc = window_coding(windows ? windows + 4 * (size_t)i : nullptr, reduce, w[i]))
+    {
+      fail(i, rc);
+      continue;
+    }
+    const Rect& r = w[i].rect;
+    const uint32_t q[4] = {r.x0, r.y0, r.x1, r.y1};
+    memcpy(rects_out + 4 * (size_t)i, q, sizeof(q));
+    if(ref == n)
+      ref = i;
+    else if(b2k_batch_window_check(w[ref].h, w[ref].wc, ref, w[i].h, w[i].wc, i))
+      fail(i, 1);
+  }
+  if(ref == n)
+    return failures();
+  const b2k_coding cp = w[ref].wc.vcp;
+  *cp_out = cp;
+  if(!imgs)
+    return failures();
+  int jrc = 0;
+  b2k_device_job* J = cached_batch_job(e, cp, n, &jrc);
+  if(jrc < 0)
+    return -1;
+  if(jrc)
+  {
+    for(uint32_t i = 0; i < n; ++i)
+      if(!status[i])
+        fail(i, jrc);
+    return failures();
+  }
+  e->have_window_stats = false;
+  bool refinement = false;
+  const bool whole = w[ref].wc.whole;
+  if(whole ? parse_streams(e, J, n, cs, len, h.data(), h[ref].flags(), true, status, e->batch_errors.data(), &refinement)
+           : parse_windows(e, J, n, cs, len, w.data(), ref, reduce, true, status, e->batch_errors.data(), &refinement))
+    return -1;
+  uint64_t bytes = 0;
+  for(uint32_t i = 0; i < n && whole; ++i)
+    bytes += status[i] ? 0 : len[i];
+  note_window_stats(e, J, whole ? bytes : b2k_t2_window_bytes(J->t2w));
+  std::vector<Rect> rects(n);
+  for(uint32_t i = 0; i < n; ++i)
+  {
+    rects[i] = w[i].rect;
+    if(!status[i])
+      if(int rc = check_device_planes(e, &cp, &imgs[i]))
+        fail(i, rc);
+  }
+  if(decode_slots(e, J, n, imgs, rects.data(), refinement, false, caller, ms_total, status, e->batch_errors.data()))
+    return -1;
+  return failures();
 }
 
 /* ---- images in device memory to code streams (b2k_encode_codestream_device / b2k_encode_codestreams_device) -----------

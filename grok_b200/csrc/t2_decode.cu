@@ -38,23 +38,12 @@
 
 using namespace b2k;
 using namespace b2k::t2;
+static_assert(WINDOW_MAX_RES == B2K_MAX_RES, "a need rectangle per resolution");
 
 void b2k_set_error(const char* msg); /* engine.cu */
 
 namespace
 {
-/* a coded block of a windowed parse's virtual coding: its box tile, the need rectangle that applies to it (resolution
-   max(resno - 1, 0)) and its rectangle in band coordinates */
-struct WinBlock
-{
-  uint32_t tile, res, x0, y0, x1, y1;
-};
-struct NeedRects /* the window's need rectangles, one per resolution of the virtual coding; n = 0: no filter */
-{
-  uint32_t n;
-  uint32_t r[B2K_MAX_RES][4];
-};
-
 /* Every kernel runs over the n streams of a batch (n = 1 for a single stream), one thread per item; the threads' bodies
    are t2_parse.h's batch_* functions, which tests/t2_batch_check.cpp runs on the host */
 __global__ void k_t2_locate(const uint8_t* __restrict__ cs, const StreamDesc* __restrict__ sd, uint32_t n, uint32_t ntiles, TileBox box,
@@ -105,35 +94,55 @@ __global__ void k_t2_walk(const uint8_t* __restrict__ cs, const StreamDesc* __re
 
 /* a thread per (stream, coded block): descriptor s * ncoded + k from template enc[s * ncoded + k], pointing into the arena.
    A stream whose parse failed (or was skipped) gets length-0 descriptors, which decode as all-zero blocks.  win != NULL (a
-   windowed parse, one stream): coded[k] is the box block of virtual coded block k; a block the window does not need stays
-   uncoded, and a parsed block's bytes are addressed where k_t2_gather puts them */
+   windowed batch): t2_parse.h's window_block, the need filter and the address of the block's gathered bytes */
 __global__ void k_t2_desc(const StreamDesc* __restrict__ sd, uint32_t n, const ParsedBlock* __restrict__ blk, uint64_t nblocks,
                           const uint32_t* __restrict__ coded, uint32_t ncoded, const HtBlockDesc* __restrict__ enc,
                           const float* __restrict__ quant, HtBlockDesc* __restrict__ dec, const WinBlock* __restrict__ win,
                           const NeedRects* __restrict__ need, const PartRange* __restrict__ parts, const uint32_t* __restrict__ head,
-                          const uint64_t* __restrict__ body_at, ParseStatus* status)
+                          uint32_t bt, const uint64_t* __restrict__ body_at, ParseStatus* status)
 {
   const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if(g >= (uint64_t)n * ncoded)
     return;
   uint32_t s = 0;
-  ParsedBlock b = batch_block(blk, nblocks, coded, g, ncoded, status, &s);
-  uint64_t at = b.offset;
-  if(win && b.length)
+  uint64_t slot_off = 0;
+  ParsedBlock b;
+  if(win)
+    b = window_block(blk, nblocks, coded, g, ncoded, status, sd, win, need, parts, head, bt, body_at, &s, &slot_off);
+  else
   {
-    const WinBlock w = win[g];
-    if(need->n && !window_needs(need->r[w.res], w.x0, w.y0, w.x1, w.y1))
-      b = ParsedBlock{};
-    at = b.length ? gathered_offset(parts, head[w.tile], body_at, b.offset) : 0;
+    b = batch_block(blk, nblocks, coded, g, ncoded, status, &s);
+    slot_off = sd[s].at + b.offset;
   }
   HtBlockDesc d = enc[g];
   d.length = b.length;
-  d.slot_off = sd[s].at + at;
+  d.slot_off = slot_off;
   block_decode_fields(b, d.kmax, &d.mmsbs, &d.passes, &d.length2);
   d.quant = quant[g]; /* stepsize / 2^(31-Kmax) */
   dec[g] = d;
   if(d.passes > 1)
     status[s].refinement = 1;
+}
+
+/* a windowed batch's arena layout, one CTA: sd[s].at for every stream (window_arena_at), each thread a run of streams
+   whose start is the scan of the runs before it */
+__global__ void __launch_bounds__(1024) k_t2_window_at(StreamDesc* __restrict__ sd, const ParseStatus* __restrict__ status, uint32_t n)
+{
+  __shared__ uint64_t sum[1024];
+  const uint32_t per = (n + 1023) / 1024, s0 = min(n, threadIdx.x * per), s1 = min(n, s0 + per);
+  uint64_t mine = 0;
+  for(uint32_t s = s0; s < s1; ++s)
+    mine += window_gathered_bytes(status[s]);
+  sum[threadIdx.x] = mine;
+  __syncthreads();
+  for(uint32_t d = 1; d < 1024; d <<= 1)
+  {
+    const uint64_t v = threadIdx.x >= d ? sum[threadIdx.x - d] : 0;
+    __syncthreads();
+    sum[threadIdx.x] += v;
+    __syncthreads();
+  }
+  window_arena_at(sd, status, s0, s1, sum[threadIdx.x] - mine);
 }
 
 /* one copy per entry of a (source, length, destination) table: entry e (blockIdx.y strided) by a strip of CTAs along x;
@@ -161,20 +170,19 @@ __global__ void k_copy_table(const CopyEntry* __restrict__ tab, uint32_t n, uint
   }
 }
 
-/* the wanted tile parts' packet data, end to end: part p (blockIdx.y strided) by a strip of CTAs along x */
-__global__ void k_t2_gather(const uint8_t* __restrict__ cs, const PartRange* __restrict__ parts, const uint64_t* __restrict__ body_at,
-                            uint32_t nparts, uint8_t* __restrict__ out)
+/* a windowed batch's gather: item g (blockIdx.y strided) of window_gather_part, over (stream, part), by a strip of CTAs
+   along x */
+__global__ void k_t2_gather(const StreamDesc* __restrict__ sd, const PartRange* __restrict__ parts, const uint64_t* __restrict__ body_at,
+                            const ParseStatus* __restrict__ status, uint64_t items, uint64_t per, uint8_t* __restrict__ out)
 {
-  for(uint32_t p = blockIdx.y; p < nparts; p += gridDim.y)
+  for(uint64_t g = blockIdx.y; g < items; g += gridDim.y)
   {
-    const PartRange R = parts[p];
-    if(R.end <= R.begin)
+    const uint8_t* src = nullptr;
+    uint64_t dst = 0, len = 0;
+    if(!window_gather_part(sd, parts, body_at, status, g, per, &src, &dst, &len))
       continue;
-    const uint64_t n = R.end - R.begin;
-    const uint8_t* src = cs + R.begin;
-    uint8_t* dst = out + body_at[p];
-    for(uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
-      dst[i] = src[i];
+    for(uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < len; i += (uint64_t)gridDim.x * blockDim.x)
+      out[dst + i] = src[i];
   }
 }
 
@@ -219,11 +227,11 @@ struct T2Parse
   uint32_t reduce = 0;
   std::vector<uint32_t> vmap;      /* every virtual block -> its box block */
   WinBlock* d_win = nullptr;
-  NeedRects* d_need = nullptr;
+  NeedRects* d_need = nullptr;     /* per stream */
   NeedRects* h_need = nullptr;     /* pinned */
   uint64_t* d_body_at = nullptr;   /* per recorded part, parts_cap of them */
-  uint32_t* d_wcount = nullptr;    /* tile parts seen per stream tile */
-  uint32_t wcount_cap = 0;
+  uint32_t* d_wcount = nullptr;    /* tile parts seen per stream tile, per stream */
+  uint64_t wcount_cap = 0;
 };
 
 #define T2P_TRY(expr)                                                                                                          \
@@ -315,7 +323,7 @@ int b2k_t2_parse_create(const b2k_coding& cp, uint32_t flags, const b2k_block* b
 }
 
 int b2k_t2_window_create(const b2k::t2::WindowCoding& wc, uint32_t flags, uint32_t reduce, const b2k_block* vblocks, uint64_t nv,
-                         const uint32_t* coded_index, uint64_t ncoded, T2Parse** out)
+                         const uint32_t* coded_index, uint64_t ncoded, T2Parse** out, uint32_t streams)
 {
   *out = nullptr;
   std::vector<b2k_block> box_blocks;
@@ -332,7 +340,7 @@ int b2k_t2_window_create(const b2k::t2::WindowCoding& wc, uint32_t flags, uint32
     win[k] = WinBlock{v.tile, v.resno ? v.resno - 1u : 0u, v.x0, v.y0, v.x1, v.y1};
   }
   T2Parse* J = nullptr;
-  if(b2k_t2_parse_create(wc.box, flags, box_blocks.data(), box_blocks.size(), bg.nx * bg.ny, coded_box.data(), ncoded, &J))
+  if(b2k_t2_parse_create(wc.box, flags, box_blocks.data(), box_blocks.size(), bg.nx * bg.ny, coded_box.data(), ncoded, &J, streams))
     return -1;
   struct Guard
   {
@@ -343,18 +351,18 @@ int b2k_t2_window_create(const b2k::t2::WindowCoding& wc, uint32_t flags, uint32
   J->box = wc.box;
   J->reduce = reduce;
   J->vmap.swap(vmap);
-  T2P_TRY(cudaMalloc(&J->d_win, std::max<uint64_t>(ncoded, 1) * sizeof(WinBlock) + sizeof(NeedRects)));
+  T2P_TRY(cudaMalloc(&J->d_win, std::max<uint64_t>(ncoded, 1) * sizeof(WinBlock) + J->streams * sizeof(NeedRects)));
   J->d_need = reinterpret_cast<NeedRects*>(J->d_win + std::max<uint64_t>(ncoded, 1));
   T2P_TRY(cudaMemcpy(J->d_win, win.data(), ncoded * sizeof(WinBlock), cudaMemcpyHostToDevice));
-  T2P_TRY(cudaHostAlloc(&J->h_need, sizeof(NeedRects), cudaHostAllocDefault));
+  T2P_TRY(cudaHostAlloc(&J->h_need, J->streams * sizeof(NeedRects), cudaHostAllocDefault));
   *out = J;
   J = nullptr;
   return 0;
 }
 
-bool b2k_t2_window_matches(const T2Parse* J, const b2k_coding& box, uint32_t flags, uint32_t reduce)
+bool b2k_t2_window_matches(const T2Parse* J, const b2k_coding& box, uint32_t flags, uint32_t reduce, uint32_t streams)
 {
-  return J && J->window && J->flags == flags && J->reduce == reduce && memcmp(&J->box, &box, sizeof(box)) == 0;
+  return J && J->window && J->flags == flags && J->reduce == reduce && J->streams == streams && memcmp(&J->box, &box, sizeof(box)) == 0;
 }
 
 void b2k_t2_parse_destroy(T2Parse* J)
@@ -374,7 +382,8 @@ void b2k_t2_parse_destroy(T2Parse* J)
 uint32_t b2k_t2_parse_flags(const T2Parse* J) { return J->flags; }
 
 /* the five launches over the plan's tiles, which are the tiles of `box` among each stream's ntiles, for the n streams whose
-   h_sd[s].at / len / sot the caller filled in (sot = 0: not parsed); the part table is laid out here */
+   h_sd[s].at / len / sot / base the caller filled in (sot = 0: not parsed); the part table is laid out here.  A windowed
+   batch lays its arena out on the device (k_t2_window_at) before the descriptors point into it */
 static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint32_t n, uint32_t ntiles, const TileBox& box, uint32_t* d_count,
                          const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
 {
@@ -406,7 +415,7 @@ static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint32_t n, uint32_t nti
   /* statuses and stream table in one copy */
   T2P_TRY(cudaMemcpyAsync(J->d_status, J->h_status, S * sizeof(ParseStatus) + n * sizeof(StreamDesc), cudaMemcpyHostToDevice, st));
   if(J->window)
-    T2P_TRY(cudaMemcpyAsync(J->d_need, J->h_need, sizeof(NeedRects), cudaMemcpyHostToDevice, st));
+    T2P_TRY(cudaMemcpyAsync(J->d_need, J->h_need, n * sizeof(NeedRects), cudaMemcpyHostToDevice, st));
   const uint32_t tpb = 32; /* streams, tiles and packets are few and each thread is a long serial chain: spread them over the SMs */
   auto grid = [&](uint64_t items) { return (unsigned)((items + tpb - 1) / tpb); };
   k_t2_locate<<<grid(n), tpb, 0, st>>>(cs, J->d_sd, n, ntiles, box, J->d_parts, J->d_head, J->d_last, d_count, J->d_body_at, J->d_status);
@@ -428,11 +437,16 @@ static int enqueue_parse(T2Parse* J, const uint8_t* cs, uint32_t n, uint32_t nti
                                                            J->d_kmax, J->d_tile_first, J->nblocks, tags, J->d_blk, J->d_tags, J->d_indexed,
                                                            J->d_marked, sop, eph, J->d_status);
   b2k_count_launch();
+  if(d_dec && J->window)
+  {
+    k_t2_window_at<<<1, 1024, 0, st>>>(J->d_sd, J->d_status, n);
+    b2k_count_launch();
+  }
   if(d_dec && J->ncoded)
   {
     k_t2_desc<<<(unsigned)((n * J->ncoded + 127) / 128), 128, 0, st>>>(J->d_sd, n, J->d_blk, J->nblocks, J->d_coded, (uint32_t)J->ncoded,
                                                                        d_enc, d_quant, d_dec, J->d_win, J->d_need, J->d_parts, J->d_head,
-                                                                       J->d_body_at, J->d_status);
+                                                                       box.tiles(), J->d_body_at, J->d_status);
     b2k_count_launch();
   }
   T2P_TRY(cudaMemcpyAsync(J->h_status, J->d_status, n * sizeof(ParseStatus), cudaMemcpyDeviceToHost, st));
@@ -449,47 +463,80 @@ int b2k_t2_batch_enqueue(T2Parse* J, const uint8_t* arena, uint32_t n, const uin
     return -1;
   }
   for(uint32_t s = 0; s < n; ++s)
-    J->h_sd[s] = StreamDesc{at[s], len[s], sot[s], 0, 0};
+    J->h_sd[s] = StreamDesc{at[s], len[s], sot[s], 0, 0, nullptr};
   return enqueue_parse(J, arena, n, J->ntiles, TileBox{J->ntiles, 0, 0, J->ntiles, 1}, J->d_count, d_enc, d_quant, d_dec, st);
 }
 
 uint32_t b2k_t2_parse_streams(const T2Parse* J) { return J->streams; }
 
-int b2k_t2_window_enqueue(T2Parse* J, const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t grid_nx, uint32_t ntiles,
-                          const b2k::t2::WindowCoding& wc, const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
+int b2k_t2_window_enqueue(T2Parse* J, uint32_t n, const uint8_t* const* cs, const uint64_t* len, const uint64_t* sot,
+                          const std::vector<Rect>* const* need, const TileBox& box, uint32_t ntiles, const HtBlockDesc* d_enc,
+                          const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st)
 {
-  if(ntiles > J->wcount_cap)
+  if(n > J->streams)
+  {
+    b2k_set_error("internal: more code streams than the parse was made for");
+    return -1;
+  }
+  if((uint64_t)n * ntiles > J->wcount_cap)
   {
     cudaFree(J->d_wcount);
     J->d_wcount = nullptr;
     J->wcount_cap = 0;
-    T2P_TRY(cudaMalloc(&J->d_wcount, ntiles * sizeof(uint32_t)));
-    J->wcount_cap = ntiles;
+    const uint64_t cap = (uint64_t)J->streams * ntiles;
+    T2P_TRY(cudaMalloc(&J->d_wcount, cap * sizeof(uint32_t)));
+    J->wcount_cap = cap;
   }
-  NeedRects& n = *J->h_need;
-  n.n = (uint32_t)std::min<size_t>(wc.need.size(), B2K_MAX_RES);
-  for(uint32_t r = 0; r < n.n; ++r)
+  for(uint32_t s = 0; s < n; ++s)
   {
-    n.r[r][0] = wc.need[r].x0;
-    n.r[r][1] = wc.need[r].y0;
-    n.r[r][2] = wc.need[r].x1;
-    n.r[r][3] = wc.need[r].y1;
+    NeedRects& N = J->h_need[s];
+    N.n = need[s] ? (uint32_t)std::min<size_t>(need[s]->size(), WINDOW_MAX_RES) : 0;
+    for(uint32_t r = 0; r < N.n; ++r)
+    {
+      const Rect& R = (*need[s])[r];
+      N.r[r][0] = R.x0;
+      N.r[r][1] = R.y0;
+      N.r[r][2] = R.x1;
+      N.r[r][3] = R.y1;
+    }
+    J->h_sd[s] = StreamDesc{0, len[s], sot[s], 0, 0, cs[s]};
   }
-  J->h_sd[0] = StreamDesc{0, len, sot, 0, 0};
-  return enqueue_parse(J, cs, 1, ntiles, TileBox{grid_nx, wc.ta_x, wc.ta_y, wc.tb_x, wc.tb_y}, J->d_wcount, d_enc, d_quant, d_dec, st);
+  return enqueue_parse(J, nullptr, n, ntiles, box, J->d_wcount, d_enc, d_quant, d_dec, st);
 }
 
-uint64_t b2k_t2_window_bytes(const T2Parse* J) { return J->h_status->bytes; }
-
-int b2k_t2_window_gather(const T2Parse* J, const uint8_t* cs, uint8_t* out, cudaStream_t st)
+uint64_t b2k_t2_window_bytes(const T2Parse* J)
 {
-  const uint32_t nparts = J->h_status->nparts;
-  const uint64_t bytes = J->h_status->bytes;
-  if(!nparts || !bytes)
+  uint64_t bytes = 0;
+  for(uint32_t s = 0; s < J->last_n; ++s)
+    if(status_reason(J->h_status[s]) == PR_NONE)
+      bytes += J->h_status[s].bytes;
+  return bytes;
+}
+
+uint64_t b2k_t2_window_arena(const T2Parse* J)
+{
+  uint64_t bytes = 0;
+  for(uint32_t s = 0; s < J->last_n; ++s)
+    bytes += window_gathered_bytes(J->h_status[s]);
+  return bytes;
+}
+
+int b2k_t2_window_gather(const T2Parse* J, uint8_t* out, cudaStream_t st)
+{
+  uint64_t per = 0, bytes = 0, parts = 0;
+  for(uint32_t s = 0; s < J->last_n; ++s)
+    if(status_reason(J->h_status[s]) == PR_NONE)
+    {
+      per = std::max<uint64_t>(per, J->h_status[s].nparts);
+      bytes += J->h_status[s].bytes;
+      parts += J->h_status[s].nparts;
+    }
+  if(!parts || !bytes)
     return 0;
-  const uint64_t per_part = bytes / nparts;
-  const unsigned gx = (unsigned)std::min<uint64_t>(256, per_part / (256 * 16) + 1);
-  k_t2_gather<<<dim3(gx, std::min<uint32_t>(nparts, 65535)), 256, 0, st>>>(cs, J->d_parts, J->d_body_at, nparts, out);
+  const uint64_t items = J->last_n * per;
+  const unsigned gx = (unsigned)std::min<uint64_t>(256, bytes / parts / (256 * 16) + 1);
+  k_t2_gather<<<dim3(gx, (unsigned)std::min<uint64_t>(items, 65535)), 256, 0, st>>>(J->d_sd, J->d_parts, J->d_body_at, J->d_status, items,
+                                                                                     per, out);
   b2k_count_launch();
   T2P_TRY(cudaGetLastError());
   return 0;

@@ -5,6 +5,7 @@
 #include <vector>
 #include "b2k_internal.h"
 #include "t2_plan.h"
+#include "t2_parse.h"
 
 struct T2Parse; /* a job's packet plan and device buffers for one progression order and SOP / EPH setting */
 
@@ -43,22 +44,28 @@ void b2k_t2_parse_stats(const T2Parse* j, uint32_t* indexed, uint32_t* walked);
 /* after a result of 0: the block table b2k_codestream_parse returns (offsets into cs) into out[0, nblocks) */
 int b2k_t2_parse_blocks(const T2Parse* j, b2k_block* out, cudaStream_t st);
 
-/* ---- windowed parse (b2k_codestream_parse_window on a stream in device memory) ----------------------------------------
+/* ---- windowed parse (b2k_codestream_parse_window on streams in device memory; a single stream is a batch of one) -------
  * The plan is the box coding's (wc.box: the wanted tiles at full resolution), so the same five launches parse exactly the
- * wanted tiles' packets; the virtual coding's blocks vblocks[0, nv) map onto box blocks, and its coded blocks
- * vblocks[coded_index[k]] get descriptors.  Keyed by the box coding, flags and reduce.  0, or -1 with b2k_last_error set. */
+ * wanted tiles' packets of every stream; the virtual coding's blocks vblocks[0, nv) map onto box blocks, and its coded
+ * blocks vblocks[coded_index[k]] get descriptors.  Keyed by the box coding, flags, reduce and the stream capacity.  0, or
+ * -1 with b2k_last_error set. */
 int b2k_t2_window_create(const b2k::t2::WindowCoding& wc, uint32_t flags, uint32_t reduce, const b2k_block* vblocks, uint64_t nv,
-                         const uint32_t* coded_index, uint64_t ncoded, T2Parse** out);
-bool b2k_t2_window_matches(const T2Parse* j, const b2k_coding& box, uint32_t flags, uint32_t reduce);
-/* on st: the parse of cs[0, len) (read in place) for the wanted tiles of a stream of ntiles tiles, grid_nx wide, with
-   wc's need rectangles; the descriptors address the packet data as b2k_t2_window_gather lays it out */
-int b2k_t2_window_enqueue(T2Parse* j, const uint8_t* cs, uint64_t len, uint64_t sot, uint32_t grid_nx, uint32_t ntiles,
-                          const b2k::t2::WindowCoding& wc, const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec,
-                          cudaStream_t st);
-/* after the status: bytes of packet data in the wanted tiles' parts */
+                         const uint32_t* coded_index, uint64_t ncoded, T2Parse** out, uint32_t streams = 1);
+bool b2k_t2_window_matches(const T2Parse* j, const b2k_coding& box, uint32_t flags, uint32_t reduce, uint32_t streams);
+/* on st: the parse of the n streams cs[s][0, len[s]) (read in place, each from its own buffer; sot[s] = 0: not parsed) for
+   the tiles of `box` among each stream's ntiles, with need[s]'s rectangles (NULL or empty: no filter); with d_dec the
+   arena layout (each stream's gathered packet data at a 256-byte boundary) and descriptor s * ncoded + k of every stream's
+   coded block k, addressing the bytes where b2k_t2_window_gather puts them.  The statuses to the host. */
+int b2k_t2_window_enqueue(T2Parse* j, uint32_t n, const uint8_t* const* cs, const uint64_t* len, const uint64_t* sot,
+                          const std::vector<b2k::Rect>* const* need, const b2k::t2::TileBox& box, uint32_t ntiles,
+                          const HtBlockDesc* d_enc, const float* d_quant, HtBlockDesc* d_dec, cudaStream_t st);
+/* after the status: bytes of packet data in the wanted tiles' parts, over the streams that parsed */
 uint64_t b2k_t2_window_bytes(const T2Parse* j);
-/* on st, one launch: those bytes from cs, end to end, into out (b2k_t2_window_bytes of them) */
-int b2k_t2_window_gather(const T2Parse* j, const uint8_t* cs, uint8_t* out, cudaStream_t st);
-/* after a result of 0: b2k_codestream_parse_window's block table (offsets into cs) of the virtual coding into out[0, nv) */
+/* after the status: the arena bytes the gather lays the streams' packet data out in (the decoder's slack not included) */
+uint64_t b2k_t2_window_arena(const T2Parse* j);
+/* on st, one launch: the packet data of the streams that parsed, from their buffers into out as the descriptors address it */
+int b2k_t2_window_gather(const T2Parse* j, uint8_t* out, cudaStream_t st);
+/* after a result of 0 (a batch of one): b2k_codestream_parse_window's block table (offsets into cs) of the virtual coding
+   into out[0, nv) */
 int b2k_t2_window_blocks(const T2Parse* j, const b2k_block* vblocks, uint64_t nv, const std::vector<b2k::Rect>& need, b2k_block* out,
                          cudaStream_t st);

@@ -515,13 +515,17 @@ B2K_HD bool window_needs(const uint32_t* need, uint32_t x0, uint32_t y0, uint32_
 
 /* ---- batches: n code streams of one coding parsed by the same five launches -------------------------------------------
  * The plan (packets, tag-tree offsets, Kmax) is shared; every other piece of parse state is sliced per stream.  Stream s
- * lies at byte at of the arena (batch_arena_next), its tile parts in entries [parts0, parts0 + parts_cap) of the part
+ * lies at byte at of the arena (batch_arena_next) or, in a windowed batch, is read in place from its own buffer, its gathered
+ * packet data going to byte at of the arena (window_arena_at); its tile parts in entries [parts0, parts0 + parts_cap) of the part
  * table (a prefix sum of part_capacity), and its blocks, packets, tiles and tag scratch in slice s of their arrays.
  * sot = 0: the stream failed before its tile parts and is not parsed. */
 struct StreamDesc
 {
   uint64_t at, len, sot, parts0, parts_cap;
+  const uint8_t* base; /* the stream's own buffer, read in place (a windowed batch); NULL: the stream is byte `at` of the arena */
 };
+/* stream s's first byte: its own buffer, or its place in the arena */
+B2K_HD const uint8_t* stream_bytes(const uint8_t* arena, const StreamDesc& D) { return D.base ? D.base : arena + D.at; }
 /* item i of stream s in a launch over n streams of `per` items each, flattened as g = s * per + i */
 struct StreamItem
 {
@@ -589,7 +593,7 @@ B2K_HD uint32_t status_reason(const ParseStatus& st)
 }
 
 /* The five kernels' threads over a batch (t2_decode.cu runs them as kernels, tests/t2_batch_check.cpp on the host in the same
- * order).  cs is the arena; stream s is sd[s], its status status[s].  A stream whose status is set before the first step
+ * order).  cs is the arena; stream s is sd[s] (stream_bytes), its status status[s].  A stream whose status is set before the first step
  * (PR_SKIPPED) is left alone.  The per-stream arrays are sliced: head / last (bt = box.tiles() each), count (ntiles each),
  * indexed / marked (plan tiles each), blk (nblocks each), start / end / part_end (np each), tags (tag_nodes each). */
 /* step 1, thread s: the tile-part walk of stream s */
@@ -602,7 +606,7 @@ B2K_HD void batch_locate(const uint8_t* cs, const StreamDesc* sd, uint32_t s, ui
   const uint64_t bt = box.tiles();
   uint32_t np = 0;
   uint64_t bytes = 0;
-  status[s].locate = locate_tile_parts_box(cs + D.at, D.len, D.sot, ntiles, box, parts + D.parts0, D.parts_cap, head + s * bt, last + s * bt,
+  status[s].locate = locate_tile_parts_box(stream_bytes(cs, D), D.len, D.sot, ntiles, box, parts + D.parts0, D.parts_cap, head + s * bt, last + s * bt,
                                            count + (uint64_t)s * ntiles, &np, body_at ? body_at + D.parts0 : nullptr, &bytes);
   status[s].nparts = np;
   status[s].bytes = bytes;
@@ -623,7 +627,7 @@ B2K_HD void batch_plt(const uint8_t* cs, const StreamDesc* sd, uint64_t g, const
     blk[i] = ParsedBlock{};
   const Part T = tiles[t];
   const uint64_t o = s * np;
-  const bool ix = plt_index(cs + sd[s].at, parts + sd[s].parts0, head[g], T.p1 - T.p0, start + o + T.p0, end + o + T.p0, part_end + o + T.p0);
+  const bool ix = plt_index(stream_bytes(cs, sd[s]), parts + sd[s].parts0, head[g], T.p1 - T.p0, start + o + T.p0, end + o + T.p0, part_end + o + T.p0);
   indexed[g] = ix;
   marked[g] = 0;
   if(ix && T.p1 > T.p0)
@@ -646,7 +650,7 @@ B2K_HD void batch_packet(const uint8_t* cs, const StreamDesc* sd, uint64_t g, co
     return;
   uint64_t at = start[g];
   const Packet& P = packets[it.i];
-  if(parse_packet(cs + sd[s].at, P, &at, part_end[g], kmax, blk + s * nblocks, tags + s * tag_nodes + P.tag_at, sop, eph) != PR_NONE ||
+  if(parse_packet(stream_bytes(cs, sd[s]), P, &at, part_end[g], kmax, blk + s * nblocks, tags + s * tag_nodes + P.tag_at, sop, eph) != PR_NONE ||
      at != end[g])
     marked[t] = 1; /* the walk decides */
 }
@@ -672,7 +676,7 @@ B2K_HD void batch_walk(const uint8_t* cs, const StreamDesc* sd, uint64_t g, cons
       blk[i] = ParsedBlock{};
   if(head[g] != PART_NONE)
     status_add(&status[s].walked, 1u);
-  const uint32_t r = parse_tile(cs + sd[s].at, parts + sd[s].parts0, head[g], packets + T.p0, T.p1 - T.p0, kmax, blk,
+  const uint32_t r = parse_tile(stream_bytes(cs, sd[s]), parts + sd[s].parts0, head[g], packets + T.p0, T.p1 - T.p0, kmax, blk,
                                 tags + s * tag_nodes + packets[T.p0].tag_at, sop, eph);
   if(r != PR_NONE)
     status_min(&status[s].tile_err, ((unsigned long long)t << 8) | r);
@@ -696,6 +700,76 @@ B2K_HD uint64_t gathered_offset(const PartRange* parts, uint32_t first, const ui
     if(off >= parts[p].begin && off < parts[p].end)
       return body_at[p] + (off - parts[p].begin);
   return 0;
+}
+
+/* ---- windowed batches: n streams parsed against the plan of one box coding, read in place -----------------------------
+ * Every stream wants the same tile box; its tile parts are recorded under their box tile index (batch_locate with the box
+ * and body_at), and only their packet data is gathered into the arena, stream s's at sd[s].at (window_arena_at). */
+constexpr uint32_t WINDOW_MAX_RES = 33; /* resolutions of a coding (B2K_MAX_RES) */
+/* a coded block of the virtual coding (the plan's, shared by every stream): its box tile, the need rectangle that applies
+   to it (resolution max(resno - 1, 0)) and its rectangle in band coordinates */
+struct WinBlock
+{
+  uint32_t tile, res, x0, y0, x1, y1;
+};
+/* one stream's need rectangles, one per resolution of the virtual coding; n = 0: no filter */
+struct NeedRects
+{
+  uint32_t n;
+  uint32_t r[WINDOW_MAX_RES][4];
+};
+
+/* the arena bytes stream s's gathered packet data takes: its wanted parts' packet data up to the next 256-byte boundary
+   (batch_arena_next), none when its tile-part walk failed or it is not parsed */
+B2K_HD uint64_t window_gathered_bytes(const ParseStatus& st) { return st.locate == PR_NONE ? batch_arena_next(0, st.bytes) : 0; }
+
+/* where each stream's gathered data starts: sd[s].at for s in [s0, s1), from `at` on (the streams laid end to end) */
+B2K_HD uint64_t window_arena_at(StreamDesc* sd, const ParseStatus* status, uint32_t s0, uint32_t s1, uint64_t at)
+{
+  for(uint32_t s = s0; s < s1; ++s)
+  {
+    sd[s].at = at;
+    at += window_gathered_bytes(status[s]);
+  }
+  return at;
+}
+
+/* step 5 of a windowed batch, thread g = s * ncoded + k: batch_block's block, left uncoded when stream s's need rectangles
+   leave it out, and *slot_off: where its bytes lie in the arena once k_t2_gather has put stream s's wanted parts' packet
+   data end to end at sd[s].at.  win[k] is coded block k's; head is sliced per stream (bt box tiles each), parts and
+   body_at from sd[s].parts0 */
+B2K_HD ParsedBlock window_block(const ParsedBlock* blk, uint64_t nblocks, const uint32_t* coded, uint64_t g, uint64_t ncoded,
+                                const ParseStatus* status, const StreamDesc* sd, const WinBlock* win, const NeedRects* need,
+                                const PartRange* parts, const uint32_t* head, uint32_t bt, const uint64_t* body_at, uint32_t* s_out,
+                                uint64_t* slot_off)
+{
+  ParsedBlock b = batch_block(blk, nblocks, coded, g, ncoded, status, s_out);
+  const uint32_t s = *s_out;
+  const WinBlock w = win[g % ncoded];
+  const NeedRects& N = need[s];
+  if(b.length && N.n && !window_needs(N.r[w.res], w.x0, w.y0, w.x1, w.y1))
+    b = ParsedBlock{};
+  const StreamDesc& D = sd[s];
+  *slot_off = D.at + (b.length ? gathered_offset(parts + D.parts0, head[(uint64_t)s * bt + w.tile], body_at + D.parts0, b.offset) : 0);
+  return b;
+}
+
+/* the gather of a windowed batch, item g = s * per + j (per: the most parts a stream recorded): part j of stream s, when
+   stream s parsed and recorded it -- len bytes from *src to arena byte *dst.  False: nothing to copy */
+B2K_HD bool window_gather_part(const StreamDesc* sd, const PartRange* parts, const uint64_t* body_at, const ParseStatus* status, uint64_t g,
+                               uint64_t per, const uint8_t** src, uint64_t* dst, uint64_t* len)
+{
+  const StreamItem it = split_stream_item(g, per);
+  const StreamDesc& D = sd[it.s];
+  if(status_reason(status[it.s]) != PR_NONE || it.i >= status[it.s].nparts)
+    return false;
+  const PartRange R = parts[D.parts0 + it.i];
+  if(R.end <= R.begin)
+    return false;
+  *src = D.base + R.begin;
+  *dst = D.at + body_at[D.parts0 + it.i];
+  *len = R.end - R.begin;
+  return true;
 }
 
 } // namespace t2

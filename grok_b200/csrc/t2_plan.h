@@ -70,6 +70,12 @@ int b2k_parse_main_header(const uint8_t* cs, uint64_t len, b2k::t2::MainHeader& 
    another progression order, SOP or EPH) */
 int b2k_batch_coding_check(const b2k::t2::MainHeader& ref, uint32_t ref_index, const b2k::t2::MainHeader& h, uint32_t index);
 
+/* a windowed batch (b2k_decode_codestreams_window_device) takes the window coding ref_wc of stream ref_index (main header
+   ref): 0 when stream `index` (main header h, window coding wc) may join it -- the same virtual coding, box coding, tile
+   grid and wanted tiles, progression order, SOP and EPH -- else 1 with b2k_last_error naming both streams */
+int b2k_batch_window_check(const b2k::t2::MainHeader& ref, const b2k::t2::WindowCoding& ref_wc, uint32_t ref_index,
+                           const b2k::t2::MainHeader& h, const b2k::t2::WindowCoding& wc, uint32_t index);
+
 /* the wanted tiles, the virtual coding and the window's need rectangles of b2k_codestream_parse_window(window, reduce) on a
    stream of coding cp: 0, or its return code and text for the window errors, in its order */
 int b2k_window_coding(const b2k_coding& cp, const uint32_t* window, uint32_t reduce, b2k::t2::WindowCoding& w);

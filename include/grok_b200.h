@@ -613,6 +613,32 @@ B2K_API int32_t b2k_decode_codestream_window_device(b2k_engine* e, const uint8_t
 /* last windowed device parse: wanted tiles, and bytes of their tile parts copied into the job's arena (the packet data of
  * their tile parts; the whole stream when every tile was wanted at reduce 0) */
 B2K_API int32_t b2k_codestream_window_device_stats(b2k_engine* e, uint32_t* tiles_wanted, uint64_t* arena_bytes);
+/* A batch of windows: n HTJ2K code streams in device memory, each with its own window (windows[4 i .. 4 i + 3] = x0, y0,
+ * x1, y1 on its full-resolution canvas; windows == NULL: every whole image) and one `reduce` -> n images in device memory,
+ * in one launch chain.  status[i] and b2k_decode_codestreams_error(e, i) are what b2k_decode_codestream_window_device(e,
+ * cs[i], len[i], &windows[4 i], reduce, &imgs[i], ...) returns alone and its b2k_last_error text, the checks in the same
+ * order: cs[i]'s memory, the main header, the window (b2k_codestream_parse_window's window errors), the tile parts and
+ * packets of the wanted tiles only (damage outside the window passes, as it does alone), imgs[i], the HT decoder's
+ * verdict on stream i's blocks.  Status 0: imgs[i] holds exactly the single call's pixels and rects_out[4 i .. 4 i + 3]
+ * is its rect_out; any other status (-2 included): imgs[i] is not written.
+ * The batch's coding is the virtual coding of the lowest-index stream whose header and window pass (*cp_out receives it).
+ * Another stream whose virtual coding, tile grid or wanted tiles differ, or whose progression order, SOP or EPH differ,
+ * gets status 1 with a text naming that stream.  So any windows go together for single-tile streams (the box is always
+ * the one tile); tiled streams go together when their windows touch the same tiles, e.g. one window for the whole batch.
+ * Different tile boxes in one call are not supported.
+ * imgs == NULL: headers only -- cp_out, rects_out and the statuses up to the coding match.  rects_out holds zeros for a
+ * stream that fails before its window's coding.  Streams are read in place after the work queued on cuda_stream, which
+ * then waits for the image writes; only the wanted tiles' packet data is copied, into the engine's arena.
+ * Synchronisations: the header prefixes, the parse statuses, the end (as b2k_decode_codestreams_device).  For a fixed
+ * virtual coding the launch count does not depend on n once n x tiles reaches the pipeline's chunk count.
+ * Memory: the batch job of the virtual coding (n virtual-image-sized int32 plane sets), kept as b2k_decode_codestreams_device
+ * keeps its own.  Returns < 0 for a failure of the whole call (NULL arrays, n == 0, imgs whose sample_bytes differ, a CUDA
+ * error), b2k_last_error set; else the number of streams whose status is not 0.  b2k_codestream_window_device_stats then
+ * reports the box's wanted tiles and the bytes gathered for all streams together. */
+B2K_API int32_t b2k_decode_codestreams_window_device(b2k_engine* e, uint32_t n, const uint8_t* const* cs, const uint64_t* len,
+                                                     const uint32_t* windows, uint32_t reduce, const b2k_device_planes* imgs,
+                                                     void* cuda_stream, b2k_coding* cp_out, uint32_t* rects_out, int32_t* status,
+                                                     double* ms_total);
 
 /* Geometry only (host): enumerate the blocks of the selected tiles, lengths zero.  Returns the
  * count; fills at most cap entries. */
